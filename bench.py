@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- MJump/s of the B200 kangaroo jump engine (BASELINE.json metric) + roofline + CPU baseline.
+"""bench.py -- MJump/s of the H100 kangaroo jump engine (BASELINE.json metric) + roofline + CPU baseline.
 
-One "step" = one GPUEngine::Launch on the full herd: NB_RUN=64 jumps for every kangaroo of the default B200
-grid (2*148 x 128 threads x 128 = 4,849,664 kangaroos, the size the reference's GetGridSize picks,
-GPUEngine.cu:301-303), jump table of the in80 configuration (VC_CUDA8/in80.txt: 2^79.8 range -> rangePower 80,
+One "step" = one GPUEngine::Launch on the full herd: NB_RUN=64 jumps for every kangaroo of the default
+grid (2*SMs x 128 threads x 128; on an H100 SXM 2*132 x 128 x 128 = 4,325,376 kangaroos, the size the reference's
+GetGridSize picks, GPUEngine.cu:301-303), jump table of the in80 configuration (VC_CUDA8/in80.txt: 2^79.8 range -> rangePower 80,
 dp = 16), the reference's own throughput accounting `nbKangaroo * NB_RUN` per Launch (Kangaroo.cpp:575).
 
   value : jumps / device time of exactly K launches (state resident in HBM, DP slabs left on the device)
@@ -12,18 +12,20 @@ dp = 16), the reference's own throughput accounting `nbKangaroo * NB_RUN` per La
           them, exactly what Kangaroo::SolveKeyGPU consumes.  The herd itself is resident by design of the
           reference interface (SetKangaroos once, GPUEngine.cu:381-433), so h2d per step is 0 payload bytes.
   roofline : integer-multiply bound (SURVEY.md 8d): 416 IMAD.WIDE per jump (5 ModMult x 74 + ModSqr x 46) against
-          the MEASURED wide-IMAD issue rate of this box (scripts/ubench, profiles/), plus the HBM view.
+          the wide-IMAD issue rate measured in the same run (kgx_bench_raw), plus the HBM view.
   cpu_baseline : the reference's SolveKeyCPU inner loop (oracle/_ref/libkref.so = unmodified SECPK1 code) on all
           host cores for a bounded sample.
 
 `--impl reference` times that CPU implementation alone.  Under torchrun (N>1) one rank per GPU, independent
 herds (weak scaling), DP records gathered to rank 0 over NCCL every step.
+`--dump-outputs DIR` writes what the last timed step computed (see dump_outputs) so two builds can be compared.
 """
 import argparse
 import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -46,14 +48,14 @@ def host_cores():
 
 
 _CPU_THREADS = None
-CALIB_PATH = os.path.join(ROOT, ".kgx_cpu_calibration.json")
+CALIB_PATH = os.path.join(tempfile.gettempdir(), "kgx_cpu_calibration.json")   # never inside the (possibly read-only) tree
 
 
 def cpu_threads(be):
-    """Thread count of the CPU arm, calibrated ONCE per box and shared by `--impl reference`, the cpu_baseline leg and the
-    product-level run (VERDICT r1 weak #6: two calibrations in one driver run picked 64 and 32 threads).  The visible CPU
-    count can exceed what the container may run (cgroup quota), so the candidate with the best short-run rate is kept and
-    cached on disk next to bench.py, keyed by host name and visible core count."""
+    """Thread count of the CPU arm, calibrated ONCE per host and shared by `--impl reference`, the cpu_baseline leg and the
+    product-level run, so that all three use the same count.  The visible CPU count can exceed what the container may run
+    (cgroup quota), so the candidate with the best short-run rate is kept and cached in the temporary directory, keyed by
+    host name and visible core count."""
     global _CPU_THREADS
     if _CPU_THREADS is not None:
         return _CPU_THREADS
@@ -140,8 +142,8 @@ def cpu_product_run(threads, seconds=20.0):
 
 
 class ClockSampler(threading.Thread):
-    """One long-lived `nvidia-smi -lms 50` whose lines are stamped on arrival; result() keeps the samples that fell
-    inside the timed regions (the recipe's clocks line, B200_PROFILING.md)."""
+    """One long-lived `nvidia-smi -lms 50` (read-only queries) whose lines are stamped on arrival; result() keeps the
+    samples that fell inside the timed regions."""
     Q = "clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
     NAMES = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
@@ -202,7 +204,7 @@ def load_in80_table():
 def build_herd(eng, case, rank):
     """Synthetic herd shaped like Kangaroo::CreateHerd (Kangaroo.cpp:670-738): every kangaroo gets its own uniform
     random distance in the 2^80 range (numpy PCG64, seeded per rank), wild ones shifted by -width/2 (mod n) and started
-    at key + d*G.  The point arithmetic runs on the device (kgx_create_herd), so all 4.85 M walkers are distinct valid
+    at key + d*G.  The point arithmetic runs on the device (kgx_create_herd), so all walkers are distinct valid
     curve points; no part of the oracle is involved."""
     import numpy as np
     from kangaroo_b200 import random_herd_arrays
@@ -270,6 +272,38 @@ def shim_run(prep, gx, gy, local_rank, dp, warmup, steps):
             pass
 
 
+def _limbs32(a):
+    """(n, k) uint64 limbs -> (n, 2k) float64 of 32-bit limbs, little-endian: exact in float64."""
+    import numpy as np
+    return np.ascontiguousarray(a, dtype=np.uint64).view(np.uint32).astype(np.float64)
+
+
+def dump_outputs(out_dir, eng, lib, max_found, sample=65536, seed=0):
+    """What the last timed launch computed, as a caller of the device-resident path receives it: the DP records of that
+    launch (sorted by kangaroo index, then x: their order in the slab depends on thread timing) and the herd state it
+    leaves behind, for a fixed seeded sample of kangaroos.  Every array is float64 (256-bit values as 32-bit limbs)."""
+    import ctypes
+    import numpy as np
+    from kangaroo_b200._lib import Item
+    os.makedirs(out_dir, exist_ok=True)
+    items = (Item * max_found)()
+    nI, nF = ctypes.c_uint32(0), ctypes.c_uint32(0)
+    rc = lib.kgx_collect(eng._h, items, max_found, ctypes.byref(nI), ctypes.byref(nF), 0, 0)   # no relaunch: read the slab
+    assert rc == 0, lib.kgx_last_error(eng._h)
+    raw = np.frombuffer(items, dtype=np.uint64, count=int(nI.value) * 7).reshape(-1, 7)
+    words = raw.view(np.uint32)                                       # x: words 0..7, d: 8..11, kidx: 12..13
+    order = np.lexsort(tuple(words[:, w] for w in range(7, -1, -1)) + (raw[:, 6],))
+    raw = raw[order]
+    ax, ay, ad = eng.GetKangaroosRaw()
+    rng = np.random.Generator(np.random.PCG64(seed))
+    idx = np.sort(rng.choice(ax.shape[0], size=min(sample, ax.shape[0]), replace=False))
+    arrays = {"dp_count": np.array([nF.value], dtype=np.float64), "dp_x": _limbs32(raw[:, 0:4]), "dp_d": _limbs32(raw[:, 4:6]),
+              "dp_kidx": raw[:, 6].astype(np.float64), "state_index": idx.astype(np.float64),
+              "state_x": _limbs32(ax[idx]), "state_y": _limbs32(ay[idx]), "state_d": _limbs32(ad[idx])}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -279,7 +313,11 @@ def main():
     ap.add_argument("--grid", default="", help="x,y override (default 2*SMs,128)")
     ap.add_argument("--dp", type=int, default=16)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the DP records and a sampled herd state of the last timed step as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
 
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -331,7 +369,7 @@ def main():
     herd_scalars = build_herd(eng, case, rank)
     try:
         shim_prep = shim_prepare(eng, case, herd_scalars, local_rank)
-    except OSError as exc:                                         # e.g. no room for the 466 MB herd file: keep the C-ABI e2e leg
+    except OSError as exc:                                         # e.g. no room for the ~0.4 GB herd file: keep the C-ABI e2e leg
         print("bench.py: C++ shim leg skipped on rank %d: %s" % (rank, exc), file=sys.stderr)
         shim_prep = None
     del herd_scalars
@@ -377,6 +415,8 @@ def main():
     # the K timed launches are exactly the K kernels completed inside the region: (K-1) collected + the one synced
     kernel_ms = kernel_ms[1:] + [eng.last_launch_ms()]
     dev_s = sum(kernel_ms) / 1e3
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, lib, max_found)
 
     # ---- end-to-end leg through the C ABI with HOST buffers: kgx_collect(..., relaunch=1) is exactly the body of
     # GPUEngine::Launch (GPUEngine.cu:607-679): wait for the kernel, start the next one, copy this launch's DP records
@@ -448,7 +488,7 @@ def main():
 
     if rank == 0:
         clocks = sampler.result()
-        mhz = clocks["sm_mhz"] or 1965.0
+        mhz = clocks["sm_mhz"] or clocks["sm_max_mhz"] or 1980.0    # 1980 MHz: H100 SXM maximum SM clock
         sms = torch.cuda.get_device_properties(local_rank).multi_processor_count
         # multiplier roofline: IMAD.WIDE.U32 issue rate measured NOW on this GPU (kgx_bench_raw kind 0, best of 3)
         imad_peak = 0.0
@@ -457,7 +497,7 @@ def main():
             assert lib.kgx_bench_raw(local_rank, 0, 20000, ctypes.byref(ms_), ctypes.byref(ops_)) == 0
             imad_peak = max(imad_peak, ops_.value / (ms_.value * 1e-3))
         # second measured view: what the multiplier pipe sustains inside real carry chains (kgx_bench_raw kind 1: dependent fe_mul
-        # chains, 73 wide IMAD each) -- on B200 this runs ABOVE the accumulate-probe, so the larger of the two is the measured peak
+        # chains, 73 wide IMAD each) -- it can run above the accumulate-probe, so the larger of the two is the measured peak
         chain_peak = 0.0
         for _ in range(2):
             ms_, ops_ = ctypes.c_float(0), ctypes.c_double(0)
@@ -468,15 +508,8 @@ def main():
         nominal_peak = sms * 32.0 * mhz * 1e6          # quarter-rate pipe: 32 lane-ops/clk/SM at the SM clock seen during the run
         achieved = kernel_value * 1e6 * ALGO_IMAD_PER_JUMP
         mode = eng.kernel
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get(mode)
-        except Exception:
-            traffic = None
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-            hbm_peak, hbm_src = float(peaks["hbm_gbs"]), "measured"
-        except Exception:
-            hbm_peak, hbm_src = 6650.0, "fallback"
+        hbm_peak, hbm_src = 3350.0, "H100 SXM data sheet (HBM3)"
+        l2_mb = torch.cuda.get_device_properties(local_rank).L2_cache_size / 2**20
         hbm_ach = kernel_value * 1e6 * ALGO_BYTES_PER_JUMP / 1e9
         out = dict(
             metric="MJump/s (kangaroo jumps/sec)", value=value, unit="MJump/s", n_gpus=world, steps=steps, warmup=max(warmup, 3),
@@ -484,7 +517,8 @@ def main():
             dtype="u32x8 (256-bit modular integer)", data="synthetic",
             config={"workload": "in80.txt: rangePower 80 jump table, dp=%d, grid %dx%d -> %d kangaroos/GPU x NB_RUN=64 jumps per step"
                                 % (args.dp, gx, gy, n),
-                    "state_bytes_per_gpu": n * 80, "l2_note": "388 MB of kangaroo state per GPU > 126 MB L2; every step streams all of it",
+                    "state_bytes_per_gpu": n * 80,
+                    "l2_note": "%.0f MB of kangaroo state per GPU > %.0f MB L2; every step streams all of it" % (n * 80 / 1e6, l2_mb),
                     "dp_found_per_step": found / max(steps, 1)},
             kernel_only={"value": kernel_value, "unit": "MJump/s/GPU", "ms_per_launch": dev_s / steps * 1e3,
                          "how": "CUDA events on the engine stream around each jump_kernel launch"},
@@ -500,19 +534,20 @@ def main():
             e2e_c_abi={"value": cabi_value, "unit": "MJump/s", "d2h_bytes_per_step": d2h / max(steps, 1),
                        "how": "kgx_collect(relaunch=1) from Python/ctypes into a host array of 56-byte items: the C ABI alone, no Int marshalling"},
             roofline={"bound": "imad", "achieved": achieved / 1e12, "peak": imad_peak / 1e12, "unit": "TIMAD/s (32x32->64 multiply-adds)",
-                      "frac": achieved / imad_peak, "traffic": traffic,
+                      "frac": achieved / imad_peak,
                       "algorithmic_imad_per_jump": ALGO_IMAD_PER_JUMP,
                       "peak_how": "best of two live measurements of the wide-multiply pipe on this GPU: independent IMAD.WIDE accumulate probe "
                                   "(kgx_bench_raw kind 0: %.2f T/s = %.1f lane-ops/clk/SM) and 73 x the dependent fe_mul-chain rate (kind 1: %.2f T/s "
-                                  "= %.1f lane-ops/clk/SM) at %.0f MHz on %d SMs; this pipe (fmaheavy), not HBM or tensor cores, bounds the kernel"
+                                  "= %.1f lane-ops/clk/SM) at %.0f MHz on %d SMs.  Whether this pipe or HBM (hbm.designed_frac) bounds the kernel is not "
+                                  "measured: no DRAM byte counter is read"
                                   % (probe_peak / 1e12, probe_peak / sms / (mhz * 1e6), chain_peak / 1e12, chain_peak / sms / (mhz * 1e6), mhz, sms),
                       "nominal": {"peak": nominal_peak / 1e12, "frac": achieved / nominal_peak,
                                   "how": "32 lane-ops/clk/SM (quarter-rate pipe) x %d SMs x %.0f MHz -- never reached by any probe" % (sms, mhz)},
-                      "traffic_how": "dram__bytes_read.sum + dram__bytes_write.sum per launch, ncu --set full (profiles/traffic.json)",
                       "hbm": {"bound": "hbm", "achieved": hbm_ach, "peak": hbm_peak, "unit": "GB/s", "frac": hbm_ach / hbm_peak,
                               "peak_source": hbm_src, "algorithmic_bytes_per_jump": ALGO_BYTES_PER_JUMP,
                               "designed_bytes_per_jump": DESIGN_BYTES_PER_JUMP.get(mode),
-                              "designed_gbs": kernel_value * 1e6 * DESIGN_BYTES_PER_JUMP.get(mode, 0) / 1e9}},
+                              "designed_gbs": kernel_value * 1e6 * DESIGN_BYTES_PER_JUMP.get(mode, 0) / 1e9,
+                              "designed_frac": kernel_value * 1e6 * DESIGN_BYTES_PER_JUMP.get(mode, 0) / 1e9 / hbm_peak}},
             kernel_mode=mode,
             gpu_launches=int(gpu_launches), clocks=clocks)
         if rt_steps:

@@ -1,5 +1,5 @@
 /*
- * kgx.h -- C ABI of the B200-native kangaroo jump engine (libkgx.so).
+ * kgx.h -- C ABI of the H100-native kangaroo jump engine (libkgx.so).
  *
  * This is the drop-in boundary for ONE path of JeanLucPons/Kangaroo: the GPU jump engine behind
  * `class GPUEngine` (reference GPU/GPUEngine.h:40-84, GPU/GPUEngine.cu).  The reference's interface is a C++
@@ -53,9 +53,9 @@ kgx_engine* kgx_create(int dev, int groups, int threads_per_group, uint32_t max_
 #define KGX_KERNEL_AUTO     0
 #define KGX_KERNEL_STREAM   1
 #define KGX_KERNEL_RESIDENT 2
-#define KGX_KERNEL_TMEM     3   /* tile kernel with y and the prefix products in tensor memory (tcgen05.ld/st): 2048-kangaroo tiles */
+#define KGX_KERNEL_TMEM     3   /* cluster tile kernel: one 1792-kangaroo tile in the shared memory of a 2-CTA cluster */
 kgx_engine* kgx_create_ex(int dev, int groups, int threads_per_group, uint32_t max_found, int kernel, int stream_g);
-/* 1 = stream kernel, 2 = resident kernel, 3 = TMEM tile kernel (what kgx_create / kgx_create_ex resolved to) */
+/* 1 = stream kernel, 2 = resident kernel, 3 = cluster tile kernel (what kgx_create / kgx_create_ex resolved to) */
 int         kgx_kernel_kind(kgx_engine* e);
 void        kgx_destroy(kgx_engine* e);
 const char* kgx_last_error(kgx_engine* e);      /* e may be NULL: error of the last failed kgx_create */

@@ -5,7 +5,7 @@
  * per DP `AddToTable` -> HashTable::Add (HashTable.cpp:221-307) -> on ADD_COLLISION `CollisionCheck`), and the server-side
  * drain of Thread.cpp:165-234, for the in-box multi-GPU case where the DP records of ALL ranks arrive on rank 0 as one
  * buffer per step (NCCL gather, kangaroo_b200/dist.py).  The table itself is the reference's own `class HashTable`,
- * UNCHANGED: this library is compiled against /root/reference (HashTable.cpp + SECPK1) exactly like the drop-in binary
+ * UNCHANGED: this library is compiled against the reference sources (HashTable.cpp + SECPK1) exactly like the drop-in binary
  * (kangaroo_b200/csrc/build_ingest.sh); only the driver around it is new: records are inserted by a pool of worker threads
  * sharded by bucket index (h mod threads) -- buckets are independent in the reference's table, so no lock is needed --
  * instead of one thread under one mutex.

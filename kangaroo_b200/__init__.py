@@ -1,4 +1,4 @@
-"""kangaroo_b200 -- B200-native (sm_100a) Pollard's-kangaroo jump engine for secp256k1.
+"""kangaroo_b200 -- H100-native (sm_90a) Pollard's-kangaroo jump engine for secp256k1.
 
 One hot path of JeanLucPons/Kangaroo rebuilt from scratch: the GPU jump engine behind `class GPUEngine`
 (reference GPU/GPUEngine.h:40-84).  The product is the CUDA library `csrc/libkgx.so` (C ABI: include/kgx.h);

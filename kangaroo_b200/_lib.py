@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.environ.get("KGX_LIB_OVERRIDE") or os.path.join(CSRC, "libkgx.so")   # override: A/B builds in scripts/ experiments
 HOSTTEST_PATH = os.path.join(CSRC, "libkgx_hosttest.so")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 
@@ -60,7 +60,7 @@ _lib = None
 
 
 def build_library(verbose=False):
-    """Compile every CUDA source for sm_100a into csrc/libkgx.so (nvcc cross-compiles without a GPU) and the
+    """Compile every CUDA source for sm_90a into csrc/libkgx.so (nvcc cross-compiles without a GPU) and the
     host-only unit-test helper csrc/libkgx_hosttest.so."""
     src = os.path.join(CSRC, "kgx_engine.cu")
     cmd = ["nvcc"] + NVCC_FLAGS + ["-o", LIB_PATH, src]

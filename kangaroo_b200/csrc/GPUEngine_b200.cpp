@@ -1,7 +1,7 @@
 // GPUEngine_b200.cpp -- drop-in implementation of the reference's `class GPUEngine` on top of libkgx.so.
 //
 // The class declaration is the reference's own, UNCHANGED header GPU/GPUEngine.h:40-84 (found on the include path
-// at build time: -I/root/reference; this file replaces GPU/GPUEngine.cu in the link).  Every member keeps the
+// at build time: -I$KANGAROO_REF; this file replaces GPU/GPUEngine.cu in the link).  Every member keeps the
 // semantics documented in SURVEY.md 8(b); the private data members of the verbatim header are reused as opaque
 // storage (inputKangaroo -> kgx_engine*, outputItemPinned -> kgx_item staging) because the header cannot change.
 //
@@ -132,7 +132,7 @@ void GPUEngine::SetParams(uint64_t dpMask, Int* distance, Int* px, Int* py) {  /
   if (kgx_set_params(KGX(inputKangaroo), dpMask, jd, jx, jy) != 0) printf("GPUEngine: SetParams: %s\n", kgx_last_error(KGX(inputKangaroo)));
 }
 
-// Int <-> limb marshalling of a whole herd (4.85 M kangaroos x 3 Int on the default grid) on several host threads: the
+// Int <-> limb marshalling of a whole herd (4.3 M kangaroos x 3 Int on the default H100 grid) on several host threads: the
 // checkpoint path (Kangaroo.cpp:618-626) parks the GPU thread on GetKangaroos, so its duration is GPU idle time.
 template <typename F>
 static void parallel_for(uint64_t n, F body) {

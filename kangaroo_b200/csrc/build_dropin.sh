@@ -1,5 +1,5 @@
 #!/bin/bash
-# build_dropin.sh -- link the reference's UNMODIFIED host program against the B200 engine.
+# build_dropin.sh -- link the reference's UNMODIFIED host program against the H100 engine.
 #   build/kangaroo_b200     = reference main.cpp Kangaroo.cpp Check.cpp Thread.cpp Backup.cpp Network.cpp Merge.cpp
 #                             PartMerge.cpp HashTable.cpp Timer.cpp SECPK1/*.cpp   (compiled where they lie, -DWITHGPU)
 #                           + kangaroo_b200/csrc/GPUEngine_b200.cpp (replaces GPU/GPUEngine.cu) + libkgx.so
@@ -8,9 +8,9 @@
 #                             engine mode behind the shim (SURVEY 8f/f4)
 #   build/kangaroo_b200_stats, build/kangaroo_b200_sym_stats = both again with the reference's -DSTATS
 #   build/kgx_shim_bench    = shim_bench.cpp: end-to-end timing through `class GPUEngine` (bench.py's e2e leg)
-# Needs the reference sources at $REF (default /root/reference); nothing is copied into the repo.
+# Needs the reference sources at $REF (default $KANGAROO_REF); nothing is copied into the repo.
 set -e
-REF=${REF:-/root/reference}
+REF=${REF:-$KANGAROO_REF}
 HERE=$(cd "$(dirname "$0")" && pwd)
 ROOT=$(cd "$HERE/../.." && pwd)
 OUT=$ROOT/build

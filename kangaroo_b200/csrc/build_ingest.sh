@@ -1,9 +1,9 @@
 #!/bin/bash
 # build_ingest.sh -- build/libkgx_ingest.so: the rank-0 DP ingest (kgx_ingest.cpp, C ABI include/kgx_ingest.h) linked
 # with the reference's UNMODIFIED HashTable.cpp + SECPK1 + Timer.cpp, compiled where they lie under $REF.
-# Needs the reference sources at build time only; the built library travels to the GPU box (build/ is git-ignored).
+# Needs the reference sources ($REF, default $KANGAROO_REF) at build time only; build/ is git-ignored.
 set -e
-REF=${REF:-/root/reference}
+REF=${REF:-$KANGAROO_REF}
 HERE=$(cd "$(dirname "$0")" && pwd)
 ROOT=$(cd "$HERE/../.." && pwd)
 OUT=$ROOT/build

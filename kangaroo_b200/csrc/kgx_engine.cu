@@ -1,4 +1,4 @@
-// kgx_engine.cu -- host side of the B200 jump engine behind the C ABI of include/kgx.h.
+// kgx_engine.cu -- host side of the H100 jump engine behind the C ABI of include/kgx.h.
 //
 // Replaces the host half of the reference's GPU/GPUEngine.cu (ctor/dtor :144-263, SetKangaroos/GetKangaroos/
 // SetKangaroo :381-538, callKernel :540-557, SetParams :559-590, Launch :607-679) with a stream-ordered
@@ -27,12 +27,12 @@ struct kgx_engine {
   uint4* state = nullptr;
   uint4* pre = nullptr;      // streaming mode: prefix-product scratch
   bool streamMode = false;
-  bool tmemMode = false;     // TMEM-backed tile kernel (jump_kernel_tmem<16>)
+  bool tmemMode = false;     // cluster tile kernel (jump_kernel_cluster; selector KGX_KERNEL_TMEM)
   int streamCtas = 2;
   bool symmetry = false;     // USE_SYMMETRY engine mode (kgx_set_symmetry): class switch + cycle rule, signed distances
   int symRule = 0;           // KGX_SYM_LASTJUMP / KGX_SYM_CLASS
-  int pfDist = 2;            // KGX_STREAM_PF: L2 prefetch distance of the stream kernel in kangaroos (measured: 0 -> 14.04,
-                             // 2 -> 14.44, 4 -> 14.40, 8 -> 14.24 GJump/s, profiles/r2c_sweep_prefetch.txt)
+  int pfDist = 2;            // KGX_STREAM_PF: L2 prefetch distance of the stream kernel in kangaroos (0 = off).  H100 SXM at
+                             // 700 W, default herd, kernel time: 0 -> 10.45, 2 -> 11.31, 4 -> 9.91 GJump/s (one run each)
   uint8_t* aux = nullptr;    // symmetric mode: lastJump per slot
   bool warpInv = true;       // stream kernel: one warp-wide shuffle-butterfly inverse per pass (false: one per thread)
   u32* slab[2] = {nullptr, nullptr};   // DP slabs [count][maxFound*14]
@@ -65,7 +65,7 @@ struct kgx_engine {
     }                                                                                          \
   } while (0)
 
-// Tile geometries compiled in.  The default was picked by the sweep recorded in profiles/ (KGX_CFG="T,K" overrides).
+// Tile geometries compiled in.  The default is the largest tile of 128 threads that still fits two CTAs per SM (KGX_CFG="T,K" overrides).
 // kernSym: the symmetric-mode (USE_SYMMETRY) instantiation; only the default geometry carries one (others: NULL).
 struct CfgEntry { int T, K, smem, ctas; void (*kern)(LaunchParams); void (*kernSym)(LaunchParams); };
 #define KGX_CFG_ENTRY(T_, K_) { T_, K_, Cfg<T_, K_>::SMEM_BYTES, Cfg<T_, K_>::CTAS_PER_SM, jump_kernel<T_, K_, false>, nullptr }
@@ -79,7 +79,7 @@ static const int g_ncfg = sizeof(g_cfgs) / sizeof(g_cfgs[0]);
 #define KGX_DEFAULT_CFG 0
 #endif
 #ifndef KGX_DEFAULT_STREAM
-#define KGX_DEFAULT_STREAM 1   // streaming kernel is the faster one on B200 (profiles/r1_sweep.txt); KGX_MODE=resident selects the tile kernel
+#define KGX_DEFAULT_STREAM 1   // streaming kernel for large herds; KGX_MODE=resident selects the tile kernel
 #endif
 
 extern "C" {
@@ -97,7 +97,7 @@ int kgx_grid_default(int dev, int* x, int* y) {
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return -1;
   if (*x <= 0) *x = 2 * prop.multiProcessorCount;   // GPUEngine.cu:301
-  if (*y <= 0) *y = 128;                            // GPUEngine.cu:303 (sm_100 is not in the reference's core table)
+  if (*y <= 0) *y = 128;                            // GPUEngine.cu:303 (sm_90 is not in the reference's core table)
   return 0;
 }
 
@@ -171,14 +171,14 @@ kgx_engine* kgx_create_ex(int dev, int groups, int threads_per_group, uint32_t m
     else if (kernel != KGX_KERNEL_AUTO) { snprintf(g_create_err, sizeof g_create_err, "kgx_create_ex: bad kernel selector %d", kernel); delete e; return nullptr; }
     // default: the streaming kernel for herds of 400 k kangaroos and more (it wants many kangaroos per thread on every
     // SM to amortise the per-thread inverse), the shared-memory tile kernel below that (its inverse is shared by a whole
-    // tile, so it keeps ~6.9 GJump/s down to ~270 k kangaroos) -- measured crossover, profiles/r1g_sweep.txt
+    // tile, so it keeps its rate on herds too small to give every stream thread a long group)
     e->streamMode = mode ? (strcmp(mode, "stream") == 0) : (KGX_DEFAULT_STREAM != 0 && e->n >= 400000ull);
     if (mode && strcmp(mode, "stream") && strcmp(mode, "resident") && strcmp(mode, "tmem")) {
       snprintf(g_create_err, sizeof g_create_err, "kgx_create: KGX_MODE must be stream, resident or tmem"); delete e; return nullptr;
     }
     if (mode && !strcmp(mode, "tmem")) {
       e->tmemMode = true;
-      e->T = CfgTm<16>::T; e->K = CfgTm<16>::K; e->smemBytes = CfgTm<16>::SMEM_BYTES; e->ctasPerSM = 2;
+      e->T = CfgCl::T; e->K = CfgCl::K; e->smemBytes = CfgCl::SMEM_BYTES; e->ctasPerSM = 2;
     }
     if (e->streamMode) {
       // kangaroos per thread: 128 (the reference's GPU_GRP_SIZE) when the herd fills two CTAs per SM with it; smaller
@@ -203,7 +203,7 @@ kgx_engine* kgx_create_ex(int dev, int groups, int threads_per_group, uint32_t m
       if (g < 2 || g > 4096 || (g & 1)) { snprintf(g_create_err, sizeof g_create_err, "kgx_create: stream group size (KGX_STREAM_G) must be an even number in [2, 4096]"); delete e; return nullptr; }
       // group inverse: the warp-wide shuffle butterfly (one uniform inverse per warp and pass) for long groups, one inverse per
       // thread for short ones, where the butterfly's 10 extra multiplications per lane weigh more than lane divergence inside
-      // the variable-time inverse -- measured equal at G = 128 (14.16 vs 14.23 GJump/s), 3 % apart at G = 28 (profiles/r2b_sweep.txt)
+      // the variable-time inverse
       if (!invChosen) e->warpInv = g >= 64;
       if (const char* pf = getenv("KGX_STREAM_PF")) e->pfDist = atoi(pf);
       e->streamCtas = ctas;
@@ -235,8 +235,8 @@ kgx_engine* kgx_create_ex(int dev, int groups, int threads_per_group, uint32_t m
   }
   if ((s = cudaHostAlloc(&e->slabPinned, e->slabBytes, cudaHostAllocDefault)) != cudaSuccess) return fail("cudaHostAlloc", s);
   if (e->tmemMode) {
-    if ((s = cudaFuncSetAttribute(jump_kernel_tmem<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, e->smemBytes)) != cudaSuccess)
-      return fail("cudaFuncSetAttribute(smem, tmem kernel)", s);
+    if ((s = cudaFuncSetAttribute(jump_kernel_cluster, cudaFuncAttributeMaxDynamicSharedMemorySize, e->smemBytes)) != cudaSuccess)
+      return fail("cudaFuncSetAttribute(smem, cluster kernel)", s);
   } else if (!e->streamMode &&
       (s = cudaFuncSetAttribute(g_cfgs[e->cfg].kern, cudaFuncAttributeMaxDynamicSharedMemorySize, e->smemBytes)) != cudaSuccess)
     return fail("cudaFuncSetAttribute(smem)", s);
@@ -269,7 +269,7 @@ int kgx_set_jumps_per_launch(kgx_engine* e, int n_run) {
 int kgx_set_symmetry(kgx_engine* e, int on) {
   CK(e, cudaSetDevice(e->dev));
   if (e->inflight) { snprintf(e->err, sizeof e->err, "kgx_set_symmetry: a launch is in flight"); return -1; }
-  if (on && e->tmemMode) { snprintf(e->err, sizeof e->err, "kgx_set_symmetry: the TMEM tile kernel has no symmetric instantiation"); return -1; }
+  if (on && e->tmemMode) { snprintf(e->err, sizeof e->err, "kgx_set_symmetry: the cluster tile kernel has no symmetric instantiation"); return -1; }
   if (on && !e->streamMode && !g_cfgs[e->cfg].kernSym) {
     snprintf(e->err, sizeof e->err, "kgx_set_symmetry: tile geometry %d,%d has no symmetric instantiation", e->T, e->K); return -1;
   }
@@ -445,7 +445,8 @@ int kgx_launch_async(kgx_engine* e) {
   CK(e, cudaMemsetAsync(e->slab[sidx], 0, 4, e->stream));            // GPUEngine.cu:543
   CK(e, cudaEventRecord(e->evStart[sidx], e->stream));
   u32 grid = (u32)(e->ctasPerSM * e->sms);
-  if (grid > e->numTiles) grid = e->numTiles;
+  const u32 ctasPerTile = e->tmemMode ? CfgCl::CLUSTER : 1;             // the cluster kernel spreads a tile over 2 CTAs
+  if (grid > e->numTiles * ctasPerTile) grid = e->numTiles * ctasPerTile;
   if (e->streamMode) {
     if (e->symmetry) stream_kernel<128, 2, true, true><<<grid, 128, 0, e->stream>>>(p);
     else if (e->streamCtas == 3) {
@@ -456,7 +457,7 @@ int kgx_launch_async(kgx_engine* e) {
       else stream_kernel<128, 2, false, false><<<grid, 128, 0, e->stream>>>(p);
     }
   }
-  else if (e->tmemMode) jump_kernel_tmem<16><<<grid, 128, e->smemBytes, e->stream>>>(p);
+  else if (e->tmemMode) jump_kernel_cluster<<<grid, CfgCl::T, e->smemBytes, e->stream>>>(p);
   else if (e->symmetry) g_cfgs[e->cfg].kernSym<<<grid, e->T, e->smemBytes, e->stream>>>(p);
   else g_cfgs[e->cfg].kern<<<grid, e->T, e->smemBytes, e->stream>>>(p);
   e->launches++;

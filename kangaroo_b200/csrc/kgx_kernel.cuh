@@ -1,4 +1,4 @@
-// kgx_kernel.cuh -- the kangaroo jump kernels for sm_100a (B200).
+// kgx_kernel.cuh -- the kangaroo jump kernels for sm_90a (H100).
 //
 // Replace the reference's GPU/GPUCompute.h:22-117 (ComputeKangaroos) + comp_kangaroos (GPUEngine.cu:35-40).
 // Same mathematics (SURVEY.md App. A.2), different machine mapping:
@@ -16,8 +16,8 @@
 //                    spans the tile: per-thread chains -> per-lane chains across the warps -> XOR-butterfly product over
 //                    the 32 lanes with warp shuffles -> ONE warp-uniform inverse per tile per jump -> back down the tree;
 //                    several CTAs per SM overlap one tile's serial inverse with another's parallel phase.
-//   jump_kernel_tmem : (opt-in) the resident kernel with y and the prefix products in TENSOR MEMORY (tcgen05.alloc/ld/st as a
-//                    lane-private store): 2048-kangaroo tiles, 4096 resident kangaroos per SM.
+//   jump_kernel_cluster : (opt-in) the resident kernel with one 1792-kangaroo tile spread over the shared memory of a 2-CTA
+//                    thread-block cluster; one inverse per tile through distributed shared memory.
 //   SYM instantiations of the first two add the reference's USE_SYMMETRY paths (class switch + lastJump / symClass rule).
 //
 //   Both use the same fused per-kangaroo pass: back-substitution of this jump's inverse, the affine add, the
@@ -26,6 +26,7 @@
 #pragma once
 #include "kgx_field.cuh"
 #include "kgx_modinv.h"
+#include <cooperative_groups.h>
 
 namespace kgx {
 
@@ -297,122 +298,142 @@ __global__ void __launch_bounds__(T, Cfg<T, K>::CTAS_PER_SM) jump_kernel(LaunchP
 }
 
 // =====================================================================================================
-// TMEM-backed tile kernel (sm_100a only; KGX_MODE=tmem / KGX_KERNEL_TMEM).  VERDICT r1 weak #4 asked for the "TMEM-doubled
-// resident tile" to be MEASURED instead of costed.  Tensor memory (256 KB per SM, 512 columns x 128 lanes x 32 bit) is used as
-// a lane-private state store: thread t of the 128-thread CTA owns TMEM lane t, and keeps y (8 columns) and the prefix product
-// (8 columns) of each of its K kangaroos there (tcgen05.st / tcgen05.ld, 32x32b.x8: one 256-bit field element per lane per
-// instruction, SASS STTM / LDTM); x and the distance stay in shared memory because the tile inverse and the DP path read
-// them across threads.  Shared memory per kangaroo drops from 112 to 48 bytes: K = 16 -> tiles of 2048 kangaroos, two CTAs
-// per SM (2 x 256 TMEM columns = all of it), 4096 resident kangaroos per SM instead of 1792.
-// Everything else -- arithmetic, fused pass, tile-wide inverse -- is jump_kernel's.
+// Cluster tile kernel (KGX_MODE=tmem / KGX_KERNEL_TMEM; the selector keeps its name).  One tile of 1792 kangaroos (K = 14 rows
+// of T = 128) is shared by the two CTAs of a thread-block cluster, each holding 7 rows -- x, y, prefix products and distances
+// -- in its own shared memory (105 KB, so two CTAs fit on one SM).  The tile still takes ONE inverse per jump: each CTA
+// reduces its 128 thread totals to one product (tile_inverse's chain + butterfly), the two products meet through
+// distributed shared memory across a cluster barrier, both CTAs invert the same tile product and walk their own tree back.
+// That doubles the kangaroos per inverse of a 2-CTA-per-SM resident tile without needing more shared memory per SM.
+// Everything else -- arithmetic, fused pass -- is jump_kernel's (no symmetric instantiation).
 // =====================================================================================================
-template <int K_>
-struct CfgTm {
-  static constexpr int T = 128, K = K_, W = 4, TILE = T * K_;
+struct CfgCl {
+  static constexpr int T = 128, K = 14, KH = 7, W = 4, TILE = T * K, CLUSTER = 2;   // KH rows per CTA
   static constexpr int S_X = 0;
-  static constexpr int S_D = S_X + K * 2 * T;
-  static constexpr int S_TOT = S_D + K * T;
-  static constexpr int S_JT = S_TOT + 2 * T;
-  static constexpr int SLOT_OFF = S_JT * 16 + JT_WORDS * 4;        // u32: TMEM base address written by tcgen05.alloc
-  static constexpr int SMEM_BYTES = SLOT_OFF + 16;
-  static constexpr int COLS = K * 16;                                // y: 8 columns, prefix: 8 columns per kangaroo
-  static_assert(COLS == 32 || COLS == 64 || COLS == 128 || COLS == 256 || COLS == 512, "TMEM allocations are powers of two >= 32 columns");
+  static constexpr int S_Y = S_X + KH * 2 * T;
+  static constexpr int S_P = S_Y + KH * 2 * T;
+  static constexpr int S_D = S_P + KH * 2 * T;
+  static constexpr int S_TOT = S_D + KH * T;
+  static constexpr int S_XCH = S_TOT + 2 * T;                      // 2 x 2 uint4: this CTA's product, double-buffered
+  static constexpr int S_JT = S_XCH + 4;
+  static constexpr int SMEM_BYTES = S_JT * 16 + JT_WORDS * 4;
 };
 
-__device__ __forceinline__ void tmem_ld_fe(u32* r, u32 taddr) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
+// Called by every thread of both CTAs (it contains a cluster barrier).  Warp 0 turns the T totals of sTot into their
+// inverses like tile_inverse, but with the product of BOTH CTAs' totals inverted: `mine` is this CTA's exchange slot,
+// `peer` the same slot of the other CTA (distributed shared memory).
+template <int T, int W>
+__device__ __noinline__ void cluster_tile_inverse(uint4* sTot, uint4* mine, const uint4* peer, int t) {
+  const int lane = t & 31;
+  u32 tw[W][8], c[W][8], v[8], sib[5][8];
+  if (t < 32) {
+#pragma unroll
+    for (int w = 0; w < W; w++) lds_fe(tw[w], sTot, 32 * w + lane, T + 32 * w + lane);
+    fe_copy(c[0], tw[0]);
+#pragma unroll
+    for (int w = 1; w < W; w++) fe_mul(c[w], c[w - 1], tw[w]);
+    fe_copy(v, c[W - 1]);
+#pragma unroll
+    for (int l = 0; l < 5; l++) {
+      shfl_xor_fe(sib[l], v, 1 << l);
+      fe_mul(v, v, sib[l]);
+    }
+    if (lane == 0) sts_fe(mine, 0, 1, v);         // product of this CTA's 128 totals
+  }
+  cooperative_groups::this_cluster().sync();      // release / acquire: both products are visible cluster-wide
+  if (t < 32) {
+    u32 pv[8], inv[8];
+    lds_fe(pv, peer, 0, 1);
+    fe_mul(inv, v, pv);
+    fe_inv(inv, inv);                             // 1 / tile product, identical in both CTAs
+    fe_mul(inv, inv, pv);                         // -> 1 / this CTA's product
+#pragma unroll
+    for (int l = 4; l >= 0; l--) fe_mul(inv, inv, sib[l]);
+#pragma unroll
+    for (int w = W - 1; w >= 1; w--) {
+      u32 o[8];
+      fe_mul(o, inv, c[w - 1]);
+      sts_fe(sTot, 32 * w + lane, T + 32 * w + lane, o);
+      fe_mul(inv, inv, tw[w]);
+    }
+    sts_fe(sTot, lane, T + lane, inv);
+  }
 }
-__device__ __forceinline__ void tmem_st_fe(u32 taddr, const u32* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};\n"
-               :: "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory"); }
 
-template <int K>
-__global__ void __launch_bounds__(128, 2) jump_kernel_tmem(LaunchParams p) {
-  using C = CfgTm<K>;
-  constexpr int T = C::T, TILE = C::TILE;
+__global__ void __cluster_dims__(CfgCl::CLUSTER, 1, 1) __launch_bounds__(CfgCl::T, 2) jump_kernel_cluster(LaunchParams p) {
+  using C = CfgCl;
+  constexpr int T = C::T, KH = C::KH, TILE = C::TILE;
   extern __shared__ uint4 smem[];
   uint4* sX = smem + C::S_X;
+  uint4* sY = smem + C::S_Y;
+  uint4* sP = smem + C::S_P;
   uint4* sD = smem + C::S_D;
   uint4* sTot = smem + C::S_TOT;
   uint4* jt = smem + C::S_JT;
-  u32* slot = reinterpret_cast<u32*>(reinterpret_cast<uint8_t*>(smem) + C::SLOT_OFF);
+  cooperative_groups::cluster_group cluster = cooperative_groups::this_cluster();
+  const u32 rank = cluster.block_rank();
+  uint4* xch = smem + C::S_XCH;
+  const uint4* xchPeer = cluster.map_shared_rank(xch, rank ^ 1u);
   const int t = threadIdx.x;
-  const int lane = t & 31;
   const u32 mlo = (u32)p.dpMask, mhi = (u32)(p.dpMask >> 32);
 
   for (int i = t; i < JT_WORDS; i += T) reinterpret_cast<u32*>(jt)[i] = p.jtab[i];
-  if (t < 32) {                                  // one warp allocates this CTA's columns and lets the next CTA allocate
-    const u32 slot_addr = (u32)__cvta_generic_to_shared(slot);
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" :: "r"(slot_addr), "r"((u32)C::COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  const u32 tbase = *slot;
-  // TMEM address = lane << 16 | column; warp w of the CTA may only touch lanes 32w .. 32w+31, lane l of the warp gets row 32w + l
-  const u32 trow = tbase + ((u32)(t & ~31) << 16);
-  #define KGX_TM_Y(g) (trow + (u32)(g) * 16u)
-  #define KGX_TM_P(g) (trow + (u32)(g) * 16u + 8u)
 
-  for (u32 tile = blockIdx.x; tile < p.numTiles; tile += gridDim.x) {
-    __syncthreads();   // previous tile's shared state fully consumed
-    uint4* gsrc = p.state + (size_t)tile * (K * CHUNKS * T);
-#pragma unroll 1
-    for (int g = 0; g < K; g++) {
+  // Exchange slot of the next tile inverse.  It alternates on EVERY call, across tile boundaries too: a CTA can only write
+  // a slot again after the cluster barrier of the call in between, which its partner passes only after reading that slot.
+  u32 slot = 0;
+  const u32 nClusters = gridDim.x / C::CLUSTER;
+  for (u32 tile = blockIdx.x / C::CLUSTER; tile < p.numTiles; tile += nClusters) {   // both CTAs walk the same tiles
+    __syncthreads();
+    uint4* gsrc = p.state + (size_t)tile * (C::K * CHUNKS * T) + (size_t)rank * (KH * CHUNKS * T);   // rows KH*rank ..
+#pragma unroll
+    for (int g = 0; g < KH; g++) {
       sX[(g * 2 + 0) * T + t] = gsrc[(g * CHUNKS + 0) * T + t];
       sX[(g * 2 + 1) * T + t] = gsrc[(g * CHUNKS + 1) * T + t];
-      u32 y[8];
-      unpack8(y, gsrc[(g * CHUNKS + 2) * T + t], gsrc[(g * CHUNKS + 3) * T + t]);
-      tmem_st_fe(KGX_TM_Y(g), y);
+      sY[(g * 2 + 0) * T + t] = gsrc[(g * CHUNKS + 2) * T + t];
+      sY[(g * 2 + 1) * T + t] = gsrc[(g * CHUNKS + 3) * T + t];
       sD[g * T + t] = gsrc[(g * CHUNKS + 4) * T + t];
     }
     u32 P[8];
-    {   // prologue: forward chain of dx; prefix(g) = product of the dx before g
+    {   // prologue: forward chain of dx; sP[g] = product of the dx before g
       u32 x[8], jx[8], dx[8];
 #pragma unroll 1
-      for (int g = 0; g < K; g++) {
+      for (int g = 0; g < KH; g++) {
         lds_fe(x, sX, (g * 2) * T + t, (g * 2 + 1) * T + t);
         lds_jp4(jx, jt, x[0] & 31u);
         fe_sub(dx, x, jx);
         if (g == 0) {
           u32 one[8]; fe_set_one(one);
-          tmem_st_fe(KGX_TM_P(0), one);
+          sts_fe(sP, t, T + t, one);
           fe_copy(P, dx);
         } else {
-          tmem_st_fe(KGX_TM_P(g), P);
+          sts_fe(sP, (g * 2) * T + t, (g * 2 + 1) * T + t, P);
           fe_mul(P, P, dx);
         }
       }
       sts_fe(sTot, t, T + t, P);
     }
-    tmem_wait_st();
     int backward = 1;
     for (int run = 0; run < p.nRun; run++) {
       __syncthreads();
-      if (t < 32) tile_inverse<T, C::W>(sTot, lane, nullptr);
+      cluster_tile_inverse<T, C::W>(sTot, xch + 2 * slot, xchPeer + 2 * slot, t);
+      slot ^= 1u;
       __syncthreads();
       u32 I[8];
       lds_fe(I, sTot, t, T + t);
       const bool last = (run == p.nRun - 1);
 #pragma unroll 1
-      for (int i = 0; i < K; i++) {
-        const int g = backward ? (K - 1 - i) : i;
+      for (int i = 0; i < KH; i++) {
+        const int g = backward ? (KH - 1 - i) : i;
         const int i0 = (g * 2) * T + t, i1 = (g * 2 + 1) * T + t;
         u32 x[8], y[8], jx[8], jy[8], dx[8], inv[8], s[8], rx[8], ry[8];
         lds_fe(x, sX, i0, i1);
-        tmem_ld_fe(inv, KGX_TM_P(g));            // prefix of this kangaroo
+        lds_fe(inv, sP, i0, i1);
         const u32 j = x[0] & 31u;
         lds_jp4(jx, jt, j);
         fe_sub(dx, x, jx);
         fe_mul(inv, inv, I);                     // 1/dx
-        if (i != K - 1) fe_mul(I, I, dx);
-        tmem_ld_fe(y, KGX_TM_Y(g));
+        if (i != KH - 1) fe_mul(I, I, dx);
+        lds_fe(y, sY, i0, i1);
         lds_jp4(jy, jt + 64, j);
         fe_sub(s, y, jy);
         fe_mul(s, s, inv);
@@ -422,15 +443,15 @@ __global__ void __launch_bounds__(128, 2) jump_kernel_tmem(LaunchParams p) {
         fe_sub(ry, x, rx);
         fe_mul(ry, ry, s);
         fe_sub(ry, ry, y);
-        sts_fe(sX, i0, i1, rx);
-        tmem_st_fe(KGX_TM_Y(g), ry);
         uint4 dv = sD[g * T + t];
         u32 d[4] = {dv.x, dv.y, dv.z, dv.w};
         const uint4 jd = jt[128 + j];
         d128_add(d, jd.x, jd.y, jd.z, jd.w);
+        sts_fe(sX, i0, i1, rx);
+        sts_fe(sY, i0, i1, ry);
         sD[g * T + t] = make_uint4(d[0], d[1], d[2], d[3]);
         if (((rx[7] & mhi) | (rx[6] & mlo)) == 0u) {
-          const u64 kidx = (u64)tile * TILE + (u64)g * T + (u64)t;
+          const u64 kidx = (u64)tile * TILE + (u64)(rank * KH + g) * T + (u64)t;
           if (kidx < p.nKangaroos) {
             const u32 pos = atomicAdd(p.out, 1u);
             if (pos < p.maxFound) {
@@ -447,35 +468,28 @@ __global__ void __launch_bounds__(128, 2) jump_kernel_tmem(LaunchParams p) {
           fe_sub(dx, rx, jx);
           if (i == 0) {
             u32 one[8]; fe_set_one(one);
-            tmem_st_fe(KGX_TM_P(g), one);
+            sts_fe(sP, i0, i1, one);
             fe_copy(P, dx);
           } else {
-            tmem_st_fe(KGX_TM_P(g), P);
+            sts_fe(sP, i0, i1, P);
             fe_mul(P, P, dx);
           }
         }
       }
       if (!last) sts_fe(sTot, t, T + t, P);
-      tmem_wait_st();                            // this pass's y / prefix stores are visible to the next pass's loads
       backward ^= 1;
     }
     uint4* gdst = gsrc;
-#pragma unroll 1
-    for (int g = 0; g < K; g++) {
-      u32 y[8];
-      tmem_ld_fe(y, KGX_TM_Y(g));
+#pragma unroll
+    for (int g = 0; g < KH; g++) {
       gdst[(g * CHUNKS + 0) * T + t] = sX[(g * 2 + 0) * T + t];
       gdst[(g * CHUNKS + 1) * T + t] = sX[(g * 2 + 1) * T + t];
-      gdst[(g * CHUNKS + 2) * T + t] = make_uint4(y[0], y[1], y[2], y[3]);
-      gdst[(g * CHUNKS + 3) * T + t] = make_uint4(y[4], y[5], y[6], y[7]);
+      gdst[(g * CHUNKS + 2) * T + t] = sY[(g * 2 + 0) * T + t];
+      gdst[(g * CHUNKS + 3) * T + t] = sY[(g * 2 + 1) * T + t];
       gdst[(g * CHUNKS + 4) * T + t] = sD[g * T + t];
     }
   }
-  #undef KGX_TM_Y
-  #undef KGX_TM_P
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-  __syncthreads();
-  if (t < 32) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" :: "r"(tbase), "r"((u32)C::COLS) : "memory");
+  cluster.sync();   // the other CTA may still read this CTA's exchange slot
 }
 
 // =====================================================================================================

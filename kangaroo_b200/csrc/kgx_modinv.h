@@ -1,7 +1,7 @@
 // kgx_modinv.h -- modular inverse mod p = 2^256 - 0x1000003D1, variable time, host+device.
 //
 // Replaces the reference's GPU/GPUMath.h:700-803 (_ModInv: DRS62 "delayed right shift" divsteps on 64-bit
-// limbs, which sm_100a has to emulate).  Algorithm and structure: the Bernstein-Yang "safegcd" divstep iteration in
+// limbs, which sm_90a has to emulate).  Algorithm and structure: the Bernstein-Yang "safegcd" divstep iteration in
 // the variable-time signed-30-bit-limb form published by libsecp256k1 (src/modinv32_impl.h, MIT licence, P. Wuille):
 // divsteps_30_var / update_de_30 / update_fg_30 / normalize_30 and the f*g*(f^2-2) 6-bit inverse trick follow that
 // design -- third-party public code, NOT the reference -- re-typed here for one fixed modulus p (constants folded,
@@ -169,9 +169,8 @@ KGX_HD void modinv256(uint32_t out[8], const uint32_t in[8]) {
   // the batch count is data dependent (about 18 for random input; 25 bounds any 256-bit input).
   // KGX_INV_UNROLL batches run between two convergence tests: once g == 0 a further batch is the matrix (2^30, 0; 0, 1),
   // which leaves f and d unchanged (d at most re-normalised by +p), so testing less often is still exact.  The idea was to
-  // let batch k+1's divsteps (which need only the low limbs of f, g) overlap the tail of batch k's 9-limb updates; measured
-  // on a B200 (profiles/r2d_sweep_inverse_unroll.txt) it buys nothing for the warp-uniform inverse of the resident kernel
-  // (6.98 -> 7.02 GJump/s) and costs 1-4 % in the stream kernel (idle batches), so the test stays after every batch.
+  // let batch k+1's divsteps (which need only the low limbs of f, g) overlap the tail of batch k's 9-limb updates; the
+  // extra batches run idle once g == 0, so by default the test stays after every batch.
 #ifndef KGX_INV_UNROLL
 #define KGX_INV_UNROLL 1
 #endif

@@ -1,6 +1,6 @@
 """ctypes binding of build/libkgx_ingest.so (C ABI: include/kgx_ingest.h): the rank-0 distinguished-point table.
 
-The table is the reference's own `class HashTable` (HashTable.{h,cpp}, compiled unmodified from /root/reference by
+The table is the reference's own `class HashTable` (HashTable.{h,cpp}, compiled unmodified from the reference sources by
 kangaroo_b200/csrc/build_ingest.sh); the library adds the batched, bucket-sharded multi-threaded insert that replaces the
 single-mutex loop of Kangaroo::SolveKeyGPU (Kangaroo.cpp:594-612) when the DP records of all GPUs arrive on rank 0.
 No Python-side fallback: without the library DPTable() raises."""

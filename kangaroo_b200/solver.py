@@ -98,7 +98,7 @@ class Solver:
         self.dps = DPTable(threads=ingest_threads) if self.rank == 0 else None      # rank 0: the reference HashTable
         # Two pinned staging buffers: while the ingest thread inserts step k's records, step k+1's land in the other one.  The
         # NCCL kernels of a step cannot start before the jump launch that occupies every SM has finished, so without this
-        # decoupling the CPU insert (3-4 ms at 8 GPUs) sat exposed between two launches: 97 instead of 112 GJump/s.
+        # decoupling the CPU insert would sit exposed between two launches.
         self._hosts = ([torch.empty(self.world * max_found * DP40_BYTES, dtype=torch.uint8).pin_memory() for _ in range(2)]
                        if self.rank == 0 else None)
         self._hidx = 0

@@ -57,7 +57,7 @@ def _ptr(a):
 
 
 def build(ref=True):
-    """Build the oracle (and, where /root/reference exists, the reference harness)."""
+    """Build the oracle (and, where KANGAROO_REF names the reference sources, the reference harness)."""
     subprocess.check_call(["make", "-s", "-C", HERE, "oracle"] + (["ref"] if ref else []))
 
 
@@ -246,7 +246,3 @@ class Oracle(_Backend):
 class Reference(_Backend):
     prefix = "ref_"
     path = os.path.join(HERE, "_ref", "libkref.so")
-
-
-def reference_available():
-    return os.path.exists(Reference.path) or os.path.isdir("/root/reference/SECPK1")

@@ -1,9 +1,9 @@
 /*
  * kgx_oracle.h -- CPU restatement of the reference kangaroo jump path (TEST INFRASTRUCTURE ONLY).
  *
- * This is the parity oracle for the B200 jump engine.  It is NOT part of the product: only tests/,
+ * This is the parity oracle for the H100 jump engine.  It is NOT part of the product: only tests/,
  * __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may load it.
- * Every function cites the reference file:line (under /root/reference) whose algorithm it restates.
+ * Every function cites the reference file:line (of the reference sources) whose algorithm it restates.
  *
  * Pinned against: SURVEY.md Appendix C golden vectors (jump table rangePower=64, 1024-jump
  * trajectory), the known answers of the reference's sample inputs, and -- in the build container --

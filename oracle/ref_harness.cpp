@@ -2,7 +2,7 @@
  * ref_harness.cpp -- thin C wrapper that drives the UNMODIFIED reference SECPK1 / HashTable code.
  *
  * TEST / BASELINE INFRASTRUCTURE ONLY.  Compiled by oracle/Makefile against the sources where they lie
- * under /root/reference (nothing is copied into this repo) into oracle/_ref/libkref.so.  It exists to
+ * under $KANGAROO_REF (nothing is copied into this repo) into oracle/_ref/libkref.so.  It exists to
  *   (1) pin oracle/kgx_oracle.c against the reference's own arithmetic (tests/test_oracle_vs_ref.py),
  *   (2) generate the committed fixtures under tests/golden/ (tests/golden/make_golden.py),
  *   (3) serve as the "reference" CPU baseline in bench.py (the SolveKeyCPU inner loop, Kangaroo.cpp:375-433,

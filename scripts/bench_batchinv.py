@@ -1,6 +1,6 @@
 """BASELINE config 5: batch-inverse microbench -- 2^20 kangaroos x 1024 jumps (16 launches of NB_RUN=64), dpMask = all ones
-(never fires), Montgomery group sizes 32 / 64 / 128 per thread (stream kernel: one inverse per thread, or -- round 2 -- one
-warp-wide shuffle-butterfly inverse per 32 x G kangaroos), the tile-wide groups of the resident kernel and of the TMEM tile kernel.  Reports MJump/s, ModMult/s (= 6 x MJump/s, SURVEY 8d) and the fraction of the measured wide-IMAD
+(never fires), Montgomery group sizes 32 / 64 / 128 per thread (stream kernel: one inverse per thread, or one
+warp-wide shuffle-butterfly inverse per 32 x G kangaroos), the tile-wide groups of the resident kernel and of the cluster tile kernel.  Reports MJump/s, ModMult/s (= 6 x MJump/s, SURVEY 8d) and the fraction of the measured wide-IMAD
 roofline (416 IMAD.WIDE per jump)."""
 import ctypes
 import json
@@ -35,7 +35,7 @@ def main():
     variants += [("stream auto (G=28, thread inverse)", {"KGX_MODE": "stream"}),
                  ("resident tile 128x7=896", {"KGX_MODE": "resident", "KGX_CFG": "128,7"}),
                  ("resident tile 64x7=448", {"KGX_MODE": "resident", "KGX_CFG": "64,7"}),
-                 ("TMEM tile 128x16=2048", {"KGX_MODE": "tmem"})]
+                 ("cluster tile 2x(128x7)=1792", {"KGX_MODE": "tmem"})]
     lines = ["batch-inverse microbench (BASELINE config 5): 2^20 kangaroos x 1024 jumps, rangePower 64 table, dp = 64 (never fires)",
              "measured wide-IMAD peak %.3e /s ; roofline = 416 IMAD.WIDE per jump" % peak, "",
              "%-44s %10s %12s %14s %9s" % ("variant (Montgomery group)", "ms/1024j", "MJump/s", "ModMult/s", "roofline")]
@@ -57,8 +57,8 @@ def main():
         mj = n * 1024 / tot / 1e3
         lines.append("%-44s %10.2f %12.1f %14.3e %8.1f%%" % (name, tot, mj, mj * 6e6, 100 * mj * 1e6 * 416 / peak))
         print(lines[-1], flush=True)
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    open(os.path.join(ROOT, "gpurun_out", "batchinv_microbench.txt"), "w").write("\n".join(lines) + "\n")
+    os.makedirs(os.path.join(ROOT, "results"), exist_ok=True)
+    open(os.path.join(ROOT, "results", "batchinv_microbench.txt"), "w").write("\n".join(lines) + "\n")
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
 """Raw device microbenchmarks (BASELINE config 5 inputs): IMAD.WIDE issue rate, fe_mul / fe_sqr / inverse
-throughput, and jump-kernel launch time on a synthetic herd.  Writes gpurun_out/microbench.json."""
+throughput, and jump-kernel launch time on a synthetic herd.  Writes results/microbench.json."""
 import ctypes
 import json
 import os
@@ -35,7 +35,7 @@ def main():
     from kangaroo_b200 import random_herd_arrays
     from tests.golden_util import load_cases
     case = [c for c in load_cases() if c["range_power"] == 80][0]
-    for grid in ((296, 128), (74, 128), (16, 128)):
+    for grid in ((264, 128), (66, 128), (16, 128)):
         n = grid[0] * grid[1] * 128
         eng = GPUEngine(grid[0], grid[1], 0, 1 << 20)
         eng.SetParams(0xFFFF000000000000, *case["table"])
@@ -52,8 +52,8 @@ def main():
         out["jump_%dx%d" % grid] = {"kangaroos": n, "ms_per_launch": ms, "mjump_s": n * NB_RUN / ms / 1e3, "all_ms": times}
         print(grid, out["jump_%dx%d" % grid], flush=True)
         eng.close()
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    json.dump(out, open(os.path.join(ROOT, "gpurun_out", "microbench.json"), "w"), indent=1)
+    os.makedirs(os.path.join(ROOT, "results"), exist_ok=True)
+    json.dump(out, open(os.path.join(ROOT, "results", "microbench.json"), "w"), indent=1)
 
 
 if __name__ == "__main__":

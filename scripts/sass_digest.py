@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Static SASS digest of the jump kernels in kangaroo_b200/csrc/libkgx.so (VERDICT r1 next #3a): for one kernel, find the hot
+"""Static SASS digest of the jump kernels in kangaroo_b200/csrc/libkgx.so: for one kernel, find the hot
 loop (the innermost backward branch that contains the most IMAD.WIDE) and count opcode classes per loop trip.  The stream
 kernel's trip is TWO kangaroo jumps (ping-pong unroll), so counts are also given per jump.
 

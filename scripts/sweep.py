@@ -15,7 +15,7 @@ def main():
     cfgs = sys.argv[1:] or ["128,7", "128,5", "128,4", "96,6", "64,7", "64,6", "64,5", "64,4", "256,3", "32,8", "32,12"]
     case = [c for c in load_cases() if c["range_power"] == 80][0]
     sx, sy, sd = arrays(case["start"])
-    gx, gy = (int(v) for v in os.environ.get('KGX_SWEEP_GRID', '296,128').split(','))
+    gx, gy = (int(v) for v in os.environ.get('KGX_SWEEP_GRID', '264,128').split(','))
     n = gx * gy * 128
     idx = np.arange(n) % sx.shape[0]
     ax, ay = sx[idx], sy[idx]
@@ -43,8 +43,8 @@ def main():
                 out[cfg]["prof"] = [int(v) for v in pr]
         print("KGX_CFG=%-7s %8.3f ms/launch  %8.1f MJump/s%s" % (cfg, ms, out[cfg]["mjump_s"], extra), flush=True)
         eng.close()
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    json.dump(out, open(os.path.join(ROOT, "gpurun_out", "sweep.json"), "w"), indent=1)
+    os.makedirs(os.path.join(ROOT, "results"), exist_ok=True)
+    json.dump(out, open(os.path.join(ROOT, "results", "sweep.json"), "w"), indent=1)
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
-"""Round-2 sweep: MJump/s of engine variants selected through the environment, several herd sizes in one process.
-  python scripts/sweep2.py "label|ENV=VAL,ENV=VAL|gx,gy" ...      -> gpurun_out/sweep2.json + one line per variant
+"""Sweep: MJump/s of engine variants selected through the environment, several herd sizes in one process.
+  python scripts/sweep2.py "label|ENV=VAL,ENV=VAL|gx,gy" ...      -> results/sweep2.json + one line per variant
 Herd = replicated rows of the reference-generated in80 fixture (valid curve points; throughput does not depend on values)."""
 import json
 import os
@@ -52,8 +52,8 @@ def main():
         out[label] = dict(ms=ms, mjump_s=n * NB_RUN / ms / 1e3, kangaroos=n, kernel=eng.kernel, env=envs)
         print("%-44s %9d kangaroos  %-8s %8.3f ms/launch  %8.1f MJump/s" % (label, n, eng.kernel, ms, out[label]["mjump_s"]), flush=True)
         eng.close()
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    json.dump(out, open(os.path.join(ROOT, "gpurun_out", "sweep2.json"), "w"), indent=1)
+    os.makedirs(os.path.join(ROOT, "results"), exist_ok=True)
+    json.dump(out, open(os.path.join(ROOT, "results", "sweep2.json"), "w"), indent=1)
 
 
 if __name__ == "__main__":

@@ -1,7 +1,7 @@
-// ubench3.cu -- round-2 pipe probes for sm_100a (B200): FP64 (DFMA) vs wide integer multiply (IMAD.WIDE) issue rates, how
+// ubench3.cu -- pipe probes for sm_90a (H100): FP64 (DFMA) vs wide integer multiply (IMAD.WIDE) issue rates, how
 // they overlap with each other and with ALU work, and the DFMA-based 256-bit multiplier (kgx_field_fp64.cuh) against the
 // integer one (kgx_field.cuh), alone and mixed.  Cycles are MEASURED (clock64 of one thread per CTA + globaltimer), not
-// derived from a nominal clock.   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scripts/ubench3 scripts/ubench3.cu
+// derived from a nominal clock.   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/ubench3 scripts/ubench3.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a GPU machine)")
     config.addinivalue_line("markers", "slow: takes more than a few seconds on CPU")
 
 
@@ -19,19 +19,11 @@ def oracle():
     return kgo.Oracle()
 
 
-@pytest.fixture(scope="session")
-def reference():
-    from oracle import kgo
-    if not kgo.reference_available():
-        pytest.skip("reference build (oracle/_ref/libkref.so) not available")
-    return kgo.Reference()
-
-
 # Every oracle / reference-fixture parity test runs on BOTH jump kernels (kgx_create_ex): "stream128" is the benchmarked
-# configuration (stream kernel, 128 kangaroos per thread, what the default 296x128 grid resolves to), "stream" the
+# configuration (stream kernel, 128 kangaroos per thread, what the default 264x128 grid of an H100 resolves to), "stream" the
 # adaptive group size small grids get, "resident" the shared-memory tile kernel.
 KERNEL_VARIANTS = {"stream128": dict(kernel="stream", stream_g=128), "stream": dict(kernel="stream"), "resident": dict(kernel="resident"),
-                   "tmem": dict(kernel="tmem")}      # tile kernel with y / prefix products in tensor memory (2048-kangaroo tiles)
+                   "tmem": dict(kernel="tmem")}      # cluster tile kernel: one 1792-kangaroo tile over the shared memory of 2 CTAs
 
 
 @pytest.fixture(params=sorted(KERNEL_VARIANTS))

@@ -1,9 +1,9 @@
 """Generate tests/golden/jump_golden.json from the REFERENCE's own code (oracle/_ref/libkref.so, i.e. the
-unmodified /root/reference SECPK1 sources driven by oracle/ref_harness.cpp).  Run in the build container:
+unmodified reference SECPK1 sources driven by oracle/ref_harness.cpp).  Run where oracle/_ref/libkref.so is built:
 
     python tests/golden/make_golden.py
 
-The fixture is what travels to the GPU box (where /root/reference does not exist)."""
+The fixture is committed, so the tests need neither the reference sources nor oracle/_ref."""
 import json
 import os
 import sys

@@ -1,138 +1,82 @@
-"""Pin oracle/kgx_oracle.c against the reference's own SECPK1 code (oracle/_ref/libkref.so, built from
-/root/reference by oracle/Makefile).  Skipped where the reference build is unavailable."""
-import random
+"""Pin oracle/kgx_oracle.c against the reference's own SECPK1 code.  The reference's results on these seeded workloads
+are stored in tests/golden/ref_golden.json (tests/golden/make_ref_golden.py); every test recomputes the same transcript
+on the oracle and must reproduce it value for value."""
+import json
+import os
 
-import numpy as np
 import pytest
 
 from oracle import kgo
+from tests import ref_transcripts as rt
 
 P, N = kgo.P, kgo.N
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_golden.json")
 
 
-def test_field_ops(oracle, reference):
-    rng = random.Random(3)
-    edge = [0, 1, 2, P - 1, P - 2, 0x1000003D1, 2**255, 2**256 - 1 - 0x1000003D1, 2**128 - 1]
-    vals = edge + [rng.randrange(P) for _ in range(3000)]
-    for i in range(len(vals) - 1):
-        a, b = vals[i], vals[i + 1]
-        assert oracle.mod_mul(a, b) == reference.mod_mul(a, b)
-        assert oracle.mod_sqr(a) == reference.mod_sqr(a)
-        assert oracle.mod_sub(a, b) == reference.mod_sub(a, b)
-    for a in vals[:300]:
-        assert oracle.mod_inv(a) == reference.mod_inv(a)
+def check(name, transcript):
+    with open(GOLDEN) as f:
+        want = json.load(f)["transcripts"][name]
+    assert len(transcript) == want["entries"], name
+    assert rt.digest(transcript) == want["sha256"], "%s: oracle %s vs reference %s" % (name, rt.head(transcript), want["head"])
 
 
-def test_order_ops(oracle, reference):
-    rng = random.Random(4)
-    for _ in range(500):
-        a, b = rng.randrange(N), rng.randrange(N)
-        assert oracle.order_add(a, b) == reference.order_add(a, b)
-        assert oracle.order_sub(a, b) == reference.order_sub(a, b)
+def test_field_ops(oracle):
+    check("field_ops", rt.field_ops(oracle))
 
 
-def test_rng_and_rand(oracle, reference):
-    for seed in (0, 1, 0x600DCAFE, 0xFFFFFFFF):
-        oracle.rseed(seed); reference.rseed(seed)
-        assert [oracle.rndl() for _ in range(700)] == [reference.rndl() for _ in range(700)]
-        for nbit in (1, 31, 32, 33, 64, 65, 128, 255, 256):
-            assert oracle.rand_bits(nbit) == reference.rand_bits(nbit)
+def test_order_ops(oracle):
+    check("order_ops", rt.order_ops(oracle))
 
 
-def test_scalar_mult_and_add(oracle, reference):
-    rng = random.Random(5)
-    ks = [1, 2, 3, 255, 256, 257, 2**64, N - 1, N - 2] + [rng.randrange(1, N) for _ in range(40)]
-    pts = []
-    for k in ks:
-        a = oracle.ec_mul_g(k)
-        assert a == reference.ec_mul_g(k)
-        pts.append(a)
-    for i in range(len(pts) - 1):
-        if pts[i][0] != pts[i + 1][0]:
-            assert oracle.ec_add(pts[i], pts[i + 1]) == reference.ec_add(pts[i], pts[i + 1])
+def test_rng_and_rand(oracle):
+    check("rng_and_rand", rt.rng_and_rand(oracle))
 
 
-def test_jump_tables_all_range_powers(oracle, reference):
-    for rp in (32, 40, 48, 56, 64, 72, 80, 84, 110, 115, 125, 256):
-        a = oracle.create_jump_table(rp); da = oracle.last_draws
-        b = reference.create_jump_table(rp)
-        assert da == reference.last_draws
-        assert all(np.array_equal(u, v) for u, v in zip(a, b)), rp
+def test_scalar_mult_and_add(oracle):
+    check("scalar_mult_and_add", rt.scalar_mult_and_add(oracle))
 
 
-def test_herd_and_jump_loop(oracle, reference):
-    table = oracle.create_jump_table(64)
-    key = oracle.ec_mul_g(0x5B3F38AF935A3640D158E871CE6E9666DB862636383386EE510F18CCC3BD72EB)
-    for first_type in (0, 1):
-        oracle.rseed(42); reference.rseed(42)
-        a = oracle.create_herd(300, 64, 2**63 - 1, key, first_type)
-        b = reference.create_herd(300, 64, 2**63 - 1, key, first_type)
-        assert all(np.array_equal(u, v) for u, v in zip(a, b))
-    mask = oracle.dp_mask(6)
-    dps_a = oracle.jump_cpu(*a, table, 70, mask, grp=128)
-    dps_b = reference.jump_cpu(*b, table, 70, mask, grp=1024)
-    assert all(np.array_equal(u, v) for u, v in zip(a, b))
-    assert sorted(dps_a) == sorted(dps_b) and len(dps_a) > 200
-    # Check.cpp single-AddDirect replay through the reference agrees too
-    x, y, d = (kgo.from_limbs(v[7]) for v in reference.create_herd(8, 64, 2**63 - 1, key, 0))
-    xo, yo, do = x, y, d
-    for _ in range(20):
-        x, y, d = reference.jump_single(x, y, d, table)
-        xo, yo, do = oracle.jump_single(xo, yo, do, table)
-    assert (x, y, d) == (xo, yo, do)
+def test_jump_tables_all_range_powers(oracle):
+    check("jump_tables", rt.jump_tables(oracle))
 
 
-def test_hash_convert(oracle, reference):
-    rng = random.Random(6)
-    for _ in range(200):
-        x = rng.randrange(P)
-        d = rng.randrange(2**126) if rng.random() < 0.5 else N - rng.randrange(1, 2**126)
-        t = rng.randrange(2)
-        assert oracle.hash_convert(x, d, t) == reference.hash_convert(x, d, t)
+def test_herd_and_jump_loop(oracle):
+    """Herds of both types, 70 jumps of the SolveKeyCPU loop (oracle: 128 kangaroos per inverse, reference: 1024) with
+    their DPs, and 20 single-AddDirect jumps of the Check.cpp replay."""
+    t = rt.herd_and_jump_loop(oracle, grp=128)
+    assert len(t[3]) > 200
+    check("herd_and_jump_loop", t)
+
+
+def test_hash_convert(oracle):
+    check("hash_convert", rt.hash_convert(oracle))
 
 
 # ---- USE_SYMMETRY restatement (SURVEY 8f/f4) pinned to the reference's own Int / Secp256K1 code -------------------------
-@pytest.mark.parametrize("rp", [40, 56, 64, 80, 109, 125])
-def test_symmetric_jump_table_matches_reference(oracle, reference, rp):
+@pytest.mark.parametrize("rp", list(rt.SYM_RANGE_POWERS))
+def test_symmetric_jump_table_matches_reference(oracle, rp):
     """Kangaroo.cpp:742-832 USE_SYMMETRY branch: the two primes u, v come from Int::IsProbablePrime, whose Miller-Rabin bases
     are drawn from the same MT19937 stream as the distances -- the oracle reproduces that consumption exactly."""
-    a = oracle.create_jump_table_sym(rp)
-    b = reference.create_jump_table_sym(rp)
-    assert oracle.last_uv == reference.last_uv and oracle.last_draws == reference.last_draws
-    for x, y in zip(a, b):
-        assert np.array_equal(x, y)
-    jd = a[0]
+    check("symmetric_jump_table_%d" % rp, rt.symmetric_jump_table(oracle, rp))
+    jd = oracle.create_jump_table_sym(rp)[0]
     u, v = oracle.last_uv
     assert all(int(jd[i, 0]) % u == 0 for i in range(16)) and all(int(jd[i, 0]) % v == 0 for i in range(16, 32))
 
 
-def test_symmetric_herd_and_walk_match_reference(oracle, reference):
+def test_symmetric_herd_and_walk_match_reference(oracle):
     """CreateHerd (Kangaroo.cpp:670-738, sym branch) and the symmetric walk Check.cpp:534-556 replays (lastJump limiter,
-    ModPositiveK1 class switch, d = n - d): oracle (batched inverse) == reference (one AddDirect per jump), bit for bit."""
-    rp = 64
-    key = oracle.ec_mul_g(0x5B3F38AF935A3640D158E871CE6E9666DB862636383386EE0000000000123000)
-    wdiv4 = ((1 << rp) - 1) >> 2
-    table = oracle.create_jump_table_sym(rp)
-    n = 96
-    for be in (oracle, reference):
-        be.rseed(777)
-    ox, oy, od = oracle.create_herd_sym(n, rp, wdiv4, key, 0)
-    rx, ry, rd = reference.create_herd_sym(n, rp, wdiv4, key, 0)
-    assert np.array_equal(ox, rx) and np.array_equal(oy, ry) and np.array_equal(od, rd)
+    ModPositiveK1 class switch, d = n - d): oracle (batched inverse, 32 per group) == reference (24 per group), bit for bit."""
+    t, (ox, oy, od, lo) = rt.symmetric_herd_and_walk(oracle, grp=32)
+    check("symmetric_herd_and_walk", t)
+    n = ox.shape[0]
+    assert len(t[2]) > 500 and len(t[4]) > 500
+    assert set(int(v) for v in lo) == {0, 1}                                  # symclass state after the second walk
     half = (kgo.P - 1) // 2
     assert all(kgo.from_limbs(oy[i]) <= half for i in range(n))
     assert any(kgo.from_limbs(od[i]) > kgo.N // 2 for i in range(n))           # some distances went negative (mod n)
-    mask = oracle.dp_mask(4)
-    for rule, init in (("lastjump", 32), ("symclass", 0)):
-        lo, lr = np.full(n, init, dtype=np.uint8), np.full(n, init, dtype=np.uint8)
-        do = oracle.jump_sym(ox, oy, od, lo, table, 200, mask, grp=32, rule=rule)
-        dr = reference.jump_sym(rx, ry, rd, lr, table, 200, mask, grp=24, rule=rule)
-        assert np.array_equal(ox, rx) and np.array_equal(oy, ry) and np.array_equal(od, rd) and np.array_equal(lo, lr), rule
-        assert sorted(do) == sorted(dr) and len(do) > 500, rule
-        if rule == "symclass":
-            assert set(np.unique(lo)) == {0, 1}
     # invariant of the class walk: tame x == (d*G).x ; wild x == (key + d*G).x or (key - d*G).x -- a class switch negates
     # the whole point, i.e. d AND the key term, which is why CheckKey tries +-key and the four sign pairs (Kangaroo.cpp:218-253)
+    key = oracle.ec_mul_g(rt.SYM_KEY_PRIV)
     for i in (0, 1, 2, 3, 50, 95):
         dv = kgo.from_limbs(od[i])
         if i % 2 == 0:
