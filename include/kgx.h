@@ -91,6 +91,22 @@ int kgx_patch(kgx_engine* e, uint64_t kidx, const uint64_t px[4], const uint64_t
 int kgx_snapshot_begin(kgx_engine* e);
 int kgx_snapshot_read(kgx_engine* e, uint64_t* px, uint64_t* py, uint64_t* d);
 
+/* --- the herd as work-file records (Kangaroo::SaveWork -ws / FetchWalks, Backup.cpp:536-539, 211-223): 96 bytes per
+ *     kangaroo, {x[4], y[4], d[4]} u64 limbs, d = distance mod n with the wild offset removed, kIdx order.  Both calls fail
+ *     in symmetric mode.  wild_offset: 2 limbs (the bias of odd kIdx).
+ * _export: after kgx_snapshot_begin, converts the snapshot on the device (copy stream; launches queued after the snapshot
+ *     keep running) and copies records [first, first+count) to dst, host or device memory of the engine's GPU.  Call it
+ *     in chunks; the call whose range ends at n releases the snapshot.  The engine then keeps the snapshot's staging
+ *     (80 bytes per kangaroo) and the record buffer (96 bytes per kangaroo) for the next save: freeing device memory
+ *     synchronises the device, which would stall the jump launches once per save.  kgx_destroy frees both.
+ * _import: replaces kangaroos 0..count-1 (the rest of the herd is kept) in stream order after the launch in flight; recs:
+ *     count x 96 bytes of host memory.  Fails, changing nothing, when a biased distance does not fit in 128 bits (a file of
+ *     another range).  verify != 0 recomputes every position as d*G (even kIdx) / key + d*G (odd kIdx): *mismatches =
+ *     records that differ, and the herd is only replaced when there are none. --- */
+int kgx_snapshot_export(kgx_engine* e, const uint64_t wild_offset[2], uint64_t first, uint64_t count, void* dst);
+int kgx_import(kgx_engine* e, const uint64_t wild_offset[2], const void* recs, uint64_t count, const uint64_t keyx[4],
+               const uint64_t keyy[4], int verify, uint64_t* mismatches);
+
 /* --- herd creation on the device (SURVEY 8f/f2; replaces the CPU side of Kangaroo::CreateHerd, Kangaroo.cpp:670-738):
  *     kangaroo i starts at scalars[i]*G, plus `key` when (i + first_type) is odd (wild).  scalars: n x 4 limbs (mod the
  *     group order), d128: n x 2 limbs stored as the (biased) distances. --- */

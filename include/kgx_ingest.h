@@ -59,11 +59,22 @@ int kgi_resolve(kgi_table* t, const uint64_t d_old[2], const uint64_t d_new[2], 
                 const uint64_t range_start[4], uint64_t priv_out[4]);
 
 /* Work-file compatibility (SURVEY 8f/f3): write the table as a reference work file (Backup.cpp:368-394 header HEADW +
- * HashTable::SaveTable) that the reference's -winfo / -wcheck / -i / -wm read.  range_start/range_end/key: 4 limbs each. */
+ * HashTable::SaveTable) that the reference's -winfo / -wcheck / -i / -wm read.  range_start/range_end/key: 4 limbs each.
+ * No kangaroos (totalWalk = 0).  0 on success, -errno when a write fails (full disk, bad path). */
 int kgi_save_work(kgi_table* t, const char* path, uint32_t dp_bits, const uint64_t range_start[4], const uint64_t range_end[4],
                   const uint64_t keyx[4], const uint64_t keyy[4], uint64_t total_count, double total_time);
-/* Load the DP table of a reference work file (HEADW) into t; fills dp_bits / count / time when non-NULL.  0 on success. */
+/* Same, recording total_walk kangaroos (Backup.cpp:530): the file ends right after the count, and the caller appends the
+ * total_walk x 96-byte records {x[4], y[4], d[4]} (Backup.cpp:536-539) to complete it. */
+int kgi_save_work_ex(kgi_table* t, const char* path, uint32_t dp_bits, const uint64_t range_start[4], const uint64_t range_end[4],
+                     const uint64_t keyx[4], const uint64_t keyy[4], uint64_t total_count, double total_time, uint64_t total_walk);
+/* Load the DP table of a reference work file (HEADW) into t; fills dp_bits / count / time when non-NULL.  0 on success,
+ * negative when the file cannot be opened or is short. */
 int kgi_load_work(kgi_table* t, const char* path, uint32_t* dp_bits, uint64_t* total_count, double* total_time);
+/* Same (Kangaroo::LoadWork, Backup.cpp:149-207), also returning the range, the key (4 limbs each), nbLoadedWalk and the
+ * byte offset of the kangaroo block (nb_walk x 96 bytes, checked to be present).  Any output may be NULL. */
+int kgi_load_work_ex(kgi_table* t, const char* path, uint32_t* dp_bits, uint64_t range_start[4], uint64_t range_end[4],
+                     uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time, uint64_t* nb_walk,
+                     uint64_t* walk_offset);
 
 #ifdef __cplusplus
 }

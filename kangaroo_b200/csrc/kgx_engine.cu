@@ -13,6 +13,7 @@
 #include "../../include/kgx.h"
 #include "kgx_kernel.cuh"
 #include "kgx_herd.cuh"
+#include "kgx_ckpt.cuh"
 
 using namespace kgx;
 
@@ -49,6 +50,8 @@ struct kgx_engine {
   cudaEvent_t evStart[2] = {nullptr, nullptr}, evStop[2] = {nullptr, nullptr};
   cudaEvent_t evSnap = nullptr;   // snapshot (checkpoint) staging complete
   bool snapPending = false;
+  u64* herdRecs = nullptr;        // n x 96-byte work-file records (kgx_snapshot_export / kgx_import); kept, like the staging, for the next save
+  bool snapConverted = false;     // herdRecs holds the pending snapshot
   float lastMs = 0.f;
   unsigned long long* prof = nullptr;   // KGX_PROF=1: phase cycle counters
   u64 launches = 0;
@@ -116,7 +119,7 @@ void kgx_destroy(kgx_engine* e) {
   cudaSetDevice(e->dev);
   if (e->stream) cudaStreamSynchronize(e->stream);
   cudaFree(e->dp40); cudaFree(e->herdTab); cudaFree(e->state); cudaFree(e->pre); cudaFree(e->slab[0]); cudaFree(e->slab[1]); cudaFree(e->jtab);
-  cudaFree(e->stgX); cudaFree(e->stgY); cudaFree(e->stgD); cudaFree(e->aux);
+  cudaFree(e->stgX); cudaFree(e->stgY); cudaFree(e->stgD); cudaFree(e->aux); cudaFree(e->herdRecs);
   if (e->slabPinned) cudaFreeHost(e->slabPinned);
   for (int i = 0; i < 2; i++) { if (e->evStart[i]) cudaEventDestroy(e->evStart[i]); if (e->evStop[i]) cudaEventDestroy(e->evStop[i]); }
   if (e->evSnap) cudaEventDestroy(e->evSnap);
@@ -366,6 +369,7 @@ int kgx_snapshot_begin(kgx_engine* e) {
   CK(e, cudaGetLastError());
   CK(e, cudaEventRecord(e->evSnap, e->stream));
   e->snapPending = true;
+  e->snapConverted = false;
   return 0;
 }
 
@@ -380,6 +384,100 @@ int kgx_snapshot_read(kgx_engine* e, uint64_t* px, uint64_t* py, uint64_t* d) {
   e->snapPending = false;
   free_staging(e);
   return 0;
+}
+
+// Work-file records of the pending snapshot (kgx_ckpt.cuh).  The first call converts the whole snapshot on the copy stream
+// (after the snapshot's unpack, concurrently with the jump launches queued since); every call copies records
+// [first, first+count) to dst (host or device memory of this engine's GPU).  The call whose range ends at n releases the
+// snapshot.  The staging (stgX/stgY/stgD, 80 B per kangaroo) and herdRecs (96 B per kangaroo) stay allocated for the next
+// save: cudaFree synchronises the device and would wait for the jump launch in flight.
+int kgx_snapshot_export(kgx_engine* e, const uint64_t wild_offset[2], uint64_t first, uint64_t count, void* dst) {
+  CK(e, cudaSetDevice(e->dev));
+  if (e->symmetry) { snprintf(e->err, sizeof e->err, "kgx_snapshot_export: not available in symmetric mode (signed distances)"); return -1; }
+  if (!e->snapPending) { snprintf(e->err, sizeof e->err, "kgx_snapshot_export: no snapshot pending"); return -1; }
+  if (first > e->n || count > e->n - first) { snprintf(e->err, sizeof e->err, "kgx_snapshot_export: range [%llu, +%llu) outside the herd", (unsigned long long)first, (unsigned long long)count); return -1; }
+  if (!e->snapConverted) {
+    if (!e->herdRecs) CK(e, cudaMalloc(&e->herdRecs, e->n * 96));
+    CK(e, cudaStreamWaitEvent(e->copyStream, e->evSnap, 0));
+    herd_export_kernel<<<4 * e->sms, 256, 0, e->copyStream>>>(reinterpret_cast<const u32*>(e->stgX), reinterpret_cast<const u32*>(e->stgY),
+                                                             reinterpret_cast<const u32*>(e->stgD), e->herdRecs, e->n, wild_offset[0], wild_offset[1]);
+    e->launches++;
+    CK(e, cudaGetLastError());
+    e->snapConverted = true;
+  }
+  if (count) CK(e, cudaMemcpyAsync(dst, e->herdRecs + first * 12, count * 96, cudaMemcpyDefault, e->copyStream));
+  CK(e, cudaStreamSynchronize(e->copyStream));
+  if (first + count == e->n) { e->snapPending = false; e->snapConverted = false; }
+  return 0;
+}
+
+// Replace kangaroos 0..count-1 by `count` work-file records (host memory), in stream order after the launch in flight.
+// Nothing changes when a record's biased distance does not fit in 128 bits (error) or, with verify != 0, when any position
+// differs from d*G (tame) / key + d*G (wild): *mismatches then says how many do (0 = imported).
+int kgx_import(kgx_engine* e, const uint64_t wild_offset[2], const void* recs, uint64_t count, const uint64_t keyx[4],
+               const uint64_t keyy[4], int verify, uint64_t* mismatches) {
+  CK(e, cudaSetDevice(e->dev));
+  if (mismatches) *mismatches = 0;
+  if (e->symmetry) { snprintf(e->err, sizeof e->err, "kgx_import: not available in symmetric mode (signed distances)"); return -1; }
+  if (e->snapPending) { snprintf(e->err, sizeof e->err, "kgx_import: snapshot pending (export it first)"); return -1; }
+  if (count > e->n) { snprintf(e->err, sizeof e->err, "kgx_import: %llu records for a herd of %llu", (unsigned long long)count, (unsigned long long)e->n); return -1; }
+  if (count == 0) return 0;
+  if (verify && !e->herdTab) {
+    CK(e, cudaMalloc(&e->herdTab, 256 * 16 * 4));
+    herd_table_kernel<<<1, 32, 0, e->stream>>>(e->herdTab);
+    e->launches++;
+    CK(e, cudaGetLastError());
+  }
+  if (!e->herdRecs) CK(e, cudaMalloc(&e->herdRecs, e->n * 96));
+  if (ensure_staging(e)) return -1;
+  u32 *scal = nullptr, *vx = nullptr, *vy = nullptr, *dKey = nullptr;
+  unsigned long long* flags = nullptr;     // [0] lowest out-of-range index (~0 = none), [1] mismatches
+  auto body = [&]() -> int {
+    CK(e, cudaMalloc(&scal, count * 32));
+    CK(e, cudaMalloc(&flags, 16));
+    const unsigned long long init[2] = {~0ull, 0ull};
+    CK(e, cudaMemcpyAsync(flags, init, 16, cudaMemcpyHostToDevice, e->stream));
+    CK(e, cudaMemcpyAsync(e->herdRecs, recs, count * 96, cudaMemcpyHostToDevice, e->stream));
+    unpack_kernel<<<(u32)((e->n + 255) / 256), 256, 0, e->stream>>>(e->state, e->stgX, e->stgY, e->stgD, e->n, e->T, e->K);
+    e->launches++;
+    CK(e, cudaGetLastError());
+    herd_import_kernel<<<4 * e->sms, 256, 0, e->stream>>>(e->herdRecs, count, wild_offset[0], wild_offset[1], reinterpret_cast<u32*>(e->stgX),
+                                                         reinterpret_cast<u32*>(e->stgY), reinterpret_cast<u32*>(e->stgD), scal, flags);
+    e->launches++;
+    CK(e, cudaGetLastError());
+    if (verify) {
+      CK(e, cudaMalloc(&vx, count * 32));
+      CK(e, cudaMalloc(&vy, count * 32));
+      CK(e, cudaMalloc(&dKey, 64));
+      uint64_t key[8];
+      memcpy(key, keyx, 32); memcpy(key + 4, keyy, 32);
+      CK(e, cudaMemcpyAsync(dKey, key, 64, cudaMemcpyHostToDevice, e->stream));
+      herd_kernel<<<(u32)((count + 127) / 128), 128, 0, e->stream>>>(e->herdTab, scal, dKey, 0, count, vx, vy, 0, nullptr);
+      e->launches++;
+      CK(e, cudaGetLastError());
+      herd_compare_kernel<<<4 * e->sms, 256, 0, e->stream>>>(reinterpret_cast<u32*>(e->stgX), reinterpret_cast<u32*>(e->stgY), vx, vy, count, flags + 1);
+      e->launches++;
+      CK(e, cudaGetLastError());
+    }
+    unsigned long long res[2];
+    CK(e, cudaMemcpyAsync(res, flags, 16, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    if (res[0] != ~0ull) {
+      snprintf(e->err, sizeof e->err, "kgx_import: record %llu: distance does not fit the engine's 128-bit form (a file of another range?)", res[0]);
+      return -1;
+    }
+    if (mismatches) *mismatches = res[1];
+    if (res[1]) return 0;
+    pack_kernel<<<(u32)((e->nPadded + 255) / 256), 256, 0, e->stream>>>(e->state, e->stgX, e->stgY, e->stgD, e->n, e->nPadded, e->T, e->K, e->aux, e->symRule == KGX_SYM_CLASS ? 0 : 32);
+    e->launches++;
+    CK(e, cudaGetLastError());
+    CK(e, cudaStreamSynchronize(e->stream));
+    return 0;
+  };
+  const int rc = body();
+  cudaFree(scal); cudaFree(vx); cudaFree(vy); cudaFree(dKey); cudaFree(flags);
+  free_staging(e);
+  return rc;
 }
 
 int kgx_patch(kgx_engine* e, uint64_t kidx, const uint64_t px[4], const uint64_t py[4], const uint64_t d[2]) {

@@ -12,6 +12,7 @@
 // no lock is taken.  The one shared field HashTable::Add writes -- kDist/kType on ADD_COLLISION -- is not read: the stored
 // entry is looked up again by the owning worker.
 #include <atomic>
+#include <cerrno>
 #include <condition_variable>
 #include <cstdio>
 #include <cstring>
@@ -226,38 +227,71 @@ int kgi_resolve(kgi_table* t, const uint64_t d_old[2], const uint64_t d_new[2], 
   return 0;
 }
 
-int kgi_save_work(kgi_table* t, const char* path, uint32_t dp_bits, const uint64_t range_start[4], const uint64_t range_end[4],
-                  const uint64_t keyx[4], const uint64_t keyy[4], uint64_t total_count, double total_time) {
+// a failed stdio call: -errno (EIO when the C library left errno at 0)
+static int io_error() { return errno ? -errno : -EIO; }
+
+int kgi_save_work_ex(kgi_table* t, const char* path, uint32_t dp_bits, const uint64_t range_start[4], const uint64_t range_end[4],
+                     const uint64_t keyx[4], const uint64_t keyy[4], uint64_t total_count, double total_time, uint64_t total_walk) {
+  errno = 0;
   FILE* f = fopen(path, "wb");
-  if (!f) return -1;
+  if (!f) return io_error();
   // Kangaroo::SaveHeader (Backup.cpp:368-394), type HEADW
   const uint32_t head = HEADW_MAGIC, version = 0;
-  fwrite(&head, 4, 1, f); fwrite(&version, 4, 1, f);
-  fwrite(&dp_bits, 4, 1, f);
-  fwrite(range_start, 32, 1, f); fwrite(range_end, 32, 1, f);
-  fwrite(keyx, 32, 1, f); fwrite(keyy, 32, 1, f);
-  fwrite(&total_count, 8, 1, f); fwrite(&total_time, 8, 1, f);
-  t->ht->SaveTable(f, 0, HASH_SIZE, false);                       // HashTable.cpp:375-396
-  const uint64_t totalWalk = 0;                                   // no kangaroos in this file (Backup.cpp:549-551)
-  fwrite(&totalWalk, 8, 1, f);
+  bool ok = fwrite(&head, 4, 1, f) == 1 && fwrite(&version, 4, 1, f) == 1 && fwrite(&dp_bits, 4, 1, f) == 1 &&
+            fwrite(range_start, 32, 1, f) == 1 && fwrite(range_end, 32, 1, f) == 1 && fwrite(keyx, 32, 1, f) == 1 &&
+            fwrite(keyy, 32, 1, f) == 1 && fwrite(&total_count, 8, 1, f) == 1 && fwrite(&total_time, 8, 1, f) == 1;
+  if (ok) {
+    t->ht->SaveTable(f, 0, HASH_SIZE, false);                     // HashTable.cpp:375-396 (ignores fwrite results: ferror below)
+    ok = !ferror(f) && fwrite(&total_walk, 8, 1, f) == 1;         // Backup.cpp:530-531 / 549-551
+  }
+  ok = fflush(f) == 0 && ok;
+  const int err = ok ? 0 : io_error();
+  if (fclose(f) != 0 && ok) return io_error();
+  return err;
+}
+
+int kgi_save_work(kgi_table* t, const char* path, uint32_t dp_bits, const uint64_t range_start[4], const uint64_t range_end[4],
+                  const uint64_t keyx[4], const uint64_t keyy[4], uint64_t total_count, double total_time) {
+  return kgi_save_work_ex(t, path, dp_bits, range_start, range_end, keyx, keyy, total_count, total_time, 0);
+}
+
+int kgi_load_work_ex(kgi_table* t, const char* path, uint32_t* dp_bits, uint64_t range_start[4], uint64_t range_end[4],
+                     uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time, uint64_t* nb_walk,
+                     uint64_t* walk_offset) {
+  errno = 0;
+  FILE* f = fopen(path, "rb");
+  if (!f) return io_error();
+  // Kangaroo::LoadWork (Backup.cpp:149-207)
+  uint32_t head = 0, version = 0, dp = 0;
+  uint64_t hdr[16], cnt = 0, walk = 0; double tm = 0;
+  bool ok = fread(&head, 4, 1, f) == 1 && fread(&version, 4, 1, f) == 1 && head == HEADW_MAGIC;
+  ok = ok && fread(&dp, 4, 1, f) == 1 && fread(hdr, 32, 4, f) == 4 && fread(&cnt, 8, 1, f) == 1 && fread(&tm, 8, 1, f) == 1;
+  if (ok) {
+    t->ht->LoadTable(f);                                          // HashTable.cpp (Reset + per-bucket read; ignores fread results)
+    ok = !ferror(f) && !feof(f) && fread(&walk, 8, 1, f) == 1;
+  }
+  long off = ok ? ftell(f) : -1;
+  if (ok && walk) {                                               // the kangaroo block must be all there (FetchWalks, Backup.cpp:211-223)
+    ok = off >= 0 && fseek(f, 0, SEEK_END) == 0;
+    const long end = ok ? ftell(f) : -1;
+    ok = ok && end >= off && (uint64_t)(end - off) / 96 >= walk;
+  }
   fclose(f);
+  if (!ok) { t->ht->Reset(); return -EINVAL; }
+  if (dp_bits) *dp_bits = dp;
+  if (range_start) memcpy(range_start, hdr, 32);
+  if (range_end) memcpy(range_end, hdr + 4, 32);
+  if (keyx) memcpy(keyx, hdr + 8, 32);
+  if (keyy) memcpy(keyy, hdr + 12, 32);
+  if (total_count) *total_count = cnt;
+  if (total_time) *total_time = tm;
+  if (nb_walk) *nb_walk = walk;
+  if (walk_offset) *walk_offset = (uint64_t)off;
   return 0;
 }
 
 int kgi_load_work(kgi_table* t, const char* path, uint32_t* dp_bits, uint64_t* total_count, double* total_time) {
-  FILE* f = fopen(path, "rb");
-  if (!f) return -1;
-  uint32_t head = 0, version = 0, dp = 0;
-  uint64_t skip[16], cnt = 0; double tm = 0;
-  bool ok = fread(&head, 4, 1, f) == 1 && fread(&version, 4, 1, f) == 1 && head == HEADW_MAGIC;
-  ok = ok && fread(&dp, 4, 1, f) == 1 && fread(skip, 32, 4, f) == 4 && fread(&cnt, 8, 1, f) == 1 && fread(&tm, 8, 1, f) == 1;
-  if (!ok) { fclose(f); return -1; }
-  t->ht->LoadTable(f);                                            // HashTable.cpp (Reset + per-bucket read)
-  fclose(f);
-  if (dp_bits) *dp_bits = dp;
-  if (total_count) *total_count = cnt;
-  if (total_time) *total_time = tm;
-  return 0;
+  return kgi_load_work_ex(t, path, dp_bits, nullptr, nullptr, nullptr, nullptr, total_count, total_time, nullptr, nullptr);
 }
 
 }  // extern "C"

@@ -115,6 +115,81 @@ def _step_flat(self, n_found):
 DPGather.step_flat = _step_flat
 
 
+WALK_BYTES = 96          # one kangaroo of a work file (Backup.cpp:536-539)
+
+
+class HerdGather:
+    """The herds of all ranks to rank 0 as one work-file kangaroo block, in rank order (rank 0's kIdx 0..n0-1, then rank
+    1's, ...), so that the reference reads it as one herd.  Herd sizes may differ per rank (GetGridSize runs per GPU): they
+    are exchanged once here.  The block moves in chunks of at most `chunk` records that never span two ranks; every chunk
+    goes through one fixed buffer of chunk*96 bytes on `device` (a point-to-point send from its owner to rank 0).
+
+    Every rank calls chunk(j) for j in range(len(plan)) in the same order."""
+
+    def __init__(self, dist, rank, world, torch, n_local, device, chunk):
+        self.dist, self.rank, self.world, self.torch, self.device = dist, rank, world, torch, device
+        if dist is not None and world > 1:
+            mine = torch.tensor([int(n_local)], dtype=torch.int64, device=device)
+            sizes = torch.empty(world, dtype=torch.int64, device=device)
+            dist.all_gather_into_tensor(sizes, mine)
+            self.sizes = [int(v) for v in sizes.cpu().tolist()]
+        else:
+            self.sizes = [int(n_local)]
+        self.offsets = [sum(self.sizes[:r]) for r in range(len(self.sizes))]
+        self.total = sum(self.sizes)
+        self.chunk_records = int(chunk)
+        self.plan = [(r, first, min(self.chunk_records, n - first)) for r, n in enumerate(self.sizes) for first in range(0, n, self.chunk_records)]
+        self._buf = None
+
+    def chunk(self, j, export):
+        """Move chunk j of the plan to rank 0.  export(first, count, dst) writes this rank's records [first, first+count)
+        into dst (a uint8 tensor of count*96 bytes on `device`); it is called on the owning rank only.  Returns the records
+        (a view of the gather buffer, valid until the next call) on rank 0, None elsewhere."""
+        r, first, count = self.plan[j]
+        if self.rank != r and self.rank != 0:
+            return None
+        if self._buf is None:
+            self._buf = self.torch.empty(self.chunk_records * WALK_BYTES, dtype=self.torch.uint8, device=self.device)
+        view = self._buf[:count * WALK_BYTES]
+        if self.rank == r:
+            export(first, count, view)
+        if r != 0:
+            if self.rank == r:
+                self.dist.send(view, dst=0)
+            else:
+                self.dist.recv(view, src=r)
+            if self.device.type == "cuda":
+                self.torch.cuda.current_stream().synchronize()   # the next export rewrites the buffer from another stream
+        return view if self.rank == 0 else None
+
+    def scatter(self, nb_walk, read):
+        """The reverse, for a resume (FetchWalks): the first nb_walk kangaroos of a file, read on rank 0 only, to their
+        ranks through the same chunk plan and buffer.  read(first, count) -> uint8 numpy array of count*96 bytes (called on
+        rank 0).  Returns this rank's records [0, min(n_r, nb_walk - o_r)) as a uint8 numpy array."""
+        import numpy as np
+        off = self.offsets[self.rank]
+        out = np.empty(max(0, min(self.sizes[self.rank], nb_walk - off)) * WALK_BYTES, dtype=np.uint8)
+        for r, first, count in self.plan:
+            count = max(0, min(count, nb_walk - self.offsets[r] - first))
+            if count == 0 or (self.rank != r and self.rank != 0):
+                continue
+            if self._buf is None:
+                self._buf = self.torch.empty(self.chunk_records * WALK_BYTES, dtype=self.torch.uint8, device=self.device)
+            view = self._buf[:count * WALK_BYTES]
+            if self.rank == 0:
+                view.copy_(self.torch.from_numpy(read(self.offsets[r] + first, count)))
+            if r != 0:
+                if self.rank == 0:
+                    self.dist.send(view, dst=r)
+                else:
+                    self.dist.recv(view, src=0)
+                if self.device.type == "cuda":
+                    self.torch.cuda.current_stream().synchronize()
+            if self.rank == r:
+                out[first * WALK_BYTES:(first + count) * WALK_BYTES] = view.cpu().numpy()
+        return out
+
+
 def decode_records(buf):
     """uint8 tensor/bytes of 56-byte records -> list of (x, d_biased, kidx) Python ints (GPUEngine.cu:653-671)."""
     b = bytes(buf.cpu().numpy().tobytes()) if hasattr(buf, "cpu") else bytes(buf)

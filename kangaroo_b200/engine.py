@@ -196,6 +196,36 @@ class GPUEngine:
         self._ck(self._lib.kgx_snapshot_read(self._h, _p(ax), _p(ay), _p(ad)), "SnapshotRead")
         return _ints(ax), _ints(ay), [self._unbias(v, i) for i, v in enumerate(_ints(ad))]
 
+    def _wo(self):
+        return _limbs([self.wildOffset & ((1 << 128) - 1)], 2)
+
+    def SnapshotExport(self, first, count, dst=None):
+        """Work-file records [first, first+count) of the snapshot taken by SnapshotBegin (96 bytes each: x, y, unbiased d
+        mod n as 4 u64 limbs; Backup.cpp:536-539), converted on the device.  dst: a writable buffer of count*96 bytes -- a
+        numpy array, or an int address of host / device memory -- or None for a new (count, 12) uint64 array.  The chunk
+        that ends at nbKangaroo releases the snapshot."""
+        out = np.empty((count, 12), dtype=np.uint64) if dst is None else dst
+        if isinstance(out, np.ndarray):
+            assert out.flags.c_contiguous and out.nbytes >= count * 96
+            addr = out.ctypes.data
+        else:
+            addr = int(out)
+        self._ck(self._lib.kgx_snapshot_export(self._h, _p(self._wo()), int(first), int(count), ctypes.c_void_p(addr)), "SnapshotExport")
+        return out
+
+    def ImportKangaroos(self, recs, key, verify=True):
+        """Replace kangaroos 0..len(recs)-1 by work-file records (bytes / uint8 or (n,12) uint64 array; FetchWalks order),
+        converted and checked on the device.  Raises when a distance does not fit the engine's form (a file of another range).
+        verify: recompute every position as d*G (tame) / key + d*G (wild); returns the number of records that fail, and the
+        herd is left unchanged unless that number is 0."""
+        a = np.ascontiguousarray(np.frombuffer(recs, dtype=np.uint8) if not isinstance(recs, np.ndarray) else recs.view(np.uint8).reshape(-1))
+        assert a.size % 96 == 0
+        kx, ky = _limbs([key[0]], 4), _limbs([key[1]], 4)
+        bad = ctypes.c_uint64(0)
+        self._ck(self._lib.kgx_import(self._h, _p(self._wo()), a.ctypes.data_as(ctypes.c_void_p), a.size // 96, _p(kx), _p(ky),
+                                      int(bool(verify)), ctypes.byref(bad)), "ImportKangaroos")
+        return int(bad.value)
+
     def SetKangaroosRaw(self, ax, ay, ad):
         n = self.nbKangaroo
         ax, ay, ad = _limbs(ax, 4), _limbs(ay, 4), _limbs(ad, 2)

@@ -39,7 +39,12 @@ _SIGS = {
                                      ctypes.c_double]),
     "kgi_load_work": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_uint32), _u64p,
                                      ctypes.POINTER(ctypes.c_double)]),
+    "kgi_save_work_ex": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_uint32, _u64p, _u64p, _u64p, _u64p, ctypes.c_uint64,
+                                        ctypes.c_double, ctypes.c_uint64]),
+    "kgi_load_work_ex": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_uint32), _u64p, _u64p, _u64p, _u64p,
+                                        _u64p, ctypes.POINTER(ctypes.c_double), _u64p, _u64p]),
 }
+WALK_BYTES = 96          # one kangaroo of a work file: x[4], y[4], d[4] (Backup.cpp:536-539)
 EXPORTED_SYMBOLS = sorted(_SIGS)
 _lib = None
 
@@ -131,11 +136,12 @@ class DPTable:
         rc = self._lib.kgi_resolve(self._h, a, b, _limbs4(key[0]), _limbs4(key[1]), _limbs4(range_start), out)
         return sum(int(out[k]) << (64 * k) for k in range(4)) if rc == 1 else None
 
-    def save_work(self, path, dp_bits, range_start, range_end, pubkey, total_count=0, total_time=0.0):
-        rc = self._lib.kgi_save_work(self._h, os.fsencode(path), int(dp_bits), _limbs4(range_start), _limbs4(range_end),
-                                     _limbs4(pubkey[0]), _limbs4(pubkey[1]), int(total_count), float(total_time))
+    def save_work(self, path, dp_bits, range_start, range_end, pubkey, total_count=0, total_time=0.0, total_walk=0):
+        """Header + table (+ the kangaroo count: the caller appends total_walk x 96-byte records right after)."""
+        rc = self._lib.kgi_save_work_ex(self._h, os.fsencode(path), int(dp_bits), _limbs4(range_start), _limbs4(range_end),
+                                        _limbs4(pubkey[0]), _limbs4(pubkey[1]), int(total_count), float(total_time), int(total_walk))
         if rc != 0:
-            raise RuntimeError("kgi_save_work: cannot write %s" % path)
+            raise RuntimeError("kgi_save_work: cannot write %s: %s" % (path, os.strerror(-rc)))
 
     def load_work(self, path):
         dp, cnt, tm = ctypes.c_uint32(0), ctypes.c_uint64(0), ctypes.c_double(0)
@@ -143,3 +149,43 @@ class DPTable:
         if rc != 0:
             raise RuntimeError("kgi_load_work: %s is not a HEADW work file" % path)
         return dp.value, cnt.value, tm.value
+
+    def load_work_ex(self, path):
+        """Kangaroo::LoadWork (Backup.cpp:149-207): the table into this DPTable -> WorkInfo (header, nbLoadedWalk and the
+        offset of the kangaroo block)."""
+        dp, cnt, tm = ctypes.c_uint32(0), ctypes.c_uint64(0), ctypes.c_double(0)
+        rs, re_, kx, ky = (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)()
+        walk, off = ctypes.c_uint64(0), ctypes.c_uint64(0)
+        rc = self._lib.kgi_load_work_ex(self._h, os.fsencode(path), ctypes.byref(dp), rs, re_, kx, ky, ctypes.byref(cnt),
+                                        ctypes.byref(tm), ctypes.byref(walk), ctypes.byref(off))
+        if rc != 0:
+            raise RuntimeError("kgi_load_work: %s is not a complete HEADW work file" % path)
+        val = lambda a: sum(int(a[k]) << (64 * k) for k in range(4))
+        return WorkInfo(path, dp.value, val(rs), val(re_), (val(kx), val(ky)), cnt.value, tm.value, walk.value, off.value)
+
+
+def read_work_header(path):
+    """The fixed 156-byte HEADW header (Backup.cpp:368-394) without the table -> (dp_bits, range_start, range_end,
+    (key x, key y), total_count, total_time).  Needs no library."""
+    import struct
+    with open(path, "rb") as f:
+        raw = f.read(156)
+    if len(raw) != 156 or struct.unpack_from("<I", raw)[0] != 0xFA6A8001:
+        raise RuntimeError("%s is not a HEADW work file" % path)
+    val = lambda o: int.from_bytes(raw[o:o + 32], "little")
+    return (struct.unpack_from("<I", raw, 8)[0], val(12), val(44), (val(76), val(108)),
+            struct.unpack_from("<Q", raw, 140)[0], struct.unpack_from("<d", raw, 148)[0])
+
+
+class WorkInfo:
+    """Header of a HEADW work file and where its kangaroos are."""
+
+    def __init__(self, path, dp_bits, range_start, range_end, key, total_count, total_time, nb_walk, walk_offset):
+        self.path, self.dp_bits, self.range_start, self.range_end, self.key = path, dp_bits, range_start, range_end, key
+        self.total_count, self.total_time, self.nb_walk, self.walk_offset = total_count, total_time, nb_walk, walk_offset
+
+    def walks(self, first=0, count=None):
+        """kangaroos [first, first+count) of the file as a (count, 12) uint64 array of records (read from disk)."""
+        count = self.nb_walk - first if count is None else count
+        assert 0 <= first and first + count <= self.nb_walk
+        return np.fromfile(self.path, dtype=np.uint64, count=count * 12, offset=self.walk_offset + first * WALK_BYTES).reshape(count, 12)

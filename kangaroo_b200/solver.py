@@ -17,6 +17,17 @@ Per step (= one GPUEngine::Launch on every rank) nothing on the data path is Pyt
 
   single GPU :  python -m kangaroo_b200.solver in.txt --dp 12
   N GPUs     :  torchrun --nproc-per-node N -m kangaroo_b200.solver in.txt --dp 12
+
+Work files (the reference's -w / -wi / -ws / -i, Backup.cpp): --save-work FILE writes the DP table, with --save-kangaroos also
+every rank's herd (rank order, 96-byte records converted on the device, gathered to rank 0 in bounded chunks), at the end and
+every --save-interval seconds; --resume FILE continues a run from such a file, or from one the reference wrote.  A file is a
+consistent cut: its table holds the DPs of exactly the launches its herd has made, and its count is their jumps.  The save
+decided at step k snapshots the herd on the device in stream order after launch i+1 (in flight at step k); step k+1
+queues the table write on the ingest thread right behind launch i+1's DPs, so it writes the table of the cut; the herd chunks
+follow over the next steps (Solver._save_start).  The end-of-run save does the same
+with the launch in flight when the loop stops.  Kangaroos re-created at step k are re-created after the snapshot, so the
+file holds them dead: a resumed run finds them again.  A save goes to FILE.tmp, is fsynced and renamed over FILE; a failed
+save removes FILE.tmp and the run goes on.  On --resume only rank 0 reads the file.
 """
 import argparse
 import ctypes
@@ -30,11 +41,14 @@ import numpy as np
 
 from . import ecmath as ec
 from .engine import GPUEngine, NB_JUMP, NB_RUN, WILD, random_herd_arrays
-from .dist import DPGather, SlabView, DP40_BYTES
+from .dist import DPGather, HerdGather, SlabView, DP40_BYTES, WALK_BYTES
 from .ingest import DPTable, EV_RESET, EV_COLLISION
 
 ORDER = ec.N
 MAX_RESETS = 255          # per step, carried in the control broadcast
+SAVE_CHUNK = 1 << 18      # kangaroos per gather chunk of a save (24 MB buffer)
+SAVE_CHUNKS_PER_STEP = 1  # chunks a step moves while a save is in progress (default herd: 17 steps)
+SAVE_BUFFERS = 4          # rank 0's pinned chunk buffers queued to the writer
 
 
 def create_jump_table(range_power):
@@ -65,7 +79,8 @@ def dp_mask(bits):
 
 
 class Solver:
-    def __init__(self, start, end, pub, dp_bits, grid=None, max_found=1 << 17, seed=None, ingest_threads=0):
+    def __init__(self, start, end, pub, dp_bits, grid=None, max_found=1 << 17, seed=None, ingest_threads=0,
+                 save_work="", save_interval=0.0, save_kangaroos=False, resume=None):
         import torch
         self.torch = torch
         self.rank = int(os.environ.get("RANK", "0"))
@@ -102,7 +117,7 @@ class Solver:
         self._hosts = ([torch.empty(self.world * max_found * DP40_BYTES, dtype=torch.uint8).pin_memory() for _ in range(2)]
                        if self.rank == 0 else None)
         self._hidx = 0
-        self._work = queue.Queue(maxsize=1)
+        self._work = queue.Queue()
         self._done = queue.Queue()
         self._pending = 0
         self._acc_found, self._acc_resets = None, []
@@ -110,12 +125,170 @@ class Solver:
         if self.rank == 0:
             self._thread = threading.Thread(target=self._ingest_loop, daemon=True)
             self._thread.start()
-        self._ctrl = torch.zeros(2 + 2 * MAX_RESETS, dtype=torch.int64, device="cuda")
+        self._ctrl = torch.zeros(4 + 2 * MAX_RESETS, dtype=torch.int64, device="cuda")
         self.jumps = 0
         self.same_herd = 0
         self.resets_done = 0
         self.t_ingest = 0.0
         self.stop = False
+        self.save_path, self.save_interval, self.save_kangaroos = save_work, float(save_interval), bool(save_kangaroos)
+        self.time_offset = 0.0
+        self.herd = (HerdGather(self.dist, self.rank, self.world, torch, n, torch.device("cuda", self.local), SAVE_CHUNK)
+                     if save_kangaroos or resume else None)
+        self._save_due = False              # decided at the end of step k, started in step k+1
+        self._chunks_next = 0               # herd chunks step k+1 moves (decided at the end of step k)
+        self._saving = False                # herd chunks of the current save still to move
+        self._save_left, self._save_steps, self._save_stats, self._step_times = [], [], [], []
+        self._saved = queue.Queue()         # ingest thread -> main: (path, MB, seconds, error) per finished save
+        self._chunk_pool = queue.Queue()
+        if self.rank == 0 and save_kangaroos:
+            for _ in range(SAVE_BUFFERS):
+                self._chunk_pool.put(torch.empty(SAVE_CHUNK * WALK_BYTES, dtype=torch.uint8).pin_memory())
+        self.saves = []                     # (MB, seconds) per save, rank 0
+        self.save_error = None
+        if resume:
+            self._resume(resume)
+        self.jumps0 = self.jumps
+
+    # -- work files ------------------------------------------------------------------------------------------------
+    def _resume(self, path):
+        """Kangaroo::LoadWork + FetchWalks (Backup.cpp:149-231): rank 0 loads the table; rank r takes the file's kangaroos
+        [o_r, o_r + n_r) as its kIdx 0..n_r-1 (o_r = herd sizes of the lower ranks), verified on the device; the ones the
+        file lacks keep the fresh random herd made above.  Only rank 0 reads the file; it sends every rank its records."""
+        torch = self.torch
+        info = torch.zeros(4, dtype=torch.int64, device="cuda")
+        if self.rank == 0:
+            w = self.dps.load_work_ex(path)
+            info.copy_(torch.tensor([w.nb_walk, w.walk_offset, w.total_count, 0], dtype=torch.int64))
+            self.time_offset = w.total_time
+        if self.dist is not None:
+            self.dist.broadcast(info, 0)
+        nb_walk, offset, count, _ = (int(v) for v in info.cpu().tolist())
+        self.jumps = count
+        take = max(0, min(self.eng.nbKangaroo, nb_walk - self.herd.offsets[self.rank]))
+        if self.rank == 0:
+            print("Resume %s: %d DPs, count 2^%.2f, %d kangaroos in the file for %d in the herd" %
+                  (path, len(self.dps), np.log2(max(count, 1)), nb_walk, self.herd.total), flush=True)
+            if nb_walk > self.herd.total:
+                print("Warning: %d unhandled kangaroos" % (nb_walk - self.herd.total), flush=True)   # Kangaroo.cpp FectchKangaroos
+
+        def read(first, cnt):                                   # rank 0 only
+            return np.fromfile(path, dtype=np.uint8, count=cnt * WALK_BYTES, offset=offset + first * WALK_BYTES)
+
+        t0 = time.perf_counter()
+        recs = self.herd.scatter(nb_walk, read)                 # this rank's records, sent by rank 0 in bounded chunks
+        bad = self.eng.ImportKangaroos(recs, self.key, verify=True) if take else 0
+        if self.dist is not None:                               # every rank refuses together (none left waiting in a collective)
+            t = torch.tensor([bad], dtype=torch.int64, device="cuda")
+            self.dist.all_reduce(t)
+            bad = int(t.item())
+        if bad:
+            raise RuntimeError("%s: %d kangaroos are not at d*G (tame) / key + d*G (wild): the file belongs to another key "
+                               "or range" % (path, bad))
+        if take:
+            print("rank %d: %d kangaroos imported and verified in %.2f s" % (self.rank, take, time.perf_counter() - t0), flush=True)
+
+    def _export(self, first, count, dst):
+        self.eng.SnapshotExport(first, count, dst.data_ptr())
+
+    # A save runs alongside the launches.  Its first step queues the table write on the ingest thread right behind the DPs of
+    # the cut (that thread alone touches the table, so it writes the table of the cut); then every step moves up to
+    # SAVE_CHUNKS_PER_STEP herd chunks (device conversion + gather to rank 0 + copy into a free pinned buffer) and queues their
+    # writes behind it.  The ingest thread writes, fsyncs and renames.  A step moves a chunk only when rank 0 has a pinned
+    # buffer the writer has freed, so the step loop never waits for the disk: a slow disk only makes the save take more steps.
+    def _save_start(self, kangaroos, chunks):
+        """first step of a save of the current cut: with kangaroos, the snapshot was taken one step earlier"""
+        self._saving = True
+        self._save_left = list(range(len(self.herd.plan))) if kangaroos else []
+        self._save_steps = []                                  # times of the steps that moved this save
+        self._save_stats.append(self._save_steps)
+        if self.rank == 0:
+            nwalk = self.herd.total if kangaroos else 0
+            self._work.put(("begin", self.save_path, self.jumps, self.time_offset + time.time() - self.t_start, nwalk, time.perf_counter()))
+        self._save_progress(chunks)
+
+    def _save_progress(self, chunks):
+        if not self._saving:
+            return
+        while self._save_left and chunks > 0:
+            j = self._save_left.pop(0)
+            chunks -= 1
+            v = self.herd.chunk(j, self._export)
+            if self.rank == 0:
+                buf = self._chunk_pool.get()                     # back-pressure: the writer frees buffers as it goes
+                buf[:v.numel()].copy_(v)
+                self._work.put(("chunk", buf, v.numel()))
+        if not self._save_left:
+            if self.rank == 0:
+                self._work.put(("end",))
+            self._saving = False
+
+    def _write(self, job):
+        """ingest thread: one piece of a work file (jobs arrive in file order)"""
+        kind = job[0]
+        if kind == "begin":
+            path, count, total_time, nwalk, self._wt0 = job[1:]
+            self._wpath, self._wtmp, self._werr, self._wf = path, path + ".tmp", None, None
+            try:
+                self.dps.save_work(self._wtmp, self.dp_bits, self.start, self.end, self.pub, total_count=count,
+                                   total_time=total_time, total_walk=nwalk)
+                self._wf = open(self._wtmp, "ab")
+            except (OSError, RuntimeError) as e:
+                self._werr = str(e)
+        elif kind == "chunk":
+            buf, nbytes = job[1], job[2]
+            try:
+                if self._wf is not None and self._werr is None:
+                    self._wf.write(memoryview(buf.numpy()[:nbytes]))
+            except OSError as e:
+                self._werr = str(e)
+            finally:
+                self._chunk_pool.put(buf)
+        else:
+            size = 0
+            try:
+                if self._werr is None:
+                    self._wf.flush()
+                    os.fsync(self._wf.fileno())
+                    size = self._wf.tell()
+                    self._wf.close()
+                    self._wf = None
+                    os.replace(self._wtmp, self._wpath)          # the previous checkpoint stays whole until here
+                    dfd = os.open(os.path.dirname(os.path.abspath(self._wpath)), os.O_RDONLY)
+                    try:
+                        os.fsync(dfd)
+                    finally:
+                        os.close(dfd)
+            except OSError as e:
+                self._werr = str(e)
+            if self._werr is not None:
+                if self._wf is not None:
+                    self._wf.close()
+                    self._wf = None
+                try:
+                    os.remove(self._wtmp)
+                except OSError:
+                    pass
+            res = (self._wpath, size / 1048576.0, time.perf_counter() - self._wt0, self._werr)
+            self._on_saved(*res)
+            self._saved.put(res)
+
+    def _on_saved(self, path, mb, seconds, err):
+        """ingest thread, right after a save finished (or failed)"""
+
+    def _report_saves(self, block_for=0):
+        """rank 0: log the saves finished so far; block_for = saves still to wait for"""
+        while block_for > 0 or not self._saved.empty():
+            path, mb, secs, err = self._saved.get()
+            block_for -= 1
+            st = self._save_stats.pop(0) if self._save_stats else []
+            if err is not None:
+                self.save_error = err
+                print("SaveWork %s failed: %s (the previous file is kept)" % (path, err), flush=True)
+                continue
+            self.saves.append((mb, secs))
+            print("SaveWork %s: %.1f MB in %.2f s, written beside %d steps; longest of them %.1f ms (median step %.1f ms)" %
+                  (path, mb, secs, len(st), 1e3 * max(st or [0]), 1e3 * float(np.median(self._step_times[-64:] or [0]))), flush=True)
 
     # -- rank 0: ingest -------------------------------------------------------------------------------------------
     def _ingest(self, segments):
@@ -137,23 +310,32 @@ class Solver:
 
     def _ingest_loop(self):
         while True:
-            segs = self._work.get()
-            if segs is None:
+            job = self._work.get()
+            if job is None:
                 return
-            self._done.put(self._ingest(segs))
+            if job[0] == "dps":
+                self._done.put(self._ingest(job[1]))
+            else:
+                self._write(job)
 
     def _submit(self, segs):
         """hand one step's records to the ingest thread"""
-        self._work.put(segs)
+        self._work.put(("dps", segs))
         self._pending += 1
 
-    def _staging(self):
-        """the staging buffer for this step; at most one older step may still be in the ingest thread (it reads the OTHER buffer)"""
+    def _staging(self, nbytes):
+        """the staging buffer for this step; at most one older step may still be in the ingest thread (it reads the OTHER
+        pinned buffer).  While a save keeps that thread busy, further steps get a buffer of their own instead of waiting."""
+        if self._pending >= 2 and self._writes_pending():
+            return self.torch.empty(nbytes, dtype=self.torch.uint8)
         while self._pending >= 2:
             self._take(block=True)
         host = self._hosts[self._hidx]
         self._hidx ^= 1
         return host
+
+    def _writes_pending(self):
+        return self._saving or len(self._save_stats) > 0
 
     def _take(self, block):
         f, r = self._done.get(block=block)
@@ -185,19 +367,61 @@ class Solver:
         self.eng.SetKangaroo(kidx, pos[0], pos[1], d)
         self.resets_done += 1
 
-    def step(self):
+    def step(self, may_save=True):
         """one Launch on every rank; returns the private key on rank 0 when found (None otherwise)"""
         torch = self.torch
         n_found = self.eng.collect_count(relaunch=True)                  # launch i done, launch i+1 running
+        self._gather(n_found)
+        found, resets = None, []
+        self._save_work_done = self._save_due or self._saving
+        if self._save_due:                                               # decided at the end of the previous step
+            self._save_due = False
+            self._last_save = time.time()
+            self._save_start(self.save_kangaroos, self._chunks_next)     # behind launch i+1's DPs: the cut
+        elif self._saving:
+            self._save_progress(self._chunks_next)
+        if self.rank == 0:
+            found, resets = self._harvest()
+        save_next = (may_save and self.save_interval > 0 and self.rank == 0 and not self._saving and
+                     time.time() - self._last_save >= self.save_interval)
+        # herd chunks the next step may move: only into pinned buffers the writer has already freed, so a step never waits for
+        # the disk (rank 0 decides, every rank follows)
+        chunks = min(SAVE_CHUNKS_PER_STEP, self._chunk_pool.qsize()) if self.rank == 0 else 0
+        # control word: stop flag + save flag + kangaroos to re-create, back to their owners
+        if self.dist is not None:
+            if self.rank == 0:
+                resets = resets[:MAX_RESETS]
+                c = [1 if found is not None else 0, len(resets), int(save_next), chunks] + [v for rk in resets for v in rk]
+                self._ctrl[:len(c)].copy_(torch.tensor(c, dtype=torch.int64))
+            self.dist.broadcast(self._ctrl, 0)
+            c = self._ctrl.cpu().tolist()
+            self.stop = bool(c[0])
+            save_next, chunks = bool(c[2]), c[3]
+            resets = [(c[4 + 2 * i], c[5 + 2 * i]) for i in range(c[1])]
+        else:
+            self.stop = found is not None
+        self._chunks_next = chunks
+        if save_next and not self.stop:
+            if self.save_kangaroos:
+                self.eng.SnapshotBegin()                                 # stream order: after launch i+1, before the resets below
+            self._save_due = True
+        for rk, kidx in resets:
+            self.same_herd += 1
+            if rk == self.rank and not self.stop:
+                self._reset_kangaroo(kidx)
+        return found
+
+    def _gather(self, n_found):
+        """this launch's DP records of every rank -> rank 0's ingest thread"""
+        torch = self.torch
         cnt = min(n_found, self.eng.maxFound)
         self.jumps += self.eng.nbKangaroo * NB_RUN * self.world
-        found, resets = None, []
         if self.gather is not None:
             res = self.gather.step_flat(cnt)                                # rank 0: (counts, cap, device tensor [world*cap*40])
             if self.rank == 0:
                 counts, cap, flat = res
                 nbytes = self.world * cap * DP40_BYTES
-                host = self._staging()
+                host = self._staging(nbytes)
                 host[:nbytes].copy_(flat[:nbytes], non_blocking=True)
                 torch.cuda.current_stream().synchronize()
                 h = host.numpy()
@@ -206,55 +430,57 @@ class Solver:
             if cnt:
                 ptr = self.eng.convert_dps_device_ptr()
                 dev = torch.as_tensor(SlabView(ptr + 4, cnt * DP40_BYTES), device="cuda")
-                host = self._staging()
+                host = self._staging(cnt * DP40_BYTES)
                 host[:cnt * DP40_BYTES].copy_(dev, non_blocking=True)
                 torch.cuda.current_stream().synchronize()
                 self._submit([(0, host.numpy()[:cnt * DP40_BYTES])])
-        if self.rank == 0:
-            found, resets = self._harvest()
-        # control word: stop flag + kangaroos to re-create, back to their owners
-        if self.dist is not None:
-            if self.rank == 0:
-                resets = resets[:MAX_RESETS]
-                c = [1 if found is not None else 0, len(resets)] + [v for rk in resets for v in rk]
-                self._ctrl[:len(c)].copy_(torch.tensor(c, dtype=torch.int64))
-            self.dist.broadcast(self._ctrl, 0)
-            c = self._ctrl.cpu().tolist()
-            self.stop = bool(c[0])
-            resets = [(c[2 + 2 * i], c[3 + 2 * i]) for i in range(c[1])]
-        else:
-            self.stop = found is not None
-        for rk, kidx in resets:
-            self.same_herd += 1
-            if rk == self.rank and not self.stop:
-                self._reset_kangaroo(kidx)
-        return found
 
     def run(self, max_steps=1 << 30, verbose=True):
         self.eng.callKernel()
         t0 = time.time()
+        self.t_start = self._last_save = t0
         key = None
         steps = 0
         self.steady = None                      # (time, jumps) after the first 32 steps: NCCL communicator set-up, first table growth
+        self._step_times = step_times = []
         for s in range(max_steps):
-            key = self.step()
+            ts = time.perf_counter()
+            key = self.step(may_save=s + 1 < max_steps)
+            step_times.append(time.perf_counter() - ts)
+            if self._save_work_done:
+                self._save_steps.append(step_times[-1])
             steps += 1
+            if self.rank == 0:
+                self._report_saves()
             if steps == 32:
                 self.steady = (time.time(), self.jumps)
             if verbose and self.rank == 0 and (s % 64 == 63 or self.stop):
                 dt = time.time() - t0
                 print("[%6.1fs] 2^%.2f jumps  %.0f MJump/s  %d DPs  dead %d  ingest %.1f ms/step" %
-                      (dt, np.log2(max(self.jumps, 1)), self.jumps / dt / 1e6, len(self.dps), self.same_herd,
+                      (dt, np.log2(max(self.jumps, 1)), (self.jumps - self.jumps0) / dt / 1e6, len(self.dps), self.same_herd,
                        1e3 * self.t_ingest / steps), flush=True)
             if self.stop:
                 break
-        self.eng.sync()
-        if self.rank == 0 and key is None:                      # the last steps' records may still be in the ingest thread
-            key, _ = self._harvest(wait_all=True)
+        if self._saving:                                        # a save still moving its herd: finish it first
+            self._save_progress(len(self._save_left))
+        if self.save_path:
+            # end-of-run cut: the launch still in flight is collected, its DPs go into the table before it is written
+            if self.save_kangaroos:
+                self.eng.SnapshotBegin()
+            self._gather(self.eng.collect_count(relaunch=False))
+        else:
+            self.eng.sync()
         t1 = time.time()
+        if self.save_path:
+            self._save_start(self.save_kangaroos, len(self.herd.plan) if self.save_kangaroos else 0)
+        if self.rank == 0:                                      # drain: the last steps' records may still be in the ingest thread
+            k2, _ = self._harvest(wait_all=True)
+            key = key if key is not None else k2
+            self._report_saves(block_for=len(self._save_stats))
         self.elapsed = t1 - t0
         self.steps = steps
-        self.steady_rate = ((self.jumps - self.steady[1]) / (t1 - self.steady[0]) if self.steady and steps > 64 else self.jumps / self.elapsed)
+        self.steady_rate = ((self.jumps - self.steady[1]) / (t1 - self.steady[0]) if self.steady and steps > 64
+                            else (self.jumps - self.jumps0) / self.elapsed)
         return key
 
     def close(self):
@@ -268,32 +494,74 @@ class Solver:
             self.dps.close()
 
 
+def _resume_header(path):
+    """the work file's header, read on rank 0 only and broadcast: the other ranks need not see the file"""
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    hdr = None
+    if int(os.environ.get("RANK", "0")) == 0:
+        from .ingest import read_work_header
+        dp, start, end, pub, _, _ = read_work_header(path)
+        hdr = (dp, start, end, pub)
+    if world > 1:
+        import torch
+        import torch.distributed as dist
+        local = int(os.environ.get("LOCAL_RANK", "0"))
+        torch.cuda.set_device(local)
+        if not dist.is_initialized():
+            dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+        box = [hdr]
+        dist.broadcast_object_list(box, 0)
+        hdr = box[0]
+    return hdr
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser()
-    ap.add_argument("config")
-    ap.add_argument("--dp", type=int, default=12)
+    ap.add_argument("config", nargs="?", help="range start, end and public keys (optional with --resume)")
+    ap.add_argument("--dp", type=int, default=None, help="distinguished-point bits (default 12, or the file's with --resume)")
     ap.add_argument("--grid", default="")
     ap.add_argument("--seed", type=int, default=None)
     ap.add_argument("--max-steps", type=int, default=1 << 30)
     ap.add_argument("--ingest-threads", type=int, default=0, help="workers of the rank-0 DP table (0 = min(8, cores))")
-    ap.add_argument("--save-work", default="", help="write the rank-0 DP table as a reference work file (HEADW) at the end")
+    ap.add_argument("--save-work", default="", help="write the DP table as a reference work file (HEADW) at the end (-w)")
+    ap.add_argument("--save-interval", type=float, default=0.0,
+                    help="also save every SECONDS while running (-wi); 0 = at the end only")
+    ap.add_argument("--save-kangaroos", action="store_true", help="save every rank's herd with the table (-ws)")
+    ap.add_argument("--resume", default="", metavar="FILE",
+                    help="continue from a work file (-i): range, key and dp come from the file unless given")
     a = ap.parse_args(argv)
-    start, end, pubs = ec.parse_config(a.config)
+    if a.resume:
+        file_dp, start, end, pub = _resume_header(a.resume)
+        pubs = [pub]
+        if a.config:
+            start, end, pubs = ec.parse_config(a.config)
+        dp = a.dp if a.dp is not None else file_dp
+    elif a.config:
+        start, end, pubs = ec.parse_config(a.config)
+        dp = a.dp if a.dp is not None else 12
+    else:
+        ap.error("a config file or --resume FILE is required")
+    if (a.save_interval > 0 or a.save_kangaroos) and not a.save_work:
+        ap.error("--save-interval and --save-kangaroos need --save-work FILE")
     grid = tuple(int(v) for v in a.grid.split(",")) if a.grid else None
     rc = 0
     for i, pub in enumerate(pubs):
-        s = Solver(start, end, pub, a.dp, grid, seed=a.seed, ingest_threads=a.ingest_threads)
+        s = Solver(start, end, pub, dp, grid, seed=a.seed, ingest_threads=a.ingest_threads, save_work=a.save_work,
+                   save_interval=a.save_interval, save_kangaroos=a.save_kangaroos, resume=a.resume or None)
         if s.rank == 0:
             print("Range width: 2^%d  kangaroos/GPU: %d  GPUs: %d  dp: %d  ingest threads: %d" %
-                  (s.range_power, s.eng.nbKangaroo, s.world, a.dp, s.dps.threads), flush=True)
+                  (s.range_power, s.eng.nbKangaroo, s.world, dp, s.dps.threads), flush=True)
         key = s.run(a.max_steps)
         if s.rank == 0:
             print("Solver rate: %.0f MJump/s steady state (after the first 32 steps), %.0f MJump/s over all %d steps (%.2f s); "
                   "rank-0 ingest %.2f ms/step; %d DPs; %d dead kangaroos re-created" %
-                  (s.steady_rate / 1e6, s.jumps / s.elapsed / 1e6, s.steps, s.elapsed, 1e3 * s.t_ingest / max(s.steps, 1), len(s.dps), s.same_herd))
-            if a.save_work:
-                s.dps.save_work(a.save_work, a.dp, start, end, pub, total_count=s.jumps, total_time=s.elapsed)
-                print("work file written: %s" % a.save_work)
+                  (s.steady_rate / 1e6, (s.jumps - s.jumps0) / s.elapsed / 1e6, s.steps, s.elapsed, 1e3 * s.t_ingest / max(s.steps, 1),
+                   len(s.dps), s.same_herd))
+            if a.save_work and s.save_error is None:
+                mb, dt_save = s.saves[-1]
+                print("work file written: %s (%.1f MB in %.2f s, count 2^%.2f)" % (a.save_work, mb, dt_save, np.log2(max(s.jumps, 1))))
+            elif a.save_work:
+                print("work file NOT written: %s: %s" % (a.save_work, s.save_error)); rc = 1
             if key is not None and ec.mul(key) == pub:
                 print("Key#%2d Pub:  0x%064X\n       Priv: 0x%X" % (i, pub[0], key))
             else:
