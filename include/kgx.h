@@ -140,9 +140,41 @@ uint64_t kgx_kernel_launches(kgx_engine* e);
  * out = {serial section, modular inverse alone, parallel phase, tile-steps}; resets them. -1 when disabled. */
 int      kgx_debug_prof(kgx_engine* e, uint64_t out[4]);
 
-/* --- device-side unit-test / microbenchmark hooks (kgx_field.cuh, kgx_modinv.h) --- */
-/* op: 0 = mul, 1 = sqr, 2 = sub, 3 = inv.  a, b, out: n x 4 limbs on the HOST. */
+/* --- device-side unit-test / microbenchmark hooks (kgx_field.cuh, kgx_modinv.h, kgx_herd.cuh, kgx_kernel.cuh) --- */
+/* One device primitive per element.  a, b, out: n x 4 limbs on the HOST; "word k" is 32-bit word k of an element (word 0 =
+ * low half of limb 0).  Results narrower than 256 bits fill the low words of out, the rest is 0.  Unknown op: error.
+ *   MUL, SQR, SUB, INV     out = fe_mul(a,b) / fe_sqr(a) / fe_sub(a,b) / modinv256(a)
+ *   *_INPLACE              the same through the aliased forms fe_mul(a,a,b) / fe_sqr(a,a) / fe_sub(a,a,b); out = a afterwards
+ *   GT_HALF                word 0 = fe_gt_half_mask(a): 0xFFFFFFFF when a > (p-1)/2, else 0
+ *   CNEG                   fe_cneg(a, mask = b word 0); out = a afterwards
+ *   D128_ADD, D128_CNEG    128-bit distance in a words 0..3: d128_add(a, b words 0..3) / d128_cneg(a, mask = b word 0)
+ *   IS_ZERO                word 0 = fe_is_zero_modp(a) (1 / 0)
+ *   NEG, DBL               out = fe_neg(a) / fe_dbl(a)
+ *   JUMP_INDEX             x0 = a word 0, aux = b word 0, rule = b word 1: word 0 = jump_index<symmetric>, word 1 = jump_index<plain>
+ *   SYM_NEXT_AUX           j = a word 0, neg mask = a word 1, aux = b word 0, rule = b word 1: word 0 = sym_next_aux */
+#define KGX_TF_MUL           0
+#define KGX_TF_SQR           1
+#define KGX_TF_SUB           2
+#define KGX_TF_INV           3
+#define KGX_TF_MUL_INPLACE   4
+#define KGX_TF_SQR_INPLACE   5
+#define KGX_TF_SUB_INPLACE   6
+#define KGX_TF_GT_HALF       7
+#define KGX_TF_CNEG          8
+#define KGX_TF_D128_ADD      9
+#define KGX_TF_D128_CNEG     10
+#define KGX_TF_IS_ZERO       11
+#define KGX_TF_NEG           12
+#define KGX_TF_DBL           13
+#define KGX_TF_JUMP_INDEX    14
+#define KGX_TF_SYM_NEXT_AUX  15
 int kgx_test_field(int dev, int op, int n, const uint64_t* a, const uint64_t* b, uint64_t* out);
+/* The device HashTable::Convert (kgx_convert_dps) on crafted input: a DP slab [u32 count][max_found x 56-byte records] is
+ * built from `count` and recs56 (min(count, max_found) records, kgx_item layout), converted with wild_offset (2 limbs) or,
+ * with signed_mode != 0, as signed distances, and the whole [u32 count][max_found x 40-byte records] buffer is copied to
+ * `out` (4 + max_found * 40 bytes; slots past the count keep the device fill 0xFF). */
+int kgx_test_dp_convert(int dev, uint32_t count, uint32_t max_found, const void* recs56, const uint64_t wild_offset[2],
+                        int signed_mode, void* out);
 /* Raw device throughput probes: kind 0 = IMAD.WIDE.U32 issue rate (the multiplier roofline bench.py reports against),
  * 1 = ModMult chains, 2 = ModSqr chains, 3 = modular inverses.  *ms = device time, *ops = operations executed. */
 int kgx_bench_raw(int dev, int kind, int iters, float* ms, double* ops);

@@ -53,6 +53,8 @@ _SIGS = {
     "kgx_kernel_launches": (ctypes.c_uint64, [ctypes.c_void_p]),
     "kgx_debug_prof": (ctypes.c_int, [ctypes.c_void_p, _u64p]),
     "kgx_test_field": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, _u64p, _u64p, _u64p]),
+    "kgx_test_dp_convert": (ctypes.c_int, [ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_void_p, _u64p, ctypes.c_int,
+                                           ctypes.c_void_p]),
     "kgx_bench_raw": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_float),
                                      ctypes.POINTER(ctypes.c_double)]),
 }

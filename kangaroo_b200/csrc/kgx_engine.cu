@@ -14,6 +14,7 @@
 #include "kgx_kernel.cuh"
 #include "kgx_herd.cuh"
 #include "kgx_ckpt.cuh"
+#include "kgx_testhooks.cuh"
 
 using namespace kgx;
 
@@ -631,6 +632,10 @@ void* kgx_dp_slab_device(kgx_engine* e) { return e->done >= 0 ? (void*)e->slab[e
 #define CKH(call) do { cudaError_t _s = (call); if (_s != cudaSuccess) { snprintf(g_create_err, sizeof g_create_err, "%s: %s", #call, cudaGetErrorString(_s)); return -1; } } while (0)
 
 int kgx_test_field(int dev, int op, int n, const uint64_t* a, const uint64_t* b, uint64_t* out) {
+  if (op < KGX_TF_MUL || op > KGX_TF_SYM_NEXT_AUX || n <= 0) {
+    snprintf(g_create_err, sizeof g_create_err, "kgx_test_field: bad op %d or count %d", op, n);
+    return -1;
+  }
   CKH(cudaSetDevice(dev));
   u32 *da, *db, *dout;
   CKH(cudaMalloc(&da, (size_t)n * 32)); CKH(cudaMalloc(&db, (size_t)n * 32)); CKH(cudaMalloc(&dout, (size_t)n * 32));
@@ -641,6 +646,30 @@ int kgx_test_field(int dev, int op, int n, const uint64_t* a, const uint64_t* b,
   CKH(cudaMemcpy(out, dout, (size_t)n * 32, cudaMemcpyDeviceToHost));
   cudaFree(da); cudaFree(db); cudaFree(dout);
   return 0;
+}
+
+int kgx_test_dp_convert(int dev, uint32_t count, uint32_t max_found, const void* recs56, const uint64_t wild_offset[2],
+                        int signed_mode, void* out) {
+  if (max_found == 0) { snprintf(g_create_err, sizeof g_create_err, "kgx_test_dp_convert: max_found must be > 0"); return -1; }
+  CKH(cudaSetDevice(dev));
+  const u32 stored = count < max_found ? count : max_found;
+  const size_t slabBytes = 4 + (size_t)max_found * KGX_ITEM_SIZE, outBytes = 4 + (size_t)max_found * 40;
+  u32 *slab = nullptr, *out40 = nullptr;
+  auto body = [&]() -> int {
+    CKH(cudaMalloc(&slab, slabBytes));
+    CKH(cudaMalloc(&out40, outBytes));
+    CKH(cudaMemset(slab, 0, slabBytes));
+    CKH(cudaMemset(out40, 0xFF, outBytes));
+    CKH(cudaMemcpy(slab, &count, 4, cudaMemcpyHostToDevice));
+    if (stored) CKH(cudaMemcpy(slab + 1, recs56, (size_t)stored * KGX_ITEM_SIZE, cudaMemcpyHostToDevice));
+    dp_convert_kernel<<<64, 256>>>(slab, out40, max_found, wild_offset[0], wild_offset[1], signed_mode ? 1 : 0);   // kgx_convert_dps's launch
+    CKH(cudaGetLastError());
+    CKH(cudaMemcpy(out, out40, outBytes, cudaMemcpyDeviceToHost));
+    return 0;
+  };
+  const int rc = body();
+  cudaFree(slab); cudaFree(out40);
+  return rc;
 }
 
 int kgx_bench_raw(int dev, int kind, int iters, float* ms, double* ops) {

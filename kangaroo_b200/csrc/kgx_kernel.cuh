@@ -744,21 +744,7 @@ __global__ void dp_convert_kernel(const u32* __restrict__ slab, u32* __restrict_
   }
 }
 
-// ---- unit-test / microbench kernels ------------------------------------------------------------------
-__global__ void test_field_kernel(int op, int n, const u32* a, const u32* b, u32* out) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  u32 x[8], y[8], r[8];
-#pragma unroll
-  for (int w = 0; w < 8; w++) { x[w] = a[i * 8 + w]; y[w] = b[i * 8 + w]; }
-  if (op == 0) fe_mul(r, x, y);
-  else if (op == 1) fe_sqr(r, x);
-  else if (op == 2) fe_sub(r, x, y);
-  else fe_inv(r, x);
-#pragma unroll
-  for (int w = 0; w < 8; w++) out[i * 8 + w] = r[w];
-}
-
+// ---- microbench kernel (the unit-test kernel is in kgx_testhooks.cuh) ------------------------------------
 // kind 0: dependent-free IMAD.WIDE.U32 issue-rate probe; kind 1: fe_mul chains; kind 2: fe_sqr chains; kind 3: fe_inv
 __global__ void bench_raw_kernel(int kind, int iters, u32* sink) {
   const u32 seed = blockIdx.x * blockDim.x + threadIdx.x + 1u;

@@ -22,6 +22,53 @@ def test_header_symbols_are_exported():
     assert declared == set(_lib.EXPORTED_SYMBOLS)
 
 
+def compiled_jump_kernels(src):
+    """The jump-kernel instantiations kgx_engine.cu launches in the non-symmetric engine: ("resident", "T,K") per KGX_CFG_ENTRY
+    (the first entry is the default geometry), ("stream", CTAS, inverse) per stream_kernel launch, and the cluster kernel."""
+    geoms = re.findall(r"KGX_CFG_ENTRY(?:_SYM)?\(\s*(\d+)\s*,\s*(\d+)\s*\)", src)
+    kernels = {("resident", "%s,%s" % g) for g in geoms}
+    for ctas, warp in re.findall(r"stream_kernel<\s*128\s*,\s*(\d+)\s*,\s*(true|false)\s*,\s*false\s*>\s*<<<", src):
+        kernels.add(("stream", ctas, "warp" if warp == "true" else "thread"))
+    if re.search(r"jump_kernel_cluster\s*<<<", src):
+        kernels.add(("tmem",))
+    return kernels, "%s,%s" % geoms[0]
+
+
+def variant_kernel(env, default_geometry):
+    """The instantiation a tests/test_gpu_modes.py variant selects, or None where that depends on the herd size."""
+    mode = env["KGX_MODE"]
+    if mode == "resident":
+        return ("resident", env.get("KGX_CFG", default_geometry))
+    if mode == "tmem":
+        return ("tmem",)
+    inv = env.get("KGX_STREAM_INV") or ("warp" if int(env.get("KGX_STREAM_G", "0")) >= 64 else None)
+    return ("stream", env.get("KGX_STREAM_CTAS", "2"), inv) if inv else None
+
+
+def check_variants_cover(src, variants):
+    kernels, default_geometry = compiled_jump_kernels(src)
+    selected = {variant_kernel(v, default_geometry) for v in variants} - {None}
+    assert kernels - selected == set(), "compiled jump kernels that no entry of VARIANTS runs"
+    assert selected - kernels == set(), "VARIANTS entries that select no compiled jump kernel"
+
+
+def test_every_compiled_jump_kernel_has_a_gpu_test():
+    """tests/test_gpu_modes.py runs every entry of VARIANTS; a geometry or stream instantiation added to kgx_engine.cu without
+    an entry there fails here, on a machine without a GPU."""
+    from tests.test_gpu_modes import VARIANTS
+    src = open(os.path.join(ROOT, "kangaroo_b200", "csrc", "kgx_engine.cu")).read()
+    kernels, _ = compiled_jump_kernels(src)
+    assert {("resident", "128,7"), ("resident", "96,6"), ("stream", "3", "thread"), ("tmem",)} <= kernels   # the parser finds them
+    check_variants_cover(src, VARIANTS)
+    # the guard itself: one more geometry, or one variant fewer, must fail it
+    extra = src.replace("KGX_CFG_ENTRY(32, 12),", "KGX_CFG_ENTRY(32, 12), KGX_CFG_ENTRY(160, 3),")
+    assert extra != src
+    with pytest.raises(AssertionError):
+        check_variants_cover(extra, VARIANTS)
+    with pytest.raises(AssertionError):
+        check_variants_cover(src, [v for v in VARIANTS if v.get("KGX_CFG") != "96,6"])
+
+
 def test_no_oracle_in_product():
     # the product package must never import / link the oracle
     for dirpath, _, files in os.walk(os.path.join(ROOT, "kangaroo_b200")):
