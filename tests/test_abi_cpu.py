@@ -23,8 +23,9 @@ def test_header_symbols_are_exported():
 
 
 def compiled_jump_kernels(src):
-    """The jump-kernel instantiations kgx_engine.cu launches in the non-symmetric engine: ("resident", "T,K") per KGX_CFG_ENTRY
-    (the first entry is the default geometry), ("stream", CTAS, inverse) per stream_kernel launch, and the cluster kernel."""
+    """The jump-kernel instantiations kgx_engine.cu launches in the non-symmetric engine: ("resident", "T,K") per KGX_CFG_ENTRY or
+    KGX_CFG_ENTRY_SYM (the first entry is the default geometry), ("stream", CTAS, inverse) per stream_kernel<128, CTAS, WARPINV,
+    false> launch, and the cluster kernel."""
     geoms = re.findall(r"KGX_CFG_ENTRY(?:_SYM)?\(\s*(\d+)\s*,\s*(\d+)\s*\)", src)
     kernels = {("resident", "%s,%s" % g) for g in geoms}
     for ctas, warp in re.findall(r"stream_kernel<\s*128\s*,\s*(\d+)\s*,\s*(true|false)\s*,\s*false\s*>\s*<<<", src):
@@ -45,28 +46,57 @@ def variant_kernel(env, default_geometry):
     return ("stream", env.get("KGX_STREAM_CTAS", "2"), inv) if inv else None
 
 
-def check_variants_cover(src, variants):
+def compiled_symmetric_jump_kernels(src):
+    """The instantiations the symmetric engine (kgx_set_symmetry) launches: ("resident", "T,K") per KGX_CFG_ENTRY_SYM and
+    ("stream", CTAS, inverse) per stream_kernel<128, CTAS, WARPINV, true> launch."""
+    kernels = {("resident", "%s,%s" % g) for g in re.findall(r"KGX_CFG_ENTRY_SYM\(\s*(\d+)\s*,\s*(\d+)\s*\)", src)}
+    for ctas, warp in re.findall(r"stream_kernel<\s*128\s*,\s*(\d+)\s*,\s*(true|false)\s*,\s*true\s*>\s*<<<", src):
+        kernels.add(("stream", ctas, "warp" if warp == "true" else "thread"))
+    return kernels
+
+
+def symmetric_variant_kernel(env, default_geometry):
+    """The instantiation a SYM_VARIANTS entry selects.  The symmetric engine ignores KGX_STREAM_INV: its stream kernel always
+    takes the warp inverse."""
+    mode = env["KGX_MODE"]
+    if mode == "resident":
+        return ("resident", env.get("KGX_CFG", default_geometry))
+    if mode == "tmem":
+        return ("tmem",)
+    return ("stream", env.get("KGX_STREAM_CTAS", "2"), "warp")
+
+
+def check_variants_cover(src, variants, sym_variants):
     kernels, default_geometry = compiled_jump_kernels(src)
     selected = {variant_kernel(v, default_geometry) for v in variants} - {None}
     assert kernels - selected == set(), "compiled jump kernels that no entry of VARIANTS runs"
     assert selected - kernels == set(), "VARIANTS entries that select no compiled jump kernel"
+    kernels = compiled_symmetric_jump_kernels(src)
+    selected = {symmetric_variant_kernel(v, default_geometry) for v in sym_variants}
+    assert kernels - selected == set(), "compiled symmetric jump kernels that no entry of SYM_VARIANTS runs"
+    assert selected - kernels == set(), "SYM_VARIANTS entries that select no compiled symmetric jump kernel"
 
 
 def test_every_compiled_jump_kernel_has_a_gpu_test():
-    """tests/test_gpu_modes.py runs every entry of VARIANTS; a geometry or stream instantiation added to kgx_engine.cu without
-    an entry there fails here, on a machine without a GPU."""
-    from tests.test_gpu_modes import VARIANTS
+    """tests/test_gpu_modes.py runs every entry of VARIANTS and SYM_VARIANTS; a geometry or stream instantiation added to
+    kgx_engine.cu without an entry there fails here, on a machine without a GPU."""
+    from tests.test_gpu_modes import SYM_VARIANTS, VARIANTS
     src = open(os.path.join(ROOT, "kangaroo_b200", "csrc", "kgx_engine.cu")).read()
     kernels, _ = compiled_jump_kernels(src)
     assert {("resident", "128,7"), ("resident", "96,6"), ("stream", "3", "thread"), ("tmem",)} <= kernels   # the parser finds them
-    check_variants_cover(src, VARIANTS)
-    # the guard itself: one more geometry, or one variant fewer, must fail it
+    assert compiled_symmetric_jump_kernels(src) == {("resident", "128,7"), ("stream", "2", "warp")}
+    check_variants_cover(src, VARIANTS, SYM_VARIANTS)
+    # the guard itself: one more geometry, one more symmetric geometry, or one variant fewer, must fail it
     extra = src.replace("KGX_CFG_ENTRY(32, 12),", "KGX_CFG_ENTRY(32, 12), KGX_CFG_ENTRY(160, 3),")
-    assert extra != src
+    extra_sym = src.replace("KGX_CFG_ENTRY(64, 7),", "KGX_CFG_ENTRY_SYM(64, 7),")
+    assert extra != src and extra_sym != src
+    for bad_src in (extra, extra_sym):
+        with pytest.raises(AssertionError):
+            check_variants_cover(bad_src, VARIANTS, SYM_VARIANTS)
     with pytest.raises(AssertionError):
-        check_variants_cover(extra, VARIANTS)
+        check_variants_cover(src, [v for v in VARIANTS if v.get("KGX_CFG") != "96,6"], SYM_VARIANTS)
     with pytest.raises(AssertionError):
-        check_variants_cover(src, [v for v in VARIANTS if v.get("KGX_CFG") != "96,6"])
+        check_variants_cover(src, VARIANTS, [v for v in SYM_VARIANTS if v["KGX_MODE"] != "resident"])
 
 
 def test_no_oracle_in_product():
