@@ -112,6 +112,24 @@ int kgx_import(kgx_engine* e, const uint64_t wild_offset[2], const void* recs, u
  *     group order), d128: n x 2 limbs stored as the (biased) distances. --- */
 int kgx_create_herd(kgx_engine* e, const uint64_t* scalars, const uint64_t* d128, const uint64_t keyx[4], const uint64_t keyy[4], int first_type);
 
+/* --- multi-key herd: one tame herd shared by several keys (the solver's --batch-keys).  Not in the reference, which solves
+ *     the keys of an input file one after another with a new herd each (Kangaroo::Run, Kangaroo.cpp:1021-1066).
+ * _create_herd_multi: kgx_create_herd with a key table of n_keys (1..KGX_MAX_KEYS) keys, keys: n_keys x 8 limbs (x[4], y[4]),
+ *     and a target per kangaroo, targets: n entries in kIdx order, each below n_keys: wild kangaroo i starts at
+ *     keys[targets[i]] + scalars[i]*G (the entries of tame kangaroos are not used).  The engine keeps the table and the
+ *     targets (kgx_create_herd drops them).  Fails in symmetric mode.
+ * _retarget: every wild kangaroo whose target is `from` moves to key b = to[(kIdx >> 1) % n_to] (1 <= n_to <= n_keys): its
+ *     point gets keys[b] - keys[from] added, its distance stays, so it is at keys[b] + d*G again, and its target becomes b.
+ *     Stream-ordered after the launch in flight, like kgx_patch, and the call does not wait for that launch.  Padding
+ *     slots keep walking their old copy (their DPs are dropped).  kgx_upload / kgx_patch / kgx_import change no target.
+ *     kgx_set_symmetry(on) drops the key table; _retarget and _targets fail in symmetric mode.
+ * _targets: the n targets (kIdx order) after every retarget queued so far. --- */
+#define KGX_MAX_KEYS 65535
+int kgx_create_herd_multi(kgx_engine* e, const uint64_t* scalars, const uint64_t* d128, const uint64_t* keys, uint32_t n_keys,
+                          const uint16_t* targets, int first_type);
+int kgx_retarget(kgx_engine* e, uint32_t from, const uint16_t* to, uint32_t n_to);
+int kgx_targets(kgx_engine* e, uint16_t* out);
+
 /* --- GPUEngine::callKernel (GPUEngine.cu:540-557): zero the DP count, start NB_RUN jumps, asynchronous --- */
 int kgx_launch_async(kgx_engine* e);
 /* First half of GPUEngine::Launch (GPUEngine.cu:607-675): wait for the in-flight launch (sleeping unless

@@ -58,6 +58,14 @@ int kgi_add_items(kgi_table* t, const void* items56, uint32_t n, uint32_t rank, 
 int kgi_resolve(kgi_table* t, const uint64_t d_old[2], const uint64_t d_new[2], const uint64_t keyx[4], const uint64_t keyy[4],
                 const uint64_t range_start[4], uint64_t priv_out[4]);
 
+/* The same against a list of keys (the solver's --batch-keys: the stored entry carries no kIdx, so which key the wild side
+ * belongs to is found here).  keys: n_keys x 8 limbs (x[4], y[4]) of keyToSearch = P - start*G each.  The four candidates are
+ * formed once (four scalar multiplications), then compared with every key and its negative: returns 1 with the index of
+ * the first matching key in *key_index_out and its private key, which equals kgi_resolve's on that key, or 0 when no key
+ * matches. */
+int kgi_resolve_multi(kgi_table* t, const uint64_t d_old[2], const uint64_t d_new[2], const uint64_t* keys, uint32_t n_keys,
+                      const uint64_t range_start[4], uint32_t* key_index_out, uint64_t priv_out[4]);
+
 /* Work-file compatibility (SURVEY 8f/f3): write the table as a reference work file (Backup.cpp:368-394 header HEADW +
  * HashTable::SaveTable) that the reference's -winfo / -wcheck / -i / -wm read.  range_start/range_end/key: 4 limbs each.
  * No kangaroos (totalWalk = 0).  0 on success, -errno when a write fails (full disk, bad path). */

@@ -19,6 +19,7 @@ class Item(ctypes.Structure):
 
 
 _u64p = ctypes.POINTER(ctypes.c_uint64)
+_u16p = ctypes.POINTER(ctypes.c_uint16)
 _SIGS = {
     "kgx_device_count": (ctypes.c_int, []),
     "kgx_grid_default": (ctypes.c_int, [ctypes.c_int, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]),
@@ -37,6 +38,9 @@ _SIGS = {
     "kgx_download": (ctypes.c_int, [ctypes.c_void_p, _u64p, _u64p, _u64p]),
     "kgx_patch": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_uint64, _u64p, _u64p, _u64p]),
     "kgx_create_herd": (ctypes.c_int, [ctypes.c_void_p, _u64p, _u64p, _u64p, _u64p, ctypes.c_int]),
+    "kgx_create_herd_multi": (ctypes.c_int, [ctypes.c_void_p, _u64p, _u64p, _u64p, ctypes.c_uint32, _u16p, ctypes.c_int]),
+    "kgx_retarget": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_uint32, _u16p, ctypes.c_uint32]),
+    "kgx_targets": (ctypes.c_int, [ctypes.c_void_p, _u16p]),
     "kgx_snapshot_begin": (ctypes.c_int, [ctypes.c_void_p]),
     "kgx_snapshot_read": (ctypes.c_int, [ctypes.c_void_p, _u64p, _u64p, _u64p]),
     "kgx_snapshot_export": (ctypes.c_int, [ctypes.c_void_p, _u64p, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_void_p]),

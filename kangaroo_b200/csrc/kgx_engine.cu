@@ -53,6 +53,13 @@ struct kgx_engine {
   bool snapPending = false;
   u64* herdRecs = nullptr;        // n x 96-byte work-file records (kgx_snapshot_export / kgx_import); kept, like the staging, for the next save
   bool snapConverted = false;     // herdRecs holds the pending snapshot
+  // multi-key herd (kgx_create_herd_multi / kgx_retarget): none of it is jump-kernel state
+  u32* keys = nullptr;            // key table: keyCap x 16 words (x, y); the first nKeys hold the herd's keys
+  uint16_t* targets = nullptr;    // n: key of every wild kangaroo, kIdx order
+  u32* rtDelta = nullptr;         // keyCap x 16 words: keys[to[j]] - keys[from] of the retarget in stream order
+  u32* rtTo = nullptr;            // keyCap: to[j] | infinity flag
+  u32 nKeys = 0, keyCap = 0;      // nKeys == 0: no key table (a herd of kgx_create_herd or kgx_upload)
+  int firstType = 0;
   float lastMs = 0.f;
   unsigned long long* prof = nullptr;   // KGX_PROF=1: phase cycle counters
   u64 launches = 0;
@@ -121,6 +128,7 @@ void kgx_destroy(kgx_engine* e) {
   if (e->stream) cudaStreamSynchronize(e->stream);
   cudaFree(e->dp40); cudaFree(e->herdTab); cudaFree(e->state); cudaFree(e->pre); cudaFree(e->slab[0]); cudaFree(e->slab[1]); cudaFree(e->jtab);
   cudaFree(e->stgX); cudaFree(e->stgY); cudaFree(e->stgD); cudaFree(e->aux); cudaFree(e->herdRecs);
+  cudaFree(e->keys); cudaFree(e->targets); cudaFree(e->rtDelta); cudaFree(e->rtTo);
   if (e->slabPinned) cudaFreeHost(e->slabPinned);
   for (int i = 0; i < 2; i++) { if (e->evStart[i]) cudaEventDestroy(e->evStart[i]); if (e->evStop[i]) cudaEventDestroy(e->evStop[i]); }
   if (e->evSnap) cudaEventDestroy(e->evSnap);
@@ -250,7 +258,10 @@ kgx_engine* kgx_create_ex(int dev, int groups, int threads_per_group, uint32_t m
 
 uint64_t kgx_num_kangaroos(kgx_engine* e) { return e->n; }
 int kgx_kernel_kind(kgx_engine* e) { return e->streamMode ? KGX_KERNEL_STREAM : (e->tmemMode ? KGX_KERNEL_TMEM : KGX_KERNEL_RESIDENT); }
-uint64_t kgx_memory_bytes(kgx_engine* e) { return e->stateBytes + (e->pre ? e->nPadded * 32 : 0) + 2 * e->slabBytes + JT_WORDS * 4; }
+uint64_t kgx_memory_bytes(kgx_engine* e) {
+  return e->stateBytes + (e->pre ? e->nPadded * 32 : 0) + 2 * e->slabBytes + JT_WORDS * 4 +
+         (e->targets ? e->n * 2 : 0) + (u64)e->keyCap * (64 + 64 + 4);
+}
 uint32_t kgx_max_found(kgx_engine* e) { return e->maxFound; }
 float kgx_last_launch_ms(kgx_engine* e) { return e->lastMs; }
 uint64_t kgx_kernel_launches(kgx_engine* e) { return e->launches; }
@@ -284,6 +295,7 @@ int kgx_set_symmetry(kgx_engine* e, int on) {
   if (on && !e->aux) CK(e, cudaMalloc(&e->aux, e->nPadded));
   if (on) CK(e, cudaMemsetAsync(e->aux, on == KGX_SYM_CLASS ? 0 : 32, e->nPadded, e->stream));
   e->symRule = on;
+  if (on) e->nKeys = 0;        // a multi-key herd is not available in symmetric mode (kgx_create_herd_multi): drop its table
   if (on && !e->streamMode)
     CK(e, cudaFuncSetAttribute(g_cfgs[e->cfg].kernSym, cudaFuncAttributeMaxDynamicSharedMemorySize, e->smemBytes));
   e->symmetry = on != 0;
@@ -453,7 +465,7 @@ int kgx_import(kgx_engine* e, const uint64_t wild_offset[2], const void* recs, u
       uint64_t key[8];
       memcpy(key, keyx, 32); memcpy(key + 4, keyy, 32);
       CK(e, cudaMemcpyAsync(dKey, key, 64, cudaMemcpyHostToDevice, e->stream));
-      herd_kernel<<<(u32)((count + 127) / 128), 128, 0, e->stream>>>(e->herdTab, scal, dKey, 0, count, vx, vy, 0, nullptr);
+      herd_kernel<<<(u32)((count + 127) / 128), 128, 0, e->stream>>>(e->herdTab, scal, dKey, nullptr, 0, count, vx, vy, 0, nullptr);
       e->launches++;
       CK(e, cudaGetLastError());
       herd_compare_kernel<<<4 * e->sms, 256, 0, e->stream>>>(reinterpret_cast<u32*>(e->stgX), reinterpret_cast<u32*>(e->stgY), vx, vy, count, flags + 1);
@@ -495,10 +507,14 @@ int kgx_patch(kgx_engine* e, uint64_t kidx, const uint64_t px[4], const uint64_t
 
 // Kangaroo::CreateHerd on the device (Kangaroo.cpp:670-738): positions d*G (tame) / key + d*G (wild) for all n
 // kangaroos straight into the engine state.  scalars: n x 4 limbs (d mod group order, exactly what the reference
-// feeds ComputePublicKeys); d128: n x 2 limbs (the biased distances to store); key: x[4], y[4].
-int kgx_create_herd(kgx_engine* e, const uint64_t* scalars, const uint64_t* d128, const uint64_t keyx[4], const uint64_t keyy[4], int first_type) {
+// feeds ComputePublicKeys); d128: n x 2 limbs (the biased distances to store).  keys: n_keys x 8 limbs (x, y); targets
+// NULL: one key, no key table kept; else the wild term of kangaroo i is keys[targets[i]] and the table and the targets stay
+// in the engine for kgx_retarget.
+static int create_herd(kgx_engine* e, const char* what, const uint64_t* scalars, const uint64_t* d128, const uint64_t* keys,
+                       uint32_t n_keys, const uint16_t* targets, int first_type) {
   CK(e, cudaSetDevice(e->dev));
-  if (e->snapPending) { snprintf(e->err, sizeof e->err, "kgx_create_herd: snapshot pending (read it first)"); return -1; }
+  if (e->snapPending) { snprintf(e->err, sizeof e->err, "%s: snapshot pending (read it first)", what); return -1; }
+  e->nKeys = 0;
   if (!e->herdTab) {
     CK(e, cudaMalloc(&e->herdTab, 256 * 16 * 4));
     herd_table_kernel<<<1, 32, 0, e->stream>>>(e->herdTab);
@@ -507,16 +523,33 @@ int kgx_create_herd(kgx_engine* e, const uint64_t* scalars, const uint64_t* d128
   }
   if (ensure_staging(e)) return -1;
   u32 *dScal = nullptr, *dKey = nullptr;
-  uint64_t key[8];
-  memcpy(key, keyx, 32); memcpy(key + 4, keyy, 32);
   auto body = [&]() -> int {      // CK returns from the lambda, so the scratch buffers are always released below
     CK(e, cudaMalloc(&dScal, e->n * 32));
-    CK(e, cudaMalloc(&dKey, 64));
+    if (targets) {
+      if (n_keys > e->keyCap) {
+        cudaFree(e->keys); cudaFree(e->rtDelta); cudaFree(e->rtTo);
+        e->keys = e->rtDelta = e->rtTo = nullptr;
+        e->keyCap = 0;
+        CK(e, cudaMalloc(&e->keys, (size_t)n_keys * 64));
+        CK(e, cudaMalloc(&e->rtDelta, (size_t)n_keys * 64));
+        CK(e, cudaMalloc(&e->rtTo, (size_t)n_keys * 4));
+        e->keyCap = n_keys;
+      }
+      if (!e->targets) CK(e, cudaMalloc(&e->targets, e->n * 2));
+      // load the retarget kernels now: kgx_retarget must not be the first launch of a kernel, which can wait for the device
+      cudaFuncAttributes fa;
+      CK(e, cudaFuncGetAttributes(&fa, retarget_delta_kernel));
+      CK(e, cudaFuncGetAttributes(&fa, retarget_kernel));
+      CK(e, cudaMemcpyAsync(e->keys, keys, (size_t)n_keys * 64, cudaMemcpyHostToDevice, e->stream));
+      CK(e, cudaMemcpyAsync(e->targets, targets, e->n * 2, cudaMemcpyHostToDevice, e->stream));
+    } else {
+      CK(e, cudaMalloc(&dKey, 64));
+      CK(e, cudaMemcpyAsync(dKey, keys, 64, cudaMemcpyHostToDevice, e->stream));
+    }
     CK(e, cudaMemcpyAsync(dScal, scalars, e->n * 32, cudaMemcpyHostToDevice, e->stream));
-    CK(e, cudaMemcpyAsync(dKey, key, 64, cudaMemcpyHostToDevice, e->stream));
     CK(e, cudaMemcpyAsync(e->stgD, d128, e->n * 16, cudaMemcpyHostToDevice, e->stream));
-    herd_kernel<<<(u32)((e->n + 127) / 128), 128, 0, e->stream>>>(e->herdTab, dScal, dKey, first_type, e->n,
-                                                                 reinterpret_cast<u32*>(e->stgX), reinterpret_cast<u32*>(e->stgY),
+    herd_kernel<<<(u32)((e->n + 127) / 128), 128, 0, e->stream>>>(e->herdTab, dScal, targets ? e->keys : dKey, targets ? e->targets : nullptr,
+                                                                 first_type, e->n, reinterpret_cast<u32*>(e->stgX), reinterpret_cast<u32*>(e->stgY),
                                                                  e->symmetry ? 1 : 0, reinterpret_cast<u32*>(e->stgD));
     e->launches++;
     CK(e, cudaGetLastError());
@@ -530,7 +563,62 @@ int kgx_create_herd(kgx_engine* e, const uint64_t* scalars, const uint64_t* d128
   const int rc = body();
   cudaFree(dScal); cudaFree(dKey);
   free_staging(e);
+  if (rc == 0 && targets) { e->nKeys = n_keys; e->firstType = first_type; }
   return rc;
+}
+
+int kgx_create_herd(kgx_engine* e, const uint64_t* scalars, const uint64_t* d128, const uint64_t keyx[4], const uint64_t keyy[4], int first_type) {
+  uint64_t key[8];
+  memcpy(key, keyx, 32); memcpy(key + 4, keyy, 32);
+  return create_herd(e, "kgx_create_herd", scalars, d128, key, 1, nullptr, first_type);
+}
+
+int kgx_create_herd_multi(kgx_engine* e, const uint64_t* scalars, const uint64_t* d128, const uint64_t* keys, uint32_t n_keys,
+                          const uint16_t* targets, int first_type) {
+  if (e->symmetry) { snprintf(e->err, sizeof e->err, "kgx_create_herd_multi: not available in symmetric mode"); return -1; }
+  if (n_keys == 0 || n_keys > KGX_MAX_KEYS) { snprintf(e->err, sizeof e->err, "kgx_create_herd_multi: n_keys must be in [1, %d]", KGX_MAX_KEYS); return -1; }
+  for (u64 i = 0; i < e->n; i++)
+    if (targets[i] >= n_keys) {
+      snprintf(e->err, sizeof e->err, "kgx_create_herd_multi: target %u of kangaroo %llu is not below n_keys = %u", targets[i], (unsigned long long)i, n_keys);
+      return -1;
+    }
+  return create_herd(e, "kgx_create_herd_multi", scalars, d128, keys, n_keys, targets, first_type);
+}
+
+// Moves the wild kangaroos of key `from` to the keys in `to`, in stream order after the launch in flight (like kgx_patch),
+// without waiting for it: the destination list reaches the device as kernel parameters (retarget_delta_kernel), one
+// affine addition per moved kangaroo follows (retarget_kernel).
+int kgx_retarget(kgx_engine* e, uint32_t from, const uint16_t* to, uint32_t n_to) {
+  CK(e, cudaSetDevice(e->dev));
+  if (e->symmetry) { snprintf(e->err, sizeof e->err, "kgx_retarget: not available in symmetric mode"); return -1; }
+  if (!e->nKeys) { snprintf(e->err, sizeof e->err, "kgx_retarget: the herd has no key table (kgx_create_herd_multi)"); return -1; }
+  if (from >= e->nKeys) { snprintf(e->err, sizeof e->err, "kgx_retarget: key %u is not below n_keys = %u", from, e->nKeys); return -1; }
+  if (n_to == 0 || n_to > e->nKeys) { snprintf(e->err, sizeof e->err, "kgx_retarget: n_to must be in [1, n_keys = %u]", e->nKeys); return -1; }
+  for (u32 j = 0; j < n_to; j++)
+    if (to[j] >= e->nKeys) { snprintf(e->err, sizeof e->err, "kgx_retarget: to[%u] = %u is not below n_keys = %u", j, to[j], e->nKeys); return -1; }
+  for (u32 j0 = 0; j0 < n_to; j0 += RETARGET_CHUNK) {
+    const u32 cnt = n_to - j0 < (u32)RETARGET_CHUNK ? n_to - j0 : (u32)RETARGET_CHUNK;
+    RetargetChunk c;
+    memset(&c, 0, sizeof c);
+    memcpy(c.to, to + j0, (size_t)cnt * 2);
+    retarget_delta_kernel<<<(cnt + 127) / 128, 128, 0, e->stream>>>(e->keys, from, c, j0, cnt, e->rtDelta, e->rtTo);
+    e->launches++;
+    CK(e, cudaGetLastError());
+  }
+  retarget_kernel<<<(u32)((e->n + 255) / 256), 256, 0, e->stream>>>(e->state, e->T, e->K, e->n, e->firstType, e->targets, from,
+                                                                   e->rtDelta, e->rtTo, n_to);
+  e->launches++;
+  CK(e, cudaGetLastError());
+  return 0;
+}
+
+int kgx_targets(kgx_engine* e, uint16_t* out) {
+  CK(e, cudaSetDevice(e->dev));
+  if (e->symmetry) { snprintf(e->err, sizeof e->err, "kgx_targets: not available in symmetric mode"); return -1; }
+  if (!e->nKeys) { snprintf(e->err, sizeof e->err, "kgx_targets: the herd has no key table (kgx_create_herd_multi)"); return -1; }
+  CK(e, cudaMemcpyAsync(out, e->targets, e->n * 2, cudaMemcpyDeviceToHost, e->stream));   // stream order: after the retargets
+  CK(e, cudaStreamSynchronize(e->stream));
+  return 0;
 }
 
 int kgx_launch_async(kgx_engine* e) {

@@ -5,6 +5,7 @@
 // mixed additions over the set bits of d, and ONE inversion per kangaroo.
 #pragma once
 #include "kgx_field.cuh"
+#include "kgx_kernel.cuh"
 #include "kgx_modinv.h"
 
 namespace kgx {
@@ -48,12 +49,26 @@ __global__ void herd_table_kernel(u32* tab) {
   }
 }
 
-// One thread per kangaroo: (x,y) = d*G [+ key].  scal: n x 8 words (d mod group order), key: 16 words or NULL rows
-// where isWild[i]==0.  Writes AoS px,py (n x 8 words each) in kIdx order.
+// canonical residue: fe_mul / fe_sub leave values < 2^256 congruent mod p; subtract p once if needed
+// (subtracting p mod 2^256 == adding 0x1000003D1)
+__device__ __forceinline__ void fe_canon(u32* V) {
+  const u32 pm[8] = {0xFFFFFC2Fu, 0xFFFFFFFEu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
+  bool ge = true;
+  for (int w = 7; w >= 0; w--) { if (V[w] != pm[w]) { ge = V[w] > pm[w]; break; } }
+  if (ge) {
+    u64 acc = (u64)V[0] + 0x3D1u; V[0] = (u32)acc;
+    acc = (u64)V[1] + 1u + (acc >> 32); V[1] = (u32)acc;
+    for (int w = 2; w < 8; w++) { acc = (u64)V[w] + (acc >> 32); V[w] = (u32)acc; }
+  }
+}
+
+// One thread per kangaroo: (x,y) = d*G [+ key].  scal: n x 8 words (d mod group order).  keys: the key table, 16 words
+// (x then y) per key; the wild term of kangaroo i is key targets[i], or key 0 when targets is NULL (a single-key herd).
+// Kangaroo i is wild when (i + firstType) is odd.  Writes AoS px,py (n x 8 words each) in kIdx order.
 // sym != 0 (USE_SYMMETRY herd, Kangaroo.cpp:730-734): a point whose y is in the upper half is replaced by its negative and
 // the stored (signed 128-bit) distance dist[i] is negated with it.
-__global__ void herd_kernel(const u32* __restrict__ tab, const u32* __restrict__ scal, const u32* __restrict__ key,
-                            int firstType, u64 n, u32* px, u32* py, int sym, u32* dist) {
+__global__ void herd_kernel(const u32* __restrict__ tab, const u32* __restrict__ scal, const u32* __restrict__ keys,
+                            const uint16_t* __restrict__ targets, int firstType, u64 n, u32* px, u32* py, int sym, u32* dist) {
   u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   u32 k[8];
@@ -69,7 +84,7 @@ __global__ void herd_kernel(const u32* __restrict__ tab, const u32* __restrict__
       if (!((k[b >> 5] >> (b & 31)) & 1u)) continue;
       q = tab + b * 16;
     } else {
-      q = key;
+      q = keys + (targets ? 16u * targets[i] : 0u);
     }
     u32 qx[8], qy[8];
 #pragma unroll
@@ -130,19 +145,8 @@ __global__ void herd_kernel(const u32* __restrict__ tab, const u32* __restrict__
   fe_mul(X, X, zi2);
   fe_mul(zi2, zi2, zi);
   fe_mul(Y, Y, zi2);
-  // canonical residues: fe_mul leaves values < 2^256 congruent mod p; subtract p once if needed
-  // (subtracting p mod 2^256 == adding 0x1000003D1)
-  const u32 pm[8] = {0xFFFFFC2Fu, 0xFFFFFFFEu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
-  for (int c = 0; c < 2; c++) {
-    u32* V = c ? Y : X;
-    bool ge = true;
-    for (int w = 7; w >= 0; w--) { if (V[w] != pm[w]) { ge = V[w] > pm[w]; break; } }
-    if (ge) {
-      u64 acc = (u64)V[0] + 0x3D1u; V[0] = (u32)acc;
-      acc = (u64)V[1] + 1u + (acc >> 32); V[1] = (u32)acc;
-      for (int w = 2; w < 8; w++) { acc = (u64)V[w] + (acc >> 32); V[w] = (u32)acc; }
-    }
-  }
+  fe_canon(X);
+  fe_canon(Y);
   if (sym) {
     const u32 neg = fe_gt_half_mask(Y);
     fe_cneg(Y, neg);
@@ -152,6 +156,84 @@ __global__ void herd_kernel(const u32* __restrict__ tab, const u32* __restrict__
   }
 #pragma unroll
   for (int w = 0; w < 8; w++) { px[i * 8 + w] = X[w]; py[i * 8 + w] = Y[w]; }
+}
+
+// ---- multi-key herd: moving the wild kangaroos of a solved key to other keys (kgx_retarget) ----------------------------
+// (x1, y1) += (x2, y2) in affine coordinates with one inverse; canonical result.  Same x: doubling when the points are
+// equal, the point at infinity (returns false, x1 / y1 then meaningless) when they are opposite -- the group law, as in
+// herd_kernel.
+__device__ bool affine_add(u32* x1, u32* y1, const u32* x2, const u32* y2) {
+  u32 num[8], den[8], s[8], t[8];
+  fe_sub(den, x2, x1);
+  fe_sub(num, y2, y1);
+  if (fe_is_zero_modp(den)) {
+    if (!fe_is_zero_modp(num)) return false;
+    // s = 3 x^2 / 2 y
+    fe_sqr(t, x1);
+    fe_dbl(num, t); fe_neg(s, t); fe_sub(num, num, s);
+    fe_dbl(den, y1);
+  }
+  modinv256(t, den);
+  fe_mul(s, num, t);
+  fe_sqr(t, s); fe_sub(t, t, x1); fe_sub(t, t, x2);     // x3 = s^2 - x1 - x2
+  fe_sub(num, x1, t); fe_mul(num, num, s); fe_sub(y1, num, y1);   // y3 = s (x1 - x3) - y1
+  fe_copy(x1, t);
+  fe_canon(x1);
+  fe_canon(y1);
+  return true;
+}
+
+// The destination list of one kgx_retarget travels as kernel parameters, copied at launch: the call returns without
+// waiting for the launch in flight and leaves no host buffer behind that the device still has to read.
+constexpr int RETARGET_CHUNK = 1024;
+struct RetargetChunk { uint16_t to[RETARGET_CHUNK]; };
+
+// delta[j0 + j] = keys[to[j]] - keys[from] (16 words), rtTo[j0 + j] = to[j], bit 31 set when the difference is the point
+// at infinity (the same key listed twice: the moved kangaroo keeps its point).
+__global__ void retarget_delta_kernel(const u32* __restrict__ keys, u32 from, RetargetChunk c, u32 j0, u32 cnt, u32* delta,
+                                      u32* rtTo) {
+  const u32 j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= cnt) return;
+  const u32 b = c.to[j];
+  u32 x[8], y[8], fx[8], fy[8];
+#pragma unroll
+  for (int w = 0; w < 8; w++) { x[w] = keys[16 * b + w]; y[w] = keys[16 * b + 8 + w]; fx[w] = keys[16 * from + w]; fy[w] = keys[16 * from + 8 + w]; }
+  fe_neg(fy, fy);
+  const bool inf = !affine_add(x, y, fx, fy);
+#pragma unroll
+  for (int w = 0; w < 8; w++) { delta[16 * (j0 + j) + w] = x[w]; delta[16 * (j0 + j) + 8 + w] = y[w]; }
+  rtTo[j0 + j] = b | (inf ? 0x80000000u : 0u);
+}
+
+// Every wild kangaroo s < n (kIdx order; wild when s + firstType is odd) whose target is `from` moves to key
+// b = rtTo[(s >> 1) % nTo]: its point gets keys[b] - keys[from] added in place in the tile layout (slot s -> tile s / TILE,
+// row (s % TILE) / T, column s % T, as pack_kernel), its distance stays, its target becomes b.  Padding slots are left
+// stale, like patch_kernel leaves them.
+__global__ void retarget_kernel(uint4* state, int T, int K, u64 n, int firstType, uint16_t* targets, u32 from,
+                                const u32* __restrict__ delta, const u32* __restrict__ rtTo, u32 nTo) {
+  const u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n || !((s + (u64)firstType) & 1ull) || targets[s] != from) return;
+  const u32 j = (u32)((s >> 1) % nTo);
+  const u32 tj = rtTo[j];
+  targets[s] = (uint16_t)(tj & 0xFFFFu);
+  if (tj >> 31) return;
+  const int TILE = T * K;
+  const u64 tile = s / TILE; const int r = (int)(s % TILE); const int g = r / T, t = r % T;
+  uint4* st = state + tile * (K * CHUNKS * T);
+  uint4 c[4];
+#pragma unroll
+  for (int k = 0; k < 4; k++) c[k] = st[(g * CHUNKS + k) * T + t];
+  u32 x[8] = {c[0].x, c[0].y, c[0].z, c[0].w, c[1].x, c[1].y, c[1].z, c[1].w};
+  u32 y[8] = {c[2].x, c[2].y, c[2].z, c[2].w, c[3].x, c[3].y, c[3].z, c[3].w};
+  if (!affine_add(x, y, delta + 16 * j, delta + 16 * j + 8)) {
+    // keys[b] + d*G is the point at infinity: stored as (0, 0), as herd_kernel does
+#pragma unroll
+    for (int w = 0; w < 8; w++) { x[w] = 0; y[w] = 0; }
+  }
+  st[(g * CHUNKS + 0) * T + t] = make_uint4(x[0], x[1], x[2], x[3]);
+  st[(g * CHUNKS + 1) * T + t] = make_uint4(x[4], x[5], x[6], x[7]);
+  st[(g * CHUNKS + 2) * T + t] = make_uint4(y[0], y[1], y[2], y[3]);
+  st[(g * CHUNKS + 3) * T + t] = make_uint4(y[4], y[5], y[6], y[7]);
 }
 
 }  // namespace kgx

@@ -227,6 +227,53 @@ int kgi_resolve(kgi_table* t, const uint64_t d_old[2], const uint64_t d_new[2], 
   return 0;
 }
 
+int kgi_resolve_multi(kgi_table* t, const uint64_t d_old[2], const uint64_t d_new[2], const uint64_t* keys, uint32_t n_keys,
+                      const uint64_t range_start[4], uint32_t* key_index_out, uint64_t priv_out[4]) {
+  int128_t a, b;
+  a.i64[0] = d_old[0]; a.i64[1] = d_old[1]; b.i64[0] = d_new[0]; b.i64[1] = d_new[1];
+  Int da, db; uint32_t ta, tb;
+  HashTable::CalcDistAndType(a, &da, &ta);
+  HashTable::CalcDistAndType(b, &db, &tb);
+  if (ta == tb) return 0;
+  Int Td, Wd;
+  if (ta == 0) { Td.Set(&da); Wd.Set(&db); } else { Td.Set(&db); Wd.Set(&da); }
+  // the four candidates of Kangaroo::CheckKey (Kangaroo.cpp:218-253), each one scalar multiplication, whatever n_keys is
+  Int pk[4];
+  Point P[4];
+  Int negY[4];
+  for (int type = 0; type < 4; type++) {
+    Int d1(&Td), d2(&Wd);
+    if (type & 1) d1.ModNegK1order();
+    if (type & 2) d2.ModNegK1order();
+    pk[type].Set(&d1);
+    pk[type].ModAddK1order(&d2);
+    P[type] = t->secp->ComputePublicKey(&pk[type]);
+    negY[type].Set(&P[type].y);
+    negY[type].ModNeg();
+  }
+  // then only comparisons per key: key k matches when a candidate is +-keys[k]; for that key the candidates are tried in
+  // kgi_resolve's order, so both calls give the same private key
+  for (uint32_t k = 0; k < n_keys; k++) {
+    Int kx, ky;
+    kx.SetInt32(0); ky.SetInt32(0);
+    for (int w = 0; w < 4; w++) { kx.bits64[w] = keys[8 * k + w]; ky.bits64[w] = keys[8 * k + 4 + w]; }
+    for (int type = 0; type < 4; type++) {
+      if (!P[type].x.IsEqual(&kx)) continue;
+      Int priv(&pk[type]);
+      if (P[type].y.IsEqual(&ky)) { }
+      else if (negY[type].IsEqual(&ky)) priv.ModNegK1order();
+      else continue;
+      Int start; start.SetInt32(0);
+      for (int w = 0; w < 4; w++) start.bits64[w] = range_start[w];
+      priv.ModAddK1order(&start);
+      for (int w = 0; w < 4; w++) priv_out[w] = priv.bits64[w];
+      *key_index_out = k;
+      return 1;
+    }
+  }
+  return 0;
+}
+
 // a failed stdio call: -errno (EIO when the C library left errno at 0)
 static int io_error() { return errno ? -errno : -EIO; }
 

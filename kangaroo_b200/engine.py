@@ -18,6 +18,7 @@ TAME, WILD = 0, 1   # Constants.h:38-39
 ORDER = 0xFFFFFFFFFFFFFFFFFFFFFFFFFFFFFFFEBAAEDCE6AF48A03BBFD25E8CD0364141
 _M64 = 0xFFFFFFFFFFFFFFFF
 _u64p = ctypes.POINTER(ctypes.c_uint64)
+_u16p = ctypes.POINTER(ctypes.c_uint16)
 
 
 class ITEM:
@@ -260,6 +261,30 @@ class GPUEngine:
         assert sc.shape[0] == n and ad.shape[0] == n
         kx, ky = _limbs([key[0]], 4), _limbs([key[1]], 4)
         self._ck(self._lib.kgx_create_herd(self._h, _p(sc), _p(ad), _p(kx), _p(ky), TAME), "CreateHerd")
+
+    def CreateHerdMulti(self, scalars, d128, keys, targets):
+        """CreateHerdRaw with a key table (not in the reference): keys = list of (x, y) points, targets = n key indices in
+        kIdx order; wild kangaroo i (odd kIdx) starts at keys[targets[i]] + scalars[i]*G.  The engine keeps the table and
+        the targets for Retarget."""
+        n = self.nbKangaroo
+        sc, ad = _limbs(scalars, 4), _limbs(d128, 2)
+        kt = np.ascontiguousarray(np.hstack([_limbs([k[0] for k in keys], 4), _limbs([k[1] for k in keys], 4)]))
+        tg = np.ascontiguousarray(targets, dtype=np.uint16)
+        assert sc.shape[0] == n and ad.shape[0] == n and tg.shape == (n,)
+        self._ck(self._lib.kgx_create_herd_multi(self._h, _p(sc), _p(ad), _p(kt), len(keys), tg.ctypes.data_as(_u16p), TAME),
+                 "CreateHerdMulti")
+
+    def Retarget(self, frm, to):
+        """Move every wild kangaroo of key `frm` to key to[(kIdx >> 1) % len(to)] (point += keys[new] - keys[frm], distance
+        kept), stream-ordered after the launch in flight; does not wait for it."""
+        t = np.ascontiguousarray(to, dtype=np.uint16)
+        self._ck(self._lib.kgx_retarget(self._h, int(frm), t.ctypes.data_as(_u16p), t.size), "Retarget")
+
+    def Targets(self):
+        """the key index of every kangaroo (kIdx order, uint16; meaningful for wild kangaroos), after the retargets queued"""
+        out = np.empty(self.nbKangaroo, dtype=np.uint16)
+        self._ck(self._lib.kgx_targets(self._h, out.ctypes.data_as(_u16p)), "Targets")
+        return out
 
     def callKernel(self):
         """GPUEngine.cu:540-557."""

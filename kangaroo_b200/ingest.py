@@ -35,6 +35,8 @@ _SIGS = {
     "kgi_add_items": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32, _u64p, ctypes.POINTER(Event),
                                      ctypes.c_uint32, ctypes.POINTER(ctypes.c_uint32)]),
     "kgi_resolve": (ctypes.c_int, [ctypes.c_void_p, _u64p, _u64p, _u64p, _u64p, _u64p, _u64p]),
+    "kgi_resolve_multi": (ctypes.c_int, [ctypes.c_void_p, _u64p, _u64p, _u64p, ctypes.c_uint32, _u64p, ctypes.POINTER(ctypes.c_uint32),
+                                         _u64p]),
     "kgi_save_work": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_uint32, _u64p, _u64p, _u64p, _u64p, ctypes.c_uint64,
                                      ctypes.c_double]),
     "kgi_load_work": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_uint32), _u64p,
@@ -135,6 +137,25 @@ class DPTable:
         out = (ctypes.c_uint64 * 4)()
         rc = self._lib.kgi_resolve(self._h, a, b, _limbs4(key[0]), _limbs4(key[1]), _limbs4(range_start), out)
         return sum(int(out[k]) << (64 * k) for k in range(4)) if rc == 1 else None
+
+    @staticmethod
+    def key_table(keys):
+        """keys (list of (x, y); None = the point at infinity, stored as (0, 0)) -> the (K, 8) uint64 table resolve_multi takes"""
+        out = np.zeros((len(keys), 8), dtype=np.uint64)
+        for i, k in enumerate(keys):
+            if k is not None:
+                out[i] = [(int(k[c]) >> (64 * w)) & _M64 for c in (0, 1) for w in range(4)]
+        return out
+
+    def resolve_multi(self, d_old, d_new, keys, range_start):
+        """resolve() against a key table (key_table(), or a list of points) -> (key index, private key) of the first key
+        matched, or None"""
+        kt = keys if isinstance(keys, np.ndarray) else self.key_table(keys)
+        kt = np.ascontiguousarray(kt, dtype=np.uint64)
+        a = (ctypes.c_uint64 * 2)(*d_old); b = (ctypes.c_uint64 * 2)(*d_new)
+        idx, out = ctypes.c_uint32(0), (ctypes.c_uint64 * 4)()
+        rc = self._lib.kgi_resolve_multi(self._h, a, b, kt.ctypes.data_as(_u64p), kt.shape[0], _limbs4(range_start), ctypes.byref(idx), out)
+        return (int(idx.value), sum(int(out[k]) << (64 * k) for k in range(4))) if rc == 1 else None
 
     def save_work(self, path, dp_bits, range_start, range_end, pubkey, total_count=0, total_time=0.0, total_walk=0):
         """Header + table (+ the kangaroo count: the caller appends total_walk x 96-byte records right after)."""

@@ -46,6 +46,8 @@ from .ingest import DPTable, EV_RESET, EV_COLLISION
 
 ORDER = ec.N
 MAX_RESETS = 255          # per step, carried in the control broadcast
+MAX_KEYS = 65535          # --batch-keys: keys of one run (KGX_MAX_KEYS, the engine's uint16 targets)
+MAX_SOLVED = 64           # --batch-keys: keys one step's control broadcast announces solved; more wait for the next step
 SAVE_CHUNK = 1 << 18      # kangaroos per gather chunk of a save (24 MB buffer)
 SAVE_CHUNKS_PER_STEP = 1  # chunks a step moves while a save is in progress (default herd: 17 steps)
 SAVE_BUFFERS = 4          # rank 0's pinned chunk buffers queued to the writer
@@ -108,7 +110,7 @@ class Solver:
         n = self.eng.nbKangaroo
         self.rng = np.random.Generator(np.random.PCG64((seed if seed is not None else int(time.time())) * 1000 + self.rank))
         sc, d128 = random_herd_arrays(n, self.range_power, self.wdiv2, self.rng)
-        self.eng.CreateHerdRaw(sc, d128, self.key)
+        self._create_herd(sc, d128)
         self.gather = DPGather(self.eng, self.dist, self.rank, self.world, torch, wire="dp40") if self.world > 1 else None
         self.dps = DPTable(threads=ingest_threads) if self.rank == 0 else None      # rank 0: the reference HashTable
         # Two pinned staging buffers: while the ingest thread inserts step k's records, step k+1's land in the other one.  The
@@ -149,6 +151,9 @@ class Solver:
         if resume:
             self._resume(resume)
         self.jumps0 = self.jumps
+
+    def _create_herd(self, sc, d128):
+        self.eng.CreateHerdRaw(sc, d128, self.key)
 
     # -- work files ------------------------------------------------------------------------------------------------
     def _resume(self, path):
@@ -352,13 +357,16 @@ class Solver:
         self._acc_found, self._acc_resets = None, []
         return found, resets
 
+    def _wild_key(self, kidx):
+        return self.key
+
     def _reset_kangaroo(self, kidx):
         """Kangaroo.cpp:601-609: CreateHerd(1, type) + SetKangaroo(kIdx) on the owning engine."""
         v = int(self.rng.integers(0, 1 << 62)) | (int(self.rng.integers(0, 1 << 62)) << 62) | (int(self.rng.integers(0, 1 << 62)) << 124)
         v &= (1 << self.range_power) - 1
         if kidx % 2 == WILD:
             d = (v - self.wdiv2) % ORDER
-            pos = ec.add(self.key, ec.mul(d))
+            pos = ec.add(self._wild_key(kidx), ec.mul(d))
         else:
             d = v
             pos = ec.mul(d)
@@ -494,6 +502,202 @@ class Solver:
             self.dps.close()
 
 
+# -- --batch-keys: every key of the input in one run, one tame herd shared by all of them -------------------------------------
+# The reference solves the keys of an input one after another, each with a new herd and an empty table (Kangaroo::Run,
+# Kangaroo.cpp:1021-1066).  Tame trails (d*G) and their DPs do not depend on the key, so here one engine, one herd and one
+# table serve them all: the wild half of the herd is spread over the unsolved keys, and when a key is solved its wilds move
+# on to the others (kgx_retarget), keeping their distance.  Rank 0 finds the key of a tame/wild collision with
+# kgi_resolve_multi, since the stored entry carries no kIdx.
+def spread(kidx, live):
+    """The key of wild kangaroo kIdx among the live keys (in input order): live[(kIdx >> 1) % len(live)].  The herd's first
+    assignment and kgx_retarget both follow it, so the wilds of every rank are spread evenly over the live keys."""
+    kidx = np.asarray(kidx, dtype=np.int64)
+    return np.asarray(live, dtype=np.uint16)[(kidx >> 1) % len(live)]
+
+
+def assign_targets(n, live):
+    """targets of a new multi-key herd of n kangaroos: the wild ones (odd kIdx) spread over the live keys, the tame ones 0"""
+    t = np.zeros(n, dtype=np.uint16)
+    wild = np.arange(WILD, n, 2)
+    t[wild] = spread(wild, live)
+    return t
+
+
+def retarget_targets(targets, frm, live):
+    """the host mirror of kgx_retarget(frm, live): the wilds of key frm move to spread(kIdx, live)"""
+    kidx = np.arange(targets.size)
+    moved = (kidx % 2 == WILD) & (targets == frm)
+    out = targets.copy()
+    out[moved] = spread(kidx[moved], live)
+    return out
+
+
+def key_classes(keys):
+    """Keys that are the same point, or each other's negative, share one search: -> (rep, neg) with rep[i] the first key of
+    i's class in input order and neg[i] true when keys[i] == -keys[rep[i]].  None (the point at infinity) is its own class."""
+    rep, neg, first = list(range(len(keys))), [False] * len(keys), {}
+    for i, k in enumerate(keys):
+        if k is None:
+            continue
+        j = first.setdefault(k[0], i)                   # same x: the same point or its negative
+        if j != i:
+            rep[i], neg[i] = j, k[1] != keys[j][1]
+    return rep, neg
+
+
+def class_privs(start, priv_rep, neg):
+    """the private key of a key of the class solved with priv_rep: keyToSearch = priv - start*G, so the negative of a key
+    has priv 2*start - priv_rep"""
+    return (2 * start - priv_rep) % ORDER if neg else priv_rep
+
+
+class BatchSolver(Solver):
+    """--batch-keys.  pubs: every public key of the input.  After run(), rank 0 holds priv[i] (None: not found)."""
+
+    def __init__(self, start, end, pubs, dp_bits, grid=None, max_found=1 << 17, seed=None, ingest_threads=0):
+        self.pubs = list(pubs)
+        if not 1 <= len(self.pubs) <= MAX_KEYS:
+            raise ValueError("--batch-keys takes 1 to %d keys, not %d" % (MAX_KEYS, len(self.pubs)))
+        # Kangaroo::InitSearchKey per key; pub == start*G leaves the point at infinity: solved at start, priv = start
+        self.keys = [ec.add(p, ec.neg(ec.mul(start))) if start else p for p in self.pubs]
+        self.priv = [start if k is None else None for k in self.keys]
+        # a key listed twice, or the negative of another, is searched once, as the first of its class: kgi_resolve_multi
+        # reports the first matching key, so the later ones would never be hit
+        self.rep, self.neg = key_classes(self.keys)
+        self.live = [i for i, k in enumerate(self.keys) if k is not None and self.rep[i] == i]
+        self._announce = []                 # rank 0: keys solved, not yet in a control broadcast
+        super().__init__(start, end, self.pubs[0], dp_bits, grid, max_found, seed, ingest_threads)
+        self.key_table = DPTable.key_table(self.keys)
+        self._ctrl = self.torch.zeros(2 + MAX_SOLVED + 2 * MAX_RESETS, dtype=self.torch.int64, device="cuda")
+
+    def _create_herd(self, sc, d128):
+        self.targets = assign_targets(self.eng.nbKangaroo, self.live or [0])         # host mirror of the engine's targets
+        self.eng.CreateHerdMulti(sc, d128, [k or (0, 0) for k in self.keys], self.targets)
+
+    def _wild_key(self, kidx):
+        return self.keys[int(self.targets[kidx])]
+
+    def _ingest(self, segments):
+        """rank 0, ingest thread -> (hits [(key index, private key, rank, kIdx)], resets)"""
+        hits, resets = [], []
+        t0 = time.perf_counter()
+        for r, buf in segments:
+            if buf.size == 0:
+                continue
+            for kind, rk, kidx, d_old, d_new in self.dps.add_dp40(buf, r):
+                if kind == EV_COLLISION:
+                    m = self.dps.resolve_multi(d_old, d_new, self.key_table, self.start)
+                    if m is None:
+                        resets.append((rk, kidx))                # matches no key: "unexpected wrong collision, reset kangaroo"
+                    else:
+                        hits.append(m + (rk, kidx))
+                elif kind == EV_RESET:
+                    resets.append((rk, kidx))                    # same herd, wild/wild across keys included
+        self.t_ingest += time.perf_counter() - t0
+        return hits, resets
+
+    def _take(self, block):
+        f, r = self._done.get(block=block)
+        self._pending -= 1
+        self._acc_found = (self._acc_found or []) + f
+        self._acc_resets += r
+
+    def _claim(self, hits, resets):
+        """rank 0: a hit on an unsolved key solves it.  A hit on a solved key resets the kangaroo that made it: a tame one that
+        ran onto the abandoned trail of a moved wild would re-walk it, or a wild DP from before its move."""
+        for idx, priv, rk, kidx in hits or []:
+            r = self.rep[idx]
+            if self.priv[r] is None:
+                self.priv[r] = class_privs(self.start, priv, self.neg[idx])
+                for i in range(len(self.keys)):                 # the other keys of its class
+                    if self.rep[i] == r:
+                        self.priv[i] = class_privs(self.start, self.priv[r], self.neg[i])
+                self._announce.append(r)
+            else:
+                resets.append((rk, kidx))
+
+    def step(self, may_save=False):
+        """one Launch on every rank; control broadcast [n_solved, n_resets, solved keys..., (rank, kIdx)...]; every rank moves
+        the wilds of each solved key to the live ones"""
+        torch = self.torch
+        n_found = self.eng.collect_count(relaunch=True)                  # launch i done, launch i+1 running
+        self._gather(n_found)
+        self._save_work_done = False
+        solved, resets = [], []
+        if self.rank == 0:
+            hits, resets = self._harvest()
+            self._claim(hits, resets)
+            solved, self._announce = self._announce[:MAX_SOLVED], self._announce[MAX_SOLVED:]
+        if self.dist is not None:
+            if self.rank == 0:
+                resets = resets[:MAX_RESETS]
+                c = [len(solved), len(resets)] + solved + [v for rk in resets for v in rk]
+                self._ctrl[:len(c)].copy_(torch.tensor(c, dtype=torch.int64))
+            self.dist.broadcast(self._ctrl, 0)
+            c = self._ctrl.cpu().tolist()
+            ns, nr = c[0], c[1]
+            solved = c[2:2 + ns]
+            resets = [(c[2 + ns + 2 * i], c[3 + ns + 2 * i]) for i in range(nr)]
+        for idx in solved:
+            self.live.remove(idx)
+            if self.live:
+                self.eng.Retarget(idx, self.live)                        # stream order: after launch i+1, before the resets
+                self.targets = retarget_targets(self.targets, idx, self.live)
+        self.stop = not self.live
+        for rk, kidx in resets:
+            self.same_herd += 1
+            if rk == self.rank and not self.stop:
+                self._reset_kangaroo(kidx)                               # at its current key
+        return None
+
+    def run(self, max_steps=1 << 30, verbose=True):
+        if not self.live:                                                # every key solved at start
+            self.elapsed, self.steps, self.steady_rate = 1e-9, 0, 0.0
+            return None
+        left = super().run(max_steps, verbose)
+        if self.rank == 0:
+            self._claim(left, [])                                        # hits of the last steps' records
+        return None
+
+
+def _run_batch(start, end, pubs, dp, grid, a):
+    t0 = time.perf_counter()
+    s = BatchSolver(start, end, pubs, dp, grid, seed=a.seed, ingest_threads=a.ingest_threads)
+    t_setup = time.perf_counter() - t0
+    if s.rank == 0:
+        print("Range width: 2^%d  kangaroos/GPU: %d  GPUs: %d  dp: %d  ingest threads: %d  keys: %d in one run" %
+              (s.range_power, s.eng.nbKangaroo, s.world, dp, s.dps.threads, len(pubs)), flush=True)
+    t0 = time.perf_counter()
+    s.run(a.max_steps)
+    t_run = time.perf_counter() - t0
+    t0 = time.perf_counter()
+    rc = 0
+    if s.rank == 0:
+        print("Solver rate: %.0f MJump/s steady state (after the first 32 steps), %.0f MJump/s over all %d steps (%.2f s); "
+              "rank-0 ingest %.2f ms/step; %d DPs; %d dead kangaroos re-created" %
+              (s.steady_rate / 1e6, (s.jumps - s.jumps0) / s.elapsed / 1e6, s.steps, s.elapsed, 1e3 * s.t_ingest / max(s.steps, 1),
+               len(s.dps), s.same_herd))
+        for i, pub in enumerate(pubs):
+            if s.priv[i] is not None and ec.mul(s.priv[i]) == pub:
+                print("Key#%2d Pub:  0x%064X\n       Priv: 0x%X" % (i, pub[0], s.priv[i]))
+            else:
+                print("Key#%2d not found" % i); rc = 1
+        solved = sum(1 for i, pub in enumerate(pubs) if s.priv[i] is not None and ec.mul(s.priv[i]) == pub)
+        print("Batch: %d/%d keys solved, %d jumps (2^%.2f) in total, %.3f sqrt(N) jumps per key (N = 2^%d), %d DPs" %
+              (solved, len(pubs), s.jumps, np.log2(max(s.jumps, 1)), s.jumps / len(pubs) / 2.0 ** (s.range_power / 2),
+               s.range_power, len(s.dps)), flush=True)
+    t_results = time.perf_counter() - t0
+    t0 = time.perf_counter()
+    s.close()
+    if s.rank == 0:
+        # where the time outside the jump loop goes: the loop ends when the last key is found, the DP records still queued
+        # are then inserted, and closing frees the engine and every entry of the table
+        print("Batch time: set-up %.2f s (engine, herd, table), jump loop %.2f s, after the loop %.2f s (last DPs into the table), "
+              "results %.2f s, close %.2f s (engine and table freed)" %
+              (t_setup, s.elapsed, t_run - s.elapsed, t_results, time.perf_counter() - t0), flush=True)
+    return rc
+
+
 def _resume_header(path):
     """the work file's header, read on rank 0 only and broadcast: the other ranks need not see the file"""
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -529,7 +733,15 @@ def main(argv=None):
     ap.add_argument("--save-kangaroos", action="store_true", help="save every rank's herd with the table (-ws)")
     ap.add_argument("--resume", default="", metavar="FILE",
                     help="continue from a work file (-i): range, key and dp come from the file unless given")
+    ap.add_argument("--batch-keys", action="store_true",
+                    help="solve every key of the config in one run: one tame herd and one DP table shared by all keys, the "
+                         "wild kangaroos spread over the unsolved ones")
     a = ap.parse_args(argv)
+    if a.batch_keys and (a.resume or a.save_work or a.save_interval or a.save_kangaroos):
+        ap.error("--batch-keys cannot be combined with --save-work, --save-interval, --save-kangaroos or --resume "
+                 "(a work file carries one key)")
+    if a.batch_keys and not a.config:
+        ap.error("--batch-keys needs a config file")
     if a.resume:
         file_dp, start, end, pub = _resume_header(a.resume)
         pubs = [pub]
@@ -543,9 +755,13 @@ def main(argv=None):
         ap.error("a config file or --resume FILE is required")
     if (a.save_interval > 0 or a.save_kangaroos) and not a.save_work:
         ap.error("--save-interval and --save-kangaroos need --save-work FILE")
+    if a.batch_keys and not pubs:
+        ap.error("--batch-keys needs a config with at least one public key")
+    if a.batch_keys and len(pubs) > MAX_KEYS:
+        ap.error("--batch-keys takes at most %d keys, the config has %d" % (MAX_KEYS, len(pubs)))
     grid = tuple(int(v) for v in a.grid.split(",")) if a.grid else None
-    rc = 0
-    for i, pub in enumerate(pubs):
+    rc = _run_batch(start, end, pubs, dp, grid, a) if a.batch_keys else 0
+    for i, pub in enumerate([] if a.batch_keys else pubs):
         s = Solver(start, end, pub, dp, grid, seed=a.seed, ingest_threads=a.ingest_threads, save_work=a.save_work,
                    save_interval=a.save_interval, save_kangaroos=a.save_kangaroos, resume=a.resume or None)
         if s.rank == 0:
