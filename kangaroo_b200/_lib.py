@@ -6,7 +6,9 @@ import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-LIB_PATH = os.environ.get("KGX_LIB_OVERRIDE") or os.path.join(CSRC, "libkgx.so")   # override: A/B builds in scripts/ experiments
+BUILD_PATH = os.path.join(CSRC, "libkgx.so")   # what build_library() writes
+OVERRIDE = os.environ.get("KGX_LIB_OVERRIDE")    # A/B builds in scripts/ experiments: loaded as they are, never rebuilt or overwritten
+LIB_PATH = OVERRIDE or BUILD_PATH
 HOSTTEST_PATH = os.path.join(CSRC, "libkgx_hosttest.so")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -71,15 +73,17 @@ def build_library(verbose=False):
     """Compile every CUDA source for sm_90a into csrc/libkgx.so (nvcc cross-compiles without a GPU) and the
     host-only unit-test helper csrc/libkgx_hosttest.so."""
     src = os.path.join(CSRC, "kgx_engine.cu")
-    cmd = ["nvcc"] + NVCC_FLAGS + ["-o", LIB_PATH, src]
+    cmd = ["nvcc"] + NVCC_FLAGS + ["-o", BUILD_PATH, src]
     if verbose:
         cmd += ["-Xptxas", "-v"]
     subprocess.check_call(cmd, cwd=CSRC)
     subprocess.check_call(["g++", "-O2", "-frounding-math", "-ffp-contract=off", "-fPIC", "-shared", "-o", HOSTTEST_PATH, os.path.join(CSRC, "kgx_hosttest.cpp")])
-    return LIB_PATH
+    return BUILD_PATH
 
 
 def _needs_build():
+    if OVERRIDE:                  # a library built from other sources: rebuilding it from these would make A equal B
+        return False
     if not os.path.exists(LIB_PATH):
         return True
     t = os.path.getmtime(LIB_PATH)

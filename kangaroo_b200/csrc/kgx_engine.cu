@@ -28,13 +28,15 @@ struct kgx_engine {
   int nRun = KGX_NB_RUN;
   uint4* state = nullptr;
   uint4* pre = nullptr;      // streaming mode: prefix-product scratch
+  uint8_t* jlog = nullptr;   // streaming mode: jump-index log, LOG_RUNS bytes per kangaroo (kgx_kernel.cuh stream_fold)
   bool streamMode = false;
   bool tmemMode = false;     // cluster tile kernel (jump_kernel_cluster; selector KGX_KERNEL_TMEM)
   int streamCtas = 2;
   bool symmetry = false;     // USE_SYMMETRY engine mode (kgx_set_symmetry): class switch + cycle rule, signed distances
   int symRule = 0;           // KGX_SYM_LASTJUMP / KGX_SYM_CLASS
   int pfDist = 2;            // KGX_STREAM_PF: L2 prefetch distance of the stream kernel in kangaroos (0 = off).  H100 SXM at
-                             // 700 W, default herd, kernel time: 0 -> 10.45, 2 -> 11.31, 4 -> 9.91 GJump/s (one run each)
+                             // 700 W, default herd, kernel time (scripts/sweep2.py, one run each): 0 -> 11.54, 1 -> 12.33,
+                             // 2 -> 12.88, 3 -> 12.42, 4 -> 11.65 GJump/s; 3 CTAs/SM at distance 2: 12.39
   uint8_t* aux = nullptr;    // symmetric mode: lastJump per slot
   bool warpInv = true;       // stream kernel: one warp-wide shuffle-butterfly inverse per pass (false: one per thread)
   u32* slab[2] = {nullptr, nullptr};   // DP slabs [count][maxFound*14]
@@ -126,7 +128,7 @@ void kgx_destroy(kgx_engine* e) {
   if (!e) return;
   cudaSetDevice(e->dev);
   if (e->stream) cudaStreamSynchronize(e->stream);
-  cudaFree(e->dp40); cudaFree(e->herdTab); cudaFree(e->state); cudaFree(e->pre); cudaFree(e->slab[0]); cudaFree(e->slab[1]); cudaFree(e->jtab);
+  cudaFree(e->dp40); cudaFree(e->herdTab); cudaFree(e->state); cudaFree(e->pre); cudaFree(e->jlog); cudaFree(e->slab[0]); cudaFree(e->slab[1]); cudaFree(e->jtab);
   cudaFree(e->stgX); cudaFree(e->stgY); cudaFree(e->stgD); cudaFree(e->aux); cudaFree(e->herdRecs);
   cudaFree(e->keys); cudaFree(e->targets); cudaFree(e->rtDelta); cudaFree(e->rtTo);
   if (e->slabPinned) cudaFreeHost(e->slabPinned);
@@ -236,6 +238,7 @@ kgx_engine* kgx_create_ex(int dev, int groups, int threads_per_group, uint32_t m
   }
   if ((s = cudaMalloc(&e->state, e->stateBytes)) != cudaSuccess) return fail("cudaMalloc(state)", s);
   if (e->streamMode && (s = cudaMalloc(&e->pre, (size_t)e->nPadded * 32)) != cudaSuccess) return fail("cudaMalloc(pre)", s);
+  if (e->streamMode && (s = cudaMalloc(&e->jlog, (size_t)e->nPadded * LOG_RUNS)) != cudaSuccess) return fail("cudaMalloc(jlog)", s);
   for (int i = 0; i < 2; i++) {
     if ((s = cudaMalloc(&e->slab[i], e->slabBytes)) != cudaSuccess) return fail("cudaMalloc(slab)", s);
     if ((s = cudaMemsetAsync(e->slab[i], 0, 4, e->stream)) != cudaSuccess) return fail("cudaMemset(slab)", s);  // Check.cpp:526 collects before any launch
@@ -259,7 +262,7 @@ kgx_engine* kgx_create_ex(int dev, int groups, int threads_per_group, uint32_t m
 uint64_t kgx_num_kangaroos(kgx_engine* e) { return e->n; }
 int kgx_kernel_kind(kgx_engine* e) { return e->streamMode ? KGX_KERNEL_STREAM : (e->tmemMode ? KGX_KERNEL_TMEM : KGX_KERNEL_RESIDENT); }
 uint64_t kgx_memory_bytes(kgx_engine* e) {
-  return e->stateBytes + (e->pre ? e->nPadded * 32 : 0) + 2 * e->slabBytes + JT_WORDS * 4 +
+  return e->stateBytes + (e->pre ? e->nPadded * 32 : 0) + (e->jlog ? e->nPadded * LOG_RUNS : 0) + 2 * e->slabBytes + JT_WORDS * 4 +
          (e->targets ? e->n * 2 : 0) + (u64)e->keyCap * (64 + 64 + 4);
 }
 uint32_t kgx_max_found(kgx_engine* e) { return e->maxFound; }
@@ -628,7 +631,7 @@ int kgx_launch_async(kgx_engine* e) {
   int sidx = e->cur ^ 1;
   LaunchParams p;
   p.state = e->state; p.jtab = e->jtab; p.out = e->slab[sidx]; p.dpMask = e->dpMask; p.nKangaroos = e->n;
-  p.numTiles = e->numTiles; p.maxFound = e->maxFound; p.nRun = e->nRun; p.prof = e->prof; p.pre = e->pre; p.G = e->K; p.aux = e->aux; p.symRule = e->symRule; p.pfDist = e->pfDist;
+  p.numTiles = e->numTiles; p.maxFound = e->maxFound; p.nRun = e->nRun; p.prof = e->prof; p.pre = e->pre; p.G = e->K; p.aux = e->aux; p.symRule = e->symRule; p.pfDist = e->pfDist; p.jlog = e->jlog;
   CK(e, cudaMemsetAsync(e->slab[sidx], 0, 4, e->stream));            // GPUEngine.cu:543
   CK(e, cudaEventRecord(e->evStart[sidx], e->stream));
   u32 grid = (u32)(e->ctasPerSM * e->sms);

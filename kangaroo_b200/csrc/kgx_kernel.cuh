@@ -6,8 +6,9 @@
 //   reference      : every thread owns 128 kangaroos in LOCAL memory (18.5 KB stack/thread): px/py/dx/subp arrays are
 //                    re-read and re-written through L1/L2 several times per jump (~416 B/jump), three passes.
 //   stream_kernel  : (default for herds >= 4e5 kangaroos, kgx_engine.cu) every thread owns G kangaroos that live in HBM as
-//                    coalesced 16-byte SoA chunks; ONE fused pass per jump reads prefix/x/y/d and writes x'/y'/d'/next
-//                    prefix (224 B/jump) with the next kangaroo prefetched into a second register buffer and the pair two
+//                    coalesced 16-byte SoA chunks; ONE fused pass per jump reads prefix/x/y and writes x'/y'/next prefix
+//                    and a one-byte jump-index log entry (the distances are folded from the log at the end of the launch;
+//                    ~194.5 B/jump) with the next kangaroo prefetched into a second register buffer and the pair two
 //                    trips ahead pulled into L2; no barriers.  Group inverse once per G jumps: the 32 lane products of a warp
 //                    are multiplied by a shuffle butterfly and ONE warp-uniform safegcd inverse serves 32*G kangaroos
 //                    (WARPINV), or every thread inverts its own product (short groups).
@@ -63,6 +64,7 @@ struct LaunchParams {
   uint8_t* aux;          // symmetric mode only: one state byte per kangaroo, [numTiles][G or K][T] (see jump_index)
   int symRule;           // KGX_SYM_LASTJUMP / KGX_SYM_CLASS
   int pfDist;            // stream kernel: L2 prefetch distance in kangaroos (0 = off; KGX_STREAM_PF)
+  uint8_t* jlog;         // stream kernel only: jump-index log [numTiles][LOG_RUNS][G][T] (see stream_fold)
   unsigned long long* prof;   // optional: [0]=sum serial cycles, [1]=sum modinv cycles, [2]=sum parallel cycles, [3]=tile-steps (warp 0 of every CTA)
 };
 
@@ -497,11 +499,18 @@ __global__ void __cluster_dims__(CfgCl::CLUSTER, 1, 1) __launch_bounds__(CfgCl::
 // ([tile][g][chunk][t], 16-byte chunks, lanes contiguous -> every warp access is one 512-byte line set).
 // No barriers, no cross-thread traffic: a thread inverts its own group product (lanes diverge inside the
 // variable-time safegcd, other warps fill the pipes meanwhile) and then makes ONE fused pass over its G
-// kangaroos per jump: read prefix/x/y/d (112 B), write x'/y'/d'/next prefix (112 B), software-prefetching the
-// next kangaroo while the current one is in the multiplier.  HBM traffic 224 B/jump instead of 2.5, but no
-// serial section at all; selected with KGX_MODE=stream (see DESIGN.md for the measured trade-off).
+// kangaroos per jump: read prefix/x/y (96 B), write x'/y'/next prefix (96 B) and one jump-log byte, software-prefetching
+// the next kangaroo while the current one is in the multiplier.  The distance chunk stays out of the hot loop: the
+// log is folded into it at the end of the launch (stream_fold), so at every launch boundary the state holds the exact
+// distance.  HBM traffic ~194.5 B/jump instead of 2.5, but no serial section at all; selected with KGX_MODE=stream
+// (see DESIGN.md for the measured trade-off).
 // =====================================================================================================
-struct KangLoad { uint4 p0, p1, x0, x1, y0, y1, d; u32 lj; };
+struct KangLoad { uint4 p0, p1, x0, x1, y0, y1; u32 lj; };
+
+// Runs a jump-log window holds.  A thread folds its log into the distances after its tile's last run and after every
+// LOG_RUNS runs, so the log takes LOG_RUNS bytes per kangaroo whatever kgx_set_jumps_per_launch says.
+constexpr int LOG_RUNS = 64;
+
 
 // sg / pg point at this thread's column of kangaroo g: sg = st + g*CHUNKS*T, pg = pr + g*2*T (running pointers: the
 // hot loop does no index multiplications -- IMAD shares the binding pipe)
@@ -510,32 +519,84 @@ __device__ __forceinline__ void stream_load(KangLoad& k, const uint4* sg, const 
   k.p0 = pg[0]; k.p1 = pg[T];
   k.x0 = sg[0]; k.x1 = sg[T];
   k.y0 = sg[2 * T]; k.y1 = sg[3 * T];
-  k.d = sg[4 * T];
   if (SYM) k.lj = ag[0];
+}
+
+// Replays one jump-log byte on a distance: bits 0-4 the jump index, bit 5 the class switch of symmetric mode -- exactly
+// the distance update of the jump (d += jD[j]; d = -d after a switch).
+template <bool SYM>
+__device__ __forceinline__ void replay_jump(u32* d, u32 b, const uint4* jt) {
+  const uint4 jd = jt[128 + (b & 31u)];
+  d128_add(d, jd.x, jd.y, jd.z, jd.w);
+  if (SYM) d128_cneg(d, 0u - ((b >> 5) & 1u));
+}
+
+// Replays the first n (<= LOG_RUNS) bytes of one kangaroo's log window on its distance: l = the window's first byte, its
+// runs lie runStride bytes apart.  The bytes are loaded in two batches of LOG_RUNS / 2 before any of a batch is applied
+// (the window is always allocated), so the replay waits for two memory latencies, not one per jump.  The log is read
+// with ordinary loads: this thread wrote it in this launch.
+template <bool SYM>
+__device__ __forceinline__ void replay_window(u32* d, const uint8_t* l, size_t runStride, int n, const uint4* jt) {
+  constexpr int HALF = LOG_RUNS / 2;
+#pragma unroll
+  for (int h = 0; h < LOG_RUNS; h += HALF) {
+    u32 b[HALF];
+#pragma unroll
+    for (int r = 0; r < HALF; r++) b[r] = l[(size_t)(h + r) * runStride];
+#pragma unroll
+    for (int r = 0; r < HALF; r++)
+      if (h + r < n) replay_jump<SYM>(d, b[r], jt);
+  }
 }
 
 // DP record append (GPUCompute.h:96-105, GPUMath.h:173-188): rare path (2^-dp per jump), kept out of line so the jump loop
 // stays one basic block.  The record is re-read from the kangaroo's own state chunks, which stream_body has just
 // written (same thread, program order): the hot loop keeps neither x' nor d' alive for it -- no local-memory home, no
-// extra registers.
-template <int T>
-__device__ __noinline__ void emit_dp_from_state(u32* out, const u32 maxFound, const u64 nKangaroos, const uint4* sg, u64 kidx) {
+// extra registers.  d' is the distance of the last fold plus the `runs` + 1 log bytes of this window, the last one at lg.
+template <int T, bool SYM>
+__device__ __noinline__ void emit_dp_from_state(u32* out, const u32 maxFound, const u64 nKangaroos, const uint4* sg, const uint8_t* lg,
+                                                int runs, size_t runStride, const uint4* jt, u64 kidx) {
   if (kidx >= nKangaroos) return;                      // padding slot
   const u32 pos = atomicAdd(out, 1u);
   if (pos >= maxFound) return;                         // GPUEngine.cu:641-648: counted, not stored
-  const uint4 x0 = sg[0], x1 = sg[T], d = sg[4 * T];
+  const uint4 x0 = sg[0], x1 = sg[T], dv = sg[4 * T];
+  u32 d[4] = {dv.x, dv.y, dv.z, dv.w};
+  replay_window<SYM>(d, lg - (ptrdiff_t)runs * (ptrdiff_t)runStride, runStride, runs + 1, jt);
   u32* o = out + 1 + (size_t)pos * 14;
   o[0] = x0.x; o[1] = x0.y; o[2] = x0.z; o[3] = x0.w; o[4] = x1.x; o[5] = x1.y; o[6] = x1.z; o[7] = x1.w;
-  o[8] = d.x; o[9] = d.y; o[10] = d.z; o[11] = d.w;
+  o[8] = d[0]; o[9] = d[1]; o[10] = d[2]; o[11] = d[3];
   o[12] = (u32)kidx; o[13] = (u32)(kidx >> 32);
 }
 
-// One kangaroo of the fused pass (see the file header): back-substitute, jump, start the next chain.  Branch-free:
-// returns whether the new point is distinguished (x' and d' are in the state chunks for emit_dp_from_state).
+// Folds the `runs` logged jumps of this thread's G kangaroos into their distance chunks.  st / lt: this thread's column
+// of the tile's state and log.  Every warp load of the log is one 32-byte sector; the next kangaroo's log lines are
+// pulled into L2 while one is replayed (lane l: runs l and l + 32).
 template <int T, bool SYM>
-__device__ __forceinline__ bool stream_body(const KangLoad& cur, uint4* sg, uint4* pg, uint8_t* ag, const uint4* jt, u32* I, u32* P,
-                                            const u32 mlo, const u32 mhi, const int rule) {
-  u32 x[8], y[8], jx[8], jy[8], dx[8], inv[8], s[8], rx[8], ry[8], d[4];
+__device__ __noinline__ void stream_fold(uint4* st, const uint8_t* lt, const int G, const int runs, const uint4* jt) {
+  const size_t runStride = (size_t)G * T;
+  const int lane = threadIdx.x & 31;
+  const uint8_t* pf = lt - threadIdx.x + (size_t)lane * runStride;
+#pragma unroll 1
+  for (int g = 0; g < G; g++) {
+    const uint8_t* l = lt + (size_t)g * T;
+    if (g + 1 < G) {
+      asm volatile("prefetch.global.L2 [%0];" ::"l"(pf + (size_t)(g + 1) * T));
+      asm volatile("prefetch.global.L2 [%0];" ::"l"(pf + (size_t)(g + 1) * T + 32 * runStride));
+    }
+    uint4* dp = st + (size_t)(g * CHUNKS + 4) * T;
+    const uint4 dv = *dp;
+    u32 d[4] = {dv.x, dv.y, dv.z, dv.w};
+    replay_window<SYM>(d, l, runStride, runs, jt);
+    *dp = make_uint4(d[0], d[1], d[2], d[3]);
+  }
+}
+
+// One kangaroo of the fused pass (see the file header): back-substitute, jump, log the jump, start the next chain.
+// Branch-free: returns whether the new point is distinguished (x' is in the state chunks for emit_dp_from_state).
+template <int T, bool SYM>
+__device__ __forceinline__ bool stream_body(const KangLoad& cur, uint4* sg, uint4* pg, uint8_t* ag, uint8_t* lg, const uint4* jt, u32* I,
+                                            u32* P, const u32 mlo, const u32 mhi, const int rule) {
+  u32 x[8], y[8], jx[8], jy[8], dx[8], inv[8], s[8], rx[8], ry[8];
   unpack8(x, cur.x0, cur.x1);
   unpack8(inv, cur.p0, cur.p1);
   const u32 j = jump_index<SYM>(x[0], cur.lj, rule);
@@ -554,21 +615,19 @@ __device__ __forceinline__ bool stream_body(const KangLoad& cur, uint4* sg, uint
   fe_sub(ry, x, rx);
   fe_mul(ry, ry, s);
   fe_sub(ry, ry, y);                       // ry = s (x - rx) - y
-  d[0] = cur.d.x; d[1] = cur.d.y; d[2] = cur.d.z; d[3] = cur.d.w;
-  const uint4 jd = jt[128 + j];
-  d128_add(d, jd.x, jd.y, jd.z, jd.w);
+  u32 lb = j;                              // jump-log byte (replay_jump): d += jD[j] happens in the fold
   if (SYM) {                               // equivalence class switch (Check.cpp:551-556): y > (p-1)/2 -> (x, p - y), d -> -d
     const u32 neg = fe_gt_half_mask(ry);
     fe_cneg(ry, neg);
-    d128_cneg(d, neg);                     // signed 128-bit distance
+    lb |= neg & 32u;                       // signed 128-bit distance: negated after the add
     auxn = sym_next_aux(cur.lj, j, neg, rule);
     ag[0] = (uint8_t)auxn;                 // lastJump / symClass
   }
+  lg[0] = (uint8_t)lb;
   sg[0] = make_uint4(rx[0], rx[1], rx[2], rx[3]);
   sg[T] = make_uint4(rx[4], rx[5], rx[6], rx[7]);
   sg[2 * T] = make_uint4(ry[0], ry[1], ry[2], ry[3]);
   sg[3 * T] = make_uint4(ry[4], ry[5], ry[6], ry[7]);
-  sg[4 * T] = make_uint4(d[0], d[1], d[2], d[3]);
   // next jump's dx and prefix product, accumulated in THIS order (P starts at 1 for the first kangaroo of a pass)
   lds_jp4(jx, jt, jump_index<SYM>(rx[0], auxn, rule));
   fe_sub(dx, rx, jx);
@@ -613,6 +672,8 @@ __global__ void __launch_bounds__(T, CTAS) stream_kernel(LaunchParams p) {
     uint4* pr = p.pre + (size_t)tile * (G * 2 * T) + t;
     const u64 kbase = (u64)tile * (T * G) + (u64)t;
     uint8_t* au = SYM ? (p.aux + (size_t)tile * ((size_t)G * T) + t) : nullptr;
+    uint8_t* lt = p.jlog + (size_t)tile * ((size_t)LOG_RUNS * G * T) + t;    // [run][g] bytes of this thread's column
+    const size_t runStride = (size_t)G * T;
     u32 P[8];
     fe_set_one(P);
     {   // prologue: forward chain, pr[g] = product of the dx before g
@@ -627,6 +688,7 @@ __global__ void __launch_bounds__(T, CTAS) stream_kernel(LaunchParams p) {
       }
     }
     int backward = 1;
+    int logged = 0;                               // runs in the log since the last fold
     for (int run = 0; run < p.nRun; run++) {
       u32 I[8];
       stream_group_inverse<WARPINV>(I, P);       // 1 / (dx_0 ... dx_{G-1}) of this thread's G kangaroos
@@ -638,20 +700,20 @@ __global__ void __launch_bounds__(T, CTAS) stream_kernel(LaunchParams p) {
       uint4* sg = st + (size_t)g0 * (CHUNKS * T);
       uint4* pg = pr + (size_t)g0 * (2 * T);
       uint8_t* ag = SYM ? (au + (size_t)g0 * T) : nullptr;
+      uint8_t* lg = lt + (size_t)logged * runStride + (size_t)g0 * T;
       u64 kidx = kbase + (u64)g0 * T;
       KangLoad A, B;                              // ping-pong prefetch buffers (no register copies)
       stream_load<T, SYM>(A, sg, pg, ag);
-      // L2 prefetch of the pair p.pfDist trips ahead (no registers held): a pair is 14 planes (2 x {x lo, x hi, y lo, y hi, d} of the
-      // state, 2 x {lo, hi} of the prefix products) of 512 B per warp = 56 lines of 128 B.  Each LANE asks for a different line --
-      // lane -> (plane lane/4, line lane%4) -- so two instructions cover the pair instead of one per plane (14).
+      // L2 prefetch of the pair p.pfDist trips ahead (no registers held): a pair is 12 planes (2 x {x lo, x hi, y lo, y hi} of the
+      // state, 2 x {lo, hi} of the prefix products) of 512 B per warp = 48 lines of 128 B.  Each LANE asks for a different line --
+      // lane -> (plane lane/4, line lane%4) -- so two instructions cover the pair instead of one per plane (12).
       const int pl = lane >> 2;
       const ptrdiff_t lineOff = (ptrdiff_t)((lane & 3) * 8) - lane;                       // uint4 units, from this thread's own address
-      const uint4* q1 = pl < 5 ? sg + (ptrdiff_t)p.pfDist * ds + pl * T + lineOff         // first kangaroo: 5 state planes,
-                               : pg + (ptrdiff_t)p.pfDist * dp + (pl < 7 ? (pl - 5) * T : dp) + lineOff;   // its 2 prefix planes, the second's low one
-      const uint4* q2 = pl < 5 ? sg + (ptrdiff_t)(p.pfDist + 1) * ds + pl * T + lineOff   // second kangaroo: 5 state planes,
-                               : pg + (ptrdiff_t)(p.pfDist + 1) * dp + T + lineOff;       // its high prefix plane (lanes 20..23)
-      const ptrdiff_t qs = 2 * (pl < 5 ? ds : dp);
-      const bool q2on = pl < 6;
+      const uint4* q1 = pl < 4 ? sg + (ptrdiff_t)p.pfDist * ds + pl * T + lineOff         // first kangaroo: 4 state planes,
+                               : pg + (ptrdiff_t)p.pfDist * dp + (pl < 6 ? (pl - 4) * T : dp + (pl - 6) * T) + lineOff;   // both kangaroos' 2 prefix planes
+      const uint4* q2 = sg + (ptrdiff_t)(p.pfDist + 1) * ds + pl * T + lineOff;          // second kangaroo: 4 state planes (lanes 0..15)
+      const ptrdiff_t qs = 2 * (pl < 4 ? ds : dp);
+      const bool q2on = pl < 4;
 #pragma unroll 1
       for (int i = 0; i < G; i += 2) {
         if (p.pfDist > 0 && i + p.pfDist + 1 < G) {
@@ -660,15 +722,24 @@ __global__ void __launch_bounds__(T, CTAS) stream_kernel(LaunchParams p) {
         }
         q1 += qs; q2 += qs;
         stream_load<T, SYM>(B, sg + ds, pg + dp, ag + dk);
-        const bool ha = stream_body<T, SYM>(A, sg, pg, ag, jt, I, P, mlo, mhi, p.symRule);
+        const bool ha = stream_body<T, SYM>(A, sg, pg, ag, lg, jt, I, P, mlo, mhi, p.symRule);
         if (i + 2 < G) stream_load<T, SYM>(A, sg + 2 * ds, pg + 2 * dp, ag + 2 * dk);
-        const bool hb = stream_body<T, SYM>(B, sg + ds, pg + dp, ag + dk, jt, I, P, mlo, mhi, p.symRule);
-        if (ha) emit_dp_from_state<T>(p.out, p.maxFound, p.nKangaroos, sg, kidx);
-        if (hb) emit_dp_from_state<T>(p.out, p.maxFound, p.nKangaroos, sg + ds, kidx + dk);
-        sg += 2 * ds; pg += 2 * dp; kidx += 2 * dk;
+        const bool hb = stream_body<T, SYM>(B, sg + ds, pg + dp, ag + dk, lg + dk, jt, I, P, mlo, mhi, p.symRule);
+        if (__any_sync(0xffffffffu, ha | hb)) {      // warp-uniform: taken about once per 2^dp / 64 pairs
+          if (ha) emit_dp_from_state<T, SYM>(p.out, p.maxFound, p.nKangaroos, sg, lg, logged, runStride, jt, kidx);
+          if (hb) emit_dp_from_state<T, SYM>(p.out, p.maxFound, p.nKangaroos, sg + ds, lg + dk, logged, runStride, jt, kidx + dk);
+          __syncwarp();   // the lanes back from a DP record rejoin their warp here.  Left to themselves they ran the rest of the
+                          // launch as a separate group (the shuffles of the group inverse do not merge them): on the H100, 4 200
+                          // DPs per launch cost a third of the kernel's speed.
+        }
+        sg += 2 * ds; pg += 2 * dp; lg += 2 * dk; kidx += 2 * dk;
         if (SYM) ag += 2 * dk;
       }
       backward ^= 1;
+      if (++logged == LOG_RUNS || run == p.nRun - 1) {
+        stream_fold<T, SYM>(st, lt, G, logged, jt);
+        logged = 0;
+      }
     }
   }
 }
