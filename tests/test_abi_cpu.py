@@ -99,6 +99,53 @@ def test_every_compiled_jump_kernel_has_a_gpu_test():
         check_variants_cover(src, VARIANTS, [v for v in SYM_VARIANTS if v["KGX_MODE"] != "resident"])
 
 
+def adaptive_group_bounds(src):
+    """The (smallest, largest) stream group size kgx_create_ex picks from the herd size; the largest is the benchmarked one."""
+    lo, hi = (int(re.search(r"if \(g %s (\d+)\) g = \1;" % op, src).group(1)) for op in "<>")
+    return lo, hi
+
+
+def check_log_variants_cover(src, log_variants, sym_log_variants):
+    """tests/test_gpu_jumplog.py's matrices, in each engine mode: every stream instantiation at the adaptive group size, the
+    stream kernel at the smallest group size (CTAs loop over tiles) and one step above the largest (the longest log run
+    stride), in the non-symmetric engine also at the largest (the benchmarked kernel), and as controls without a log the
+    default tile and the cluster kernel where the mode compiles them."""
+    kernels, default_geometry = compiled_jump_kernels(src)
+    lo, hi = adaptive_group_bounds(src)
+    for name, variants, compiled, select, sizes in (
+            ("LOG_VARIANTS", log_variants, kernels, variant_kernel, {lo, hi, hi + 2}),
+            ("SYM_LOG_VARIANTS", sym_log_variants, compiled_symmetric_jump_kernels(src), symmetric_variant_kernel, {lo, hi + 2})):
+        streams = {k for k in compiled if k[0] == "stream"}
+        adaptive = {select(v, default_geometry) for v in variants if v["KGX_MODE"] == "stream" and "KGX_STREAM_G" not in v}
+        assert streams - adaptive == set(), "stream instantiations that no entry of %s runs at the adaptive group size" % name
+        explicit = {int(v["KGX_STREAM_G"]) for v in variants if "KGX_STREAM_G" in v}
+        assert sizes - explicit == set(), "stream group sizes that no entry of %s runs" % name
+        selected = {select(v, default_geometry) for v in variants} - {None}
+        controls = {("resident", default_geometry), ("tmem",)} & compiled
+        assert controls - selected == set(), "kernels without a log that %s does not run as controls" % name
+        assert selected - compiled == set(), "%s entries that select no compiled kernel" % name
+
+
+def test_every_stream_instantiation_runs_multi_window_launches():
+    """tests/test_gpu_jumplog.py runs LOG_VARIANTS and SYM_LOG_VARIANTS over several jump-log windows per launch; a stream
+    instantiation added to kgx_engine.cu without an entry there, or an entry dropped, fails here."""
+    from tests.test_gpu_jumplog import LOG_VARIANTS, SYM_LOG_VARIANTS
+    src = open(os.path.join(ROOT, "kangaroo_b200", "csrc", "kgx_engine.cu")).read()
+    assert adaptive_group_bounds(src) == (2, 128)
+    check_log_variants_cover(src, LOG_VARIANTS, SYM_LOG_VARIANTS)
+    # the guard itself: a 3-CTA symmetric stream kernel, or any one entry fewer in either list, must fail it
+    sym3 = src.replace("stream_kernel<128, 2, true, true>", "stream_kernel<128, 3, true, true>")
+    assert sym3 != src
+    with pytest.raises(AssertionError):
+        check_log_variants_cover(sym3, LOG_VARIANTS, SYM_LOG_VARIANTS)
+    for i in range(len(LOG_VARIANTS)):
+        with pytest.raises(AssertionError):
+            check_log_variants_cover(src, LOG_VARIANTS[:i] + LOG_VARIANTS[i + 1:], SYM_LOG_VARIANTS)
+    for i in range(len(SYM_LOG_VARIANTS)):
+        with pytest.raises(AssertionError):
+            check_log_variants_cover(src, LOG_VARIANTS, SYM_LOG_VARIANTS[:i] + SYM_LOG_VARIANTS[i + 1:])
+
+
 def test_no_oracle_in_product():
     # the product package must never import / link the oracle
     for dirpath, _, files in os.walk(os.path.join(ROOT, "kangaroo_b200")):

@@ -94,10 +94,10 @@ SHAPE_GRID = (61, 127)            # 61 x 127 x 128 = 991,616 kangaroos: a multip
 SAMPLE = 2048
 
 
-def shape_sample(n):
+def shape_sample(n, size=SAMPLE):
     """A strided sample plus the last 128 kangaroos, which sit in the padded last tile of every geometry."""
     import numpy as np
-    return np.unique(np.concatenate([np.arange(0, n, n // SAMPLE), np.arange(n - 128, n)]))
+    return np.unique(np.concatenate([np.arange(0, n, n // size), np.arange(n - 128, n)]))
 
 
 @pytest.fixture(scope="module")
@@ -210,19 +210,29 @@ def sym_shape_herd(oracle):
     n = SHAPE_GRID[0] * SHAPE_GRID[1] * 128
     sc, d128 = sym_herd_arrays(n, np.random.Generator(np.random.PCG64(4343)))
     idx = shape_sample(n)
+    for i in idx.tolist():
+        d = kgo.from_limbs(d128[i])
+        assert ((d - (1 << 128)) if d >> 127 else d) % kgo.N == kgo.from_limbs(sc[i])
+    x, y, d, flipped = herd_start_state(oracle, key, sc, d128, idx, symmetric=True)
+    assert 0 < flipped < len(idx)
+    return dict(n=n, sc=sc, d128=d128, key=key, idx=idx, table=oracle.create_jump_table_sym(SYM_RP), x=x, y=y, d=d)
+
+
+def herd_start_state(oracle, key, sc, d128, idx, symmetric=False):
+    """The start state CreateHerdRaw(sc, d128, key) must give the sample idx: d*G (tame, even kIdx) or key + d*G (wild) with
+    the distance d128 as stored; in symmetric mode the class representative, with d negated wherever y was flipped.
+    -> x, y (m,4) and d (m,2) limb arrays, and how many kangaroos were flipped."""
+    from oracle import kgo
     xs, ys, ds, flipped = [], [], [], 0
     for i in idx.tolist():
-        s, d = kgo.from_limbs(sc[i]), kgo.from_limbs(d128[i])
-        assert ((d - (1 << 128)) if d >> 127 else d) % kgo.N == s
-        pt = oracle.ec_mul_g(s)
+        pt = oracle.ec_mul_g(kgo.from_limbs(sc[i]))
         if i % 2:
             pt = oracle.ec_add(key, pt)
-        flip = pt[1] > (kgo.P - 1) // 2
+        d = kgo.from_limbs(d128[i])
+        flip = symmetric and pt[1] > (kgo.P - 1) // 2
         xs.append(pt[0]); ys.append(kgo.P - pt[1] if flip else pt[1]); ds.append(-d & M128 if flip else d)
         flipped += flip
-    assert 0 < flipped < len(idx)
-    return dict(n=n, sc=sc, d128=d128, key=key, idx=idx, table=oracle.create_jump_table_sym(SYM_RP),
-                x=kgo.ints_to_array(xs), y=kgo.ints_to_array(ys), d=kgo.ints_to_array(ds, 2))
+    return kgo.ints_to_array(xs), kgo.ints_to_array(ys), kgo.ints_to_array(ds, 2), flipped
 
 
 def fresh_sym_kangaroo(oracle, key, kidx, stale, init, rule):
@@ -317,12 +327,20 @@ def test_symmetric_variant_shapes_match_oracle(env, rule, init, n_run, sym_shape
         assert got == exp and len(exp) > 50, launch
 
 
-def long_walks_agree(monkeypatch, rule=None, sym_table=None):
-    """1,048,576 kangaroos x 100 launches of 64 jumps on every kernel that runs `rule` (None: the non-symmetric engine; else
-    the symmetric engine with that jump rule and sym_table): bit-identical end states and DP multisets."""
+LONG_WALK = (64,) * 100
+# The same 6400 jumps for the stream kernel in launches that end its jump-log windows at every kind of place: after one run,
+# one short of and exactly at a full window, one run past it, around two windows, and 5823 = 90 x 64 + 63 (91 folds).
+LONG_WALK_IRREGULAR = (1, 63, 64, 65, 127, 128, 129, 5823)
+
+
+def long_walks_agree(monkeypatch, rule=None, sym_table=None, stream_runs=LONG_WALK):
+    """1,048,576 kangaroos x 6400 jumps on every kernel that runs `rule` (None: the non-symmetric engine; else the symmetric
+    engine with that jump rule and sym_table): bit-identical end states and DP multisets.  The stream kernel takes its jumps
+    in launches of stream_runs jumps, the tile kernels in LONG_WALK's 100 launches of 64."""
     import numpy as np
     from kangaroo_b200 import GPUEngine, random_herd_arrays
     from tests.golden_util import load_cases
+    assert sum(stream_runs) == sum(LONG_WALK)
     case = [c for c in load_cases() if c["range_power"] == 80][0]
     rng = np.random.Generator(np.random.PCG64(2024))
     if rule is None:
@@ -340,11 +358,14 @@ def long_walks_agree(monkeypatch, rule=None, sym_table=None):
         eng.SetParams(0xFFFFF00000000000, *table)          # dp = 20
         eng.SetWildOffset(case["width_div2"])               # not applied in symmetric mode
         eng.CreateHerdRaw(sc, d128, case["key"])
+        runs = stream_runs if mode == "stream" else LONG_WALK
         dps = []
+        eng.set_jumps_per_launch(runs[0])
         eng.callKernel()
-        for _ in range(99):
-            dps += [(it.x, it.d, it.kIdx) for it in eng.Launch()]
-        dps += [(it.x, it.d, it.kIdx) for it in eng.Launch(relaunch=False)]
+        for nxt in runs[1:] + (None,):
+            if nxt:
+                eng.set_jumps_per_launch(nxt)               # read when Launch() starts the next launch
+            dps += [(it.x, it.d, it.kIdx) for it in eng.Launch(relaunch=nxt is not None)]
         ax, ay, ad = eng.GetKangaroosRaw()
         results[mode] = (ax, ay, ad, sorted(dps))
         eng.close()
@@ -367,6 +388,19 @@ def test_stream_and_resident_agree_over_a_long_symmetric_walk(rule, oracle, monk
     """The same cross-validation in symmetric mode, stream against resident kernel: their per-kangaroo state bytes carry the
     jump rule across all 100 launches, and the resident CTAs loop over tiles."""
     long_walks_agree(monkeypatch, rule, oracle.create_jump_table_sym(SYM_RP))
+
+
+def test_stream_walk_in_irregular_launches_agrees_with_the_tile_kernels(monkeypatch):
+    """The long walk with the stream kernel's 6400 jumps in launches of 1 to 5823 jumps: a fold after a short window, several
+    folds inside one launch and DPs rebuilt after them must leave the same states and DPs as the tile kernels, which keep no
+    jump log."""
+    long_walks_agree(monkeypatch, stream_runs=LONG_WALK_IRREGULAR)
+
+
+@pytest.mark.parametrize("rule", ["lastjump", "symclass"])
+def test_stream_symmetric_walk_in_irregular_launches_agrees_with_the_resident_kernel(rule, oracle, monkeypatch):
+    """The same in symmetric mode, where the folds inside a launch also replay the class switches logged in bit 5."""
+    long_walks_agree(monkeypatch, rule, oracle.create_jump_table_sym(SYM_RP), LONG_WALK_IRREGULAR)
 
 
 def test_cluster_kernel_odd_jump_count_over_several_tiles_per_cluster(monkeypatch):
