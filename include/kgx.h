@@ -154,6 +154,48 @@ int      kgx_set_jumps_per_launch(kgx_engine* e, int n_run);
 /* Number of kernels this engine has launched so far (jump + pack/unpack/patch), for bench.py's gpu_launches. */
 uint64_t kgx_kernel_launches(kgx_engine* e);
 
+/* --- device-resident DP table (kgx_dptable.cuh): the reference's HashTable (HashTable.cpp:262-307, 2^18 buckets of
+ *     ENTRY {int128 x; int128 d}) in the memory of one GPU, fed the 40-byte records of kgx_convert_dps.  Every sequence of
+ *     adds gives exactly the events, count, per-bucket nbItem / maxItem and work files of the host table of
+ *     include/kgx_ingest.h (kgi_add / kgi_save_work_ex / kgi_load_work_ex) fed the same records in the same order.
+ * _create: a table of `capacity` entries (fixed; 1 .. 2^32-2) on device dev; NULL without a device or memory, reason in
+ *     kgx_dptable_last_error(NULL).  _bytes_for: device bytes a table of that capacity takes (48 per entry + fixed scratch).
+ * _add: records of n_ranks rank segments (1 .. KGX_DPT_MAX_RANKS), segment r = counts[r] records at recs + r*stride*40
+ *     (device memory; counts on the host), inserted in segment order then record order, stream-ordered on `stream`
+ *     (a cudaStream_t; NULL = the legacy default stream); the call waits for its own work only.  Events in arrival order:
+ *     the first `cap` are copied to ev (host), *n_ev = all of them.  Returns 0; -1 when records with h >= 2^18 were
+ *     skipped (the others inserted, as kgi_add); -2 when count + records > capacity: nothing inserted, reason in
+ *     kgx_dptable_last_error; -3 on a CUDA error.
+ * _reserve: allocates now the per-call scratch of adds of up to n_records records (about 70 bytes per record) and of `cap`
+ *     events, which adds otherwise grow on demand; a caller that sizes the table to the free memory reserves first.
+ * _save_work / _load_work: kgi_save_work_ex / kgi_load_work_ex on this table (same header arguments and results, same
+ *     bytes; the entries move in bounded chunks through pinned memory), after the work queued on `stream`.  A load that
+ *     holds more entries than the capacity fails with -ENOSPC and leaves the table empty, like any failed load. --- */
+typedef struct kgx_dptable kgx_dptable;
+typedef struct {                     /* = kgi_event (include/kgx_ingest.h) */
+  uint32_t kind, rank, kidx, h;
+  uint64_t d_old[2], d_new[2];
+} kgx_dp_event;
+#define KGX_DPT_EV_RESET     1
+#define KGX_DPT_EV_COLLISION 2
+#define KGX_DPT_MAX_RANKS    256
+kgx_dptable* kgx_dptable_create(int dev, uint64_t capacity);
+void         kgx_dptable_destroy(kgx_dptable* t);
+const char*  kgx_dptable_last_error(kgx_dptable* t);
+uint64_t     kgx_dptable_count(kgx_dptable* t);
+uint64_t     kgx_dptable_capacity(kgx_dptable* t);
+uint64_t     kgx_dptable_memory_bytes(kgx_dptable* t);
+uint64_t     kgx_dptable_bytes_for(uint64_t capacity);
+int          kgx_dptable_reserve(kgx_dptable* t, uint32_t n_records, uint32_t cap);
+int kgx_dptable_add(kgx_dptable* t, const void* recs, const uint32_t* counts, uint32_t n_ranks, uint64_t stride, kgx_dp_event* ev,
+                    uint32_t cap, uint32_t* n_ev, void* stream);
+int kgx_dptable_save_work(kgx_dptable* t, const char* path, uint32_t dp_bits, const uint64_t range_start[4], const uint64_t range_end[4],
+                          const uint64_t keyx[4], const uint64_t keyy[4], uint64_t total_count, double total_time, uint64_t total_walk,
+                          void* stream);
+int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, uint64_t range_start[4], uint64_t range_end[4],
+                          uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time, uint64_t* nb_walk,
+                          uint64_t* walk_offset, void* stream);
+
 /* Debug (KGX_PROF=1 in the environment at kgx_create): phase cycle counters summed over warp 0 of every CTA:
  * out = {serial section, modular inverse alone, parallel phase, tile-steps}; resets them. -1 when disabled. */
 int      kgx_debug_prof(kgx_engine* e, uint64_t out[4]);

@@ -63,6 +63,20 @@ _SIGS = {
                                            ctypes.c_void_p]),
     "kgx_bench_raw": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_float),
                                      ctypes.POINTER(ctypes.c_double)]),
+    "kgx_dptable_create": (ctypes.c_void_p, [ctypes.c_int, ctypes.c_uint64]),
+    "kgx_dptable_destroy": (None, [ctypes.c_void_p]),
+    "kgx_dptable_last_error": (ctypes.c_char_p, [ctypes.c_void_p]),
+    "kgx_dptable_count": (ctypes.c_uint64, [ctypes.c_void_p]),
+    "kgx_dptable_capacity": (ctypes.c_uint64, [ctypes.c_void_p]),
+    "kgx_dptable_memory_bytes": (ctypes.c_uint64, [ctypes.c_void_p]),
+    "kgx_dptable_bytes_for": (ctypes.c_uint64, [ctypes.c_uint64]),
+    "kgx_dptable_reserve": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32]),
+    "kgx_dptable_add": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint32), ctypes.c_uint32, ctypes.c_uint64,
+                                       ctypes.c_void_p, ctypes.c_uint32, ctypes.POINTER(ctypes.c_uint32), ctypes.c_void_p]),
+    "kgx_dptable_save_work": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_uint32, _u64p, _u64p, _u64p, _u64p, ctypes.c_uint64,
+                                             ctypes.c_double, ctypes.c_uint64, ctypes.c_void_p]),
+    "kgx_dptable_load_work": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_uint32), _u64p, _u64p, _u64p, _u64p,
+                                             _u64p, ctypes.POINTER(ctypes.c_double), _u64p, _u64p, ctypes.c_void_p]),
 }
 EXPORTED_SYMBOLS = sorted(_SIGS)
 

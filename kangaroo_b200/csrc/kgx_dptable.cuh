@@ -1,0 +1,608 @@
+// kgx_dptable.cuh -- the rank-0 distinguished-point table in the memory of one GPU (C ABI: include/kgx.h, kgx_dptable_*).
+//
+// Semantics: exactly those of the reference's HashTable::Add driven record by record in arrival order (HashTable.cpp:262-307)
+// with kgx_ingest.cpp's event mapping (kgx_ingest.cpp:68-83): 2^18 buckets h = x.bits64[2] & 0x3FFFF, one ENTRY {x, d} per
+// distinct x of a bucket, per-bucket nbItem / maxItem counted like the reference (maxItem 16 on the first Add of a bucket, +4
+// on every later Add -- stored or not -- that finds nbItem >= maxItem - 1), and work files that are byte for byte what
+// HashTable::SaveTable writes (buckets in order, entries sorted by unsigned (x.hi, x.lo)).
+//
+// Layout (fixed capacity C entries, no growth):
+//   ent[C]      32-byte entries {x, d}, dense in insertion order; ent_h[C] their bucket
+//   slots[S]    open-addressing index over (h, x), S = C + C/2 (load <= 2/3), linear probing: 64-bit word
+//               (entry index << 32) | tag, tag = (h + 1) | 13 bits of x.hi << 19, 0 = empty
+//   nb/mx[2^18] the reference's nbItem / maxItem
+// 48 bytes per entry of capacity, plus 2 MB of bucket counters and the save scratch (SAVE_CHUNK entries, 56 bytes each).
+//
+// One add call, stream-ordered on the caller's stream:
+//   1. key  = h of every record (2^18 for a malformed one), value = arrival index (rank segments in order, then records)
+//   2. stable radix sort by key: the records of one bucket together, in arrival order
+//   3. one thread per bucket present walks its records in order: the reference's sequence of Add calls on that bucket, with
+//      the (h, x) index in place of its binary search.  Buckets never share an entry, so threads of different buckets only
+//      meet in the index, where an insert claims an empty slot with a CAS after its entry is written.
+//   4. the events, written at their arrival index, are compacted in arrival order; the first `cap` go back to the host.
+#include <cerrno>
+#include <cub/cub.cuh>
+
+namespace kgx_dpt {
+
+typedef unsigned long long ull;
+constexpr uint32_t NBUCKET = 1u << 18;                  // HASH_SIZE (HashTable.h)
+constexpr uint64_t TYPE_BIT = 0x4000000000000000ull;    // b126 of the tagged distance: herd type (HashTable::CalcDistAndType)
+constexpr uint64_t SAVE_CHUNK = 1ull << 21;             // entries per device->host chunk of a save / host->device chunk of a load
+constexpr uint32_t HEADW = 0xFA6A8001u;                 // Kangaroo.h:120
+
+struct Entry { uint64_t x0, x1, d0, d1; };              // ENTRY {int128 x; int128 d}
+struct Res { ull count; uint32_t nsel; uint32_t bad; };
+struct Ranks { uint32_t n; uint32_t pre[KGX_DPT_MAX_RANKS + 1]; };
+
+__device__ __forceinline__ uint32_t rank_of(const Ranks& R, uint32_t i) {
+  uint32_t lo = 0, hi = R.n - 1;                        // the last rank whose segment starts at or before i
+  while (lo < hi) {
+    const uint32_t m = (lo + hi + 1) >> 1;
+    if (R.pre[m] <= i) lo = m; else hi = m - 1;
+  }
+  return lo;
+}
+
+__device__ __forceinline__ const uint64_t* record(const uint8_t* recs, uint64_t stride, const Ranks& R, uint32_t i, uint32_t r) {
+  return reinterpret_cast<const uint64_t*>(recs + ((uint64_t)r * stride + (i - R.pre[r])) * 40ull);
+}
+
+__host__ __device__ __forceinline__ uint32_t slot_tag(uint32_t h, uint64_t x1) { return (h + 1) | ((uint32_t)(x1 >> 51) << 19); }
+
+__device__ __forceinline__ uint64_t slot_home(uint32_t h, uint64_t x0, uint64_t x1, uint64_t nslots) {
+  uint64_t k = (x0 ^ (x1 * 0x9E3779B97F4A7C15ull) ^ ((uint64_t)h << 40)) * 0xD6E8FEB86659FD93ull;
+  k ^= k >> 32;
+  return __umul64hi(k, nslots);
+}
+
+__device__ __forceinline__ void index_insert(ull* slots, uint64_t nslots, uint64_t home, ull word) {
+  uint64_t p = home;
+  while (atomicCAS(&slots[p], 0ull, word) != 0ull)
+    if (++p == nslots) p = 0;
+}
+
+__global__ void k_keys(const uint8_t* recs, uint64_t stride, Ranks R, uint32_t n, uint32_t* keys, uint32_t* vals,
+                       uint8_t* evFlag, Res* res) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t h = (uint32_t)(record(recs, stride, R, i, rank_of(R, i))[0] >> 32);
+  keys[i] = h < NBUCKET ? h : NBUCKET;
+  vals[i] = i;
+  evFlag[i] = 0;
+  if (h >= NBUCKET) res->bad = 1;                       // skipped, like kgx_ingest.cpp's workers; the call returns -1
+}
+
+// one thread per bucket present in the call: HashTable::Add(h, x, d) for each of its records in arrival order
+__global__ void k_insert(const uint32_t* keys, const uint32_t* vals, uint32_t n, const uint8_t* recs, uint64_t stride, Ranks R,
+                         Entry* ent, uint32_t* ent_h, ull* slots, uint64_t nslots, uint32_t* nb, uint32_t* mx, Res* res,
+                         kgx_dp_event* evArr, uint8_t* evFlag) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const uint32_t h = keys[j];
+  if (h >= NBUCKET || (j > 0 && keys[j - 1] == h)) return;
+  uint32_t nbv = nb[h], mxv = mx[h];
+  for (uint32_t k = j; k < n && keys[k] == h; k++) {
+    const uint32_t i = vals[k], r = rank_of(R, i);
+    const uint64_t* rec = record(recs, stride, R, i, r);
+    const uint64_t w0 = rec[0], x0 = rec[1], x1 = rec[2], d0 = rec[3], d1 = rec[4];
+    const uint32_t tag = slot_tag(h, x1);
+    const uint64_t home = slot_home(h, x0, x1, nslots);
+    if (mxv == 0) mxv = 16;                             // HashTable.cpp:264-267
+    if (nbv != 0) {
+      if (nbv >= mxv - 1) mxv += 4;                     // HashTable.cpp:275-278: before the search, whatever it finds
+      uint64_t p = home;
+      for (;;) {
+        const ull s = *reinterpret_cast<volatile ull*>(&slots[p]);
+        if (s == 0) break;
+        if ((uint32_t)s == tag) {
+          const Entry* e = ent + (s >> 32);
+          if (__ldcg(&e->x0) == x0 && __ldcg(&e->x1) == x1) {
+            const uint64_t o0 = __ldcg(&e->d0), o1 = __ldcg(&e->d1);
+            kgx_dp_event ev;
+            ev.rank = r; ev.kidx = (uint32_t)w0; ev.h = h;
+            ev.d_new[0] = d0; ev.d_new[1] = d1;
+            if (o0 == d0 && o1 == d1) {                 // ADD_DUPLICATE
+              ev.kind = KGX_DPT_EV_RESET; ev.d_old[0] = 0; ev.d_old[1] = 0;
+            } else {                                    // ADD_COLLISION: same herd -> reset (Kangaroo.cpp:258-262)
+              ev.kind = ((o1 ^ d1) & TYPE_BIT) ? KGX_DPT_EV_COLLISION : KGX_DPT_EV_RESET;
+              ev.d_old[0] = o0; ev.d_old[1] = o1;
+            }
+            evArr[i] = ev;
+            evFlag[i] = 1;
+            goto next;
+          }
+        }
+        if (++p == nslots) p = 0;
+      }
+    }
+    {                                                   // ADD_OK: a new entry
+      const ull e = atomicAdd(&res->count, 1ull);
+      ent[e] = Entry{x0, x1, d0, d1};
+      ent_h[e] = h;
+      __threadfence();                                  // the entry before the slot that publishes it
+      index_insert(slots, nslots, home, (e << 32) | tag);
+      nbv++;
+    }
+  next:;
+  }
+  nb[h] = nbv; mx[h] = mxv;
+}
+
+__global__ void k_events_out(const kgx_dp_event* evArr, const uint32_t* sel, const Res* res, uint32_t cap, kgx_dp_event* out) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < cap && t < res->nsel) out[t] = evArr[sel[t]];
+}
+
+// a load: entries [first, first + n) are already in ent / ent_h
+__global__ void k_index_entries(const Entry* ent, const uint32_t* ent_h, uint64_t first, uint64_t n, ull* slots, uint64_t nslots) {
+  const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  const uint64_t e = first + t;
+  const Entry v = ent[e];
+  const uint32_t h = ent_h[e];
+  index_insert(slots, nslots, slot_home(h, v.x0, v.x1, nslots), ((ull)e << 32) | slot_tag(h, v.x1));
+}
+
+// a save: the entries of buckets [b0, b1), in any order
+__global__ void k_save_select(const uint32_t* ent_h, uint64_t count, uint32_t b0, uint32_t b1, uint32_t* idx, uint32_t* cursor) {
+  const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= count) return;
+  const uint32_t h = ent_h[e];
+  if (h >= b0 && h < b1) idx[atomicAdd(cursor, 1u)] = (uint32_t)e;
+}
+
+__global__ void k_save_key(const Entry* ent, const uint32_t* ent_h, const uint32_t* idx, uint32_t n, int which, uint32_t b0, uint64_t* key) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  const uint32_t e = idx[t];
+  if (which == 0) key[t] = ent[e].x0;
+  else if (which == 1) key[t] = ent[e].x1;
+  else reinterpret_cast<uint32_t*>(key)[t] = ent_h[e] - b0;
+}
+
+__global__ void k_save_out(const Entry* ent, const uint32_t* idx, uint32_t n, Entry* out) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < n) out[t] = ent[idx[t]];
+}
+
+inline uint64_t slots_for(uint64_t capacity) { return capacity + capacity / 2 + 64; }
+inline uint64_t save_chunk_for(uint64_t capacity) { return capacity < SAVE_CHUNK ? (capacity ? capacity : 1) : SAVE_CHUNK; }
+
+}  // namespace kgx_dpt
+
+static char g_dpt_create_err[256] = "";
+
+struct kgx_dptable {
+  int dev = 0;
+  uint64_t capacity = 0, nslots = 0, count = 0;           // count: host mirror of res->count after the last call
+  kgx_dpt::Entry* ent = nullptr;
+  uint32_t* ent_h = nullptr;
+  kgx_dpt::ull* slots = nullptr;
+  uint32_t *nb = nullptr, *mx = nullptr;
+  kgx_dpt::Res* res = nullptr;                             // device
+  kgx_dpt::Res* resHost = nullptr;                         // pinned
+  // add scratch, grown to the largest call so far
+  uint32_t scratchN = 0, evCap = 0;
+  uint32_t *keyIn = nullptr, *keyOut = nullptr, *valIn = nullptr, *valOut = nullptr, *sel = nullptr;
+  kgx_dp_event *evArr = nullptr, *evOut = nullptr;
+  uint8_t* evFlag = nullptr;
+  void* cubTmp = nullptr;
+  size_t cubTmpBytes = 0;
+  uint64_t scratchBytes = 0;
+  // save / load scratch: chunk entries on the device, pinned on the host
+  uint64_t chunk = 0;
+  uint32_t *sIdxA = nullptr, *sIdxB = nullptr, *sCursor = nullptr;
+  uint64_t *sKeyA = nullptr, *sKeyB = nullptr;
+  kgx_dpt::Entry* sOut = nullptr;
+  void* sTmp = nullptr;
+  size_t sTmpBytes = 0;
+  kgx_dpt::Entry* hostEnt = nullptr;                       // pinned, chunk entries (allocated by the first save or load)
+  uint32_t* hostH = nullptr;
+  uint64_t bytes = 0;
+  char err[256] = "";
+};
+
+#define DPT_CK(t, call)                                                                        \
+  do {                                                                                         \
+    cudaError_t _s = (call);                                                                   \
+    if (_s != cudaSuccess) {                                                                   \
+      snprintf((t)->err, sizeof((t)->err), "%s: %s", #call, cudaGetErrorString(_s));           \
+      return -3;                                                                               \
+    }                                                                                          \
+  } while (0)
+
+static int dpt_alloc(kgx_dptable* t, void** p, size_t n) {
+  cudaError_t s = cudaMalloc(p, n ? n : 1);
+  if (s != cudaSuccess) {
+    snprintf(t->err, sizeof t->err, "cudaMalloc(%zu bytes): %s", n, cudaGetErrorString(s));
+    cudaGetLastError();
+    *p = nullptr;
+    return -3;
+  }
+  t->bytes += n;
+  return 0;
+}
+
+static void dpt_free_scratch(kgx_dptable* t) {
+  cudaFree(t->keyIn); cudaFree(t->keyOut); cudaFree(t->valIn); cudaFree(t->valOut); cudaFree(t->sel);
+  cudaFree(t->evArr); cudaFree(t->evFlag); cudaFree(t->cubTmp);
+  t->keyIn = t->keyOut = t->valIn = t->valOut = t->sel = nullptr;
+  t->evArr = nullptr; t->evFlag = nullptr; t->cubTmp = nullptr;
+  t->bytes -= t->scratchBytes;
+  t->scratchN = 0; t->cubTmpBytes = 0; t->scratchBytes = 0;
+}
+
+// grow-only per-call scratch for n records (rounded up to a power of two).  Every add ends with a synchronisation of its
+// stream, so no earlier call still reads the scratch freed here.
+static int dpt_scratch(kgx_dptable* t, uint32_t n) {
+  if (n <= t->scratchN) return 0;
+  dpt_free_scratch(t);
+  const uint64_t before = t->bytes;
+  uint32_t m = 1024;
+  while (m < n) m <<= 1;
+  size_t a = 0, b = 0;
+  DPT_CK(t, cub::DeviceRadixSort::SortPairs(nullptr, a, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)m, 0, 19));
+  DPT_CK(t, cub::DeviceSelect::Flagged(nullptr, b, (uint32_t*)nullptr, (uint8_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)m));
+  const size_t tmp = a > b ? a : b;
+  if (dpt_alloc(t, (void**)&t->keyIn, 4ull * m) || dpt_alloc(t, (void**)&t->keyOut, 4ull * m) || dpt_alloc(t, (void**)&t->valIn, 4ull * m) ||
+      dpt_alloc(t, (void**)&t->valOut, 4ull * m) || dpt_alloc(t, (void**)&t->sel, 4ull * m) ||
+      dpt_alloc(t, (void**)&t->evArr, sizeof(kgx_dp_event) * (size_t)m) || dpt_alloc(t, (void**)&t->evFlag, m) ||
+      dpt_alloc(t, &t->cubTmp, tmp)) {
+    t->scratchBytes = t->bytes - before;
+    dpt_free_scratch(t);
+    return -3;
+  }
+  t->scratchN = m; t->cubTmpBytes = tmp; t->scratchBytes = t->bytes - before;
+  return 0;
+}
+
+static int dpt_reset(kgx_dptable* t, cudaStream_t st) {
+  DPT_CK(t, cudaMemsetAsync(t->slots, 0, 8ull * t->nslots, st));
+  DPT_CK(t, cudaMemsetAsync(t->nb, 0, 4ull * kgx_dpt::NBUCKET, st));
+  DPT_CK(t, cudaMemsetAsync(t->mx, 0, 4ull * kgx_dpt::NBUCKET, st));
+  DPT_CK(t, cudaMemsetAsync(t->res, 0, sizeof(kgx_dpt::Res), st));
+  DPT_CK(t, cudaStreamSynchronize(st));
+  t->count = 0;
+  return 0;
+}
+
+static int dpt_pinned(kgx_dptable* t) {
+  if (t->hostEnt) return 0;
+  DPT_CK(t, cudaHostAlloc((void**)&t->hostEnt, sizeof(kgx_dpt::Entry) * t->chunk, cudaHostAllocDefault));
+  DPT_CK(t, cudaHostAlloc((void**)&t->hostH, 4ull * t->chunk, cudaHostAllocDefault));
+  return 0;
+}
+
+static int dpt_io_error() { return errno ? -errno : -EIO; }
+
+extern "C" {
+
+uint64_t kgx_dptable_bytes_for(uint64_t capacity) {
+  const uint64_t c = kgx_dpt::save_chunk_for(capacity);
+  return capacity * (sizeof(kgx_dpt::Entry) + 4) + 8 * kgx_dpt::slots_for(capacity) + 8ull * kgx_dpt::NBUCKET +
+         c * (4 + 4 + 8 + 8 + sizeof(kgx_dpt::Entry)) + 2 * 8 * c + (64ull << 20);   // the last two: radix-sort scratch, estimated
+}
+
+const char* kgx_dptable_last_error(kgx_dptable* t) { return t ? t->err : g_dpt_create_err; }
+
+void kgx_dptable_destroy(kgx_dptable* t) {
+  if (!t) return;
+  cudaSetDevice(t->dev);
+  cudaDeviceSynchronize();
+  cudaFree(t->ent); cudaFree(t->ent_h); cudaFree(t->slots); cudaFree(t->nb); cudaFree(t->mx); cudaFree(t->res);
+  dpt_free_scratch(t);
+  cudaFree(t->evOut);
+  cudaFree(t->sIdxA); cudaFree(t->sIdxB); cudaFree(t->sCursor); cudaFree(t->sKeyA); cudaFree(t->sKeyB); cudaFree(t->sOut); cudaFree(t->sTmp);
+  if (t->resHost) cudaFreeHost(t->resHost);
+  if (t->hostEnt) cudaFreeHost(t->hostEnt);
+  if (t->hostH) cudaFreeHost(t->hostH);
+  delete t;
+}
+
+kgx_dptable* kgx_dptable_create(int dev, uint64_t capacity) {
+  int cnt = 0;
+  cudaError_t s = cudaGetDeviceCount(&cnt);
+  if (s != cudaSuccess || cnt == 0) {
+    snprintf(g_dpt_create_err, sizeof g_dpt_create_err, "kgx_dptable_create: no CUDA device (%s)", cudaGetErrorString(s));
+    cudaGetLastError();
+    return nullptr;
+  }
+  if (capacity == 0 || capacity >= 0xFFFFFFFFull) {
+    snprintf(g_dpt_create_err, sizeof g_dpt_create_err, "kgx_dptable_create: capacity %llu is not in 1 .. 2^32-2 entries",
+             (unsigned long long)capacity);
+    return nullptr;
+  }
+  if ((s = cudaSetDevice(dev)) != cudaSuccess) {
+    snprintf(g_dpt_create_err, sizeof g_dpt_create_err, "kgx_dptable_create: cudaSetDevice(%d): %s", dev, cudaGetErrorString(s));
+    cudaGetLastError();
+    return nullptr;
+  }
+  kgx_dptable* t = new kgx_dptable();
+  t->dev = dev; t->capacity = capacity; t->nslots = kgx_dpt::slots_for(capacity);
+  t->chunk = kgx_dpt::save_chunk_for(capacity);
+  const uint64_t c = t->chunk;
+  size_t tmpA = 0, tmpB = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, tmpA, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)c, 0, 64);
+  cub::DeviceRadixSort::SortPairs(nullptr, tmpB, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)c, 0, 19);
+  t->sTmpBytes = tmpA > tmpB ? tmpA : tmpB;
+  bool ok = !dpt_alloc(t, (void**)&t->ent, sizeof(kgx_dpt::Entry) * capacity) && !dpt_alloc(t, (void**)&t->ent_h, 4ull * capacity) &&
+            !dpt_alloc(t, (void**)&t->slots, 8ull * t->nslots) && !dpt_alloc(t, (void**)&t->nb, 4ull * kgx_dpt::NBUCKET) &&
+            !dpt_alloc(t, (void**)&t->mx, 4ull * kgx_dpt::NBUCKET) && !dpt_alloc(t, (void**)&t->res, sizeof(kgx_dpt::Res)) &&
+            !dpt_alloc(t, (void**)&t->sIdxA, 4ull * c) && !dpt_alloc(t, (void**)&t->sIdxB, 4ull * c) &&
+            !dpt_alloc(t, (void**)&t->sCursor, 4) && !dpt_alloc(t, (void**)&t->sKeyA, 8ull * c) &&
+            !dpt_alloc(t, (void**)&t->sKeyB, 8ull * c) && !dpt_alloc(t, (void**)&t->sOut, sizeof(kgx_dpt::Entry) * c) &&
+            !dpt_alloc(t, &t->sTmp, t->sTmpBytes);
+  if (ok && cudaHostAlloc((void**)&t->resHost, sizeof(kgx_dpt::Res), cudaHostAllocDefault) != cudaSuccess) {
+    snprintf(t->err, sizeof t->err, "cudaHostAlloc failed");
+    ok = false;
+  }
+  if (ok) ok = dpt_reset(t, 0) == 0;
+  if (!ok) {
+    snprintf(g_dpt_create_err, sizeof g_dpt_create_err, "kgx_dptable_create(%llu entries, %.2f GB): %.180s",
+             (unsigned long long)capacity, kgx_dptable_bytes_for(capacity) / 1e9, t->err);
+    cudaGetLastError();
+    kgx_dptable_destroy(t);
+    return nullptr;
+  }
+  return t;
+}
+
+uint64_t kgx_dptable_count(kgx_dptable* t) { return t->count; }
+uint64_t kgx_dptable_capacity(kgx_dptable* t) { return t->capacity; }
+uint64_t kgx_dptable_memory_bytes(kgx_dptable* t) { return t->bytes + (t->evOut ? sizeof(kgx_dp_event) * (uint64_t)t->evCap : 0); }
+
+static int dpt_events(kgx_dptable* t, uint32_t cap) {
+  if (cap <= t->evCap) return 0;
+  cudaFree(t->evOut);
+  t->evOut = nullptr; t->evCap = 0;
+  DPT_CK(t, cudaMalloc((void**)&t->evOut, sizeof(kgx_dp_event) * (size_t)cap));
+  t->evCap = cap;
+  return 0;
+}
+
+int kgx_dptable_reserve(kgx_dptable* t, uint32_t n_records, uint32_t cap) {
+  DPT_CK(t, cudaSetDevice(t->dev));
+  if (n_records >= 0x80000000u) {
+    snprintf(t->err, sizeof t->err, "kgx_dptable_reserve: %u records (at most 2^31-1)", n_records);
+    return -3;
+  }
+  if (n_records && dpt_scratch(t, n_records)) return -3;
+  return dpt_events(t, cap);
+}
+
+int kgx_dptable_add(kgx_dptable* t, const void* recs, const uint32_t* counts, uint32_t n_ranks, uint64_t stride, kgx_dp_event* ev,
+                    uint32_t cap, uint32_t* n_ev, void* stream) {
+  using namespace kgx_dpt;
+  *n_ev = 0;
+  if (n_ranks == 0 || n_ranks > KGX_DPT_MAX_RANKS) {
+    snprintf(t->err, sizeof t->err, "kgx_dptable_add: %u ranks (1 .. %d)", n_ranks, KGX_DPT_MAX_RANKS);
+    return -3;
+  }
+  Ranks R;
+  R.n = n_ranks;
+  uint64_t n64 = 0;
+  for (uint32_t r = 0; r < n_ranks; r++) {
+    if (counts[r] > stride && n_ranks > 1) {
+      snprintf(t->err, sizeof t->err, "kgx_dptable_add: rank %u has %u records, more than the stride %llu", r, counts[r], (unsigned long long)stride);
+      return -3;
+    }
+    R.pre[r] = (uint32_t)n64;
+    n64 += counts[r];
+  }
+  R.pre[n_ranks] = (uint32_t)n64;
+  if (n64 >= 0x80000000ull) {
+    snprintf(t->err, sizeof t->err, "kgx_dptable_add: %llu records in one call (at most 2^31-1)", (unsigned long long)n64);
+    return -3;
+  }
+  if (t->count + n64 > t->capacity) {                      // checked before anything runs: a full table changes nothing
+    snprintf(t->err, sizeof t->err, "DP table full: %llu entries + %llu records of this call > capacity %llu",
+             (unsigned long long)t->count, (unsigned long long)n64, (unsigned long long)t->capacity);
+    return -2;
+  }
+  const uint32_t n = (uint32_t)n64;
+  if (n == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  DPT_CK(t, cudaSetDevice(t->dev));
+  if (dpt_scratch(t, n)) return -3;
+  if (dpt_events(t, cap)) return -3;
+  const uint8_t* rp = static_cast<const uint8_t*>(recs);
+  DPT_CK(t, cudaMemsetAsync(&t->res->nsel, 0, 8, st));
+  const uint32_t B = 256, G = (n + B - 1) / B;
+  k_keys<<<G, B, 0, st>>>(rp, stride, R, n, t->keyIn, t->valIn, t->evFlag, t->res);
+  DPT_CK(t, cudaGetLastError());
+  size_t tb = t->cubTmpBytes;
+  DPT_CK(t, cub::DeviceRadixSort::SortPairs(t->cubTmp, tb, t->keyIn, t->keyOut, t->valIn, t->valOut, (int)n, 0, 19, st));
+  k_insert<<<G, B, 0, st>>>(t->keyOut, t->valOut, n, rp, stride, R, t->ent, t->ent_h, t->slots, t->nslots, t->nb, t->mx, t->res,
+                            t->evArr, t->evFlag);
+  DPT_CK(t, cudaGetLastError());
+  tb = t->cubTmpBytes;
+  DPT_CK(t, cub::DeviceSelect::Flagged(t->cubTmp, tb, t->valIn, t->evFlag, t->sel, &t->res->nsel, (int)n, st));
+  const uint32_t nout = cap < n ? cap : n;
+  if (nout) {
+    k_events_out<<<(nout + B - 1) / B, B, 0, st>>>(t->evArr, t->sel, t->res, cap, t->evOut);
+    DPT_CK(t, cudaGetLastError());
+  }
+  DPT_CK(t, cudaMemcpyAsync(t->resHost, t->res, sizeof(Res), cudaMemcpyDeviceToHost, st));
+  DPT_CK(t, cudaStreamSynchronize(st));
+  t->count = t->resHost->count;
+  *n_ev = t->resHost->nsel;
+  const uint32_t ncopy = *n_ev < cap ? *n_ev : cap;
+  if (ncopy) {
+    DPT_CK(t, cudaMemcpyAsync(ev, t->evOut, sizeof(kgx_dp_event) * (size_t)ncopy, cudaMemcpyDeviceToHost, st));
+    DPT_CK(t, cudaStreamSynchronize(st));
+  }
+  return t->resHost->bad ? -1 : 0;
+}
+
+int kgx_dptable_save_work(kgx_dptable* t, const char* path, uint32_t dp_bits, const uint64_t range_start[4], const uint64_t range_end[4],
+                          const uint64_t keyx[4], const uint64_t keyy[4], uint64_t total_count, double total_time, uint64_t total_walk,
+                          void* stream) {
+  using namespace kgx_dpt;
+  cudaStream_t st = (cudaStream_t)stream;
+  DPT_CK(t, cudaSetDevice(t->dev));
+  DPT_CK(t, cudaStreamSynchronize(st));                    // every add queued on this stream is in the table
+  if (dpt_pinned(t)) return -3;
+  uint32_t* nbH = (uint32_t*)malloc(8ull * NBUCKET);
+  if (!nbH) { snprintf(t->err, sizeof t->err, "out of host memory"); return -ENOMEM; }
+  uint32_t* mxH = nbH + NBUCKET;
+  if (cudaMemcpy(nbH, t->nb, 4ull * NBUCKET, cudaMemcpyDeviceToHost) != cudaSuccess ||
+      cudaMemcpy(mxH, t->mx, 4ull * NBUCKET, cudaMemcpyDeviceToHost) != cudaSuccess) {
+    free(nbH);
+    snprintf(t->err, sizeof t->err, "kgx_dptable_save_work: bucket counters: %s", cudaGetErrorString(cudaGetLastError()));
+    return -3;
+  }
+  errno = 0;
+  FILE* f = fopen(path, "wb");
+  if (!f) { const int e = dpt_io_error(); free(nbH); snprintf(t->err, sizeof t->err, "%s: %s", path, strerror(-e)); return e; }
+  setvbuf(f, nullptr, _IOFBF, 1 << 22);
+  // Kangaroo::SaveHeader (Backup.cpp:368-394), type HEADW -- the header kgi_save_work_ex writes
+  const uint32_t head = HEADW, version = 0;
+  bool ok = fwrite(&head, 4, 1, f) == 1 && fwrite(&version, 4, 1, f) == 1 && fwrite(&dp_bits, 4, 1, f) == 1 &&
+            fwrite(range_start, 32, 1, f) == 1 && fwrite(range_end, 32, 1, f) == 1 && fwrite(keyx, 32, 1, f) == 1 &&
+            fwrite(keyy, 32, 1, f) == 1 && fwrite(&total_count, 8, 1, f) == 1 && fwrite(&total_time, 8, 1, f) == 1;
+  int rc = 0;
+  // HashTable::SaveTable (HashTable.cpp:375-396) in chunks of whole buckets: select, sort by (h, x.hi, x.lo), copy out
+  uint32_t b0 = 0;
+  while (ok && rc == 0 && b0 < NBUCKET) {
+    uint64_t m = 0;
+    uint32_t b1 = b0;
+    while (b1 < NBUCKET && (m + nbH[b1] <= t->chunk || b1 == b0)) m += nbH[b1++];
+    if (m > t->chunk) {                                   // one bucket larger than a chunk
+      snprintf(t->err, sizeof t->err, "kgx_dptable_save_work: bucket %u holds %llu entries, more than a save chunk (%llu)", b0,
+               (unsigned long long)m, (unsigned long long)t->chunk);
+      rc = -3;
+      break;
+    }
+    if (m) {
+      const uint32_t n = (uint32_t)m, B = 256, G = (n + B - 1) / B;
+      size_t tb = t->sTmpBytes;
+      int bits = 1;
+      while ((1u << bits) < b1 - b0) bits++;
+      bool good = cudaMemsetAsync(t->sCursor, 0, 4, st) == cudaSuccess;
+      k_save_select<<<(unsigned)((t->count + B - 1) / B), B, 0, st>>>(t->ent_h, t->count, b0, b1, t->sIdxA, t->sCursor);
+      k_save_key<<<G, B, 0, st>>>(t->ent, t->ent_h, t->sIdxA, n, 0, b0, t->sKeyA);
+      good = good && cub::DeviceRadixSort::SortPairs(t->sTmp, tb, t->sKeyA, t->sKeyB, t->sIdxA, t->sIdxB, (int)n, 0, 64, st) == cudaSuccess;
+      k_save_key<<<G, B, 0, st>>>(t->ent, t->ent_h, t->sIdxB, n, 1, b0, t->sKeyA);
+      good = good && cub::DeviceRadixSort::SortPairs(t->sTmp, tb, t->sKeyA, t->sKeyB, t->sIdxB, t->sIdxA, (int)n, 0, 64, st) == cudaSuccess;
+      k_save_key<<<G, B, 0, st>>>(t->ent, t->ent_h, t->sIdxA, n, 2, b0, t->sKeyA);
+      good = good && cub::DeviceRadixSort::SortPairs(t->sTmp, tb, (uint32_t*)t->sKeyA, (uint32_t*)t->sKeyB, t->sIdxA, t->sIdxB, (int)n, 0,
+                                                     bits, st) == cudaSuccess;
+      k_save_out<<<G, B, 0, st>>>(t->ent, t->sIdxB, n, t->sOut);
+      good = good && cudaMemcpyAsync(t->hostEnt, t->sOut, sizeof(Entry) * m, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+             cudaStreamSynchronize(st) == cudaSuccess;
+      if (!good) {
+        snprintf(t->err, sizeof t->err, "kgx_dptable_save_work: %s", cudaGetErrorString(cudaGetLastError()));
+        rc = -3;
+        break;
+      }
+    }
+    uint64_t off = 0;
+    for (uint32_t b = b0; ok && b < b1; b++) {
+      ok = fwrite(&nbH[b], 4, 1, f) == 1 && fwrite(&mxH[b], 4, 1, f) == 1 &&
+           (nbH[b] == 0 || fwrite(t->hostEnt + off, sizeof(Entry), nbH[b], f) == nbH[b]);
+      off += nbH[b];
+    }
+    b0 = b1;
+  }
+  free(nbH);
+  ok = ok && fwrite(&total_walk, 8, 1, f) == 1;           // Backup.cpp:530-531 / 549-551
+  ok = fflush(f) == 0 && ok;
+  int err = rc ? rc : (ok ? 0 : dpt_io_error());
+  if (fclose(f) != 0 && err == 0) err = dpt_io_error();
+  if (err < 0 && err != -3) snprintf(t->err, sizeof t->err, "%s: %s", path, strerror(-err));
+  return err;
+}
+
+int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, uint64_t range_start[4], uint64_t range_end[4],
+                          uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time, uint64_t* nb_walk,
+                          uint64_t* walk_offset, void* stream) {
+  using namespace kgx_dpt;
+  cudaStream_t st = (cudaStream_t)stream;
+  DPT_CK(t, cudaSetDevice(t->dev));
+  DPT_CK(t, cudaStreamSynchronize(st));
+  if (dpt_reset(t, st)) return -3;                         // HashTable::LoadTable starts with Reset()
+  if (dpt_pinned(t)) return -3;
+  errno = 0;
+  FILE* f = fopen(path, "rb");
+  if (!f) { const int e = dpt_io_error(); snprintf(t->err, sizeof t->err, "%s: %s", path, strerror(-e)); return e; }
+  setvbuf(f, nullptr, _IOFBF, 1 << 22);
+  // Kangaroo::LoadWork (Backup.cpp:149-207)
+  uint32_t head = 0, version = 0, dp = 0;
+  uint64_t hdr[16], cnt = 0, walk = 0;
+  double tm = 0;
+  bool ok = fread(&head, 4, 1, f) == 1 && fread(&version, 4, 1, f) == 1 && head == HEADW;
+  ok = ok && fread(&dp, 4, 1, f) == 1 && fread(hdr, 32, 4, f) == 4 && fread(&cnt, 8, 1, f) == 1 && fread(&tm, 8, 1, f) == 1;
+  uint32_t* nbH = (uint32_t*)malloc(8ull * NBUCKET);
+  if (!nbH) { fclose(f); snprintf(t->err, sizeof t->err, "out of host memory"); return -ENOMEM; }
+  uint32_t* mxH = nbH + NBUCKET;
+  int rc = 0;
+  uint64_t staged = 0, total = 0;
+  auto flush = [&]() -> bool {                            // staged entries -> ent[count ..], then into the index
+    if (!staged) return true;
+    if (t->count + staged > t->capacity) {
+      rc = -ENOSPC;
+      return false;
+    }
+    const uint64_t B = 256;
+    bool good = cudaMemcpyAsync(t->ent + t->count, t->hostEnt, sizeof(Entry) * staged, cudaMemcpyHostToDevice, st) == cudaSuccess &&
+                cudaMemcpyAsync(t->ent_h + t->count, t->hostH, 4 * staged, cudaMemcpyHostToDevice, st) == cudaSuccess;
+    if (good) k_index_entries<<<(unsigned)((staged + B - 1) / B), (unsigned)B, 0, st>>>(t->ent, t->ent_h, t->count, staged, t->slots, t->nslots);
+    good = good && cudaStreamSynchronize(st) == cudaSuccess;    // the pinned buffers are refilled next
+    if (!good) { rc = -3; snprintf(t->err, sizeof t->err, "kgx_dptable_load_work: %s", cudaGetErrorString(cudaGetLastError())); return false; }
+    t->count += staged;
+    staged = 0;
+    return true;
+  };
+  for (uint32_t h = 0; ok && h < NBUCKET; h++) {           // HashTable::LoadTable (HashTable.cpp:439-459)
+    ok = fread(&nbH[h], 4, 1, f) == 1 && fread(&mxH[h], 4, 1, f) == 1;
+    uint32_t left = ok ? nbH[h] : 0;
+    total += left;
+    if (ok && total > t->capacity) { rc = -ENOSPC; ok = false; break; }
+    while (ok && left) {
+      if (staged == t->chunk && !flush()) { ok = false; break; }
+      const uint32_t k = (uint32_t)std::min<uint64_t>(left, t->chunk - staged);
+      ok = fread(t->hostEnt + staged, sizeof(Entry), k, f) == k;
+      for (uint32_t q = 0; q < k; q++) t->hostH[staged + q] = h;
+      staged += k;
+      left -= k;
+    }
+  }
+  ok = ok && flush();
+  ok = ok && fread(&walk, 8, 1, f) == 1;
+  long off = ok ? ftell(f) : -1;
+  if (ok && walk) {                                       // the kangaroo block must be all there (FetchWalks, Backup.cpp:211-223)
+    ok = off >= 0 && fseek(f, 0, SEEK_END) == 0;
+    const long end = ok ? ftell(f) : -1;
+    ok = ok && end >= off && (uint64_t)(end - off) / 96 >= walk;
+  }
+  fclose(f);
+  if (ok) {
+    ok = cudaMemcpy(t->nb, nbH, 4ull * NBUCKET, cudaMemcpyHostToDevice) == cudaSuccess &&
+         cudaMemcpy(t->mx, mxH, 4ull * NBUCKET, cudaMemcpyHostToDevice) == cudaSuccess;
+    const ull c = t->count;
+    ok = ok && cudaMemcpy(&t->res->count, &c, 8, cudaMemcpyHostToDevice) == cudaSuccess;
+    if (!ok) rc = -3;
+  }
+  free(nbH);
+  if (!ok) {
+    if (rc == -ENOSPC)
+      snprintf(t->err, sizeof t->err, "%s holds more than the table's capacity of %llu entries", path, (unsigned long long)t->capacity);
+    else if (rc == 0)
+      snprintf(t->err, sizeof t->err, "%s is not a complete HEADW work file", path);
+    dpt_reset(t, st);
+    return rc ? rc : -EINVAL;
+  }
+  if (dp_bits) *dp_bits = dp;
+  if (range_start) memcpy(range_start, hdr, 32);
+  if (range_end) memcpy(range_end, hdr + 4, 32);
+  if (keyx) memcpy(keyx, hdr + 8, 32);
+  if (keyy) memcpy(keyy, hdr + 12, 32);
+  if (total_count) *total_count = cnt;
+  if (total_time) *total_time = tm;
+  if (nb_walk) *nb_walk = walk;
+  if (walk_offset) *walk_offset = (uint64_t)off;
+  return 0;
+}
+
+}  // extern "C"

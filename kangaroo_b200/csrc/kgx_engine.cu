@@ -784,3 +784,5 @@ int kgx_bench_raw(int dev, int kind, int iters, float* ms, double* ops) {
 }
 
 }  // extern "C"
+
+#include "kgx_dptable.cuh"   // the device-resident DP table (kgx_dptable_*)

@@ -185,6 +185,124 @@ class DPTable:
         return WorkInfo(path, dp.value, val(rs), val(re_), (val(kx), val(ky)), cnt.value, tm.value, walk.value, off.value)
 
 
+class TableFull(RuntimeError):
+    """An add that would take a DeviceDPTable past its capacity: nothing of it was inserted."""
+
+
+class DeviceDPTable:
+    """The rank-0 DP table in the memory of one GPU (libkgx.so, kgx_dptable_*): DPTable's add / __len__ / save_work /
+    load_work_ex with exactly its results for the same records in the same order, inserted by CUDA kernels straight from device
+    memory.  Its capacity (entries) is fixed at creation; an add that could pass it raises TableFull and changes nothing.
+    resolve / resolve_multi are the host table's (kgi_resolve: the reference's CheckKey), on a DPTable that holds no entry."""
+
+    def __init__(self, capacity, device=None, max_events=4096):
+        from ._lib import load_library as load_engine
+        self._lib = load_engine()
+        self.device = int(device if device is not None else 0)
+        self._h = ctypes.c_void_p(self._lib.kgx_dptable_create(self.device, int(capacity)))
+        if not self._h:
+            raise RuntimeError(self._lib.kgx_dptable_last_error(None).decode())
+        self.capacity = int(capacity)
+        self._ev = (Event * max_events)()
+        self._cap = max_events
+        self.threads = 0                     # no host workers
+        self._resolver = None
+
+    @staticmethod
+    def bytes_for(capacity):
+        from ._lib import load_library as load_engine
+        return int(load_engine().kgx_dptable_bytes_for(int(capacity)))
+
+    def close(self):
+        if self._h:
+            self._lib.kgx_dptable_destroy(self._h)
+            self._h = None
+        if self._resolver is not None:
+            self._resolver.close()
+            self._resolver = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __len__(self):
+        return int(self._lib.kgx_dptable_count(self._h))
+
+    def memory_bytes(self):
+        return int(self._lib.kgx_dptable_memory_bytes(self._h))
+
+    def _err(self):
+        return self._lib.kgx_dptable_last_error(self._h).decode()
+
+    def reserve(self, n_records):
+        """allocate now the scratch of adds of up to n_records records (adds otherwise grow it on demand)"""
+        if self._lib.kgx_dptable_reserve(self._h, int(n_records), self._cap) != 0:
+            raise RuntimeError("kgx_dptable_reserve: " + self._err())
+
+    def add_raw(self, ptr, counts, stride, stream=0):
+        """counts[r] records of rank r at device address ptr + r*stride*40 -> (return code, total events, Event array of the
+        first min(total, max_events)).  Raises TableFull (-2) and RuntimeError on a CUDA error (-3); -1 = malformed records
+        skipped."""
+        counts = [int(c) for c in counts]
+        cnt = (ctypes.c_uint32 * len(counts))(*counts)
+        ne = ctypes.c_uint32(0)
+        rc = self._lib.kgx_dptable_add(self._h, ctypes.c_void_p(int(ptr)), cnt, len(counts), int(stride),
+                                       ctypes.cast(self._ev, ctypes.c_void_p), self._cap, ctypes.byref(ne), ctypes.c_void_p(int(stream)))
+        if rc == -2:
+            raise TableFull(self._err())
+        if rc < -1:
+            raise RuntimeError("kgx_dptable_add: " + self._err())
+        return rc, ne.value, self._ev
+
+    def add(self, ptr, counts, stride, stream=0):
+        """every rank's records of one step (device memory) -> list of (kind, rank, kidx, d_old, d_new) events"""
+        rc, n, _ = self.add_raw(ptr, counts, stride, stream)
+        if rc != 0:
+            raise RuntimeError("kgx_dptable_add: malformed DP record (h >= 2^18)")
+        return DPTable._events(self, n)
+
+    def add_dp40(self, buf, rank=0, stream=0):
+        """DPTable.add_dp40 for records in device memory: buf = a CUDA uint8 tensor of n x 40 bytes"""
+        assert buf.is_cuda and buf.numel() % DP40_BYTES == 0
+        n = buf.numel() // DP40_BYTES
+        counts = [0] * rank + [n]
+        return self.add(buf.data_ptr() - rank * n * DP40_BYTES, counts, n, stream) if n else []
+
+    def save_work(self, path, dp_bits, range_start, range_end, pubkey, total_count=0, total_time=0.0, total_walk=0, stream=0):
+        rc = self._lib.kgx_dptable_save_work(self._h, os.fsencode(path), int(dp_bits), _limbs4(range_start), _limbs4(range_end),
+                                             _limbs4(pubkey[0]), _limbs4(pubkey[1]), int(total_count), float(total_time), int(total_walk),
+                                             ctypes.c_void_p(int(stream)))
+        if rc != 0:
+            raise RuntimeError("kgx_dptable_save_work: cannot write %s: %s" % (path, self._err()))
+
+    def load_work_ex(self, path, stream=0):
+        """DPTable.load_work_ex into the device table; a file of more entries than the capacity raises TableFull"""
+        dp, cnt, tm = ctypes.c_uint32(0), ctypes.c_uint64(0), ctypes.c_double(0)
+        rs, re_, kx, ky = (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)()
+        walk, off = ctypes.c_uint64(0), ctypes.c_uint64(0)
+        rc = self._lib.kgx_dptable_load_work(self._h, os.fsencode(path), ctypes.byref(dp), rs, re_, kx, ky, ctypes.byref(cnt),
+                                             ctypes.byref(tm), ctypes.byref(walk), ctypes.byref(off), ctypes.c_void_p(int(stream)))
+        if rc == -28:                                            # -ENOSPC
+            raise TableFull(self._err())
+        if rc != 0:
+            raise RuntimeError("kgx_dptable_load_work: %s" % self._err())
+        val = lambda a: sum(int(a[k]) << (64 * k) for k in range(4))
+        return WorkInfo(path, dp.value, val(rs), val(re_), (val(kx), val(ky)), cnt.value, tm.value, walk.value, off.value)
+
+    def _host(self):
+        if self._resolver is None:
+            self._resolver = DPTable(threads=1)
+        return self._resolver
+
+    def resolve(self, d_old, d_new, key, range_start):
+        return self._host().resolve(d_old, d_new, key, range_start)
+
+    def resolve_multi(self, d_old, d_new, keys, range_start):
+        return self._host().resolve_multi(d_old, d_new, keys, range_start)
+
+
 def read_work_header(path):
     """The fixed 156-byte HEADW header (Backup.cpp:368-394) without the table -> (dp_bits, range_start, range_end,
     (key x, key y), total_count, total_time).  Needs no library."""

@@ -15,6 +15,10 @@ Per step (= one GPUEngine::Launch on every rank) nothing on the data path is Pyt
                                              (Kangaroo.cpp:601-609: CreateHerd(1) + SetKangaroo)
   all ranks   one small broadcast: [stop, n_resets, (rank, kIdx) ...]
 
+With --dp-table device, rank 0's table is ingest.DeviceDPTable in its GPU's memory (same events and work files): the step's
+records are copied device to device into a staging buffer and inserted from there by the ingest thread on its own stream, no
+host copy of them.  Its capacity is fixed; a full table stops the run (with --save-work, after writing the table it holds).
+
   single GPU :  python -m kangaroo_b200.solver in.txt --dp 12
   N GPUs     :  torchrun --nproc-per-node N -m kangaroo_b200.solver in.txt --dp 12
 
@@ -42,7 +46,7 @@ import numpy as np
 from . import ecmath as ec
 from .engine import GPUEngine, NB_JUMP, NB_RUN, WILD, random_herd_arrays
 from .dist import DPGather, HerdGather, SlabView, DP40_BYTES, WALK_BYTES
-from .ingest import DPTable, EV_RESET, EV_COLLISION
+from .ingest import DPTable, DeviceDPTable, TableFull, EV_RESET, EV_COLLISION
 
 ORDER = ec.N
 MAX_RESETS = 255          # per step, carried in the control broadcast
@@ -51,6 +55,33 @@ MAX_SOLVED = 64           # --batch-keys: keys one step's control broadcast anno
 SAVE_CHUNK = 1 << 18      # kangaroos per gather chunk of a save (24 MB buffer)
 SAVE_CHUNKS_PER_STEP = 1  # chunks a step moves while a save is in progress (default herd: 17 steps)
 SAVE_BUFFERS = 4          # rank 0's pinned chunk buffers queued to the writer
+DP_TABLE_MARGIN = 4 << 30 # --dp-table device without a capacity: rank 0's free GPU memory after the engine, its staging
+                          # buffers and the table's reserved per-add scratch, less this margin for NCCL, the gather buffer
+                          # and torch's allocator.  Nothing else grows on the GPU: steps queued behind a save wait in host RAM
+
+
+class DeviceBatch:
+    """one step's records of every rank for the device table: a device buffer, rank r's counts[r] records at r*stride*40"""
+
+    def __init__(self, buf, counts, stride, event, jumps_before):
+        self.buf, self.counts, self.stride, self.event, self.jumps_before = buf, counts, stride, event, jumps_before
+
+
+def scratch_bytes(n_records):
+    """GPU memory of the device table's per-add scratch for adds of up to n_records records (kgx_dptable_reserve), rounded up"""
+    m = 1024
+    while m < n_records:
+        m <<= 1
+    return m * 80 + (16 << 20)
+
+
+def default_table_capacity(free_bytes, margin=DP_TABLE_MARGIN):
+    """the largest capacity whose device table fits in free_bytes - margin"""
+    room = free_bytes - margin
+    cap = max(room // 48, 0)
+    while cap > 0 and DeviceDPTable.bytes_for(cap) > room:
+        cap = cap * 63 // 64
+    return int(min(cap, (1 << 32) - 2))
 
 
 def create_jump_table(range_power):
@@ -82,7 +113,7 @@ def dp_mask(bits):
 
 class Solver:
     def __init__(self, start, end, pub, dp_bits, grid=None, max_found=1 << 17, seed=None, ingest_threads=0,
-                 save_work="", save_interval=0.0, save_kangaroos=False, resume=None):
+                 save_work="", save_interval=0.0, save_kangaroos=False, resume=None, dp_table="host", dp_table_capacity=None):
         import torch
         self.torch = torch
         self.rank = int(os.environ.get("RANK", "0"))
@@ -112,12 +143,32 @@ class Solver:
         sc, d128 = random_herd_arrays(n, self.range_power, self.wdiv2, self.rng)
         self._create_herd(sc, d128)
         self.gather = DPGather(self.eng, self.dist, self.rank, self.world, torch, wire="dp40") if self.world > 1 else None
-        self.dps = DPTable(threads=ingest_threads) if self.rank == 0 else None      # rank 0: the reference HashTable
-        # Two pinned staging buffers: while the ingest thread inserts step k's records, step k+1's land in the other one.  The
-        # NCCL kernels of a step cannot start before the jump launch that occupies every SM has finished, so without this
-        # decoupling the CPU insert would sit exposed between two launches.
-        self._hosts = ([torch.empty(self.world * max_found * DP40_BYTES, dtype=torch.uint8).pin_memory() for _ in range(2)]
-                       if self.rank == 0 else None)
+        self.dev_table = dp_table == "device"
+        self.table_label = "device table" if self.dev_table else "ingest"
+        # rank 0's table stopped taking records: "full" (TableFull) or "error" (any other failure of an insert), with its message
+        self.table_msg, self.table_kind, self.table_stopped = None, None, False
+        self.last_saved = None              # rank 0: path of the last save that succeeded
+        self.parked = 0                     # rank 0, device table: steps whose records waited in host RAM behind a save
+        if self.rank == 0 and self.dev_table:
+            # rank 0: the table in this GPU's memory, fed from device buffers on a stream of the ingest thread's own.  Two staging
+            # buffers (below) and one for records parked in host RAM during a save (_add_device) are all the GPU memory the
+            # records take; the table's per-add scratch is reserved up front, so the table needs no allocation while it runs.
+            nbuf = self.world * max_found * DP40_BYTES
+            self._hosts = [torch.empty(nbuf, dtype=torch.uint8, device=torch.device("cuda", self.local)) for _ in range(3)]
+            self._back = self._hosts.pop()
+            if not dp_table_capacity:
+                dp_table_capacity = default_table_capacity(torch.cuda.mem_get_info(self.local)[0] - scratch_bytes(self.world * max_found))
+            self.dps = DeviceDPTable(dp_table_capacity, device=self.local)
+            self.dps.reserve(self.world * max_found)
+            self._istream = torch.cuda.Stream(device=self.local)
+        else:
+            self.dps = DPTable(threads=ingest_threads) if self.rank == 0 else None      # rank 0: the reference HashTable
+        # Two pinned staging buffers (device buffers for the device table): while the ingest thread inserts step k's records,
+        # step k+1's land in the other one.  The NCCL kernels of a step cannot start before the jump launch that occupies every
+        # SM has finished, so without this decoupling the insert would sit exposed between two launches.
+        if not (self.rank == 0 and self.dev_table):
+            self._hosts = ([torch.empty(self.world * max_found * DP40_BYTES, dtype=torch.uint8).pin_memory() for _ in range(2)]
+                           if self.rank == 0 else None)
         self._hidx = 0
         self._work = queue.Queue()
         self._done = queue.Queue()
@@ -234,9 +285,13 @@ class Solver:
         if kind == "begin":
             path, count, total_time, nwalk, self._wt0 = job[1:]
             self._wpath, self._wtmp, self._werr, self._wf = path, path + ".tmp", None, None
+            if self.table_msg is not None and not self._full_save:
+                self._werr = "the DP table lacks DPs of the launches this file would count (%s)" % self.table_msg
+                return
+            kw = dict(stream=self._istream.cuda_stream) if self.dev_table else {}
             try:
                 self.dps.save_work(self._wtmp, self.dp_bits, self.start, self.end, self.pub, total_count=count,
-                                   total_time=total_time, total_walk=nwalk)
+                                   total_time=total_time, total_walk=nwalk, **kw)
                 self._wf = open(self._wtmp, "ab")
             except (OSError, RuntimeError) as e:
                 self._werr = str(e)
@@ -276,7 +331,7 @@ class Solver:
                     pass
             res = (self._wpath, size / 1048576.0, time.perf_counter() - self._wt0, self._werr)
             self._on_saved(*res)
-            self._saved.put(res)
+            self._saved.put(res + (not self._full_save,))   # the full-table save was not scheduled by the main thread
 
     def _on_saved(self, path, mb, seconds, err):
         """ingest thread, right after a save finished (or failed)"""
@@ -284,34 +339,73 @@ class Solver:
     def _report_saves(self, block_for=0):
         """rank 0: log the saves finished so far; block_for = saves still to wait for"""
         while block_for > 0 or not self._saved.empty():
-            path, mb, secs, err = self._saved.get()
-            block_for -= 1
-            st = self._save_stats.pop(0) if self._save_stats else []
+            path, mb, secs, err, scheduled = self._saved.get()
+            st = []
+            if scheduled:                                  # a save _save_start began: its step times
+                block_for -= 1
+                st = self._save_stats.pop(0) if self._save_stats else []
             if err is not None:
                 self.save_error = err
                 print("SaveWork %s failed: %s (the previous file is kept)" % (path, err), flush=True)
                 continue
             self.saves.append((mb, secs))
+            self.last_saved = path
             print("SaveWork %s: %.1f MB in %.2f s, written beside %d steps; longest of them %.1f ms (median step %.1f ms)" %
                   (path, mb, secs, len(st), 1e3 * max(st or [0]), 1e3 * float(np.median(self._step_times[-64:] or [0]))), flush=True)
 
     # -- rank 0: ingest -------------------------------------------------------------------------------------------
+    def _events_of(self, segments):
+        """the table's events for one step's records: segments is a list of (rank, uint8 numpy view of that rank's 40-byte
+        records) for the host table, a DeviceBatch for the device table"""
+        if isinstance(segments, DeviceBatch):
+            return self._add_device(segments)
+        return (ev for r, buf in segments if buf.size != 0 for ev in self.dps.add_dp40(buf, r))
+
+    def _add_device(self, b):
+        if self.table_msg is not None:                  # the run is stopping: later steps' DPs are not inserted
+            return []
+        if b.event is None:                             # parked in host RAM behind a save: back to the GPU, on this stream
+            with self.torch.cuda.stream(self._istream):
+                self._back[:b.buf.numel()].copy_(b.buf)
+            buf = self._back
+        else:
+            self._istream.wait_event(b.event)           # the records' copy into the staging buffer
+            buf = b.buf
+        try:
+            return self.dps.add(buf.data_ptr(), b.counts, b.stride, self._istream.cuda_stream)
+        except TableFull as e:
+            self._on_full(str(e), b.jumps_before)
+            return []
+
+    _full_save = False
+
+    def _on_full(self, msg, jumps_before):
+        """ingest thread: the table cannot take this step's records.  With --save-work, and no save open, the table is written
+        at once as the cut it is: the launches before this one, without kangaroos (their state of that cut is gone)."""
+        self.table_msg, self.table_kind = msg, "full"
+        if self.save_path and getattr(self, "_wf", None) is None:
+            self._full_save = True
+            self._write(("begin", self.save_path, jumps_before, self.time_offset + time.time() - self.t_start, 0, time.perf_counter()))
+            self._write(("end",))
+            self._full_save = False
+            self.full_saved = (self.save_path, jumps_before, getattr(self, "_werr", None))
+
     def _ingest(self, segments):
-        """segments: list of (rank, uint8 numpy view of that rank's 40-byte records).  Returns (key or None, resets)."""
+        """segments: see _events_of.  Returns (key or None, resets)."""
         found, resets = None, []
         t0 = time.perf_counter()
-        for r, buf in segments:
-            if buf.size == 0:
-                continue
-            for kind, rk, kidx, d_old, d_new in self.dps.add_dp40(buf, r):
-                if kind == EV_COLLISION and found is None:
-                    found = self.dps.resolve(d_old, d_new, self.key, self.start)     # Kangaroo.cpp:255-302
-                    if found is None:
-                        resets.append((rk, kidx))                                    # "unexpected wrong collision, reset kangaroo"
-                elif kind == EV_RESET:
-                    resets.append((rk, kidx))
+        for kind, rk, kidx, d_old, d_new in self._events_of(segments):
+            if kind == EV_COLLISION and found is None:
+                found = self.dps.resolve(d_old, d_new, self.key, self.start)     # Kangaroo.cpp:255-302
+                if found is None:
+                    resets.append((rk, kidx))                                    # "unexpected wrong collision, reset kangaroo"
+            elif kind == EV_RESET:
+                resets.append((rk, kidx))
         self.t_ingest += time.perf_counter() - t0
         return found, resets
+
+    def _no_events(self):
+        return None, []
 
     def _ingest_loop(self):
         while True:
@@ -319,7 +413,13 @@ class Solver:
             if job is None:
                 return
             if job[0] == "dps":
-                self._done.put(self._ingest(job[1]))
+                try:
+                    res = self._ingest(job[1])
+                except Exception as e:                  # the table failed: stop the run (every rank, next step) instead of
+                    if self.table_msg is None:          # leaving the main thread waiting for this step's result
+                        self.table_msg, self.table_kind = "%s: %s" % (type(e).__name__, e), "error"
+                    res = self._no_events()
+                self._done.put(res)
             else:
                 self._write(job)
 
@@ -390,6 +490,7 @@ class Solver:
             self._save_progress(self._chunks_next)
         if self.rank == 0:
             found, resets = self._harvest()
+            self.table_stopped = self.table_msg is not None
         save_next = (may_save and self.save_interval > 0 and self.rank == 0 and not self._saving and
                      time.time() - self._last_save >= self.save_interval)
         # herd chunks the next step may move: only into pinned buffers the writer has already freed, so a step never waits for
@@ -399,15 +500,17 @@ class Solver:
         if self.dist is not None:
             if self.rank == 0:
                 resets = resets[:MAX_RESETS]
-                c = [1 if found is not None else 0, len(resets), int(save_next), chunks] + [v for rk in resets for v in rk]
+                c = [2 if self.table_stopped else (1 if found is not None else 0), len(resets), int(save_next), chunks] + \
+                    [v for rk in resets for v in rk]
                 self._ctrl[:len(c)].copy_(torch.tensor(c, dtype=torch.int64))
             self.dist.broadcast(self._ctrl, 0)
             c = self._ctrl.cpu().tolist()
             self.stop = bool(c[0])
+            self.table_stopped = c[0] == 2
             save_next, chunks = bool(c[2]), c[3]
             resets = [(c[4 + 2 * i], c[5 + 2 * i]) for i in range(c[1])]
         else:
-            self.stop = found is not None
+            self.stop = found is not None or self.table_stopped
         self._chunks_next = chunks
         if save_next and not self.stop:
             if self.save_kangaroos:
@@ -423,10 +526,14 @@ class Solver:
         """this launch's DP records of every rank -> rank 0's ingest thread"""
         torch = self.torch
         cnt = min(n_found, self.eng.maxFound)
+        jumps_before = self.jumps
         self.jumps += self.eng.nbKangaroo * NB_RUN * self.world
         if self.gather is not None:
             res = self.gather.step_flat(cnt)                                # rank 0: (counts, cap, device tensor [world*cap*40])
-            if self.rank == 0:
+            if self.rank == 0 and self.dev_table:
+                counts, cap, flat = res
+                self._submit_device(flat, counts, cap, jumps_before)
+            elif self.rank == 0:
                 counts, cap, flat = res
                 nbytes = self.world * cap * DP40_BYTES
                 host = self._staging(nbytes)
@@ -435,13 +542,38 @@ class Solver:
                 h = host.numpy()
                 self._submit([(r, h[r * cap * DP40_BYTES: r * cap * DP40_BYTES + counts[r] * DP40_BYTES]) for r in range(self.world)])
         else:
-            if cnt:
+            if cnt and self.dev_table:
+                ptr = self.eng.convert_dps_device_ptr()
+                self._submit_device(torch.as_tensor(SlabView(ptr + 4, cnt * DP40_BYTES), device="cuda"), [cnt], cnt, jumps_before)
+            elif cnt:
                 ptr = self.eng.convert_dps_device_ptr()
                 dev = torch.as_tensor(SlabView(ptr + 4, cnt * DP40_BYTES), device="cuda")
                 host = self._staging(cnt * DP40_BYTES)
                 host[:cnt * DP40_BYTES].copy_(dev, non_blocking=True)
                 torch.cuda.current_stream().synchronize()
                 self._submit([(0, host.numpy()[:cnt * DP40_BYTES])])
+
+    def _submit_device(self, src, counts, stride, jumps_before):
+        """--dp-table device: the step's records stay on the GPU.  They are copied (device to device, torch's stream) into a
+        staging buffer, since the gather buffer and the engine's record buffer are rewritten by the next step, and the ingest
+        thread inserts them from there on its own stream behind that copy."""
+        nbytes = len(counts) * stride * DP40_BYTES
+        if self._pending >= 2 and self._writes_pending():
+            # a save holds the ingest thread: the steps queued behind it wait in host RAM, as with the host table, so the
+            # backlog takes no GPU memory however long the save lasts; the ingest thread copies each one back to insert it
+            buf = self.torch.empty(nbytes, dtype=self.torch.uint8)
+            buf.copy_(src[:nbytes])                     # to pageable memory: complete when it returns
+            ev = None
+            self.parked += 1
+        else:
+            buf = self._staging(nbytes)
+            buf[:nbytes].copy_(src[:nbytes], non_blocking=True)
+            ev = self.torch.cuda.Event()
+            ev.record()
+            if self.gather is None:
+                # the engine rewrites its record buffer on its own stream at the next convert, unordered with torch's stream
+                ev.synchronize()
+        self._submit(DeviceBatch(buf, list(counts), stride, ev, jumps_before))
 
     def run(self, max_steps=1 << 30, verbose=True):
         self.eng.callKernel()
@@ -464,14 +596,14 @@ class Solver:
                 self.steady = (time.time(), self.jumps)
             if verbose and self.rank == 0 and (s % 64 == 63 or self.stop):
                 dt = time.time() - t0
-                print("[%6.1fs] 2^%.2f jumps  %.0f MJump/s  %d DPs  dead %d  ingest %.1f ms/step" %
+                print("[%6.1fs] 2^%.2f jumps  %.0f MJump/s  %d DPs  dead %d  %s %.1f ms/step" %
                       (dt, np.log2(max(self.jumps, 1)), (self.jumps - self.jumps0) / dt / 1e6, len(self.dps), self.same_herd,
-                       1e3 * self.t_ingest / steps), flush=True)
+                       self.table_label, 1e3 * self.t_ingest / steps), flush=True)
             if self.stop:
                 break
         if self._saving:                                        # a save still moving its herd: finish it first
             self._save_progress(len(self._save_left))
-        if self.save_path:
+        if self.save_path and not self.table_stopped:
             # end-of-run cut: the launch still in flight is collected, its DPs go into the table before it is written
             if self.save_kangaroos:
                 self.eng.SnapshotBegin()
@@ -479,7 +611,7 @@ class Solver:
         else:
             self.eng.sync()
         t1 = time.time()
-        if self.save_path:
+        if self.save_path and not self.table_stopped:
             self._save_start(self.save_kangaroos, len(self.herd.plan) if self.save_kangaroos else 0)
         if self.rank == 0:                                      # drain: the last steps' records may still be in the ingest thread
             k2, _ = self._harvest(wait_all=True)
@@ -554,7 +686,8 @@ def class_privs(start, priv_rep, neg):
 class BatchSolver(Solver):
     """--batch-keys.  pubs: every public key of the input.  After run(), rank 0 holds priv[i] (None: not found)."""
 
-    def __init__(self, start, end, pubs, dp_bits, grid=None, max_found=1 << 17, seed=None, ingest_threads=0):
+    def __init__(self, start, end, pubs, dp_bits, grid=None, max_found=1 << 17, seed=None, ingest_threads=0, dp_table="host",
+                 dp_table_capacity=None):
         self.pubs = list(pubs)
         if not 1 <= len(self.pubs) <= MAX_KEYS:
             raise ValueError("--batch-keys takes 1 to %d keys, not %d" % (MAX_KEYS, len(self.pubs)))
@@ -566,9 +699,10 @@ class BatchSolver(Solver):
         self.rep, self.neg = key_classes(self.keys)
         self.live = [i for i, k in enumerate(self.keys) if k is not None and self.rep[i] == i]
         self._announce = []                 # rank 0: keys solved, not yet in a control broadcast
-        super().__init__(start, end, self.pubs[0], dp_bits, grid, max_found, seed, ingest_threads)
+        super().__init__(start, end, self.pubs[0], dp_bits, grid, max_found, seed, ingest_threads, dp_table=dp_table,
+                         dp_table_capacity=dp_table_capacity)
         self.key_table = DPTable.key_table(self.keys)
-        self._ctrl = self.torch.zeros(2 + MAX_SOLVED + 2 * MAX_RESETS, dtype=self.torch.int64, device="cuda")
+        self._ctrl = self.torch.zeros(3 + MAX_SOLVED + 2 * MAX_RESETS, dtype=self.torch.int64, device="cuda")
 
     def _create_herd(self, sc, d128):
         self.targets = assign_targets(self.eng.nbKangaroo, self.live or [0])         # host mirror of the engine's targets
@@ -581,20 +715,20 @@ class BatchSolver(Solver):
         """rank 0, ingest thread -> (hits [(key index, private key, rank, kIdx)], resets)"""
         hits, resets = [], []
         t0 = time.perf_counter()
-        for r, buf in segments:
-            if buf.size == 0:
-                continue
-            for kind, rk, kidx, d_old, d_new in self.dps.add_dp40(buf, r):
-                if kind == EV_COLLISION:
-                    m = self.dps.resolve_multi(d_old, d_new, self.key_table, self.start)
-                    if m is None:
-                        resets.append((rk, kidx))                # matches no key: "unexpected wrong collision, reset kangaroo"
-                    else:
-                        hits.append(m + (rk, kidx))
-                elif kind == EV_RESET:
-                    resets.append((rk, kidx))                    # same herd, wild/wild across keys included
+        for kind, rk, kidx, d_old, d_new in self._events_of(segments):
+            if kind == EV_COLLISION:
+                m = self.dps.resolve_multi(d_old, d_new, self.key_table, self.start)
+                if m is None:
+                    resets.append((rk, kidx))                    # matches no key: "unexpected wrong collision, reset kangaroo"
+                else:
+                    hits.append(m + (rk, kidx))
+            elif kind == EV_RESET:
+                resets.append((rk, kidx))                        # same herd, wild/wild across keys included
         self.t_ingest += time.perf_counter() - t0
         return hits, resets
+
+    def _no_events(self):
+        return [], []
 
     def _take(self, block):
         f, r = self._done.get(block=block)
@@ -617,8 +751,8 @@ class BatchSolver(Solver):
                 resets.append((rk, kidx))
 
     def step(self, may_save=False):
-        """one Launch on every rank; control broadcast [n_solved, n_resets, solved keys..., (rank, kIdx)...]; every rank moves
-        the wilds of each solved key to the live ones"""
+        """one Launch on every rank; control broadcast [n_solved, n_resets, table full, solved keys..., (rank, kIdx)...]; every
+        rank moves the wilds of each solved key to the live ones"""
         torch = self.torch
         n_found = self.eng.collect_count(relaunch=True)                  # launch i done, launch i+1 running
         self._gather(n_found)
@@ -628,22 +762,24 @@ class BatchSolver(Solver):
             hits, resets = self._harvest()
             self._claim(hits, resets)
             solved, self._announce = self._announce[:MAX_SOLVED], self._announce[MAX_SOLVED:]
+            self.table_stopped = self.table_msg is not None
         if self.dist is not None:
             if self.rank == 0:
                 resets = resets[:MAX_RESETS]
-                c = [len(solved), len(resets)] + solved + [v for rk in resets for v in rk]
+                c = [len(solved), len(resets), int(self.table_stopped)] + solved + [v for rk in resets for v in rk]
                 self._ctrl[:len(c)].copy_(torch.tensor(c, dtype=torch.int64))
             self.dist.broadcast(self._ctrl, 0)
             c = self._ctrl.cpu().tolist()
             ns, nr = c[0], c[1]
-            solved = c[2:2 + ns]
-            resets = [(c[2 + ns + 2 * i], c[3 + ns + 2 * i]) for i in range(nr)]
+            self.table_stopped = bool(c[2])
+            solved = c[3:3 + ns]
+            resets = [(c[3 + ns + 2 * i], c[4 + ns + 2 * i]) for i in range(nr)]
         for idx in solved:
             self.live.remove(idx)
             if self.live:
                 self.eng.Retarget(idx, self.live)                        # stream order: after launch i+1, before the resets
                 self.targets = retarget_targets(self.targets, idx, self.live)
-        self.stop = not self.live
+        self.stop = not self.live or self.table_stopped
         for rk, kidx in resets:
             self.same_herd += 1
             if rk == self.rank and not self.stop:
@@ -662,11 +798,12 @@ class BatchSolver(Solver):
 
 def _run_batch(start, end, pubs, dp, grid, a):
     t0 = time.perf_counter()
-    s = BatchSolver(start, end, pubs, dp, grid, seed=a.seed, ingest_threads=a.ingest_threads)
+    s = BatchSolver(start, end, pubs, dp, grid, seed=a.seed, ingest_threads=a.ingest_threads, dp_table=a.dp_table,
+                    dp_table_capacity=a.dp_table_capacity)
     t_setup = time.perf_counter() - t0
     if s.rank == 0:
-        print("Range width: 2^%d  kangaroos/GPU: %d  GPUs: %d  dp: %d  ingest threads: %d  keys: %d in one run" %
-              (s.range_power, s.eng.nbKangaroo, s.world, dp, s.dps.threads, len(pubs)), flush=True)
+        print("Range width: 2^%d  kangaroos/GPU: %d  GPUs: %d  dp: %d  %s  keys: %d in one run" %
+              (s.range_power, s.eng.nbKangaroo, s.world, dp, table_info(s), len(pubs)), flush=True)
     t0 = time.perf_counter()
     s.run(a.max_steps)
     t_run = time.perf_counter() - t0
@@ -674,9 +811,11 @@ def _run_batch(start, end, pubs, dp, grid, a):
     rc = 0
     if s.rank == 0:
         print("Solver rate: %.0f MJump/s steady state (after the first 32 steps), %.0f MJump/s over all %d steps (%.2f s); "
-              "rank-0 ingest %.2f ms/step; %d DPs; %d dead kangaroos re-created" %
-              (s.steady_rate / 1e6, (s.jumps - s.jumps0) / s.elapsed / 1e6, s.steps, s.elapsed, 1e3 * s.t_ingest / max(s.steps, 1),
-               len(s.dps), s.same_herd))
+              "rank-0 %s %.2f ms/step; %d DPs; %d dead kangaroos re-created" %
+              (s.steady_rate / 1e6, (s.jumps - s.jumps0) / s.elapsed / 1e6, s.steps, s.elapsed, s.table_label,
+               1e3 * s.t_ingest / max(s.steps, 1), len(s.dps), s.same_herd))
+        if s.table_stopped:
+            print(table_message(s, a)); rc = 1
         for i, pub in enumerate(pubs):
             if s.priv[i] is not None and ec.mul(s.priv[i]) == pub:
                 print("Key#%2d Pub:  0x%064X\n       Priv: 0x%X" % (i, pub[0], s.priv[i]))
@@ -696,6 +835,31 @@ def _run_batch(start, end, pubs, dp, grid, a):
               "results %.2f s, close %.2f s (engine and table freed)" %
               (t_setup, s.elapsed, t_run - s.elapsed, t_results, time.perf_counter() - t0), flush=True)
     return rc
+
+
+def table_info(s):
+    """the start-up line's description of rank 0's DP table"""
+    if not s.dev_table:
+        return "ingest threads: %d" % s.dps.threads
+    return "dp table: device, capacity %d entries (%.2f GB)" % (s.dps.capacity, s.dps.memory_bytes() / 1e9)
+
+
+def table_message(s, a):
+    """rank 0, after the run: why the table stopped it, and which work file, if any, to resume"""
+    what = "full" if s.table_kind == "full" else "failed"
+    msg = "DP table %s, run stopped: %s." % (what, s.table_msg)
+    saved = getattr(s, "full_saved", None)
+    if saved and saved[2] is None:
+        msg += (" %s holds the table as it was before this step's launch (count 2^%.2f, no kangaroos); resume it with "
+                "--dp-table host or a larger --dp-table-capacity" % (saved[0], np.log2(max(saved[1], 1))))
+    elif s.last_saved:
+        msg += (" The last work file written, %s, is a consistent cut from before the table stopped; resume it with "
+                "--dp-table host or a larger --dp-table-capacity" % s.last_saved)
+    elif a.save_work:
+        msg += " No work file was written."
+    elif what == "full":
+        msg += " Use --dp-table host or a larger --dp-table-capacity (with --save-work, the run writes a resumable file first)."
+    return msg
 
 
 def _resume_header(path):
@@ -733,6 +897,13 @@ def main(argv=None):
     ap.add_argument("--save-kangaroos", action="store_true", help="save every rank's herd with the table (-ws)")
     ap.add_argument("--resume", default="", metavar="FILE",
                     help="continue from a work file (-i): range, key and dp come from the file unless given")
+    ap.add_argument("--dp-table", choices=("host", "device"), default="host",
+                    help="where rank 0 keeps the DP table: host = the reference's HashTable in host RAM, inserted by "
+                         "--ingest-threads workers; device = a hash table with the same results in rank 0's GPU memory, inserted "
+                         "by CUDA kernels straight from the gathered records (fixed capacity: a full table stops the run)")
+    ap.add_argument("--dp-table-capacity", type=int, default=None, metavar="ENTRIES",
+                    help="--dp-table device: entries the table holds, 48 bytes of GPU memory each (default: what fits in rank "
+                         "0's free GPU memory after the engine, less %d GiB)" % (DP_TABLE_MARGIN >> 30))
     ap.add_argument("--batch-keys", action="store_true",
                     help="solve every key of the config in one run: one tame herd and one DP table shared by all keys, the "
                          "wild kangaroos spread over the unsolved ones")
@@ -742,6 +913,10 @@ def main(argv=None):
                  "(a work file carries one key)")
     if a.batch_keys and not a.config:
         ap.error("--batch-keys needs a config file")
+    if a.dp_table_capacity is not None and a.dp_table != "device":
+        ap.error("--dp-table-capacity needs --dp-table device")
+    if a.dp_table_capacity is not None and not 0 < a.dp_table_capacity < (1 << 32) - 1:
+        ap.error("--dp-table-capacity must be 1 .. 2^32-2 entries, not %d" % a.dp_table_capacity)
     if a.resume:
         file_dp, start, end, pub = _resume_header(a.resume)
         pubs = [pub]
@@ -763,17 +938,20 @@ def main(argv=None):
     rc = _run_batch(start, end, pubs, dp, grid, a) if a.batch_keys else 0
     for i, pub in enumerate([] if a.batch_keys else pubs):
         s = Solver(start, end, pub, dp, grid, seed=a.seed, ingest_threads=a.ingest_threads, save_work=a.save_work,
-                   save_interval=a.save_interval, save_kangaroos=a.save_kangaroos, resume=a.resume or None)
+                   save_interval=a.save_interval, save_kangaroos=a.save_kangaroos, resume=a.resume or None, dp_table=a.dp_table,
+                   dp_table_capacity=a.dp_table_capacity)
         if s.rank == 0:
-            print("Range width: 2^%d  kangaroos/GPU: %d  GPUs: %d  dp: %d  ingest threads: %d" %
-                  (s.range_power, s.eng.nbKangaroo, s.world, dp, s.dps.threads), flush=True)
+            print("Range width: 2^%d  kangaroos/GPU: %d  GPUs: %d  dp: %d  %s" %
+                  (s.range_power, s.eng.nbKangaroo, s.world, dp, table_info(s)), flush=True)
         key = s.run(a.max_steps)
         if s.rank == 0:
             print("Solver rate: %.0f MJump/s steady state (after the first 32 steps), %.0f MJump/s over all %d steps (%.2f s); "
-                  "rank-0 ingest %.2f ms/step; %d DPs; %d dead kangaroos re-created" %
-                  (s.steady_rate / 1e6, (s.jumps - s.jumps0) / s.elapsed / 1e6, s.steps, s.elapsed, 1e3 * s.t_ingest / max(s.steps, 1),
-                   len(s.dps), s.same_herd))
-            if a.save_work and s.save_error is None:
+                  "rank-0 %s %.2f ms/step; %d DPs; %d dead kangaroos re-created" %
+                  (s.steady_rate / 1e6, (s.jumps - s.jumps0) / s.elapsed / 1e6, s.steps, s.elapsed, s.table_label,
+                   1e3 * s.t_ingest / max(s.steps, 1), len(s.dps), s.same_herd))
+            if s.table_stopped:
+                print(table_message(s, a)); rc = 1
+            elif a.save_work and s.save_error is None:
                 mb, dt_save = s.saves[-1]
                 print("work file written: %s (%.1f MB in %.2f s, count 2^%.2f)" % (a.save_work, mb, dt_save, np.log2(max(s.jumps, 1))))
             elif a.save_work:
