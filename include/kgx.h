@@ -196,6 +196,55 @@ int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, u
                           uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time, uint64_t* nb_walk,
                           uint64_t* walk_offset, void* stream);
 
+/* --- work-file tools on one GPU (kgx_worktool.cuh): the reference's -wcheck and -wm / -wmdir for HEADW files.  Without a
+ *     device every call fails (-3); there is no CPU path.  Errors: a negative value, text in kgx_work_last_error().
+ * _check: reads `path` in chunks of `chunk` entries (0 = 2^21) through two pinned buffers, so that the disk and the device
+ *     overlap, and checks every table entry as Kangaroo::CheckHash does (Check.cpp:33-108): S = +-|d|*G, + K when wild
+ *     (K = key - start*G), OK iff S.x.bits64[2] & 0x3FFFF == h and the low 128 bits of S.x equal the stored x.  A result at
+ *     infinity is wrong.  Then every kangaroo record {x, y, d mod n}: OK as tame when (x, y) = d*G, as wild when
+ *     (x, y) = K + d*G (by value, not by position), wrong otherwise or when min(d, n - d) >= 2^128.  A file that ends right
+ *     after its table (the reference's -wm output) has no kangaroos: has_walk_count = 0.  The first `cap` wrong entries go to
+ *     wrong_entries as (bucket, index in bucket) pairs in file order, the first `cap` wrong kangaroos' indices to wrong_walks.
+ * _check_records: the same kernels on records in host memory (kind 0: n 32-byte entries with their buckets hs;
+ *     kind 1: n 96-byte kangaroo records, hs unused) for a key and range start; out[i] = 1 for a wrong entry / 0 wrong,
+ *     1 tame, 2 wild for a kangaroo.
+ * _comb: the check's fixed-base table, 480 affine points j * 2^(4w) * G (w < 32, 1 <= j <= 15) as 8 limbs (x, y) each, at
+ *     index w * 15 + j - 1.
+ * _merge: merges n_paths >= 2 files in the order given, as the reference's pairwise MergeWork calls would (Merge.cpp:33-246,
+ *     HashTable::MergeH): at equal x the entry of the earlier input is kept; a later one with the same tagged d is a
+ *     duplicate, any other a collision.  Every input is checked first (HEADW, same version, key on the curve, same range,
+ *     same key); nothing is written when one fails.  Writes tmp_path: header with the smallest dp and the summed count and
+ *     time, the merged table (maxItem = nbItem rounded up to 4), then a kangaroo count of 0.  Inputs without a kangaroo count
+ *     are accepted.  The inputs stream through the device in blocks of whole buckets of at most block_entries entries over
+ *     all inputs (0 = 2^22); a bucket larger than that is refused and tmp_path removed.  The first `cap` collisions, ordered by
+ *     bucket then x, go to coll. --- */
+typedef struct {
+  uint32_t dp_bits, has_walk_count;
+  uint64_t entries, wrong_entries;
+  uint64_t walks, walks_tame, walks_wild, wrong_walks;
+  uint32_t n_wrong_entries_listed, n_wrong_walks_listed;
+} kgx_work_check_info;
+typedef struct {
+  uint32_t dp_bits, blocks;
+  uint64_t entries, duplicates, collisions;
+  uint64_t total_count;
+  double total_time;
+  uint32_t n_listed, reserved;
+} kgx_work_merge_info;
+typedef struct {
+  uint32_t h, reserved;
+  uint64_t d_first[2];   /* tagged distance of the kept entry */
+  uint64_t d_other[2];   /* tagged distance of the later input's entry */
+} kgx_work_collision;
+const char* kgx_work_last_error(void);
+int kgx_work_check(int dev, const char* path, uint64_t chunk, kgx_work_check_info* info, uint32_t* wrong_entries, uint64_t* wrong_walks,
+                   uint32_t cap);
+int kgx_work_check_records(int dev, int kind, const void* recs, const uint32_t* hs, uint64_t n, const uint64_t keyx[4],
+                           const uint64_t keyy[4], const uint64_t range_start[4], uint8_t* out);
+int kgx_work_comb(int dev, uint64_t* out);
+int kgx_work_merge(int dev, const char* const* paths, uint32_t n_paths, const char* tmp_path, uint64_t block_entries,
+                   kgx_work_merge_info* info, kgx_work_collision* coll, uint32_t cap);
+
 /* Debug (KGX_PROF=1 in the environment at kgx_create): phase cycle counters summed over warp 0 of every CTA:
  * out = {serial section, modular inverse alone, parallel phase, tile-steps}; resets them. -1 when disabled. */
 int      kgx_debug_prof(kgx_engine* e, uint64_t out[4]);

@@ -77,6 +77,14 @@ _SIGS = {
                                              ctypes.c_double, ctypes.c_uint64, ctypes.c_void_p]),
     "kgx_dptable_load_work": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_uint32), _u64p, _u64p, _u64p, _u64p,
                                              _u64p, ctypes.POINTER(ctypes.c_double), _u64p, _u64p, ctypes.c_void_p]),
+    "kgx_work_last_error": (ctypes.c_char_p, []),
+    "kgx_work_check": (ctypes.c_int, [ctypes.c_int, ctypes.c_char_p, ctypes.c_uint64, ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint32),
+                                      _u64p, ctypes.c_uint32]),
+    "kgx_work_check_records": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint64, _u64p, _u64p,
+                                              _u64p, ctypes.c_void_p]),
+    "kgx_work_comb": (ctypes.c_int, [ctypes.c_int, _u64p]),
+    "kgx_work_merge": (ctypes.c_int, [ctypes.c_int, ctypes.POINTER(ctypes.c_char_p), ctypes.c_uint32, ctypes.c_char_p, ctypes.c_uint64,
+                                      ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32]),
 }
 EXPORTED_SYMBOLS = sorted(_SIGS)
 

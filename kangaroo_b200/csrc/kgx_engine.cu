@@ -786,3 +786,4 @@ int kgx_bench_raw(int dev, int kind, int iters, float* ms, double* ops) {
 }  // extern "C"
 
 #include "kgx_dptable.cuh"   // the device-resident DP table (kgx_dptable_*)
+#include "kgx_worktool.cuh"  // work-file check and merge (kgx_work_*)

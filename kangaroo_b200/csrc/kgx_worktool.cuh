@@ -1,0 +1,746 @@
+// kgx_worktool.cuh -- checking and merging HEADW work files on one GPU (C ABI: include/kgx.h, kgx_work_*).
+//
+// Check (the reference's -wcheck, Check.cpp:33-108, 290-411): every stored DP {x lo 128, tagged d} of bucket h is OK iff
+// S = +-|d|*G (+ K for a wild entry, K = keyToSearch = P - start*G) has S.x.bits64[2] & 0x3FFFF == h and the low 128 bits
+// of S.x equal x.  |d| < 2^126, so S comes from a fixed-base comb: 32 windows of 4 bits, 15 affine points each
+// (j * 2^(4w) * G, 30 KB in shared memory), added from the lowest window up with mixed Jacobian additions.  The partial sum
+// of windows < w has a scalar below 2^(4w) and the next term one of at least 2^(4w), so two comb terms never meet the equal
+// or opposite point; only the final +K can (S = +-K), and there the group law is followed: a doubling, or the point at
+// infinity, which is counted wrong.  Affine x comes from Montgomery's batch inverse over each thread's GROUP entries.
+// Walk records {x, y, d mod n} are checked by the same comb, magnitude min(d, n - d), compared projectively (no inverse):
+// OK as tame when (x, y) = d*G, as wild when (x, y) = K + d*G.
+//
+// Merge (the reference's -wm / -wmdir, Merge.cpp:33-346, HashTable::MergeH): the inputs stream through in blocks of whole
+// buckets, each bucket's entries uploaded in input order.  A stable radix sort by (h, x.hi, x.lo) keeps that order among
+// equal keys; one scan keeps the first entry of every run of equal (h, x) -- the earliest input's, as the reference's
+// pairwise merges do -- and classifies each later one against it: equal tagged d = a duplicate ("Dead kangaroo"), else a
+// collision returned to the host.  The kept entries are compacted, counted per bucket and written with maxItem = nbItem
+// rounded up to a multiple of 4 (HashTable.cpp:204-209).
+#include <cerrno>
+#include <vector>
+#include <algorithm>
+#include <string>
+#include <thrust/iterator/counting_iterator.h>
+
+namespace kgx_wt {
+
+using ::u32;
+using ::u64;
+typedef unsigned long long ull;
+constexpr int COMB_W = 32, COMB_J = 15, COMB_WORDS = COMB_W * COMB_J * 16;   // 480 affine points, 16 words each
+constexpr int CHECK_THREADS = 128, GROUP = 8;                                 // entries per thread share one inverse
+constexpr uint32_t NBUCKET = 1u << 18, HEADW = 0xFA6A8001u;
+constexpr uint64_t DEFAULT_CHUNK = 1ull << 21, DEFAULT_BLOCK = 1ull << 22;
+
+struct Entry { uint64_t x0, x1, d0, d1; };
+struct Coll { uint32_t h, seq; uint64_t d_first[2], d_other[2]; };
+struct MergeRes { ull dup, ncoll; };
+
+// tab[(w * 15 + j - 1) * 16]: j * 2^(4w) * G, affine x then y, canonical.  Thread w builds window w.
+__global__ void wt_comb_kernel(u32* tab) {
+  const int w = threadIdx.x;
+  if (w >= COMB_W) return;
+  u32 bx[8] = {0x16F81798u, 0x59F2815Bu, 0x2DCE28D9u, 0x029BFCDBu, 0xCE870B07u, 0x55A06295u, 0xF9DCBBACu, 0x79BE667Eu};
+  u32 by[8] = {0xFB10D4B8u, 0x9C47D08Fu, 0xA6855419u, 0xFD17B448u, 0x0E1108A8u, 0x5DA4FBFCu, 0x26A3C465u, 0x483ADA77u};
+  for (int i = 0; i < 4 * w; i++) {                 // 2^(4w) * G
+    u32 cx[8], cy[8];
+    fe_copy(cx, bx); fe_copy(cy, by);
+    kgx::affine_add(bx, by, cx, cy);
+  }
+  u32 x[8], y[8];
+  fe_copy(x, bx); fe_copy(y, by);
+  for (int j = 1; j <= COMB_J; j++) {
+    u32* o = tab + (w * COMB_J + j - 1) * 16;
+    for (int k = 0; k < 8; k++) { o[k] = x[k]; o[8 + k] = y[k]; }
+    if (j < COMB_J) kgx::affine_add(x, y, bx, by);
+  }
+}
+
+// (X, Y, Z) += (qx, qy) in Jacobian + affine coordinates, infinity as a flag.  Same x: a doubling when the points are equal,
+// the point at infinity when they are opposite (the group law, as herd_kernel).
+__device__ __forceinline__ void wt_madd(u32* X, u32* Y, u32* Z, bool& inf, const u32* qx, const u32* qy) {
+  using namespace kgx;
+  if (inf) { fe_copy(X, qx); fe_copy(Y, qy); fe_set_one(Z); inf = false; return; }
+  u32 zz[8], u2[8], s2[8], h[8], r[8], hh[8], hhh[8], v[8], t[8];
+  fe_sqr(zz, Z);
+  fe_mul(u2, qx, zz);
+  fe_mul(s2, qy, zz); fe_mul(s2, s2, Z);
+  fe_sub(h, u2, X);
+  fe_sub(r, s2, Y);
+  if (fe_is_zero_modp(h)) {
+    if (!fe_is_zero_modp(r)) { inf = true; return; }
+    u32 yy[8], S[8], M[8], m2[8], y4[8], nx[8], ny[8], nz[8];
+    fe_sqr(yy, Y);
+    fe_mul(S, X, yy); fe_dbl(S, S); fe_dbl(S, S);
+    fe_sqr(m2, X); fe_dbl(M, m2); { u32 ng[8]; fe_neg(ng, m2); fe_sub(M, M, ng); }
+    fe_sqr(nx, M); fe_sub(nx, nx, S); fe_sub(nx, nx, S);
+    fe_sqr(y4, yy); fe_dbl(y4, y4); fe_dbl(y4, y4); fe_dbl(y4, y4);
+    fe_sub(ny, S, nx); fe_mul(ny, ny, M); fe_sub(ny, ny, y4);
+    fe_mul(nz, Y, Z); fe_dbl(nz, nz);
+    fe_copy(X, nx); fe_copy(Y, ny); fe_copy(Z, nz);
+    return;
+  }
+  fe_sqr(hh, h);
+  fe_mul(hhh, hh, h);
+  fe_mul(v, X, hh);
+  fe_sqr(t, r);
+  fe_sub(t, t, hhh);
+  fe_sub(t, t, v); fe_sub(t, t, v);
+  fe_sub(v, v, t);
+  fe_mul(v, v, r);
+  fe_mul(hhh, hhh, Y);
+  fe_sub(Y, v, hhh);
+  fe_mul(Z, Z, h);
+  fe_copy(X, t);
+}
+
+// m * G for a 128-bit m (4 words) from the comb in shared memory, lowest window first
+__device__ __forceinline__ void wt_comb_mul(const u32* sc, const u32* m, u32* X, u32* Y, u32* Z, bool& inf) {
+  inf = true;
+#pragma unroll 1
+  for (int w = 0; w < COMB_W; w++) {
+    const u32 nib = (m[w >> 3] >> (4 * (w & 7))) & 15u;
+    if (nib) {
+      const u32* q = sc + (w * COMB_J + nib - 1) * 16;
+      wt_madd(X, Y, Z, inf, q, q + 8);
+    }
+  }
+}
+
+__device__ __forceinline__ void wt_load_comb(u32* sc, const u32* comb) {
+  for (int i = threadIdx.x; i < COMB_WORDS; i += blockDim.x) sc[i] = comb[i];
+  __syncthreads();
+}
+
+// Table entries: bad[i] = 1 when entry i (bucket hs[i]) is wrong.  K: 16 words (x, y), kinf = K is the point at infinity.
+// Block b checks entries [b * 128 * GROUP, (b + 1) * 128 * GROUP); thread t those at t + g * 128, g < GROUP, with one
+// inverse for its group (entries at infinity, past n or wrong, are left out of the product).
+__global__ void __launch_bounds__(CHECK_THREADS) wt_check_entries_kernel(const u32* __restrict__ comb, const Entry* __restrict__ ent,
+                                                                        const uint32_t* __restrict__ hs, uint64_t n,
+                                                                        const u32* __restrict__ K, int kinf, uint8_t* bad, ull* nbad) {
+  using namespace kgx;
+  __shared__ u32 sc[COMB_WORDS];
+  wt_load_comb(sc, comb);
+  const uint64_t base = (uint64_t)blockIdx.x * (CHECK_THREADS * GROUP) + threadIdx.x;
+  u32 X[GROUP][8], Z[GROUP][8], acc[GROUP][8];
+  bool inf[GROUP];
+  u32 run[8];
+  fe_set_one(run);
+#pragma unroll 1
+  for (int g = 0; g < GROUP; g++) {
+    const uint64_t i = base + (uint64_t)g * CHECK_THREADS;
+    inf[g] = true;
+    if (i < n) {
+      const Entry e = ent[i];
+      const bool wild = (e.d1 >> 62) & 1, neg = e.d1 >> 63;
+      const u32 m[4] = {(u32)e.d0, (u32)(e.d0 >> 32), (u32)e.d1, (u32)(e.d1 >> 32) & 0x3FFFFFFFu};
+      u32 Y[8];
+      bool f;
+      wt_comb_mul(sc, m, X[g], Y, Z[g], f);
+      if (neg && !f) { u32 t[8]; fe_neg(t, Y); fe_copy(Y, t); }
+      if (wild && !kinf) wt_madd(X[g], Y, Z[g], f, K, K + 8);
+      inf[g] = f;
+      if (!f) fe_mul(run, run, Z[g]);
+    }
+    fe_copy(acc[g], run);
+  }
+  u32 inv[8];
+  modinv256(inv, run);
+#pragma unroll 1
+  for (int g = GROUP - 1; g >= 0; g--) {
+    const uint64_t i = base + (uint64_t)g * CHECK_THREADS;
+    if (i >= n) continue;
+    bool wrong = true;
+    if (!inf[g]) {
+      u32 zi[8], x[8];
+      if (g > 0) fe_mul(zi, inv, acc[g - 1]); else fe_copy(zi, inv);
+      fe_mul(inv, inv, Z[g]);
+      fe_sqr(zi, zi);
+      fe_mul(x, X[g], zi);
+      fe_canon(x);
+      const Entry e = ent[i];
+      wrong = (x[4] & 0x3FFFFu) != hs[i] || (((u64)x[1] << 32) | x[0]) != e.x0 || (((u64)x[3] << 32) | x[2]) != e.x1;
+    }
+    bad[i] = wrong;
+    if (wrong) atomicAdd(nbad, 1ull);
+  }
+}
+
+__device__ __forceinline__ bool wt_proj_eq(const u32* X, const u32* Y, const u32* Z, const u32* x, const u32* y) {
+  using namespace kgx;
+  u32 zz[8], t[8];
+  fe_sqr(zz, Z);
+  fe_mul(t, x, zz);
+  fe_sub(t, X, t);
+  if (!fe_is_zero_modp(t)) return false;
+  fe_mul(zz, zz, Z);
+  fe_mul(t, y, zz);
+  fe_sub(t, Y, t);
+  return fe_is_zero_modp(t);
+}
+
+// Walk records (96 bytes: x[4], y[4], d[4] limbs): res[i] = 1 tame OK, 2 wild OK, 0 wrong; cnt = {tame, wild, wrong}.
+// bad[i] = 1 when wrong.  d >= n or min(d, n - d) >= 2^128 is wrong: engine distances are 128-bit.
+__global__ void __launch_bounds__(CHECK_THREADS) wt_check_walks_kernel(const u32* __restrict__ comb, const u32* __restrict__ recs,
+                                                                      uint64_t n, const u32* __restrict__ K, int kinf, uint8_t* res,
+                                                                      uint8_t* bad, ull* cnt) {
+  using namespace kgx;
+  __shared__ u32 sc[COMB_WORDS];
+  wt_load_comb(sc, comb);
+  const u32 N[8] = {0xD0364141u, 0xBFD25E8Cu, 0xAF48A03Bu, 0xBAAEDCE6u, 0xFFFFFFFEu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const u32* r = recs + i * 24;
+    u32 x[8], y[8], d[8];
+    for (int k = 0; k < 8; k++) { x[k] = r[k]; y[k] = r[8 + k]; d[k] = r[16 + k]; }
+    int kind = 0;
+    bool lt = false;                                    // d < n ?
+    for (int k = 7; k >= 0; k--) if (d[k] != N[k]) { lt = d[k] < N[k]; break; }
+    if (lt) {
+      u32 nd[8];                                        // n - d
+      u64 br = 0;
+      for (int k = 0; k < 8; k++) { const u64 s = (u64)N[k] - d[k] - br; nd[k] = (u32)s; br = (s >> 32) & 1; }
+      bool dle = true;                                  // d <= n - d ?
+      for (int k = 7; k >= 0; k--) if (d[k] != nd[k]) { dle = d[k] < nd[k]; break; }
+      const u32* m = dle ? d : nd;
+      if ((m[4] | m[5] | m[6] | m[7]) == 0) {
+        u32 X[8], Y[8], Z[8];
+        bool f;
+        wt_comb_mul(sc, m, X, Y, Z, f);
+        if (!dle && !f) { u32 t[8]; fe_neg(t, Y); fe_copy(Y, t); }
+        if (!f && wt_proj_eq(X, Y, Z, x, y)) kind = 1;
+        else {
+          if (!kinf) wt_madd(X, Y, Z, f, K, K + 8);
+          if (!f && wt_proj_eq(X, Y, Z, x, y)) kind = 2;
+        }
+      }
+    }
+    res[i] = (uint8_t)kind;
+    bad[i] = kind == 0;
+    atomicAdd(&cnt[kind == 0 ? 2 : kind - 1], 1ull);
+  }
+}
+
+// key checks: ok[0] = key (x, y) on the curve; K = key + s*G (s = -start mod n, 8 words) is left to herd_kernel
+__global__ void wt_on_curve_kernel(const u32* key, int* ok) {
+  using namespace kgx;
+  if (threadIdx.x || blockIdx.x) return;
+  u32 l[8], r[8], s[8], seven[8] = {7, 0, 0, 0, 0, 0, 0, 0};
+  fe_sqr(l, key + 8);
+  fe_sqr(r, key);
+  fe_mul(r, r, key);
+  fe_neg(s, seven);
+  fe_sub(r, r, s);                                      // x^3 + 7
+  fe_sub(l, l, r);
+  bool canon = true;                                    // coordinates must be below p, as the reference's EC() check reads them
+  u32 t[8];
+  for (int c = 0; c < 2; c++) { fe_copy(t, key + 8 * c); fe_canon(t); for (int k = 0; k < 8; k++) canon = canon && t[k] == key[8 * c + k]; }
+  *ok = fe_is_zero_modp(l) && canon;
+}
+
+// ---- merge ----
+__global__ void wt_merge_key(const Entry* ent, const uint32_t* hs, const uint32_t* idx, uint32_t n, int which, uint32_t b0, uint64_t* key) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  const uint32_t e = idx ? idx[t] : t;
+  if (which == 0) key[t] = ent[e].x0;
+  else if (which == 1) key[t] = ent[e].x1;
+  else reinterpret_cast<uint32_t*>(key)[t] = hs[e] - b0;
+}
+
+__global__ void wt_iota(uint32_t* v, uint32_t n) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < n) v[t] = t;
+}
+
+// ord: the block's entries in (h, x) order, input order among equals.  keep[i] = first of its run; later entries are
+// duplicates or collisions against that first one.  nb[h - b0] counts the kept entries of each bucket.
+__global__ void wt_merge_scan(const Entry* ent, const uint32_t* hs, const uint32_t* ord, uint32_t n, uint32_t b0, uint8_t* keep,
+                              uint32_t* nb, MergeRes* res, Coll* coll) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t e = ord[i];
+  const Entry v = ent[e];
+  const uint32_t h = hs[e];
+  uint32_t f = i;
+  while (f > 0) {
+    const uint32_t p = ord[f - 1];
+    if (hs[p] != h || ent[p].x0 != v.x0 || ent[p].x1 != v.x1) break;
+    f--;
+  }
+  keep[i] = f == i;
+  if (f == i) { atomicAdd(&nb[h - b0], 1u); return; }
+  const Entry w = ent[ord[f]];
+  if (w.d0 == v.d0 && w.d1 == v.d1) { atomicAdd(&res->dup, 1ull); return; }
+  const ull c = atomicAdd(&res->ncoll, 1ull);
+  coll[c] = Coll{h, i, {w.d0, w.d1}, {v.d0, v.d1}};
+}
+
+__global__ void wt_gather(const Entry* ent, const uint32_t* idx, uint32_t n, Entry* out) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < n) out[t] = ent[idx[t]];
+}
+
+}  // namespace kgx_wt
+
+static char g_wt_err[512] = "";
+
+#define WT_CK(call)                                                                                   \
+  do {                                                                                                \
+    cudaError_t _s = (call);                                                                          \
+    if (_s != cudaSuccess) {                                                                          \
+      snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", #call, cudaGetErrorString(_s));                   \
+      cudaGetLastError();                                                                             \
+      return -3;                                                                                      \
+    }                                                                                                 \
+  } while (0)
+
+namespace kgx_wt {
+
+struct Header {
+  uint32_t head = 0, version = 0, dp = 0;
+  uint64_t rs[4], re[4], kx[4], ky[4];
+  uint64_t count = 0;
+  double time = 0;
+};
+
+static bool read_header(FILE* f, Header& h) {
+  return fread(&h.head, 4, 1, f) == 1 && h.head == HEADW && fread(&h.version, 4, 1, f) == 1 && fread(&h.dp, 4, 1, f) == 1 &&
+         fread(h.rs, 32, 1, f) == 1 && fread(h.re, 32, 1, f) == 1 && fread(h.kx, 32, 1, f) == 1 && fread(h.ky, 32, 1, f) == 1 &&
+         fread(&h.count, 8, 1, f) == 1 && fread(&h.time, 8, 1, f) == 1;
+}
+
+// device scratch that lives for one call: freed on every return path
+struct DevBufs {
+  std::vector<void*> d, h;
+  ~DevBufs() { for (void* p : d) cudaFree(p); for (void* p : h) cudaFreeHost(p); }
+  template <class T> int dev(T** p, size_t n) {
+    if (cudaMalloc((void**)p, n ? n : 1) != cudaSuccess) {
+      snprintf(g_wt_err, sizeof g_wt_err, "cudaMalloc(%zu bytes): %s", n, cudaGetErrorString(cudaGetLastError()));
+      return -3;
+    }
+    d.push_back(*p);
+    return 0;
+  }
+  template <class T> int host(T** p, size_t n) {
+    if (cudaHostAlloc((void**)p, n ? n : 1, cudaHostAllocDefault) != cudaSuccess) {
+      snprintf(g_wt_err, sizeof g_wt_err, "cudaHostAlloc(%zu bytes): %s", n, cudaGetErrorString(cudaGetLastError()));
+      return -3;
+    }
+    h.push_back(*p);
+    return 0;
+  }
+};
+
+static int set_device(int dev) {
+  int cnt = 0;
+  cudaError_t s = cudaGetDeviceCount(&cnt);
+  if (s != cudaSuccess || cnt == 0) {
+    snprintf(g_wt_err, sizeof g_wt_err, "no CUDA device (%s)", cudaGetErrorString(s));
+    cudaGetLastError();
+    return -3;
+  }
+  WT_CK(cudaSetDevice(dev));
+  return 0;
+}
+
+// *ok = key on the curve; K (16 words on the device) = key - start*G, *kinf = K is the point at infinity
+static int key_setup(DevBufs& B, const uint64_t kx[4], const uint64_t ky[4], const uint64_t rs[4], cudaStream_t st, int* ok,
+                     u32** K, int* kinf) {
+  u32 *dKey, *tab = nullptr, *scal = nullptr, *ky_ = nullptr;
+  int* dOk;
+  if (B.dev(&dKey, 64) || B.dev(&dOk, 4)) return -3;
+  uint64_t key[8];
+  memcpy(key, kx, 32); memcpy(key + 4, ky, 32);
+  WT_CK(cudaMemcpyAsync(dKey, key, 64, cudaMemcpyHostToDevice, st));
+  wt_on_curve_kernel<<<1, 32, 0, st>>>(dKey, dOk);
+  WT_CK(cudaGetLastError());
+  WT_CK(cudaMemcpyAsync(ok, dOk, 4, cudaMemcpyDeviceToHost, st));
+  WT_CK(cudaStreamSynchronize(st));
+  if (!K || !*ok) return 0;
+  // s = (n - start mod n) mod n
+  static const uint64_t N[4] = {0xBFD25E8CD0364141ull, 0xBAAEDCE6AF48A03Bull, 0xFFFFFFFFFFFFFFFEull, 0xFFFFFFFFFFFFFFFFull};
+  uint64_t a[4], s[4];
+  memcpy(a, rs, 32);
+  auto ge = [](const uint64_t* x, const uint64_t* y) { for (int k = 3; k >= 0; k--) if (x[k] != y[k]) return x[k] > y[k]; return true; };
+  auto sub = [](uint64_t* r, const uint64_t* x, const uint64_t* y) {
+    unsigned __int128 br = 0;
+    for (int k = 0; k < 4; k++) { const unsigned __int128 t = (unsigned __int128)x[k] - y[k] - br; r[k] = (uint64_t)t; br = (t >> 64) & 1; }
+  };
+  if (ge(a, N)) sub(a, a, N);
+  if ((a[0] | a[1] | a[2] | a[3]) == 0) memset(s, 0, 32); else sub(s, N, a);
+  if (B.dev(&tab, 256 * 16 * 4) || B.dev(&scal, 32) || B.dev(K, 64) || B.dev(&ky_, 64)) return -3;
+  WT_CK(cudaMemcpyAsync(scal, s, 32, cudaMemcpyHostToDevice, st));
+  kgx::herd_table_kernel<<<1, 32, 0, st>>>(tab);
+  kgx::herd_kernel<<<1, 32, 0, st>>>(tab, scal, dKey, nullptr, 1, 1, *K, ky_, 0, nullptr);   // wild: key + s*G
+  WT_CK(cudaGetLastError());
+  WT_CK(cudaMemcpyAsync(*K + 8, ky_, 32, cudaMemcpyDeviceToDevice, st));
+  uint64_t kh[8];
+  WT_CK(cudaMemcpyAsync(kh, *K, 64, cudaMemcpyDeviceToHost, st));
+  WT_CK(cudaStreamSynchronize(st));
+  bool z = true;
+  for (int k = 0; k < 8; k++) z = z && kh[k] == 0;
+  *kinf = z;                                            // herd_kernel stores the point at infinity as (0, 0)
+  return 0;
+}
+
+static int build_comb(DevBufs& B, u32** comb, cudaStream_t st) {
+  if (B.dev(comb, COMB_WORDS * 4)) return -3;
+  wt_comb_kernel<<<1, 32, 0, st>>>(*comb);
+  WT_CK(cudaGetLastError());
+  return 0;
+}
+
+static unsigned check_blocks(uint64_t n) { return (unsigned)((n + CHECK_THREADS * GROUP - 1) / (CHECK_THREADS * GROUP)); }
+
+}  // namespace kgx_wt
+
+extern "C" {
+
+const char* kgx_work_last_error(void) { return g_wt_err; }
+
+int kgx_work_comb(int dev, uint64_t* out) {
+  using namespace kgx_wt;
+  if (set_device(dev)) return -3;
+  DevBufs B;
+  u32* comb;
+  if (build_comb(B, &comb, 0)) return -3;
+  WT_CK(cudaMemcpy(out, comb, COMB_WORDS * 4, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int kgx_work_check_records(int dev, int walks, const void* recs, const uint32_t* hs, uint64_t n, const uint64_t keyx[4],
+                           const uint64_t keyy[4], const uint64_t range_start[4], uint8_t* out) {
+  using namespace kgx_wt;
+  if (set_device(dev)) return -3;
+  DevBufs B;
+  int ok = 0, kinf = 0;
+  u32 *K = nullptr, *comb;
+  if (key_setup(B, keyx, keyy, range_start, 0, &ok, &K, &kinf)) return -3;
+  if (!ok) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_work_check_records: the key does not lie on the curve"); return -1; }
+  if (build_comb(B, &comb, 0)) return -3;
+  if (n == 0) return 0;
+  uint8_t *dRes, *dBad;
+  ull* cnt;
+  void* dRec;
+  if (B.dev(&dRec, n * (walks ? 96 : 32)) || B.dev(&dRes, n) || B.dev(&dBad, n) || B.dev(&cnt, 24)) return -3;
+  WT_CK(cudaMemcpy(dRec, recs, n * (walks ? 96 : 32), cudaMemcpyHostToDevice));
+  WT_CK(cudaMemset(cnt, 0, 24));
+  if (walks) {
+    wt_check_walks_kernel<<<(unsigned)std::min<uint64_t>((n + 127) / 128, 4096), 128>>>(comb, (const u32*)dRec, n, K, kinf, dRes, dBad, cnt);
+  } else {
+    uint32_t* dH;
+    if (B.dev(&dH, 4 * n)) return -3;
+    WT_CK(cudaMemcpy(dH, hs, 4 * n, cudaMemcpyHostToDevice));
+    wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS>>>(comb, (const Entry*)dRec, dH, n, K, kinf, dBad, cnt);
+  }
+  WT_CK(cudaGetLastError());
+  WT_CK(cudaMemcpy(out, walks ? dRes : dBad, n, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int kgx_work_check(int dev, const char* path, uint64_t chunk, kgx_work_check_info* info, uint32_t* wrong_entries, uint64_t* wrong_walks,
+                   uint32_t cap) {
+  using namespace kgx_wt;
+  memset(info, 0, sizeof *info);
+  if (set_device(dev)) return -3;
+  if (chunk == 0) chunk = DEFAULT_CHUNK;
+  if (chunk >= 0x40000000ull) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_work_check: chunk of %llu entries (at most 2^30-1)", (unsigned long long)chunk); return -1; }
+  errno = 0;
+  FILE* f = fopen(path, "rb");
+  if (!f) { const int e = errno ? errno : EIO; snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", path, strerror(e)); return -e; }
+  struct Closer { FILE* f; ~Closer() { fclose(f); } } closer{f};
+  setvbuf(f, nullptr, _IOFBF, 1 << 22);
+  Header hd;
+  if (!read_header(f, hd)) { snprintf(g_wt_err, sizeof g_wt_err, "%s is not a HEADW work file", path); return -1; }
+  info->dp_bits = hd.dp;
+  DevBufs B;
+  cudaStream_t st;
+  WT_CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  struct StreamGuard { cudaStream_t s; ~StreamGuard() { cudaStreamSynchronize(s); cudaStreamDestroy(s); } } sg{st};
+  int ok = 0, kinf = 0;
+  u32 *K = nullptr, *comb;
+  if (key_setup(B, hd.kx, hd.ky, hd.rs, st, &ok, &K, &kinf)) return -3;
+  if (!ok) { snprintf(g_wt_err, sizeof g_wt_err, "CheckWorkFile: key1 does not lie on elliptic curve"); return -1; }
+  if (build_comb(B, &comb, st)) return -3;
+  // two buffers: the host fills one from disk while the device checks the other
+  const uint64_t wchunk = chunk / 3 ? chunk / 3 : 1;    // walks per chunk: 96-byte records in the 32-byte entries' room
+  Entry *hEnt[2], *dEnt[2];
+  uint32_t *hH[2], *dH[2], *dSel[2], *hSel[2], *dNsel[2], *hNsel[2];
+  uint8_t *dBad[2], *dRes[2];
+  ull *dCnt[2], *hCnt[2];
+  std::vector<uint32_t> hIdx[2];
+  size_t selTmp = 0;
+  void* dTmp[2];
+  WT_CK(cub::DeviceSelect::Flagged(nullptr, selTmp, thrust::counting_iterator<uint32_t>(0), (uint8_t*)nullptr, (uint32_t*)nullptr,
+                                   (uint32_t*)nullptr, (int)chunk));
+  cudaEvent_t done[2];
+  for (int b = 0; b < 2; b++) {
+    if (B.host(&hEnt[b], 32 * chunk) || B.dev(&dEnt[b], 32 * chunk) || B.host(&hH[b], 4 * chunk) || B.dev(&dH[b], 4 * chunk) ||
+        B.dev(&dBad[b], chunk) || B.dev(&dRes[b], chunk) || B.dev(&dNsel[b], 4) ||
+        B.host(&hSel[b], 4ull * (cap + 1)) || B.host(&hNsel[b], 4) || B.dev(&dCnt[b], 24) || B.host(&hCnt[b], 24) ||
+        B.dev(&dTmp[b], selTmp) || B.dev(&dSel[b], 4 * chunk))
+      return -3;
+    hIdx[b].resize(chunk);
+    WT_CK(cudaEventCreateWithFlags(&done[b], cudaEventDisableTiming));
+  }
+  struct EvGuard { cudaEvent_t* e; ~EvGuard() { cudaEventDestroy(e[0]); cudaEventDestroy(e[1]); } } eg{done};
+  uint64_t pending_n[2] = {0, 0}, pending_first[2] = {0, 0};
+  int pending_kind[2] = {-1, -1};
+  uint32_t nwe = 0, nww = 0;
+  auto submit = [&](int b, int kind, uint64_t n, uint64_t first) -> int {
+    WT_CK(cudaMemsetAsync(dCnt[b], 0, 24, st));
+    if (kind == 0) {
+      WT_CK(cudaMemcpyAsync(dEnt[b], hEnt[b], 32 * n, cudaMemcpyHostToDevice, st));
+      WT_CK(cudaMemcpyAsync(dH[b], hH[b], 4 * n, cudaMemcpyHostToDevice, st));
+      wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS, 0, st>>>(comb, dEnt[b], dH[b], n, K, kinf, dBad[b], dCnt[b]);
+    } else {
+      WT_CK(cudaMemcpyAsync(dEnt[b], hEnt[b], 96 * n, cudaMemcpyHostToDevice, st));
+      wt_check_walks_kernel<<<(unsigned)std::min<uint64_t>((n + 127) / 128, 4096), 128, 0, st>>>(comb, (const u32*)dEnt[b], n, K, kinf,
+                                                                                                   dRes[b], dBad[b], dCnt[b]);
+    }
+    WT_CK(cudaGetLastError());
+    size_t tb = selTmp;
+    WT_CK(cub::DeviceSelect::Flagged(dTmp[b], tb, thrust::counting_iterator<uint32_t>(0), dBad[b], dSel[b], dNsel[b], (int)n, st));
+    WT_CK(cudaMemcpyAsync(hNsel[b], dNsel[b], 4, cudaMemcpyDeviceToHost, st));
+    if (cap) WT_CK(cudaMemcpyAsync(hSel[b], dSel[b], 4ull * std::min<uint64_t>(cap, n), cudaMemcpyDeviceToHost, st));
+    WT_CK(cudaMemcpyAsync(hCnt[b], dCnt[b], 24, cudaMemcpyDeviceToHost, st));
+    WT_CK(cudaEventRecord(done[b], st));
+    pending_n[b] = n; pending_kind[b] = kind; pending_first[b] = first;
+    return 0;
+  };
+  auto drain = [&](int b) -> int {                     // wait for buffer b's chunk and count it
+    if (pending_kind[b] < 0) return 0;
+    WT_CK(cudaEventSynchronize(done[b]));
+    const uint32_t ns = std::min<uint32_t>(*hNsel[b], cap);
+    if (pending_kind[b] == 0) {
+      info->entries += pending_n[b];
+      info->wrong_entries += hCnt[b][0];
+      for (uint32_t k = 0; k < ns && nwe < cap; k++, nwe++) {
+        wrong_entries[2 * nwe] = hH[b][hSel[b][k]];
+        wrong_entries[2 * nwe + 1] = hIdx[b][hSel[b][k]];
+      }
+    } else {
+      info->walks += pending_n[b];
+      info->walks_tame += hCnt[b][0];
+      info->walks_wild += hCnt[b][1];
+      info->wrong_walks += hCnt[b][2];
+      for (uint32_t k = 0; k < ns && nww < cap; k++, nww++) wrong_walks[nww] = pending_first[b] + hSel[b][k];
+    }
+    pending_kind[b] = -1;
+    return 0;
+  };
+  int cur = 0;
+  uint64_t fill = 0;
+  bool okr = true;
+  for (uint32_t h = 0; okr && h < NBUCKET; h++) {      // HashTable::LoadTable order; buckets may span chunks
+    uint32_t nb = 0, mx = 0;
+    okr = fread(&nb, 4, 1, f) == 1 && fread(&mx, 4, 1, f) == 1;
+    uint32_t done_in_bucket = 0;
+    while (okr && done_in_bucket < nb) {
+      if (fill == 0 && drain(cur)) return -3;           // the buffer is free once its previous chunk was counted
+      const uint32_t k = (uint32_t)std::min<uint64_t>(nb - done_in_bucket, chunk - fill);
+      okr = fread(hEnt[cur] + fill, 32, k, f) == k;
+      for (uint32_t q = 0; q < k; q++) { hH[cur][fill + q] = h; hIdx[cur][fill + q] = done_in_bucket + q; }
+      fill += k;
+      done_in_bucket += k;
+      if (fill == chunk) {
+        if (submit(cur, 0, fill, 0)) return -3;
+        cur ^= 1;
+        fill = 0;
+      }
+    }
+  }
+  if (!okr) { snprintf(g_wt_err, sizeof g_wt_err, "%s: the table is cut short", path); return -1; }
+  if (fill) {
+    if (submit(cur, 0, fill, 0)) return -3;
+    cur ^= 1;
+    fill = 0;
+  }
+  uint64_t nwalk = 0;
+  if (fread(&nwalk, 8, 1, f) == 1) {                    // files the reference's -wm wrote end right after the table
+    info->has_walk_count = 1;
+    for (uint64_t first = 0; first < nwalk;) {
+      if (drain(cur)) return -3;
+      const uint64_t k = std::min<uint64_t>(nwalk - first, wchunk);
+      if (fread(hEnt[cur], 96, k, f) != k) { snprintf(g_wt_err, sizeof g_wt_err, "%s: the kangaroo block is cut short", path); return -1; }
+      if (submit(cur, 1, k, first)) return -3;
+      cur ^= 1;
+      first += k;
+    }
+  }
+  if (drain(0) || drain(1)) return -3;
+  info->n_wrong_entries_listed = nwe;
+  info->n_wrong_walks_listed = nww;
+  return 0;
+}
+
+int kgx_work_merge(int dev, const char* const* paths, uint32_t n_paths, const char* tmp_path, uint64_t block_entries,
+                   kgx_work_merge_info* info, kgx_work_collision* coll, uint32_t cap) {
+  using namespace kgx_wt;
+  memset(info, 0, sizeof *info);
+  if (n_paths < 2) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: at least two work files are needed, %u given", n_paths); return -1; }
+  if (block_entries == 0) block_entries = DEFAULT_BLOCK;
+  if (block_entries >= 0x40000000ull) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_work_merge: block of %llu entries (at most 2^30-1)", (unsigned long long)block_entries); return -1; }
+  if (set_device(dev)) return -3;
+  std::vector<FILE*> fs(n_paths, nullptr);
+  struct Closer { std::vector<FILE*>& v; ~Closer() { for (FILE* f : v) if (f) fclose(f); } } closer{fs};
+  std::vector<Header> hd(n_paths);
+  DevBufs B;
+  // Merge.cpp:56-143: every input is checked before anything is written
+  for (uint32_t i = 0; i < n_paths; i++) {
+    errno = 0;
+    fs[i] = fopen(paths[i], "rb");
+    if (!fs[i]) { const int e = errno ? errno : EIO; snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", paths[i], strerror(e)); return -e; }
+    setvbuf(fs[i], nullptr, _IOFBF, 1 << 22);
+    if (!read_header(fs[i], hd[i])) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s is not a HEADW work file", paths[i]); return -1; }
+    if (hd[i].version != hd[0].version) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: cannot merge workfile of different version (%s)", paths[i]); return -1; }
+    int ok = 0;
+    if (key_setup(B, hd[i].kx, hd[i].ky, hd[i].rs, 0, &ok, nullptr, nullptr)) return -3;
+    if (!ok) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: key of %s does not lie on elliptic curve", paths[i]); return -1; }
+    if (memcmp(hd[i].rs, hd[0].rs, 32) || memcmp(hd[i].re, hd[0].re, 32)) {
+      snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: File range differs (%s, %s)", paths[0], paths[i]);
+      return -1;
+    }
+    if (memcmp(hd[i].kx, hd[0].kx, 32) || memcmp(hd[i].ky, hd[0].ky, 32)) {
+      snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: key differs, multiple keys not yet supported (%s, %s)", paths[0], paths[i]);
+      return -1;
+    }
+  }
+  const uint64_t C = block_entries;
+  Entry *hIn, *dIn, *dOut, *hOut;
+  uint32_t *hH, *dH, *idxA, *idxB, *dNsel, *dNb, *hNb;
+  uint64_t *keyA, *keyB;
+  uint8_t* keep;
+  MergeRes* dRes;
+  Coll* dColl;
+  size_t tA = 0, tB = 0, tC = 0;
+  WT_CK(cub::DeviceRadixSort::SortPairs(nullptr, tA, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)C, 0, 64));
+  WT_CK(cub::DeviceRadixSort::SortPairs(nullptr, tB, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)C, 0, 19));
+  WT_CK(cub::DeviceSelect::Flagged(nullptr, tC, (uint32_t*)nullptr, (uint8_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)C));
+  const size_t tmpBytes = std::max(tA, std::max(tB, tC));
+  void* dTmp;
+  if (B.host(&hIn, 32 * C) || B.dev(&dIn, 32 * C) || B.dev(&dOut, 32 * C) || B.host(&hOut, 32 * C) || B.host(&hH, 4 * C) ||
+      B.dev(&dH, 4 * C) || B.dev(&idxA, 4 * C) || B.dev(&idxB, 4 * C) || B.dev(&dNsel, 4) || B.dev(&dNb, 4ull * NBUCKET) ||
+      B.host(&hNb, 4ull * NBUCKET) || B.dev(&keyA, 8 * C) || B.dev(&keyB, 8 * C) || B.dev(&keep, C) || B.dev(&dRes, sizeof(MergeRes)) ||
+      B.dev(&dColl, sizeof(Coll) * C) || B.dev(&dTmp, tmpBytes))
+    return -3;
+  std::vector<Coll> hColl;
+  errno = 0;
+  FILE* out = fopen(tmp_path, "wb");
+  if (!out) { const int e = errno ? errno : EIO; snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: Cannot open %s for writing: %s", tmp_path, strerror(e)); return -e; }
+  setvbuf(out, nullptr, _IOFBF, 1 << 22);
+  uint32_t dp = hd[0].dp;
+  uint64_t cnt = 0;
+  double tm = 0;
+  for (uint32_t i = 0; i < n_paths; i++) { dp = std::min(dp, hd[i].dp); cnt += hd[i].count; tm += hd[i].time; }
+  const uint32_t version = 0;                         // Kangaroo::SaveHeader, Backup.cpp:368-394
+  bool okw = fwrite(&HEADW, 4, 1, out) == 1 && fwrite(&version, 4, 1, out) == 1 && fwrite(&dp, 4, 1, out) == 1 &&
+             fwrite(hd[0].rs, 32, 1, out) == 1 && fwrite(hd[0].re, 32, 1, out) == 1 && fwrite(hd[0].kx, 32, 1, out) == 1 &&
+             fwrite(hd[0].ky, 32, 1, out) == 1 && fwrite(&cnt, 8, 1, out) == 1 && fwrite(&tm, 8, 1, out) == 1;
+  int rc = 0;
+  uint64_t fill = 0;
+  uint32_t b0 = 0;
+  // one block: entries of buckets [b0, b1) in hIn (bucket by bucket, inputs in order within a bucket) -> the merged buckets
+  auto flush = [&](uint32_t b1) -> int {
+    const uint32_t n = (uint32_t)fill, T = 256, G = (n + T - 1) / T;
+    WT_CK(cudaMemsetAsync(dNb, 0, 4ull * (b1 - b0)));
+    if (n) {
+      int bits = 1;
+      while ((1u << bits) < b1 - b0) bits++;
+      size_t tb;
+      WT_CK(cudaMemcpyAsync(dIn, hIn, 32ull * n, cudaMemcpyHostToDevice));
+      WT_CK(cudaMemcpyAsync(dH, hH, 4ull * n, cudaMemcpyHostToDevice));
+      WT_CK(cudaMemsetAsync(dRes, 0, sizeof(MergeRes)));
+      wt_iota<<<G, T>>>(idxA, n);
+      wt_merge_key<<<G, T>>>(dIn, dH, nullptr, n, 0, b0, keyA);
+      tb = tmpBytes; WT_CK(cub::DeviceRadixSort::SortPairs(dTmp, tb, keyA, keyB, idxA, idxB, (int)n, 0, 64));
+      wt_merge_key<<<G, T>>>(dIn, dH, idxB, n, 1, b0, keyA);
+      tb = tmpBytes; WT_CK(cub::DeviceRadixSort::SortPairs(dTmp, tb, keyA, keyB, idxB, idxA, (int)n, 0, 64));
+      wt_merge_key<<<G, T>>>(dIn, dH, idxA, n, 2, b0, keyA);
+      tb = tmpBytes; WT_CK(cub::DeviceRadixSort::SortPairs(dTmp, tb, (uint32_t*)keyA, (uint32_t*)keyB, idxA, idxB, (int)n, 0, bits));
+      wt_merge_scan<<<G, T>>>(dIn, dH, idxB, n, b0, keep, dNb, dRes, dColl);
+      tb = tmpBytes; WT_CK(cub::DeviceSelect::Flagged(dTmp, tb, idxB, keep, idxA, dNsel, (int)n));
+      WT_CK(cudaGetLastError());
+      MergeRes r;
+      uint32_t nk = 0;
+      WT_CK(cudaMemcpy(&r, dRes, sizeof r, cudaMemcpyDeviceToHost));
+      WT_CK(cudaMemcpy(&nk, dNsel, 4, cudaMemcpyDeviceToHost));
+      wt_gather<<<(nk + T - 1) / T, T>>>(dIn, idxA, nk, dOut);
+      WT_CK(cudaGetLastError());
+      WT_CK(cudaMemcpy(hOut, dOut, 32ull * nk, cudaMemcpyDeviceToHost));
+      WT_CK(cudaMemcpy(hNb, dNb, 4ull * (b1 - b0), cudaMemcpyDeviceToHost));
+      info->duplicates += r.dup;
+      info->collisions += r.ncoll;
+      if (r.ncoll) {
+        const size_t c0 = hColl.size();
+        hColl.resize(c0 + r.ncoll);
+        WT_CK(cudaMemcpy(hColl.data() + c0, dColl, sizeof(Coll) * r.ncoll, cudaMemcpyDeviceToHost));
+        std::sort(hColl.begin() + c0, hColl.end(), [](const Coll& a, const Coll& b) { return a.h != b.h ? a.h < b.h : a.seq < b.seq; });
+        if (hColl.size() > cap) hColl.resize(cap);
+      }
+    } else {
+      memset(hNb, 0, 4ull * (b1 - b0));
+    }
+    uint64_t off = 0;
+    for (uint32_t b = b0; okw && b < b1; b++) {
+      const uint32_t nb = hNb[b - b0], md = (nb + 3) & ~3u;
+      okw = fwrite(&nb, 4, 1, out) == 1 && fwrite(&md, 4, 1, out) == 1 && (nb == 0 || fwrite(hOut + off, 32, nb, out) == nb);
+      off += nb;
+      info->entries += nb;
+    }
+    info->blocks++;
+    b0 = b1;
+    fill = 0;
+    return 0;
+  };
+  std::vector<uint32_t> nbs(n_paths);
+  for (uint32_t h = 0; rc == 0 && okw && h < NBUCKET; h++) {
+    uint64_t sum = 0;
+    for (uint32_t i = 0; i < n_paths; i++) {
+      uint32_t mx;
+      if (fread(&nbs[i], 4, 1, fs[i]) != 1 || fread(&mx, 4, 1, fs[i]) != 1) {
+        snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: the table of %s is cut short", paths[i]);
+        rc = -1;
+        break;
+      }
+      sum += nbs[i];
+    }
+    if (rc) break;
+    if (sum > C) {
+      snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: bucket %u holds %llu entries over the inputs, more than a merge block (%llu)", h,
+               (unsigned long long)sum, (unsigned long long)C);
+      rc = -1;
+      break;
+    }
+    if (fill + sum > C && (rc = flush(h)) != 0) break;
+    for (uint32_t i = 0; i < n_paths && rc == 0; i++) {
+      if (nbs[i] && fread(hIn + fill, 32, nbs[i], fs[i]) != nbs[i]) {
+        snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: the table of %s is cut short", paths[i]);
+        rc = -1;
+      }
+      for (uint32_t q = 0; q < nbs[i]; q++) hH[fill + q] = h;
+      fill += nbs[i];
+    }
+  }
+  if (rc == 0 && okw) rc = flush(NBUCKET);
+  const uint64_t zero = 0;                              // the kangaroo count: 0, so that loaders of -ws files take the result
+  okw = okw && fwrite(&zero, 8, 1, out) == 1;
+  okw = fflush(out) == 0 && okw;
+  const int ioerr = errno ? errno : EIO;
+  okw = (fclose(out) == 0) && okw;
+  if (rc == 0 && !okw) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s: %s", tmp_path, strerror(ioerr)); rc = -ioerr; }
+  if (rc) { remove(tmp_path); return rc; }
+  info->dp_bits = dp;
+  info->total_count = cnt;
+  info->total_time = tm;
+  info->n_listed = (uint32_t)hColl.size();
+  for (size_t k = 0; k < hColl.size(); k++) {
+    coll[k].h = hColl[k].h;
+    coll[k].reserved = 0;
+    memcpy(coll[k].d_first, hColl[k].d_first, 16);
+    memcpy(coll[k].d_other, hColl[k].d_other, 16);
+  }
+  return 0;
+}
+
+}  // extern "C"

@@ -1,0 +1,271 @@
+"""Work-file tools on the GPU: check and merge HEADW work files (the reference's -wcheck and -wm / -wmdir).
+
+    python -m kangaroo_b200.worktool check FILE [--device N]
+    python -m kangaroo_b200.worktool merge FILE1 FILE2 [FILE ...] -o DEST [--device N]
+    python -m kangaroo_b200.worktool merge --dir DIR -o DEST [--device N]
+
+`check` recomputes every stored DP (d*G, or key - start*G + d*G for a wild one) and every kangaroo on the GPU
+(libkgx.so, kgx_work_check) and exits 1 when anything is wrong.  `merge` combines files of the same key and range in the order
+given (the entry of the earlier file wins at equal x) with kgx_work_merge, resolves every tame/wild collision with the
+solver's resolver (the reference's CheckKey, build/libkgx_ingest.so), and either prints the key and writes nothing, or writes
+DEST through DEST.tmp, fsync and rename.  The merged file ends with a kangaroo count of 0, so the solver's --resume and the
+reference's -i take it; they start fresh herds.  There is no CPU path: without a device both commands fail."""
+import argparse
+import ctypes
+import math
+import os
+import struct
+import sys
+
+from . import ecmath as ec
+from ._lib import load_library
+
+HEADW = 0xFA6A8001
+TYPE_BIT = 1 << 126                    # b126 of a tagged distance: the herd (HashTable::CalcDistAndType)
+_M64 = (1 << 64) - 1
+
+
+class CheckInfo(ctypes.Structure):
+    """kgx_work_check_info"""
+    _fields_ = [("dp_bits", ctypes.c_uint32), ("has_walk_count", ctypes.c_uint32), ("entries", ctypes.c_uint64),
+                ("wrong_entries", ctypes.c_uint64), ("walks", ctypes.c_uint64), ("walks_tame", ctypes.c_uint64),
+                ("walks_wild", ctypes.c_uint64), ("wrong_walks", ctypes.c_uint64), ("n_wrong_entries_listed", ctypes.c_uint32),
+                ("n_wrong_walks_listed", ctypes.c_uint32)]
+
+
+class MergeInfo(ctypes.Structure):
+    """kgx_work_merge_info"""
+    _fields_ = [("dp_bits", ctypes.c_uint32), ("blocks", ctypes.c_uint32), ("entries", ctypes.c_uint64),
+                ("duplicates", ctypes.c_uint64), ("collisions", ctypes.c_uint64), ("total_count", ctypes.c_uint64),
+                ("total_time", ctypes.c_double), ("n_listed", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+class Collision(ctypes.Structure):
+    """kgx_work_collision"""
+    _fields_ = [("h", ctypes.c_uint32), ("reserved", ctypes.c_uint32), ("d_first", ctypes.c_uint64 * 2),
+                ("d_other", ctypes.c_uint64 * 2)]
+
+
+def _err(lib):
+    return lib.kgx_work_last_error().decode()
+
+
+def _limbs4(v):
+    return (ctypes.c_uint64 * 4)(*[(int(v) >> (64 * k)) & _M64 for k in range(4)])
+
+
+def is_work_file(path):
+    """a regular file that starts with the HEADW magic (Kangaroo::ReadHeader)"""
+    if not os.path.isfile(path):
+        return False
+    with open(path, "rb") as f:
+        raw = f.read(4)
+    return len(raw) == 4 and struct.unpack("<I", raw)[0] == HEADW
+
+
+class CheckResult:
+    def __init__(self, info, wrong_entries, wrong_walks):
+        for name, _ in CheckInfo._fields_:
+            setattr(self, name, getattr(info, name))
+        self.wrong_entry_positions = wrong_entries      # [(bucket, index in bucket)], file order
+        self.wrong_walk_indices = wrong_walks
+
+    @property
+    def ok(self):
+        return self.wrong_entries == 0 and self.wrong_walks == 0
+
+
+def check(path, device=0, chunk=0, cap=16):
+    """kgx_work_check on one file -> CheckResult.  A directory or a file that is not HEADW raises ValueError."""
+    if os.path.isdir(path):
+        raise ValueError("%s is a directory: partitioned work files are not supported" % path)
+    lib = load_library()
+    info = CheckInfo()
+    we = (ctypes.c_uint32 * (2 * cap))()
+    ww = (ctypes.c_uint64 * cap)()
+    rc = lib.kgx_work_check(int(device), os.fsencode(path), int(chunk), ctypes.byref(info), we, ww, cap)
+    if rc == -1:
+        raise ValueError(_err(lib))
+    if rc != 0:
+        raise RuntimeError("kgx_work_check: " + _err(lib))
+    return CheckResult(info, [(we[2 * i], we[2 * i + 1]) for i in range(info.n_wrong_entries_listed)],
+                       [ww[i] for i in range(info.n_wrong_walks_listed)])
+
+
+def check_records(kind, recs, hs, key, range_start, device=0):
+    """kgx_work_check_records: kind 0 = (n, 4) uint64 table entries with their buckets hs, kind 1 = (n, 12) uint64 kangaroo
+    records -> per-record uint8 results (entries: 1 = wrong; kangaroos: 0 wrong, 1 tame, 2 wild)"""
+    import numpy as np
+    recs = np.ascontiguousarray(recs, dtype=np.uint64)
+    n = recs.shape[0]
+    out = np.zeros(n, dtype=np.uint8)
+    hs = np.ascontiguousarray(hs if hs is not None else np.zeros(n), dtype=np.uint32)
+    lib = load_library()
+    rc = lib.kgx_work_check_records(int(device), int(kind), recs.ctypes.data_as(ctypes.c_void_p), hs.ctypes.data_as(ctypes.c_void_p), n,
+                                    _limbs4(key[0]), _limbs4(key[1]), _limbs4(range_start), out.ctypes.data_as(ctypes.c_void_p))
+    if rc != 0:
+        raise (ValueError if rc == -1 else RuntimeError)("kgx_work_check_records: " + _err(lib))
+    return out
+
+
+def comb_table(device=0):
+    """the check's fixed-base table: {(w, j): (x, y)} = j * 2^(4w) * G"""
+    lib = load_library()
+    out = (ctypes.c_uint64 * (480 * 8))()
+    if lib.kgx_work_comb(int(device), out) != 0:
+        raise RuntimeError("kgx_work_comb: " + _err(lib))
+    val = lambda o: sum(int(out[o + k]) << (64 * k) for k in range(4))
+    return {(w, j): (val(8 * (w * 15 + j - 1)), val(8 * (w * 15 + j - 1) + 4)) for w in range(32) for j in range(1, 16)}
+
+
+class MergeResult:
+    def __init__(self, info, collisions):
+        for name, _ in MergeInfo._fields_:
+            setattr(self, name, getattr(info, name))
+        self.collision_list = collisions                # [(h, d_first (2 limbs), d_other (2 limbs))], bucket then x order
+
+
+def merge_files(paths, tmp_path, device=0, block_entries=0, cap=1 << 20):
+    """kgx_work_merge: paths merged in order into tmp_path -> MergeResult.  Refusals (bad inputs, a bucket larger than a
+    block) raise ValueError and leave no tmp_path."""
+    lib = load_library()
+    arr = (ctypes.c_char_p * len(paths))(*[os.fsencode(p) for p in paths])
+    info = MergeInfo()
+    coll = (Collision * cap)()
+    rc = lib.kgx_work_merge(int(device), arr, len(paths), os.fsencode(tmp_path), int(block_entries), ctypes.byref(info), coll, cap)
+    if rc == -1:
+        raise ValueError(_err(lib))
+    if rc != 0:
+        raise RuntimeError("kgx_work_merge: " + _err(lib))
+    return MergeResult(info, [(c.h, (c.d_first[0], c.d_first[1]), (c.d_other[0], c.d_other[1])) for c in coll[:info.n_listed]])
+
+
+def dir_inputs(dirname):
+    """Kangaroo::MergeDir's inputs (Merge.cpp:255-315): every regular HEADW file of the directory, largest first (equal sizes
+    by name, so that the order does not depend on the directory's listing)"""
+    files = [os.path.join(dirname, f) for f in os.listdir(dirname)]
+    files = [f for f in files if not os.path.islink(f) and is_work_file(f)]
+    return sorted(files, key=lambda f: (-os.path.getsize(f), os.path.basename(f)))
+
+
+def validate(paths):
+    """MergeWork's refusals (Merge.cpp:56-143), before the device is touched: fewer than two inputs, a directory, a file that
+    is not HEADW, another version, a key off the curve, another range or another key -> ValueError"""
+    if len(paths) < 2:
+        raise ValueError("MergeWork: at least two work files are needed, %d given" % len(paths))
+    first = None
+    for p in paths:
+        if os.path.isdir(p):
+            raise ValueError("%s is a directory: partitioned work files are not supported" % p)
+        if not is_work_file(p):
+            raise ValueError("MergeWork: %s is not a HEADW work file" % p)
+        with open(p, "rb") as f:
+            version = struct.unpack("<I", f.read(8)[4:])[0]
+        dp, start, end, key, _, _ = read_header(p)
+        x, y = key
+        if not (x < ec.P and y < ec.P and (y * y - x * x * x - 7) % ec.P == 0):
+            raise ValueError("MergeWork: key of %s does not lie on elliptic curve" % p)
+        if first is None:
+            first = (version, start, end, key)
+            continue
+        if version != first[0]:
+            raise ValueError("MergeWork: cannot merge workfile of different version (%s)" % p)
+        if (start, end) != first[1:3]:
+            raise ValueError("MergeWork: File range differs (%s, %s)" % (paths[0], p))
+        if key != first[3]:
+            raise ValueError("MergeWork: key differs, multiple keys not yet supported (%s, %s)" % (paths[0], p))
+
+
+def read_header(path):
+    from .ingest import read_work_header
+    return read_work_header(path)
+
+
+def merge(paths, dest, device=0, block_entries=0, out=print):
+    """Merge `paths` (in order) into dest -> (exit code, private key or None).  A solved key removes DEST.tmp and writes no
+    file (Merge.cpp:218-229); otherwise DEST.tmp is synced and renamed over dest."""
+    validate(paths)
+    tmp = dest + ".tmp"
+    res = merge_files(paths, tmp, device=device, block_entries=block_entries)
+    for p in paths:
+        out("File %s: [DP%d]" % (p, read_header(p)[0]))
+    dp, start, end, pub, _, _ = read_header(tmp)
+    key = ec.add(pub, ec.neg(ec.mul(start))) if start else pub          # Kangaroo::InitSearchKey
+    unresolved, priv = 0, None
+    cross = [c for c in res.collision_list if (c[1][1] ^ c[2][1]) & (TYPE_BIT >> 64)]
+    same_herd = len(res.collision_list) - len(cross)
+    if cross:
+        from .ingest import DPTable
+        t = DPTable(threads=1)
+        try:
+            for h, d1, d2 in cross:
+                priv = t.resolve(d1, d2, key, start)
+                if priv is not None:
+                    break
+                unresolved += 1
+        finally:
+            t.close()
+    if res.n_listed < res.collisions:
+        out("Warning: %d collisions, only the first %d examined" % (res.collisions, res.n_listed))
+    if priv is not None and ec.mul(priv) == pub:
+        os.remove(tmp)
+        out("Key# 0 Pub:  0x%064X\n       Priv: 0x%X" % (pub[0], priv))
+        return 0, priv
+    with open(tmp, "rb+") as f:
+        os.fsync(f.fileno())
+    os.replace(tmp, dest)
+    out("Dead kangaroo: %d" % (res.duplicates + same_herd))
+    out("Total f1+f2: DP count 2^%.2f" % (math.log2(res.entries) if res.entries else float("-inf")))
+    if unresolved:
+        out("Unresolved tame/wild collisions: %d" % unresolved)
+    out("Merged %d files into %s: %d entries, %d duplicates, %d same-herd collisions" %
+        (len(paths), dest, res.entries, res.duplicates, same_herd))
+    return 0, None
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser(prog="python -m kangaroo_b200.worktool", description=__doc__.split("\n\n")[0])
+    sub = ap.add_subparsers(dest="cmd", required=True)
+    c = sub.add_parser("check", help="recompute every DP and kangaroo of a work file on the GPU (-wcheck)")
+    c.add_argument("file")
+    c.add_argument("--device", type=int, default=0)
+    m = sub.add_parser("merge", help="merge work files of the same key and range on the GPU (-wm / -wmdir)")
+    m.add_argument("files", nargs="*")
+    m.add_argument("--dir", default=None, help="merge every HEADW file of DIR, largest first (-wmdir)")
+    m.add_argument("-o", "--output", required=True, metavar="DEST")
+    m.add_argument("--device", type=int, default=0)
+    m.add_argument("--block-entries", type=int, default=0, help="entries per device block, summed over the inputs (0 = 2^22)")
+    a = ap.parse_args(argv)
+    try:
+        if a.cmd == "check":
+            r = check(a.file, device=a.device)
+            pct = 100.0 * (1.0 - r.wrong_entries / r.entries) if r.entries else 100.0
+            print("[%.3f%% OK]" % pct)
+            print("DP: %d" % r.entries)
+            print("DP Wrong: %d" % r.wrong_entries)
+            for h, i in r.wrong_entry_positions:
+                print("  wrong DP at bucket %06X [%d]" % (h, i))
+            if r.has_walk_count:
+                print("Kangaroos: %d (tame OK %d, wild OK %d, wrong %d)" % (r.walks, r.walks_tame, r.walks_wild, r.wrong_walks))
+                for i in r.wrong_walk_indices:
+                    print("  wrong kangaroo #%d" % i)
+            else:
+                print("Kangaroos: none (the file ends after its table)")
+            return 0 if r.ok else 1
+        if a.dir is not None:
+            if a.files:
+                ap.error("merge: give files or --dir, not both")
+            files = dir_inputs(a.dir)
+            if len(files) < 2:
+                raise ValueError("MergeDir: less than 2 work files in the directory")
+        else:
+            files = a.files
+        rc, _ = merge(files, a.output, device=a.device, block_entries=a.block_entries)
+        return rc
+    except ValueError as e:
+        print(str(e), file=sys.stderr)
+        return 2
+
+
+if __name__ == "__main__":
+    sys.exit(main())
