@@ -39,6 +39,7 @@ class DPGather:
         self._slab_fn = slab_fn if slab_fn is not None else (self._engine_slab if wire == "item56" else self._engine_dp40)
         self.total_gathered = 0
         self.last = None
+        self._flat = None                # rank 0: step_flat's receive buffer, allocated by its first call
 
     def _engine_slab(self):
         ptr = self.eng.dp_slab_device_ptr()
@@ -57,62 +58,41 @@ class DPGather:
             self._views[("dp40", ptr)] = v
         return v
 
-    def step(self, n_found):
-        """Gather this launch's DP records to rank 0.  Returns on rank 0 a list of (rank, uint8 tensor [cnt*56]);
-        None elsewhere.  n_found = records this rank produced (capped to max_found here)."""
-        torch, dist = self.torch, self.dist
+    def _gather(self, n_found, recv):
+        """The count exchange and the gather: recv(cap) -> rank 0's receive buffers, one per rank of cap records each.
+        n_found = records this rank produced (capped to max_found here).  Returns (counts list, cap, buffers or None)."""
+        torch = self.torch
         cnt = min(int(n_found), self.max_found)
         mine = torch.tensor([cnt], dtype=torch.int32, device=self.device)
         counts = torch.empty(self.world, dtype=torch.int32, device=self.device)
-        dist.all_gather_into_tensor(counts, mine)
+        self.dist.all_gather_into_tensor(counts, mine)
         counts_h = counts.cpu().tolist()
-        cap = max(ROUND, (max(counts_h) + ROUND - 1) // ROUND * ROUND)
-        cap = min(cap, self.max_found)
-        slab = self._slab_fn()
-        local = slab[4:4 + cap * self.rec]
-        if self.rank == 0:
-            bufs = [torch.empty(cap * self.rec, dtype=torch.uint8, device=self.device) for _ in range(self.world)]
-            dist.gather(local, bufs, dst=0)
-            out = [(r, bufs[r][:counts_h[r] * self.rec]) for r in range(self.world)]
-        else:
-            dist.gather(local, None, dst=0)
-            out = None
+        cap = min(max(ROUND, (max(counts_h) + ROUND - 1) // ROUND * ROUND), self.max_found)
+        local = self._slab_fn()[4:4 + cap * self.rec]
+        bufs = recv(cap) if self.rank == 0 else None
+        self.dist.gather(local, bufs, dst=0)
         if self.device.type == "cuda":
             torch.cuda.current_stream().synchronize()   # the slab is recycled by the launch after next
         self.total_gathered += sum(counts_h)
-        self.last = out
-        return out
+        return counts_h, cap, bufs
 
+    def step(self, n_found):
+        """Gather this launch's DP records to rank 0.  Returns on rank 0 a list of (rank, uint8 tensor [cnt*56]);
+        None elsewhere."""
+        counts, cap, bufs = self._gather(n_found, lambda cap: [self.torch.empty(cap * self.rec, dtype=self.torch.uint8,
+                                                                                  device=self.device) for _ in range(self.world)])
+        self.last = [(r, bufs[r][:counts[r] * self.rec]) for r in range(self.world)] if self.rank == 0 else None
+        return self.last
 
-def _step_flat(self, n_found):
-    """Like step(), but rank 0 receives every rank's records in ONE contiguous device tensor (rank r at offset r*cap*rec),
-    so that the whole step's DPs reach the host with a single copy.  Returns (counts list, cap, tensor) on rank 0, None elsewhere."""
-    torch, dist = self.torch, self.dist
-    cnt = min(int(n_found), self.max_found)
-    mine = torch.tensor([cnt], dtype=torch.int32, device=self.device)
-    counts = torch.empty(self.world, dtype=torch.int32, device=self.device)
-    dist.all_gather_into_tensor(counts, mine)
-    counts_h = counts.cpu().tolist()
-    cap = max(ROUND, (max(counts_h) + ROUND - 1) // ROUND * ROUND)
-    cap = min(cap, self.max_found)
-    local = self._slab_fn()[4:4 + cap * self.rec]
-    out = None
-    if self.rank == 0:
-        if getattr(self, "_flat", None) is None:
-            self._flat = torch.empty(self.world * self.max_found * self.rec, dtype=torch.uint8, device=self.device)
-        n = cap * self.rec
-        bufs = [self._flat[r * n:(r + 1) * n] for r in range(self.world)]
-        dist.gather(local, bufs, dst=0)
-        out = (counts_h, cap, self._flat)
-    else:
-        dist.gather(local, None, dst=0)
-    if self.device.type == "cuda":
-        torch.cuda.current_stream().synchronize()   # the slab is recycled by the launch after next
-    self.total_gathered += sum(counts_h)
-    return out
-
-
-DPGather.step_flat = _step_flat
+    def step_flat(self, n_found):
+        """Like step(), but rank 0 receives every rank's records in ONE contiguous device tensor (rank r at offset r*cap*rec),
+        so that the whole step's DPs reach rank 0's table with a single copy.  Returns (counts list, cap, tensor) on rank 0,
+        None elsewhere."""
+        if self.rank == 0 and self._flat is None:
+            self._flat = self.torch.empty(self.world * self.max_found * self.rec, dtype=self.torch.uint8, device=self.device)
+        counts, cap, _ = self._gather(n_found, lambda cap: [self._flat[r * cap * self.rec:(r + 1) * cap * self.rec]
+                                                            for r in range(self.world)])
+        return (counts, cap, self._flat) if self.rank == 0 else None
 
 
 WALK_BYTES = 96          # one kangaroo of a work file (Backup.cpp:536-539)

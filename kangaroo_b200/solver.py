@@ -13,7 +13,7 @@ Per step (= one GPUEngine::Launch on every rank) nothing on the data path is Pyt
               -> events: KGI_EV_COLLISION -> kgi_resolve (CollisionCheck/CheckKey with the reference's Secp256K1)
                          KGI_EV_RESET     -> (rank, kIdx) sent back to the owner, which re-creates that kangaroo
                                              (Kangaroo.cpp:601-609: CreateHerd(1) + SetKangaroo)
-  all ranks   one small broadcast: [stop, n_resets, (rank, kIdx) ...]
+  all ranks   one small broadcast: [table stopped, n_resets, save next, chunks, n_solved, solved keys ..., (rank, kIdx) ...]
 
 With --dp-table device, rank 0's table is ingest.DeviceDPTable in its GPU's memory (same events and work files): the step's
 records are copied device to device into a staging buffer and inserted from there by the ingest thread on its own stream, no
@@ -34,7 +34,9 @@ file holds them dead: a resumed run finds them again.  A save goes to FILE.tmp, 
 save removes FILE.tmp and the run goes on.  On --resume only rank 0 reads the file.
 """
 import argparse
+import contextlib
 import ctypes
+import functools
 import os
 import queue
 import sys
@@ -58,13 +60,6 @@ SAVE_BUFFERS = 4          # rank 0's pinned chunk buffers queued to the writer
 DP_TABLE_MARGIN = 4 << 30 # --dp-table device without a capacity: rank 0's free GPU memory after the engine, its staging
                           # buffers and the table's reserved per-add scratch, less this margin for NCCL, the gather buffer
                           # and torch's allocator.  Nothing else grows on the GPU: steps queued behind a save wait in host RAM
-
-
-class DeviceBatch:
-    """one step's records of every rank for the device table: a device buffer, rank r's counts[r] records at r*stride*40"""
-
-    def __init__(self, buf, counts, stride, event, jumps_before):
-        self.buf, self.counts, self.stride, self.event, self.jumps_before = buf, counts, stride, event, jumps_before
 
 
 def scratch_bytes(n_records):
@@ -111,6 +106,133 @@ def dp_mask(bits):
     return 0 if bits == 0 else (~((1 << (64 - min(bits, 64))) - 1)) & 0xFFFFFFFFFFFFFFFF
 
 
+# Rank 0's DP table, --dp-table host or device.  Each step's records land in one of two staging buffers: while the ingest
+# thread inserts step k's records, step k+1's land in the other one.  The NCCL kernels of a step cannot start before the jump
+# launch that occupies every SM has finished, so without this decoupling the insert would sit exposed between two launches.
+# A step parked behind a save (Solver._submit) gets a buffer of its own in host RAM instead.  stage() runs on the main
+# thread; insert() and save() (the header and the table of a work file) run on the ingest thread.
+class HostTable:
+    """the reference's HashTable in host RAM (ingest.DPTable), fed through pinned buffers"""
+    label = "ingest"
+
+    def __init__(self, torch, n_records, threads):
+        self.torch = torch
+        self.dps = DPTable(threads=threads)
+        self._bufs = [torch.empty(n_records * DP40_BYTES, dtype=torch.uint8).pin_memory() for _ in range(2)]
+        self._i = 0
+        self.save = self.dps.save_work
+        self.info = "ingest threads: %d" % self.dps.threads
+
+    def stage(self, counts, stride, src, park):
+        nbytes = len(counts) * stride * DP40_BYTES
+        if park:
+            buf = self.torch.empty(nbytes, dtype=self.torch.uint8)
+        else:
+            buf, self._i = self._bufs[self._i], self._i ^ 1
+        buf[:nbytes].copy_(src[:nbytes], non_blocking=True)
+        self.torch.cuda.current_stream().synchronize()
+        h = buf.numpy()
+        return [(r, h[r * stride * DP40_BYTES: (r * stride + c) * DP40_BYTES]) for r, c in enumerate(counts)]
+
+    def insert(self, segments):
+        return [ev for r, buf in segments if buf.size != 0 for ev in self.dps.add_dp40(buf, r)]
+
+
+class DeviceTable:
+    """ingest.DeviceDPTable in rank 0's GPU memory, fed from device staging buffers on a stream of the ingest thread's own.
+    The two staging buffers and a third one, which takes parked records back to the GPU, are all the GPU memory the records
+    take; the table's per-add scratch is reserved up front, so the table needs no allocation while it runs."""
+    label = "device table"
+
+    def __init__(self, torch, n_records, device, capacity, wait_copy):
+        """wait_copy: the records' source is rewritten unordered with torch's stream (the engine's own buffer, on one GPU)"""
+        self.torch, self._wait_copy = torch, wait_copy
+        self._bufs = [torch.empty(n_records * DP40_BYTES, dtype=torch.uint8, device=torch.device("cuda", device)) for _ in range(3)]
+        self._back = self._bufs.pop()
+        if not capacity:
+            capacity = default_table_capacity(torch.cuda.mem_get_info(device)[0] - scratch_bytes(n_records))
+        self.dps = DeviceDPTable(capacity, device=device)
+        self.dps.reserve(n_records)
+        self._stream = torch.cuda.Stream(device=device)
+        self._i = 0
+        self.save = functools.partial(self.dps.save_work, stream=self._stream.cuda_stream)
+        self.info = "dp table: device, capacity %d entries (%.2f GB)" % (self.dps.capacity, self.dps.memory_bytes() / 1e9)
+
+    def stage(self, counts, stride, src, park):
+        """the records are copied device to device (torch's stream), since the gather buffer and the engine's record buffer
+        are rewritten by the next step; insert() runs behind that copy"""
+        nbytes = len(counts) * stride * DP40_BYTES
+        if park:
+            buf = self.torch.empty(nbytes, dtype=self.torch.uint8)
+            buf.copy_(src[:nbytes])                         # to pageable memory: complete when it returns
+            return buf, list(counts), stride, None
+        buf, self._i = self._bufs[self._i], self._i ^ 1
+        buf[:nbytes].copy_(src[:nbytes], non_blocking=True)
+        ev = self.torch.cuda.Event()
+        ev.record()
+        if self._wait_copy:
+            ev.synchronize()
+        return buf, list(counts), stride, ev
+
+    def insert(self, batch):
+        buf, counts, stride, ev = batch
+        if ev is None:                                      # parked in host RAM: back to the GPU, on this stream
+            with self.torch.cuda.stream(self._stream):
+                self._back[:buf.numel()].copy_(buf)
+            buf = self._back
+        else:
+            self._stream.wait_event(ev)                     # the records' copy into the staging buffer
+        return self.dps.add(buf.data_ptr(), counts, stride, self._stream.cuda_stream)
+
+
+class WorkFile:
+    """One work file as it is written: begin() puts the header and the table in FILE.tmp, append() adds herd records and
+    finish() fsyncs it, renames it over FILE and fsyncs the directory, so the previous FILE stays whole until then.  After an
+    error nothing more is written and finish() removes FILE.tmp."""
+
+    def __init__(self, path, t0):
+        self.path, self.tmp, self.t0, self.err, self.f = path, path + ".tmp", t0, None, None
+
+    def begin(self, write_table):
+        """write_table(path): the header and the table"""
+        try:
+            write_table(self.tmp)
+            self.f = open(self.tmp, "ab")
+        except (OSError, RuntimeError) as e:
+            self.err = str(e)
+
+    def append(self, data):
+        try:
+            if self.f is not None and self.err is None:
+                self.f.write(data)
+        except OSError as e:
+            self.err = str(e)
+
+    def finish(self):
+        """-> (path, MB, seconds since t0, error or None)"""
+        size = 0
+        try:
+            if self.err is None:
+                self.f.flush()
+                os.fsync(self.f.fileno())
+                size = self.f.tell()
+                self.f.close()
+                os.replace(self.tmp, self.path)
+                dfd = os.open(os.path.dirname(os.path.abspath(self.path)), os.O_RDONLY)
+                try:
+                    os.fsync(dfd)
+                finally:
+                    os.close(dfd)
+        except OSError as e:
+            self.err = str(e)
+        if self.f is not None:
+            self.f.close()                                  # a no-op when closed above
+        if self.err is not None:
+            with contextlib.suppress(OSError):
+                os.remove(self.tmp)
+        return self.path, size / 1048576.0, time.perf_counter() - self.t0, self.err
+
+
 class Solver:
     def __init__(self, start, end, pub, dp_bits, grid=None, max_found=1 << 17, seed=None, ingest_threads=0,
                  save_work="", save_interval=0.0, save_kangaroos=False, resume=None, dp_table="host", dp_table_capacity=None):
@@ -143,42 +265,28 @@ class Solver:
         sc, d128 = random_herd_arrays(n, self.range_power, self.wdiv2, self.rng)
         self._create_herd(sc, d128)
         self.gather = DPGather(self.eng, self.dist, self.rank, self.world, torch, wire="dp40") if self.world > 1 else None
-        self.dev_table = dp_table == "device"
-        self.table_label = "device table" if self.dev_table else "ingest"
         # rank 0's table stopped taking records: "full" (TableFull) or "error" (any other failure of an insert), with its message
         self.table_msg, self.table_kind, self.table_stopped = None, None, False
         self.last_saved = None              # rank 0: path of the last save that succeeded
-        self.parked = 0                     # rank 0, device table: steps whose records waited in host RAM behind a save
-        if self.rank == 0 and self.dev_table:
-            # rank 0: the table in this GPU's memory, fed from device buffers on a stream of the ingest thread's own.  Two staging
-            # buffers (below) and one for records parked in host RAM during a save (_add_device) are all the GPU memory the
-            # records take; the table's per-add scratch is reserved up front, so the table needs no allocation while it runs.
-            nbuf = self.world * max_found * DP40_BYTES
-            self._hosts = [torch.empty(nbuf, dtype=torch.uint8, device=torch.device("cuda", self.local)) for _ in range(3)]
-            self._back = self._hosts.pop()
-            if not dp_table_capacity:
-                dp_table_capacity = default_table_capacity(torch.cuda.mem_get_info(self.local)[0] - scratch_bytes(self.world * max_found))
-            self.dps = DeviceDPTable(dp_table_capacity, device=self.local)
-            self.dps.reserve(self.world * max_found)
-            self._istream = torch.cuda.Stream(device=self.local)
-        else:
-            self.dps = DPTable(threads=ingest_threads) if self.rank == 0 else None      # rank 0: the reference HashTable
-        # Two pinned staging buffers (device buffers for the device table): while the ingest thread inserts step k's records,
-        # step k+1's land in the other one.  The NCCL kernels of a step cannot start before the jump launch that occupies every
-        # SM has finished, so without this decoupling the insert would sit exposed between two launches.
-        if not (self.rank == 0 and self.dev_table):
-            self._hosts = ([torch.empty(self.world * max_found * DP40_BYTES, dtype=torch.uint8).pin_memory() for _ in range(2)]
-                           if self.rank == 0 else None)
-        self._hidx = 0
+        self.full_saved = None              # rank 0: (path, count, error or None) of the save a full table made
+        self.parked = 0                     # rank 0: steps whose records waited in host RAM behind a save
+        self.found = None                   # rank 0: the private key, once found
+        self._announce = []                 # rank 0: keys solved, not yet in a control broadcast
+        self.dpt = self.dps = None          # rank 0: HostTable / DeviceTable, and the table it holds
+        if self.rank == 0:
+            self.dpt = (DeviceTable(torch, self.world * max_found, self.local, dp_table_capacity, self.gather is None)
+                        if dp_table == "device" else HostTable(torch, self.world * max_found, ingest_threads))
+            self.dps = self.dpt.dps
         self._work = queue.Queue()
         self._done = queue.Queue()
         self._pending = 0
-        self._acc_found, self._acc_resets = None, []
+        self._acc_hits, self._acc_resets = [], []
+        self._wf = None                     # ingest thread: the scheduled work file being written
         self._thread = None
         if self.rank == 0:
             self._thread = threading.Thread(target=self._ingest_loop, daemon=True)
             self._thread.start()
-        self._ctrl = torch.zeros(4 + 2 * MAX_RESETS, dtype=torch.int64, device="cuda")
+        self._ctrl = torch.zeros(5 + MAX_SOLVED + 2 * MAX_RESETS, dtype=torch.int64, device="cuda")
         self.jumps = 0
         self.same_herd = 0
         self.resets_done = 0
@@ -260,7 +368,7 @@ class Solver:
         self._save_stats.append(self._save_steps)
         if self.rank == 0:
             nwalk = self.herd.total if kangaroos else 0
-            self._work.put(("begin", self.save_path, self.jumps, self.time_offset + time.time() - self.t_start, nwalk, time.perf_counter()))
+            self._work.put(("begin", self.jumps, self.time_offset + time.time() - self.t_start, nwalk, time.perf_counter()))
         self._save_progress(chunks)
 
     def _save_progress(self, chunks):
@@ -280,58 +388,35 @@ class Solver:
             self._saving = False
 
     def _write(self, job):
-        """ingest thread: one piece of a work file (jobs arrive in file order)"""
+        """ingest thread: one piece of a scheduled work file (jobs arrive in file order)"""
         kind = job[0]
         if kind == "begin":
-            path, count, total_time, nwalk, self._wt0 = job[1:]
-            self._wpath, self._wtmp, self._werr, self._wf = path, path + ".tmp", None, None
-            if self.table_msg is not None and not self._full_save:
-                self._werr = "the DP table lacks DPs of the launches this file would count (%s)" % self.table_msg
-                return
-            kw = dict(stream=self._istream.cuda_stream) if self.dev_table else {}
-            try:
-                self.dps.save_work(self._wtmp, self.dp_bits, self.start, self.end, self.pub, total_count=count,
-                                   total_time=total_time, total_walk=nwalk, **kw)
-                self._wf = open(self._wtmp, "ab")
-            except (OSError, RuntimeError) as e:
-                self._werr = str(e)
+            count, total_time, nwalk, t0 = job[1:]
+            self._wf = WorkFile(self.save_path, t0)
+            if self.table_msg is not None:
+                self._wf.err = "the DP table lacks DPs of the launches this file would count (%s)" % self.table_msg
+            else:
+                self._write_table(self._wf, count, total_time, nwalk)
         elif kind == "chunk":
             buf, nbytes = job[1], job[2]
             try:
-                if self._wf is not None and self._werr is None:
-                    self._wf.write(memoryview(buf.numpy()[:nbytes]))
-            except OSError as e:
-                self._werr = str(e)
+                self._wf.append(memoryview(buf.numpy()[:nbytes]))
             finally:
                 self._chunk_pool.put(buf)
         else:
-            size = 0
-            try:
-                if self._werr is None:
-                    self._wf.flush()
-                    os.fsync(self._wf.fileno())
-                    size = self._wf.tell()
-                    self._wf.close()
-                    self._wf = None
-                    os.replace(self._wtmp, self._wpath)          # the previous checkpoint stays whole until here
-                    dfd = os.open(os.path.dirname(os.path.abspath(self._wpath)), os.O_RDONLY)
-                    try:
-                        os.fsync(dfd)
-                    finally:
-                        os.close(dfd)
-            except OSError as e:
-                self._werr = str(e)
-            if self._werr is not None:
-                if self._wf is not None:
-                    self._wf.close()
-                    self._wf = None
-                try:
-                    os.remove(self._wtmp)
-                except OSError:
-                    pass
-            res = (self._wpath, size / 1048576.0, time.perf_counter() - self._wt0, self._werr)
-            self._on_saved(*res)
-            self._saved.put(res + (not self._full_save,))   # the full-table save was not scheduled by the main thread
+            self._finish(self._wf, scheduled=True)
+            self._wf = None
+
+    def _write_table(self, wf, count, total_time, nwalk):
+        wf.begin(lambda tmp: self.dpt.save(tmp, self.dp_bits, self.start, self.end, self.pub, total_count=count,
+                                           total_time=total_time, total_walk=nwalk))
+
+    def _finish(self, wf, scheduled):
+        """ingest thread: close a work file -> its error or None.  scheduled: begun by _save_start (not the full table's save)"""
+        res = wf.finish()
+        self._on_saved(*res)
+        self._saved.put(res + (scheduled,))
+        return res[3]
 
     def _on_saved(self, path, mb, seconds, err):
         """ingest thread, right after a save finished (or failed)"""
@@ -354,58 +439,45 @@ class Solver:
                   (path, mb, secs, len(st), 1e3 * max(st or [0]), 1e3 * float(np.median(self._step_times[-64:] or [0]))), flush=True)
 
     # -- rank 0: ingest -------------------------------------------------------------------------------------------
-    def _events_of(self, segments):
-        """the table's events for one step's records: segments is a list of (rank, uint8 numpy view of that rank's 40-byte
-        records) for the host table, a DeviceBatch for the device table"""
-        if isinstance(segments, DeviceBatch):
-            return self._add_device(segments)
-        return (ev for r, buf in segments if buf.size != 0 for ev in self.dps.add_dp40(buf, r))
-
-    def _add_device(self, b):
+    def _events(self, batch, jumps_before):
+        """the table's events for one step's records"""
         if self.table_msg is not None:                  # the run is stopping: later steps' DPs are not inserted
             return []
-        if b.event is None:                             # parked in host RAM behind a save: back to the GPU, on this stream
-            with self.torch.cuda.stream(self._istream):
-                self._back[:b.buf.numel()].copy_(b.buf)
-            buf = self._back
-        else:
-            self._istream.wait_event(b.event)           # the records' copy into the staging buffer
-            buf = b.buf
         try:
-            return self.dps.add(buf.data_ptr(), b.counts, b.stride, self._istream.cuda_stream)
+            return self.dpt.insert(batch)
         except TableFull as e:
-            self._on_full(str(e), b.jumps_before)
+            self._on_full(str(e), jumps_before)
             return []
-
-    _full_save = False
 
     def _on_full(self, msg, jumps_before):
         """ingest thread: the table cannot take this step's records.  With --save-work, and no save open, the table is written
         at once as the cut it is: the launches before this one, without kangaroos (their state of that cut is gone)."""
         self.table_msg, self.table_kind = msg, "full"
-        if self.save_path and getattr(self, "_wf", None) is None:
-            self._full_save = True
-            self._write(("begin", self.save_path, jumps_before, self.time_offset + time.time() - self.t_start, 0, time.perf_counter()))
-            self._write(("end",))
-            self._full_save = False
-            self.full_saved = (self.save_path, jumps_before, getattr(self, "_werr", None))
+        if self.save_path and self._wf is None:
+            wf = WorkFile(self.save_path, time.perf_counter())
+            self._write_table(wf, jumps_before, self.time_offset + time.time() - self.t_start, 0)
+            self.full_saved = (self.save_path, jumps_before, self._finish(wf, scheduled=False))
 
-    def _ingest(self, segments):
-        """segments: see _events_of.  Returns (key or None, resets)."""
-        found, resets = None, []
-        t0 = time.perf_counter()
-        for kind, rk, kidx, d_old, d_new in self._events_of(segments):
-            if kind == EV_COLLISION and found is None:
-                found = self.dps.resolve(d_old, d_new, self.key, self.start)     # Kangaroo.cpp:255-302
-                if found is None:
+    def _ingest(self, events):
+        """rank 0, ingest thread: one step's events -> (hits [(key index, private key, rank, kIdx)], resets).  Resolving stops
+        at the first key found."""
+        hits, resets = [], []
+        for kind, rk, kidx, d_old, d_new in events:
+            if kind == EV_COLLISION and not hits:
+                priv = self.dps.resolve(d_old, d_new, self.key, self.start)      # Kangaroo.cpp:255-302
+                if priv is None:
                     resets.append((rk, kidx))                                    # "unexpected wrong collision, reset kangaroo"
+                else:
+                    hits.append((0, priv, rk, kidx))
             elif kind == EV_RESET:
                 resets.append((rk, kidx))
-        self.t_ingest += time.perf_counter() - t0
-        return found, resets
+        return hits, resets
 
-    def _no_events(self):
-        return None, []
+    def _claim(self, hits, resets):
+        """rank 0: the first hit solves the key; the run stops, so later hits are ignored"""
+        if hits and self.found is None:
+            self.found = hits[0][1]
+            self._announce.append(0)
 
     def _ingest_loop(self):
         while True:
@@ -414,48 +486,46 @@ class Solver:
                 return
             if job[0] == "dps":
                 try:
-                    res = self._ingest(job[1])
+                    t0 = time.perf_counter()
+                    res = self._ingest(self._events(*job[1:]))
+                    self.t_ingest += time.perf_counter() - t0
                 except Exception as e:                  # the table failed: stop the run (every rank, next step) instead of
                     if self.table_msg is None:          # leaving the main thread waiting for this step's result
                         self.table_msg, self.table_kind = "%s: %s" % (type(e).__name__, e), "error"
-                    res = self._no_events()
+                    res = [], []
                 self._done.put(res)
             else:
                 self._write(job)
 
-    def _submit(self, segs):
-        """hand one step's records to the ingest thread"""
-        self._work.put(("dps", segs))
+    def _submit(self, counts, stride, src, jumps_before):
+        """hand one step's records (counts[r] of rank r at src[r*stride*40:], device memory) to the ingest thread.  At most
+        one older step may still be in that thread, reading the other staging buffer.  While a save keeps it busy, further
+        steps are parked in host RAM instead of waiting: the step loop never waits for the disk, and the backlog takes no GPU
+        memory however long the save lasts."""
+        park = self._pending >= 2 and self._writes_pending()
+        if park:
+            self.parked += 1
+        while not park and self._pending >= 2:
+            self._take()
+        self._work.put(("dps", self.dpt.stage(counts, stride, src, park), jumps_before))
         self._pending += 1
-
-    def _staging(self, nbytes):
-        """the staging buffer for this step; at most one older step may still be in the ingest thread (it reads the OTHER
-        pinned buffer).  While a save keeps that thread busy, further steps get a buffer of their own instead of waiting."""
-        if self._pending >= 2 and self._writes_pending():
-            return self.torch.empty(nbytes, dtype=self.torch.uint8)
-        while self._pending >= 2:
-            self._take(block=True)
-        host = self._hosts[self._hidx]
-        self._hidx ^= 1
-        return host
 
     def _writes_pending(self):
         return self._saving or len(self._save_stats) > 0
 
-    def _take(self, block):
-        f, r = self._done.get(block=block)
+    def _take(self):
+        hits, resets = self._done.get()
         self._pending -= 1
-        if self._acc_found is None:
-            self._acc_found = f
-        self._acc_resets += r
+        self._acc_hits += hits
+        self._acc_resets += resets
 
     def _harvest(self, wait_all=False):
-        """results of the inserts finished so far -> (key or None, resets)"""
+        """results of the inserts finished so far -> (hits, resets)"""
         while self._pending and (wait_all or not self._done.empty()):
-            self._take(block=True)
-        found, resets = self._acc_found, self._acc_resets
-        self._acc_found, self._acc_resets = None, []
-        return found, resets
+            self._take()
+        res = self._acc_hits, self._acc_resets
+        self._acc_hits, self._acc_resets = [], []
+        return res
 
     def _wild_key(self, kidx):
         return self.key
@@ -475,12 +545,16 @@ class Solver:
         self.eng.SetKangaroo(kidx, pos[0], pos[1], d)
         self.resets_done += 1
 
+    def _solved(self, solved):
+        """every rank: the keys solved this step (every rank follows rank 0's broadcast) -> True when the run is done"""
+        return bool(solved)
+
     def step(self, may_save=True):
-        """one Launch on every rank; returns the private key on rank 0 when found (None otherwise)"""
+        """one Launch on every rank"""
         torch = self.torch
         n_found = self.eng.collect_count(relaunch=True)                  # launch i done, launch i+1 running
         self._gather(n_found)
-        found, resets = None, []
+        solved, resets = [], []
         self._save_work_done = self._save_due or self._saving
         if self._save_due:                                               # decided at the end of the previous step
             self._save_due = False
@@ -489,28 +563,28 @@ class Solver:
         elif self._saving:
             self._save_progress(self._chunks_next)
         if self.rank == 0:
-            found, resets = self._harvest()
+            hits, resets = self._harvest()
+            self._claim(hits, resets)
+            solved, self._announce = self._announce[:MAX_SOLVED], self._announce[MAX_SOLVED:]
             self.table_stopped = self.table_msg is not None
         save_next = (may_save and self.save_interval > 0 and self.rank == 0 and not self._saving and
                      time.time() - self._last_save >= self.save_interval)
         # herd chunks the next step may move: only into pinned buffers the writer has already freed, so a step never waits for
         # the disk (rank 0 decides, every rank follows)
         chunks = min(SAVE_CHUNKS_PER_STEP, self._chunk_pool.qsize()) if self.rank == 0 else 0
-        # control word: stop flag + save flag + kangaroos to re-create, back to their owners
+        # control word: table stopped + save flag + chunks + keys solved + kangaroos to re-create, back to their owners
         if self.dist is not None:
             if self.rank == 0:
                 resets = resets[:MAX_RESETS]
-                c = [2 if self.table_stopped else (1 if found is not None else 0), len(resets), int(save_next), chunks] + \
+                c = [int(self.table_stopped), len(resets), int(save_next), chunks, len(solved)] + solved + \
                     [v for rk in resets for v in rk]
                 self._ctrl[:len(c)].copy_(torch.tensor(c, dtype=torch.int64))
             self.dist.broadcast(self._ctrl, 0)
             c = self._ctrl.cpu().tolist()
-            self.stop = bool(c[0])
-            self.table_stopped = c[0] == 2
-            save_next, chunks = bool(c[2]), c[3]
-            resets = [(c[4 + 2 * i], c[5 + 2 * i]) for i in range(c[1])]
-        else:
-            self.stop = found is not None or self.table_stopped
+            self.table_stopped, save_next, chunks, ns = bool(c[0]), bool(c[2]), c[3], c[4]
+            solved = c[5:5 + ns]
+            resets = [(c[5 + ns + 2 * i], c[6 + ns + 2 * i]) for i in range(c[1])]
+        self.stop = self._solved(solved) or self.table_stopped          # (--batch-keys: retargets, before the resets below)
         self._chunks_next = chunks
         if save_next and not self.stop:
             if self.save_kangaroos:
@@ -520,72 +594,31 @@ class Solver:
             self.same_herd += 1
             if rk == self.rank and not self.stop:
                 self._reset_kangaroo(kidx)
-        return found
 
     def _gather(self, n_found):
         """this launch's DP records of every rank -> rank 0's ingest thread"""
-        torch = self.torch
         cnt = min(n_found, self.eng.maxFound)
         jumps_before = self.jumps
         self.jumps += self.eng.nbKangaroo * NB_RUN * self.world
+        res = None
         if self.gather is not None:
-            res = self.gather.step_flat(cnt)                                # rank 0: (counts, cap, device tensor [world*cap*40])
-            if self.rank == 0 and self.dev_table:
-                counts, cap, flat = res
-                self._submit_device(flat, counts, cap, jumps_before)
-            elif self.rank == 0:
-                counts, cap, flat = res
-                nbytes = self.world * cap * DP40_BYTES
-                host = self._staging(nbytes)
-                host[:nbytes].copy_(flat[:nbytes], non_blocking=True)
-                torch.cuda.current_stream().synchronize()
-                h = host.numpy()
-                self._submit([(r, h[r * cap * DP40_BYTES: r * cap * DP40_BYTES + counts[r] * DP40_BYTES]) for r in range(self.world)])
-        else:
-            if cnt and self.dev_table:
-                ptr = self.eng.convert_dps_device_ptr()
-                self._submit_device(torch.as_tensor(SlabView(ptr + 4, cnt * DP40_BYTES), device="cuda"), [cnt], cnt, jumps_before)
-            elif cnt:
-                ptr = self.eng.convert_dps_device_ptr()
-                dev = torch.as_tensor(SlabView(ptr + 4, cnt * DP40_BYTES), device="cuda")
-                host = self._staging(cnt * DP40_BYTES)
-                host[:cnt * DP40_BYTES].copy_(dev, non_blocking=True)
-                torch.cuda.current_stream().synchronize()
-                self._submit([(0, host.numpy()[:cnt * DP40_BYTES])])
-
-    def _submit_device(self, src, counts, stride, jumps_before):
-        """--dp-table device: the step's records stay on the GPU.  They are copied (device to device, torch's stream) into a
-        staging buffer, since the gather buffer and the engine's record buffer are rewritten by the next step, and the ingest
-        thread inserts them from there on its own stream behind that copy."""
-        nbytes = len(counts) * stride * DP40_BYTES
-        if self._pending >= 2 and self._writes_pending():
-            # a save holds the ingest thread: the steps queued behind it wait in host RAM, as with the host table, so the
-            # backlog takes no GPU memory however long the save lasts; the ingest thread copies each one back to insert it
-            buf = self.torch.empty(nbytes, dtype=self.torch.uint8)
-            buf.copy_(src[:nbytes])                     # to pageable memory: complete when it returns
-            ev = None
-            self.parked += 1
-        else:
-            buf = self._staging(nbytes)
-            buf[:nbytes].copy_(src[:nbytes], non_blocking=True)
-            ev = self.torch.cuda.Event()
-            ev.record()
-            if self.gather is None:
-                # the engine rewrites its record buffer on its own stream at the next convert, unordered with torch's stream
-                ev.synchronize()
-        self._submit(DeviceBatch(buf, list(counts), stride, ev, jumps_before))
+            res = self.gather.step_flat(cnt)                             # rank 0: (counts, cap, device tensor [world*cap*40])
+        elif cnt:
+            ptr = self.eng.convert_dps_device_ptr()
+            res = [cnt], cnt, self.torch.as_tensor(SlabView(ptr + 4, cnt * DP40_BYTES), device="cuda")
+        if res is not None:
+            self._submit(*res, jumps_before)
 
     def run(self, max_steps=1 << 30, verbose=True):
         self.eng.callKernel()
         t0 = time.time()
         self.t_start = self._last_save = t0
-        key = None
         steps = 0
         self.steady = None                      # (time, jumps) after the first 32 steps: NCCL communicator set-up, first table growth
         self._step_times = step_times = []
         for s in range(max_steps):
             ts = time.perf_counter()
-            key = self.step(may_save=s + 1 < max_steps)
+            self.step(may_save=s + 1 < max_steps)
             step_times.append(time.perf_counter() - ts)
             if self._save_work_done:
                 self._save_steps.append(step_times[-1])
@@ -598,7 +631,7 @@ class Solver:
                 dt = time.time() - t0
                 print("[%6.1fs] 2^%.2f jumps  %.0f MJump/s  %d DPs  dead %d  %s %.1f ms/step" %
                       (dt, np.log2(max(self.jumps, 1)), (self.jumps - self.jumps0) / dt / 1e6, len(self.dps), self.same_herd,
-                       self.table_label, 1e3 * self.t_ingest / steps), flush=True)
+                       self.dpt.label, 1e3 * self.t_ingest / steps), flush=True)
             if self.stop:
                 break
         if self._saving:                                        # a save still moving its herd: finish it first
@@ -614,14 +647,13 @@ class Solver:
         if self.save_path and not self.table_stopped:
             self._save_start(self.save_kangaroos, len(self.herd.plan) if self.save_kangaroos else 0)
         if self.rank == 0:                                      # drain: the last steps' records may still be in the ingest thread
-            k2, _ = self._harvest(wait_all=True)
-            key = key if key is not None else k2
+            self._claim(*self._harvest(wait_all=True))
             self._report_saves(block_for=len(self._save_stats))
         self.elapsed = t1 - t0
         self.steps = steps
         self.steady_rate = ((self.jumps - self.steady[1]) / (t1 - self.steady[0]) if self.steady and steps > 64
                             else (self.jumps - self.jumps0) / self.elapsed)
-        return key
+        return self.found
 
     def close(self):
         if self._thread is not None:
@@ -698,11 +730,9 @@ class BatchSolver(Solver):
         # reports the first matching key, so the later ones would never be hit
         self.rep, self.neg = key_classes(self.keys)
         self.live = [i for i, k in enumerate(self.keys) if k is not None and self.rep[i] == i]
-        self._announce = []                 # rank 0: keys solved, not yet in a control broadcast
         super().__init__(start, end, self.pubs[0], dp_bits, grid, max_found, seed, ingest_threads, dp_table=dp_table,
                          dp_table_capacity=dp_table_capacity)
         self.key_table = DPTable.key_table(self.keys)
-        self._ctrl = self.torch.zeros(3 + MAX_SOLVED + 2 * MAX_RESETS, dtype=self.torch.int64, device="cuda")
 
     def _create_herd(self, sc, d128):
         self.targets = assign_targets(self.eng.nbKangaroo, self.live or [0])         # host mirror of the engine's targets
@@ -711,11 +741,10 @@ class BatchSolver(Solver):
     def _wild_key(self, kidx):
         return self.keys[int(self.targets[kidx])]
 
-    def _ingest(self, segments):
-        """rank 0, ingest thread -> (hits [(key index, private key, rank, kIdx)], resets)"""
+    def _ingest(self, events):
+        """rank 0, ingest thread -> (hits [(key index, private key, rank, kIdx)], resets): every collision is resolved"""
         hits, resets = [], []
-        t0 = time.perf_counter()
-        for kind, rk, kidx, d_old, d_new in self._events_of(segments):
+        for kind, rk, kidx, d_old, d_new in events:
             if kind == EV_COLLISION:
                 m = self.dps.resolve_multi(d_old, d_new, self.key_table, self.start)
                 if m is None:
@@ -724,22 +753,12 @@ class BatchSolver(Solver):
                     hits.append(m + (rk, kidx))
             elif kind == EV_RESET:
                 resets.append((rk, kidx))                        # same herd, wild/wild across keys included
-        self.t_ingest += time.perf_counter() - t0
         return hits, resets
-
-    def _no_events(self):
-        return [], []
-
-    def _take(self, block):
-        f, r = self._done.get(block=block)
-        self._pending -= 1
-        self._acc_found = (self._acc_found or []) + f
-        self._acc_resets += r
 
     def _claim(self, hits, resets):
         """rank 0: a hit on an unsolved key solves it.  A hit on a solved key resets the kangaroo that made it: a tame one that
         ran onto the abandoned trail of a moved wild would re-walk it, or a wild DP from before its move."""
-        for idx, priv, rk, kidx in hits or []:
+        for idx, priv, rk, kidx in hits:
             r = self.rep[idx]
             if self.priv[r] is None:
                 self.priv[r] = class_privs(self.start, priv, self.neg[idx])
@@ -750,50 +769,20 @@ class BatchSolver(Solver):
             else:
                 resets.append((rk, kidx))
 
-    def step(self, may_save=False):
-        """one Launch on every rank; control broadcast [n_solved, n_resets, table full, solved keys..., (rank, kIdx)...]; every
-        rank moves the wilds of each solved key to the live ones"""
-        torch = self.torch
-        n_found = self.eng.collect_count(relaunch=True)                  # launch i done, launch i+1 running
-        self._gather(n_found)
-        self._save_work_done = False
-        solved, resets = [], []
-        if self.rank == 0:
-            hits, resets = self._harvest()
-            self._claim(hits, resets)
-            solved, self._announce = self._announce[:MAX_SOLVED], self._announce[MAX_SOLVED:]
-            self.table_stopped = self.table_msg is not None
-        if self.dist is not None:
-            if self.rank == 0:
-                resets = resets[:MAX_RESETS]
-                c = [len(solved), len(resets), int(self.table_stopped)] + solved + [v for rk in resets for v in rk]
-                self._ctrl[:len(c)].copy_(torch.tensor(c, dtype=torch.int64))
-            self.dist.broadcast(self._ctrl, 0)
-            c = self._ctrl.cpu().tolist()
-            ns, nr = c[0], c[1]
-            self.table_stopped = bool(c[2])
-            solved = c[3:3 + ns]
-            resets = [(c[3 + ns + 2 * i], c[4 + ns + 2 * i]) for i in range(nr)]
+    def _solved(self, solved):
+        """every rank moves the wilds of each solved key to the live ones (a reset kangaroo starts at its current key)"""
         for idx in solved:
             self.live.remove(idx)
             if self.live:
                 self.eng.Retarget(idx, self.live)                        # stream order: after launch i+1, before the resets
                 self.targets = retarget_targets(self.targets, idx, self.live)
-        self.stop = not self.live or self.table_stopped
-        for rk, kidx in resets:
-            self.same_herd += 1
-            if rk == self.rank and not self.stop:
-                self._reset_kangaroo(kidx)                               # at its current key
-        return None
+        return not self.live
 
     def run(self, max_steps=1 << 30, verbose=True):
         if not self.live:                                                # every key solved at start
             self.elapsed, self.steps, self.steady_rate = 1e-9, 0, 0.0
             return None
-        left = super().run(max_steps, verbose)
-        if self.rank == 0:
-            self._claim(left, [])                                        # hits of the last steps' records
-        return None
+        return super().run(max_steps, verbose)
 
 
 def _run_batch(start, end, pubs, dp, grid, a):
@@ -803,25 +792,16 @@ def _run_batch(start, end, pubs, dp, grid, a):
     t_setup = time.perf_counter() - t0
     if s.rank == 0:
         print("Range width: 2^%d  kangaroos/GPU: %d  GPUs: %d  dp: %d  %s  keys: %d in one run" %
-              (s.range_power, s.eng.nbKangaroo, s.world, dp, table_info(s), len(pubs)), flush=True)
+              (s.range_power, s.eng.nbKangaroo, s.world, dp, s.dpt.info, len(pubs)), flush=True)
     t0 = time.perf_counter()
     s.run(a.max_steps)
     t_run = time.perf_counter() - t0
     t0 = time.perf_counter()
     rc = 0
     if s.rank == 0:
-        print("Solver rate: %.0f MJump/s steady state (after the first 32 steps), %.0f MJump/s over all %d steps (%.2f s); "
-              "rank-0 %s %.2f ms/step; %d DPs; %d dead kangaroos re-created" %
-              (s.steady_rate / 1e6, (s.jumps - s.jumps0) / s.elapsed / 1e6, s.steps, s.elapsed, s.table_label,
-               1e3 * s.t_ingest / max(s.steps, 1), len(s.dps), s.same_herd))
-        if s.table_stopped:
-            print(table_message(s, a)); rc = 1
-        for i, pub in enumerate(pubs):
-            if s.priv[i] is not None and ec.mul(s.priv[i]) == pub:
-                print("Key#%2d Pub:  0x%064X\n       Priv: 0x%X" % (i, pub[0], s.priv[i]))
-            else:
-                print("Key#%2d not found" % i); rc = 1
-        solved = sum(1 for i, pub in enumerate(pubs) if s.priv[i] is not None and ec.mul(s.priv[i]) == pub)
+        rc = report(s, a)
+        solved = sum([print_key(i, pub, s.priv[i]) for i, pub in enumerate(pubs)])
+        rc |= solved < len(pubs)
         print("Batch: %d/%d keys solved, %d jumps (2^%.2f) in total, %.3f sqrt(N) jumps per key (N = 2^%d), %d DPs" %
               (solved, len(pubs), s.jumps, np.log2(max(s.jumps, 1)), s.jumps / len(pubs) / 2.0 ** (s.range_power / 2),
                s.range_power, len(s.dps)), flush=True)
@@ -837,18 +817,39 @@ def _run_batch(start, end, pubs, dp, grid, a):
     return rc
 
 
-def table_info(s):
-    """the start-up line's description of rank 0's DP table"""
-    if not s.dev_table:
-        return "ingest threads: %d" % s.dps.threads
-    return "dp table: device, capacity %d entries (%.2f GB)" % (s.dps.capacity, s.dps.memory_bytes() / 1e9)
+def report(s, a):
+    """rank 0, after the run: the rate line, then why the table stopped the run or where the work file went -> 1 when the
+    table stopped the run or the work file was not written, else 0"""
+    print("Solver rate: %.0f MJump/s steady state (after the first 32 steps), %.0f MJump/s over all %d steps (%.2f s); "
+          "rank-0 %s %.2f ms/step; %d DPs; %d dead kangaroos re-created" %
+          (s.steady_rate / 1e6, (s.jumps - s.jumps0) / s.elapsed / 1e6, s.steps, s.elapsed, s.dpt.label,
+           1e3 * s.t_ingest / max(s.steps, 1), len(s.dps), s.same_herd))
+    if s.table_stopped:
+        print(table_message(s, a))
+        return 1
+    if a.save_work and s.save_error is None:
+        mb, dt_save = s.saves[-1]
+        print("work file written: %s (%.1f MB in %.2f s, count 2^%.2f)" % (a.save_work, mb, dt_save, np.log2(max(s.jumps, 1))))
+    elif a.save_work:
+        print("work file NOT written: %s: %s" % (a.save_work, s.save_error))
+        return 1
+    return 0
+
+
+def print_key(i, pub, priv):
+    """rank 0: key i's result line -> whether priv is pub's private key"""
+    if priv is not None and ec.mul(priv) == pub:
+        print("Key#%2d Pub:  0x%064X\n       Priv: 0x%X" % (i, pub[0], priv))
+        return True
+    print("Key#%2d not found" % i)
+    return False
 
 
 def table_message(s, a):
     """rank 0, after the run: why the table stopped it, and which work file, if any, to resume"""
     what = "full" if s.table_kind == "full" else "failed"
     msg = "DP table %s, run stopped: %s." % (what, s.table_msg)
-    saved = getattr(s, "full_saved", None)
+    saved = s.full_saved
     if saved and saved[2] is None:
         msg += (" %s holds the table as it was before this step's launch (count 2^%.2f, no kangaroos); resume it with "
                 "--dp-table host or a larger --dp-table-capacity" % (saved[0], np.log2(max(saved[1], 1))))
@@ -942,24 +943,11 @@ def main(argv=None):
                    dp_table_capacity=a.dp_table_capacity)
         if s.rank == 0:
             print("Range width: 2^%d  kangaroos/GPU: %d  GPUs: %d  dp: %d  %s" %
-                  (s.range_power, s.eng.nbKangaroo, s.world, dp, table_info(s)), flush=True)
+                  (s.range_power, s.eng.nbKangaroo, s.world, dp, s.dpt.info), flush=True)
         key = s.run(a.max_steps)
         if s.rank == 0:
-            print("Solver rate: %.0f MJump/s steady state (after the first 32 steps), %.0f MJump/s over all %d steps (%.2f s); "
-                  "rank-0 %s %.2f ms/step; %d DPs; %d dead kangaroos re-created" %
-                  (s.steady_rate / 1e6, (s.jumps - s.jumps0) / s.elapsed / 1e6, s.steps, s.elapsed, s.table_label,
-                   1e3 * s.t_ingest / max(s.steps, 1), len(s.dps), s.same_herd))
-            if s.table_stopped:
-                print(table_message(s, a)); rc = 1
-            elif a.save_work and s.save_error is None:
-                mb, dt_save = s.saves[-1]
-                print("work file written: %s (%.1f MB in %.2f s, count 2^%.2f)" % (a.save_work, mb, dt_save, np.log2(max(s.jumps, 1))))
-            elif a.save_work:
-                print("work file NOT written: %s: %s" % (a.save_work, s.save_error)); rc = 1
-            if key is not None and ec.mul(key) == pub:
-                print("Key#%2d Pub:  0x%064X\n       Priv: 0x%X" % (i, pub[0], key))
-            else:
-                print("Key#%2d not found" % i); rc = 1
+            rc |= report(s, a)
+            rc |= not print_key(i, pub, key)
         s.close()
     try:
         import torch.distributed as dist
