@@ -20,17 +20,50 @@ using namespace kgx;
 
 static char g_create_err[256] = "";
 
+// Every compiled jump-kernel instantiation.  Resident tile kernels: T, K = the tile geometry (KGX_CFG="T,K"); the first entry
+// is the default, the largest tile of 128 threads that still fits two CTAs per SM.  Stream kernels: ctasPerSM (KGX_STREAM_CTAS)
+// and warpInv (KGX_STREAM_INV) select them, K is the group size chosen at engine creation.  sym: the symmetric-mode
+// (USE_SYMMETRY) instantiation, compiled for the default geometry and the 2-CTA warp-inverse stream kernel only.
+struct KernelEntry {
+  int kind, T, K, ctasPerSM;
+  bool warpInv, sym;
+  void (*fn)(LaunchParams);
+  int smem, ctasPerTile;     // dynamic shared memory; CTAs sharing one tile (the cluster kernel's 2)
+};
+#define KGX_RESIDENT(T_, K_, SYM_) { KGX_KERNEL_RESIDENT, T_, K_, Cfg<T_, K_>::CTAS_PER_SM, false, SYM_, jump_kernel<T_, K_, SYM_>, Cfg<T_, K_>::SMEM_BYTES, 1 }
+#define KGX_STREAM(CTAS_, WARPINV_, SYM_) { KGX_KERNEL_STREAM, 128, 0, CTAS_, WARPINV_, SYM_, stream_kernel<128, CTAS_, WARPINV_, SYM_>, 0, 1 }
+static const KernelEntry g_kernels[] = {
+  KGX_RESIDENT(128, 7, false), KGX_RESIDENT(128, 7, true), KGX_RESIDENT(128, 4, false), KGX_RESIDENT(128, 5, false),
+  KGX_RESIDENT(64, 7, false), KGX_RESIDENT(64, 5, false), KGX_RESIDENT(64, 6, false), KGX_RESIDENT(64, 4, false),
+  KGX_RESIDENT(96, 6, false), KGX_RESIDENT(256, 3, false), KGX_RESIDENT(32, 8, false), KGX_RESIDENT(32, 12, false),
+  KGX_STREAM(2, true, false), KGX_STREAM(2, false, false), KGX_STREAM(3, true, false), KGX_STREAM(3, false, false),
+  KGX_STREAM(2, true, true),
+  { KGX_KERNEL_TMEM, CfgCl::T, CfgCl::K * CfgCl::CLUSTER, 2, false, false, jump_kernel_cluster, CfgCl::SMEM_BYTES, CfgCl::CLUSTER },
+};
+
+// The instantiation of kernel kind `kind` for tile geometry T,K (resident), or ctas and warpInv (stream), in symmetric mode
+// or not; NULL when none is compiled.  The symmetric stream kernel always takes the warp inverse, whatever warpInv says.
+static const KernelEntry* find_kernel(int kind, int T, int K, int ctas, bool warpInv, bool sym) {
+  for (const KernelEntry& k : g_kernels) {
+    if (k.kind != kind || k.sym != sym) continue;
+    if (kind == KGX_KERNEL_RESIDENT && (k.T != T || k.K != K)) continue;
+    if (kind == KGX_KERNEL_STREAM && (k.ctasPerSM != ctas || (!sym && k.warpInv != warpInv))) continue;
+    return &k;
+  }
+  return nullptr;
+}
+
 struct kgx_engine {
   int dev = 0, groups = 0, tpg = 0, sms = 0;
-  int T = 0, K = 0, cfg = 0, ctasPerSM = 0, smemBytes = 0;   // tile geometry (kgx_kernel.cuh Cfg<T,K>)
+  int T = 0, K = 0;          // state layout: tiles of T x K kangaroos (the stream kernel's K is its group size)
+  int kind = 0;              // KGX_KERNEL_STREAM / _RESIDENT / _TMEM
+  const KernelEntry* kern = nullptr;   // the instantiation kgx_launch_async launches
   u64 n = 0, nPadded = 0;
   u32 numTiles = 0, maxFound = 0;
   int nRun = KGX_NB_RUN;
   uint4* state = nullptr;
   uint4* pre = nullptr;      // streaming mode: prefix-product scratch
   uint8_t* jlog = nullptr;   // streaming mode: jump-index log, LOG_RUNS bytes per kangaroo (kgx_kernel.cuh stream_fold)
-  bool streamMode = false;
-  bool tmemMode = false;     // cluster tile kernel (jump_kernel_cluster; selector KGX_KERNEL_TMEM)
   int streamCtas = 2;
   bool symmetry = false;     // USE_SYMMETRY engine mode (kgx_set_symmetry): class switch + cycle rule, signed distances
   int symRule = 0;           // KGX_SYM_LASTJUMP / KGX_SYM_CLASS
@@ -78,19 +111,8 @@ struct kgx_engine {
     }                                                                                          \
   } while (0)
 
-// Tile geometries compiled in.  The default is the largest tile of 128 threads that still fits two CTAs per SM (KGX_CFG="T,K" overrides).
-// kernSym: the symmetric-mode (USE_SYMMETRY) instantiation; only the default geometry carries one (others: NULL).
-struct CfgEntry { int T, K, smem, ctas; void (*kern)(LaunchParams); void (*kernSym)(LaunchParams); };
-#define KGX_CFG_ENTRY(T_, K_) { T_, K_, Cfg<T_, K_>::SMEM_BYTES, Cfg<T_, K_>::CTAS_PER_SM, jump_kernel<T_, K_, false>, nullptr }
-#define KGX_CFG_ENTRY_SYM(T_, K_) { T_, K_, Cfg<T_, K_>::SMEM_BYTES, Cfg<T_, K_>::CTAS_PER_SM, jump_kernel<T_, K_, false>, jump_kernel<T_, K_, true> }
-static const CfgEntry g_cfgs[] = {
-  KGX_CFG_ENTRY_SYM(128, 7), KGX_CFG_ENTRY(128, 4), KGX_CFG_ENTRY(128, 5), KGX_CFG_ENTRY(64, 7), KGX_CFG_ENTRY(64, 5),
-  KGX_CFG_ENTRY(64, 6), KGX_CFG_ENTRY(64, 4), KGX_CFG_ENTRY(96, 6), KGX_CFG_ENTRY(256, 3), KGX_CFG_ENTRY(32, 8), KGX_CFG_ENTRY(32, 12),
-};
-static const int g_ncfg = sizeof(g_cfgs) / sizeof(g_cfgs[0]);
-#ifndef KGX_DEFAULT_CFG
-#define KGX_DEFAULT_CFG 0
-#endif
+// state byte of a fresh kangaroo in symmetric mode: lastJump = NB_JUMP (none yet) / symClass = 0
+static int aux_init(const kgx_engine* e) { return e->symRule == KGX_SYM_CLASS ? 0 : 32; }
 #ifndef KGX_DEFAULT_STREAM
 #define KGX_DEFAULT_STREAM 1   // streaming kernel for large herds; KGX_MODE=resident selects the tile kernel
 #endif
@@ -168,15 +190,14 @@ kgx_engine* kgx_create_ex(int dev, int groups, int threads_per_group, uint32_t m
   if ((s = cudaGetDeviceProperties(&prop, dev)) != cudaSuccess) return fail("cudaGetDeviceProperties", s);
   e->dev = dev; e->groups = groups; e->tpg = threads_per_group; e->sms = prop.multiProcessorCount;
   e->n = (u64)groups * (u64)threads_per_group * KGX_GPU_GRP_SIZE;
-  e->cfg = KGX_DEFAULT_CFG;
+  e->T = g_kernels[0].T; e->K = g_kernels[0].K;
   if (const char* env = getenv("KGX_CFG")) {
-    int t = 0, k = 0, found = -1;
-    if (sscanf(env, "%d,%d", &t, &k) == 2)
-      for (int i = 0; i < g_ncfg; i++) if (g_cfgs[i].T == t && g_cfgs[i].K == k) found = i;
-    if (found < 0) { snprintf(g_create_err, sizeof g_create_err, "kgx_create: KGX_CFG=%s is not a compiled tile geometry", env); delete e; return nullptr; }
-    e->cfg = found;
+    int t = 0, k = 0;
+    if (sscanf(env, "%d,%d", &t, &k) != 2 || !find_kernel(KGX_KERNEL_RESIDENT, t, k, 0, false, false)) {
+      snprintf(g_create_err, sizeof g_create_err, "kgx_create: KGX_CFG=%s is not a compiled tile geometry", env); delete e; return nullptr;
+    }
+    e->T = t; e->K = k;
   }
-  e->T = g_cfgs[e->cfg].T; e->K = g_cfgs[e->cfg].K; e->smemBytes = g_cfgs[e->cfg].smem; e->ctasPerSM = g_cfgs[e->cfg].ctas;
   {
     const char* mode = getenv("KGX_MODE");
     if (kernel == KGX_KERNEL_STREAM) mode = "stream";
@@ -186,15 +207,12 @@ kgx_engine* kgx_create_ex(int dev, int groups, int threads_per_group, uint32_t m
     // default: the streaming kernel for herds of 400 k kangaroos and more (it wants many kangaroos per thread on every
     // SM to amortise the per-thread inverse), the shared-memory tile kernel below that (its inverse is shared by a whole
     // tile, so it keeps its rate on herds too small to give every stream thread a long group)
-    e->streamMode = mode ? (strcmp(mode, "stream") == 0) : (KGX_DEFAULT_STREAM != 0 && e->n >= 400000ull);
-    if (mode && strcmp(mode, "stream") && strcmp(mode, "resident") && strcmp(mode, "tmem")) {
-      snprintf(g_create_err, sizeof g_create_err, "kgx_create: KGX_MODE must be stream, resident or tmem"); delete e; return nullptr;
-    }
-    if (mode && !strcmp(mode, "tmem")) {
-      e->tmemMode = true;
-      e->T = CfgCl::T; e->K = CfgCl::K; e->smemBytes = CfgCl::SMEM_BYTES; e->ctasPerSM = 2;
-    }
-    if (e->streamMode) {
+    if (!mode) e->kind = KGX_DEFAULT_STREAM != 0 && e->n >= 400000ull ? KGX_KERNEL_STREAM : KGX_KERNEL_RESIDENT;
+    else if (!strcmp(mode, "stream")) e->kind = KGX_KERNEL_STREAM;
+    else if (!strcmp(mode, "resident")) e->kind = KGX_KERNEL_RESIDENT;
+    else if (!strcmp(mode, "tmem")) e->kind = KGX_KERNEL_TMEM;
+    else { snprintf(g_create_err, sizeof g_create_err, "kgx_create: KGX_MODE must be stream, resident or tmem"); delete e; return nullptr; }
+    if (e->kind == KGX_KERNEL_STREAM) {
       // kangaroos per thread: 128 (the reference's GPU_GRP_SIZE) when the herd fills two CTAs per SM with it; smaller
       // herds get a smaller group so that the grid still covers the chip (one wave of 2 CTAs/SM), at the price of more
       // inversions per jump.  KGX_STREAM_G overrides.
@@ -221,9 +239,12 @@ kgx_engine* kgx_create_ex(int dev, int groups, int threads_per_group, uint32_t m
       if (!invChosen) e->warpInv = g >= 64;
       if (const char* pf = getenv("KGX_STREAM_PF")) e->pfDist = atoi(pf);
       e->streamCtas = ctas;
-      e->T = 128; e->K = (int)g; e->smemBytes = 0; e->ctasPerSM = ctas;
+      e->K = (int)g;
     }
   }
+  e->kern = find_kernel(e->kind, e->T, e->K, e->streamCtas, e->warpInv, false);   // every non-symmetric selection is compiled
+  e->T = e->kern->T;
+  if (e->kind != KGX_KERNEL_STREAM) e->K = e->kern->K;
   const u64 TILE = (u64)e->T * e->K;
   e->numTiles = (u32)((e->n + TILE - 1) / TILE);
   e->nPadded = (u64)e->numTiles * TILE;
@@ -237,8 +258,8 @@ kgx_engine* kgx_create_ex(int dev, int groups, int threads_per_group, uint32_t m
     if ((s = cudaEventCreateWithFlags(&e->evStop[i], cudaEventBlockingSync)) != cudaSuccess) return fail("cudaEventCreate", s);
   }
   if ((s = cudaMalloc(&e->state, e->stateBytes)) != cudaSuccess) return fail("cudaMalloc(state)", s);
-  if (e->streamMode && (s = cudaMalloc(&e->pre, (size_t)e->nPadded * 32)) != cudaSuccess) return fail("cudaMalloc(pre)", s);
-  if (e->streamMode && (s = cudaMalloc(&e->jlog, (size_t)e->nPadded * LOG_RUNS)) != cudaSuccess) return fail("cudaMalloc(jlog)", s);
+  if (e->kind == KGX_KERNEL_STREAM && (s = cudaMalloc(&e->pre, (size_t)e->nPadded * 32)) != cudaSuccess) return fail("cudaMalloc(pre)", s);
+  if (e->kind == KGX_KERNEL_STREAM && (s = cudaMalloc(&e->jlog, (size_t)e->nPadded * LOG_RUNS)) != cudaSuccess) return fail("cudaMalloc(jlog)", s);
   for (int i = 0; i < 2; i++) {
     if ((s = cudaMalloc(&e->slab[i], e->slabBytes)) != cudaSuccess) return fail("cudaMalloc(slab)", s);
     if ((s = cudaMemsetAsync(e->slab[i], 0, 4, e->stream)) != cudaSuccess) return fail("cudaMemset(slab)", s);  // Check.cpp:526 collects before any launch
@@ -249,18 +270,14 @@ kgx_engine* kgx_create_ex(int dev, int groups, int threads_per_group, uint32_t m
     cudaMemset(e->prof, 0, 64);
   }
   if ((s = cudaHostAlloc(&e->slabPinned, e->slabBytes, cudaHostAllocDefault)) != cudaSuccess) return fail("cudaHostAlloc", s);
-  if (e->tmemMode) {
-    if ((s = cudaFuncSetAttribute(jump_kernel_cluster, cudaFuncAttributeMaxDynamicSharedMemorySize, e->smemBytes)) != cudaSuccess)
-      return fail("cudaFuncSetAttribute(smem, cluster kernel)", s);
-  } else if (!e->streamMode &&
-      (s = cudaFuncSetAttribute(g_cfgs[e->cfg].kern, cudaFuncAttributeMaxDynamicSharedMemorySize, e->smemBytes)) != cudaSuccess)
+  if ((s = cudaFuncSetAttribute(e->kern->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, e->kern->smem)) != cudaSuccess)
     return fail("cudaFuncSetAttribute(smem)", s);
   if ((s = cudaStreamSynchronize(e->stream)) != cudaSuccess) return fail("sync", s);
   return e;
 }
 
 uint64_t kgx_num_kangaroos(kgx_engine* e) { return e->n; }
-int kgx_kernel_kind(kgx_engine* e) { return e->streamMode ? KGX_KERNEL_STREAM : (e->tmemMode ? KGX_KERNEL_TMEM : KGX_KERNEL_RESIDENT); }
+int kgx_kernel_kind(kgx_engine* e) { return e->kind; }
 uint64_t kgx_memory_bytes(kgx_engine* e) {
   return e->stateBytes + (e->pre ? e->nPadded * 32 : 0) + (e->jlog ? e->nPadded * LOG_RUNS : 0) + 2 * e->slabBytes + JT_WORDS * 4 +
          (e->targets ? e->n * 2 : 0) + (u64)e->keyCap * (64 + 64 + 4);
@@ -287,20 +304,20 @@ int kgx_set_jumps_per_launch(kgx_engine* e, int n_run) {
 int kgx_set_symmetry(kgx_engine* e, int on) {
   CK(e, cudaSetDevice(e->dev));
   if (e->inflight) { snprintf(e->err, sizeof e->err, "kgx_set_symmetry: a launch is in flight"); return -1; }
-  if (on && e->tmemMode) { snprintf(e->err, sizeof e->err, "kgx_set_symmetry: the cluster tile kernel has no symmetric instantiation"); return -1; }
-  if (on && !e->streamMode && !g_cfgs[e->cfg].kernSym) {
-    snprintf(e->err, sizeof e->err, "kgx_set_symmetry: tile geometry %d,%d has no symmetric instantiation", e->T, e->K); return -1;
-  }
-  if (on && e->streamMode && e->streamCtas != 2) {
-    snprintf(e->err, sizeof e->err, "kgx_set_symmetry: the symmetric stream kernel is the 2-CTA variant only"); return -1;
+  const KernelEntry* kern = find_kernel(e->kind, e->T, e->K, e->streamCtas, e->warpInv, on != 0);
+  if (!kern) {
+    if (e->kind == KGX_KERNEL_TMEM) snprintf(e->err, sizeof e->err, "kgx_set_symmetry: the cluster tile kernel has no symmetric instantiation");
+    else if (e->kind == KGX_KERNEL_STREAM) snprintf(e->err, sizeof e->err, "kgx_set_symmetry: the symmetric stream kernel is the 2-CTA variant only");
+    else snprintf(e->err, sizeof e->err, "kgx_set_symmetry: tile geometry %d,%d has no symmetric instantiation", e->T, e->K);
+    return -1;
   }
   if (on != 0 && on != KGX_SYM_LASTJUMP && on != KGX_SYM_CLASS) { snprintf(e->err, sizeof e->err, "kgx_set_symmetry: mode must be 0, 1 (lastJump rule) or 2 (symClass rule)"); return -1; }
   if (on && !e->aux) CK(e, cudaMalloc(&e->aux, e->nPadded));
   if (on) CK(e, cudaMemsetAsync(e->aux, on == KGX_SYM_CLASS ? 0 : 32, e->nPadded, e->stream));
   e->symRule = on;
   if (on) e->nKeys = 0;        // a multi-key herd is not available in symmetric mode (kgx_create_herd_multi): drop its table
-  if (on && !e->streamMode)
-    CK(e, cudaFuncSetAttribute(g_cfgs[e->cfg].kernSym, cudaFuncAttributeMaxDynamicSharedMemorySize, e->smemBytes));
+  CK(e, cudaFuncSetAttribute(kern->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kern->smem));
+  e->kern = kern;
   e->symmetry = on != 0;
   return 0;
 }
@@ -346,7 +363,7 @@ int kgx_upload(kgx_engine* e, const uint64_t* px, const uint64_t* py, const uint
   CK(e, cudaMemcpyAsync(e->stgY, py, e->n * 32, cudaMemcpyHostToDevice, e->stream));
   CK(e, cudaMemcpyAsync(e->stgD, d, e->n * 16, cudaMemcpyHostToDevice, e->stream));
   u32 blocks = (u32)((e->nPadded + 255) / 256);
-  pack_kernel<<<blocks, 256, 0, e->stream>>>(e->state, e->stgX, e->stgY, e->stgD, e->n, e->nPadded, e->T, e->K, e->aux, e->symRule == KGX_SYM_CLASS ? 0 : 32);
+  pack_kernel<<<blocks, 256, 0, e->stream>>>(e->state, e->stgX, e->stgY, e->stgD, e->n, e->nPadded, e->T, e->K, e->aux, aux_init(e));
   e->launches++;
   CK(e, cudaGetLastError());
   CK(e, cudaStreamSynchronize(e->stream));
@@ -484,7 +501,7 @@ int kgx_import(kgx_engine* e, const uint64_t wild_offset[2], const void* recs, u
     }
     if (mismatches) *mismatches = res[1];
     if (res[1]) return 0;
-    pack_kernel<<<(u32)((e->nPadded + 255) / 256), 256, 0, e->stream>>>(e->state, e->stgX, e->stgY, e->stgD, e->n, e->nPadded, e->T, e->K, e->aux, e->symRule == KGX_SYM_CLASS ? 0 : 32);
+    pack_kernel<<<(u32)((e->nPadded + 255) / 256), 256, 0, e->stream>>>(e->state, e->stgX, e->stgY, e->stgD, e->n, e->nPadded, e->T, e->K, e->aux, aux_init(e));
     e->launches++;
     CK(e, cudaGetLastError());
     CK(e, cudaStreamSynchronize(e->stream));
@@ -501,7 +518,7 @@ int kgx_patch(kgx_engine* e, uint64_t kidx, const uint64_t px[4], const uint64_t
   if (kidx >= e->n) { snprintf(e->err, sizeof e->err, "kgx_patch: kidx out of range"); return -1; }
   PatchArgs a;
   memcpy(&a.c[0], px, 32); memcpy(&a.c[2], py, 32); memcpy(&a.c[4], d, 16);
-  patch_kernel<<<1, 32, 0, e->stream>>>(e->state, kidx, a, e->T, e->K, e->aux, e->symRule == KGX_SYM_CLASS ? 0 : 32);   // stream order == the reference's blocking memcpy order (Kangaroo.cpp:607)
+  patch_kernel<<<1, 32, 0, e->stream>>>(e->state, kidx, a, e->T, e->K, e->aux, aux_init(e));   // stream order == the reference's blocking memcpy order (Kangaroo.cpp:607)
   e->launches++;
   CK(e, cudaGetLastError());
   // padding slots replicate kangaroo (s % n): keep them walking their stale copy -- harmless, their DPs are dropped.
@@ -557,7 +574,7 @@ static int create_herd(kgx_engine* e, const char* what, const uint64_t* scalars,
     e->launches++;
     CK(e, cudaGetLastError());
     u32 blocks = (u32)((e->nPadded + 255) / 256);
-    pack_kernel<<<blocks, 256, 0, e->stream>>>(e->state, e->stgX, e->stgY, e->stgD, e->n, e->nPadded, e->T, e->K, e->aux, e->symRule == KGX_SYM_CLASS ? 0 : 32);
+    pack_kernel<<<blocks, 256, 0, e->stream>>>(e->state, e->stgX, e->stgY, e->stgD, e->n, e->nPadded, e->T, e->K, e->aux, aux_init(e));
     e->launches++;
     CK(e, cudaGetLastError());
     CK(e, cudaStreamSynchronize(e->stream));
@@ -634,22 +651,10 @@ int kgx_launch_async(kgx_engine* e) {
   p.numTiles = e->numTiles; p.maxFound = e->maxFound; p.nRun = e->nRun; p.prof = e->prof; p.pre = e->pre; p.G = e->K; p.aux = e->aux; p.symRule = e->symRule; p.pfDist = e->pfDist; p.jlog = e->jlog;
   CK(e, cudaMemsetAsync(e->slab[sidx], 0, 4, e->stream));            // GPUEngine.cu:543
   CK(e, cudaEventRecord(e->evStart[sidx], e->stream));
-  u32 grid = (u32)(e->ctasPerSM * e->sms);
-  const u32 ctasPerTile = e->tmemMode ? CfgCl::CLUSTER : 1;             // the cluster kernel spreads a tile over 2 CTAs
-  if (grid > e->numTiles * ctasPerTile) grid = e->numTiles * ctasPerTile;
-  if (e->streamMode) {
-    if (e->symmetry) stream_kernel<128, 2, true, true><<<grid, 128, 0, e->stream>>>(p);
-    else if (e->streamCtas == 3) {
-      if (e->warpInv) stream_kernel<128, 3, true, false><<<grid, 128, 0, e->stream>>>(p);
-      else stream_kernel<128, 3, false, false><<<grid, 128, 0, e->stream>>>(p);
-    } else {
-      if (e->warpInv) stream_kernel<128, 2, true, false><<<grid, 128, 0, e->stream>>>(p);
-      else stream_kernel<128, 2, false, false><<<grid, 128, 0, e->stream>>>(p);
-    }
-  }
-  else if (e->tmemMode) jump_kernel_cluster<<<grid, CfgCl::T, e->smemBytes, e->stream>>>(p);
-  else if (e->symmetry) g_cfgs[e->cfg].kernSym<<<grid, e->T, e->smemBytes, e->stream>>>(p);
-  else g_cfgs[e->cfg].kern<<<grid, e->T, e->smemBytes, e->stream>>>(p);
+  const KernelEntry& k = *e->kern;
+  u32 grid = (u32)(k.ctasPerSM * e->sms);
+  if (grid > e->numTiles * k.ctasPerTile) grid = e->numTiles * k.ctasPerTile;
+  k.fn<<<grid, k.T, k.smem, e->stream>>>(p);
   e->launches++;
   CK(e, cudaGetLastError());
   CK(e, cudaEventRecord(e->evStop[sidx], e->stream));

@@ -206,9 +206,8 @@ __global__ void retarget_delta_kernel(const u32* __restrict__ keys, u32 from, Re
 }
 
 // Every wild kangaroo s < n (kIdx order; wild when s + firstType is odd) whose target is `from` moves to key
-// b = rtTo[(s >> 1) % nTo]: its point gets keys[b] - keys[from] added in place in the tile layout (slot s -> tile s / TILE,
-// row (s % TILE) / T, column s % T, as pack_kernel), its distance stays, its target becomes b.  Padding slots are left
-// stale, like patch_kernel leaves them.
+// b = rtTo[(s >> 1) % nTo]: its point gets keys[b] - keys[from] added in place in the tile layout (slot_chunks), its
+// distance stays, its target becomes b.  Padding slots are left stale, like patch_kernel leaves them.
 __global__ void retarget_kernel(uint4* state, int T, int K, u64 n, int firstType, uint16_t* targets, u32 from,
                                 const u32* __restrict__ delta, const u32* __restrict__ rtTo, u32 nTo) {
   const u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x;
@@ -217,12 +216,10 @@ __global__ void retarget_kernel(uint4* state, int T, int K, u64 n, int firstType
   const u32 tj = rtTo[j];
   targets[s] = (uint16_t)(tj & 0xFFFFu);
   if (tj >> 31) return;
-  const int TILE = T * K;
-  const u64 tile = s / TILE; const int r = (int)(s % TILE); const int g = r / T, t = r % T;
-  uint4* st = state + tile * (K * CHUNKS * T);
+  uint4* st = slot_chunks(state, s, T, K);
   uint4 c[4];
 #pragma unroll
-  for (int k = 0; k < 4; k++) c[k] = st[(g * CHUNKS + k) * T + t];
+  for (int k = 0; k < 4; k++) c[k] = st[k * T];
   u32 x[8] = {c[0].x, c[0].y, c[0].z, c[0].w, c[1].x, c[1].y, c[1].z, c[1].w};
   u32 y[8] = {c[2].x, c[2].y, c[2].z, c[2].w, c[3].x, c[3].y, c[3].z, c[3].w};
   if (!affine_add(x, y, delta + 16 * j, delta + 16 * j + 8)) {
@@ -230,10 +227,10 @@ __global__ void retarget_kernel(uint4* state, int T, int K, u64 n, int firstType
 #pragma unroll
     for (int w = 0; w < 8; w++) { x[w] = 0; y[w] = 0; }
   }
-  st[(g * CHUNKS + 0) * T + t] = make_uint4(x[0], x[1], x[2], x[3]);
-  st[(g * CHUNKS + 1) * T + t] = make_uint4(x[4], x[5], x[6], x[7]);
-  st[(g * CHUNKS + 2) * T + t] = make_uint4(y[0], y[1], y[2], y[3]);
-  st[(g * CHUNKS + 3) * T + t] = make_uint4(y[4], y[5], y[6], y[7]);
+  st[0] = make_uint4(x[0], x[1], x[2], x[3]);
+  st[T] = make_uint4(x[4], x[5], x[6], x[7]);
+  st[2 * T] = make_uint4(y[0], y[1], y[2], y[3]);
+  st[3 * T] = make_uint4(y[4], y[5], y[6], y[7]);
 }
 
 }  // namespace kgx

@@ -21,9 +21,11 @@
 //                    thread-block cluster; one inverse per tile through distributed shared memory.
 //   SYM instantiations of the first two add the reference's USE_SYMMETRY paths (class switch + lastJump / symClass rule).
 //
-//   Both use the same fused per-kangaroo pass: back-substitution of this jump's inverse, the affine add, the
-//   distance update, the DP test, and the *next* jump's dx / prefix product (accumulated in the order of this pass,
-//   consumed in reverse by the next): 5 ModMult + 1 ModSqr + 7 ModSub per jump.  DESIGN.md 3 has the measurements.
+//   All three make the same fused per-kangaroo pass: back-substitution of this jump's inverse, the affine add (one copy:
+//   kangaroo_jump), the distance update, the DP test, and the *next* jump's dx / prefix product (next_dx; accumulated in
+//   the order of this pass, consumed in reverse by the next): 5 ModMult + 1 ModSqr + 7 ModSub per jump.  The two tile
+//   kernels are one body (tile_body) that differs only in rows per CTA and the inverse step, and every group inverse uses
+//   the same lane butterfly (butterfly_up / butterfly_down).  DESIGN.md 3 has the measurements.
 #pragma once
 #include "kgx_field.cuh"
 #include "kgx_modinv.h"
@@ -34,8 +36,9 @@ namespace kgx {
 constexpr int CHUNKS = 5;         // 16-byte chunks per kangaroo in HBM: x0 x1 y0 y1 d
 constexpr int JT_WORDS = 20 * 32; // jump table as uint4 jt[5][32] = {jpx lo, jpx hi, jpy lo, jpy hi, jd} x 32 jumps: one LDS.128 per half element
 
-// Tile geometry: T threads per CTA (W = T/32 warps), K kangaroos per thread.  Shared memory (uint4 units):
-//   X[K][2][T] Y[K][2][T] P[K][2][T] D[K][T] TOT[2][T] then the jump table (u32 view).
+// Tile geometry of one CTA: T threads (W = T/32 warps), K kangaroos per thread.  Shared memory (uint4 units):
+//   X[K][2][T] Y[K][2][T] P[K][2][T] D[K][T] TOT[2][T] then the jump table (u32 view), then the symmetric mode's state
+//   bytes [K][T] (the cluster kernel's CfgCl puts its exchange slots there instead).
 template <int T_, int K_>
 struct Cfg {
   static constexpr int T = T_, K = K_, W = T_ / 32, TILE = T_ * K_;
@@ -117,32 +120,37 @@ __device__ __forceinline__ u32 sym_next_aux(u32 aux, u32 j, u32 neg, int rule) {
   return rule == KGX_SYM_CLASS ? ((aux ^ neg) & 1u) : j;
 }
 
-// Warp 0 only: turn the T per-thread products in sTot into their T inverses (in place).
-// lane l chains the totals of threads {l, l+32, ...} (one per warp: conflict-free), the 32 lane products are
-// multiplied by an XOR butterfly (every lane ends with the tile product and keeps the 5 sibling factors),
-// one warp-uniform inverse, then the same tree is walked back.
-template <int T, int W>
-__device__ __noinline__ void tile_inverse(uint4* sTot, int lane, unsigned long long* prof) {
-  u32 tw[W][8], c[W][8];     // c[w] = tw[0]*...*tw[w]
-#pragma unroll
-  for (int w = 0; w < W; w++) lds_fe(tw[w], sTot, 32 * w + lane, T + 32 * w + lane);
-  fe_copy(c[0], tw[0]);
-#pragma unroll
-  for (int w = 1; w < W; w++) fe_mul(c[w], c[w - 1], tw[w]);
-  u32 v[8];
-  fe_copy(v, c[W - 1]);
-  u32 sib[5][8];
+// XOR butterfly over the 32 lanes of a warp: v becomes the product of all 32 lanes' v (identical in every lane) and sib[l]
+// keeps the sibling factor of round l.  butterfly_down walks it back: the inverse of that product becomes the inverse of this
+// lane's own v.
+__device__ __forceinline__ void butterfly_up(u32* v, u32 (*sib)[8]) {
 #pragma unroll
   for (int l = 0; l < 5; l++) {
     shfl_xor_fe(sib[l], v, 1 << l);
     fe_mul(v, v, sib[l]);
   }
-  u32 inv[8];
-  long long tq0 = prof ? clock64() : 0;
-  fe_inv(inv, v);                 // identical in all 32 lanes
-  if (prof && lane == 0) atomicAdd(prof + 1, (unsigned long long)(clock64() - tq0));
+}
+__device__ __forceinline__ void butterfly_down(u32* inv, u32 (*sib)[8]) {
 #pragma unroll
-  for (int l = 4; l >= 0; l--) fe_mul(inv, inv, sib[l]);   // -> 1 / c[W-1] of this lane
+  for (int l = 4; l >= 0; l--) fe_mul(inv, inv, sib[l]);
+}
+
+// Warp 0's tree over the T per-thread products in sTot.  tile_reduce: lane l chains the totals of threads {l, l+32, ...}
+// (one per warp: conflict-free; c[w] = tw[0]*...*tw[w]) and the butterfly multiplies the 32 lane chains into v, the
+// product of all T.  tile_walk_back takes inv = 1 / v back down the same tree and writes the T inverses to sTot.
+template <int T, int W>
+__device__ __forceinline__ void tile_reduce(u32* v, u32 (*tw)[8], u32 (*c)[8], u32 (*sib)[8], const uint4* sTot, int lane) {
+#pragma unroll
+  for (int w = 0; w < W; w++) lds_fe(tw[w], sTot, 32 * w + lane, T + 32 * w + lane);
+  fe_copy(c[0], tw[0]);
+#pragma unroll
+  for (int w = 1; w < W; w++) fe_mul(c[w], c[w - 1], tw[w]);
+  fe_copy(v, c[W - 1]);
+  butterfly_up(v, sib);
+}
+template <int T, int W>
+__device__ __forceinline__ void tile_walk_back(uint4* sTot, u32* inv, u32 (*tw)[8], u32 (*c)[8], u32 (*sib)[8], int lane) {
+  butterfly_down(inv, sib);       // -> 1 / c[W-1] of this lane
 #pragma unroll
   for (int w = W - 1; w >= 1; w--) {
     u32 o[8];
@@ -153,10 +161,83 @@ __device__ __noinline__ void tile_inverse(uint4* sTot, int lane, unsigned long l
   sts_fe(sTot, lane, T + lane, inv);
 }
 
-template <int T, int K, bool SYM>
-__global__ void __launch_bounds__(T, Cfg<T, K>::CTAS_PER_SM) jump_kernel(LaunchParams p) {
+// Warp 0 only: turn the T per-thread products in sTot into their T inverses (in place) with one warp-uniform inverse.
+template <int T, int W>
+__device__ __noinline__ void tile_inverse(uint4* sTot, int lane, unsigned long long* prof) {
+  u32 tw[W][8], c[W][8], sib[5][8], v[8], inv[8];
+  tile_reduce<T, W>(v, tw, c, sib, sTot, lane);
+  long long tq0 = prof ? clock64() : 0;
+  fe_inv(inv, v);                 // identical in all 32 lanes
+  if (prof && lane == 0) atomicAdd(prof + 1, (unsigned long long)(clock64() - tq0));
+  tile_walk_back<T, W>(sTot, inv, tw, c, sib, lane);
+}
+
+// One jump of one kangaroo: the arithmetic of the fused pass that every jump kernel shares.  pre holds the product of the
+// dx accumulated before this kangaroo in the pass (clobbered: it becomes 1/dx); strip takes this dx out of the running
+// inverse I, which the last kangaroo of a pass can skip.  y comes as its two 16-byte halves and is read only after the
+// inverse step, so that a tile kernel's shared-memory load of y does not hold 8 registers across it.  Returns (rx, ry), the jump index j and, in symmetric mode, the
+// class-switch mask (all ones when the point was negated); the caller applies the jump to the distance and the state byte.
+template <bool SYM>
+__device__ __forceinline__ u32 kangaroo_jump(u32* rx, u32* ry, u32& j, const u32* x, const uint4& y0, const uint4& y1, u32* pre,
+                                             u32* I, bool strip, u32 aux, const uint4* jt, int rule) {
+  u32 y[8], jx[8], jy[8], dx[8], s[8];
+  j = jump_index<SYM>(x[0], aux, rule);
+  lds_jp4(jx, jt, j);
+  fe_sub(dx, x, jx);
+  fe_mul(pre, pre, I);                     // 1/dx
+  if (strip) fe_mul(I, I, dx);             // strip this dx from the running inverse
+  unpack8(y, y0, y1);
+  lds_jp4(jy, jt + 64, j);
+  fe_sub(s, y, jy);                        // dy
+  fe_mul(s, s, pre);                       // s = dy/dx
+  fe_sqr(rx, s);
+  fe_sub(rx, rx, jx);
+  fe_sub(rx, rx, x);                       // rx = s^2 - jx - x
+  fe_sub(ry, x, rx);
+  fe_mul(ry, ry, s);
+  fe_sub(ry, ry, y);                       // ry = s (x - rx) - y
+  if (!SYM) return 0u;
+  const u32 neg = fe_gt_half_mask(ry);     // equivalence class switch (Check.cpp:551-556): y > (p-1)/2 -> (x, p - y), d -> -d
+  fe_cneg(ry, neg);
+  return neg;
+}
+
+// dx of the next jump of the kangaroo at x with state byte aux.
+template <bool SYM>
+__device__ __forceinline__ void next_dx(u32* dx, const u32* x, u32 aux, const uint4* jt, int rule) {
+  u32 jx[8];
+  lds_jp4(jx, jt, jump_index<SYM>(x[0], aux, rule));
+  fe_sub(dx, x, jx);
+}
+
+// Tile kernels: appends dx to the chain P and stores the product of the dx before it at (i0, i1) of sP (first: a new chain).
+__device__ __forceinline__ void chain_dx(uint4* sP, int i0, int i1, u32* P, const u32* dx, bool first) {
+  if (first) {
+    u32 one[8]; fe_set_one(one);
+    sts_fe(sP, i0, i1, one);
+    fe_copy(P, dx);
+  } else {
+    sts_fe(sP, i0, i1, P);
+    fe_mul(P, P, dx);
+  }
+}
+
+// DP record at position pos of the slab (GPUMath.h:173-188 layout): x (8 words), distance (4 words), kIdx (2 words).
+__device__ __forceinline__ void put_dp_record(u32* out, u32 pos, const u32* x, const u32* d, u64 kidx) {
+  u32* o = out + 1 + (size_t)pos * 14;
+#pragma unroll
+  for (int w = 0; w < 8; w++) o[w] = x[w];
+  o[8] = d[0]; o[9] = d[1]; o[10] = d[2]; o[11] = d[3];
+  o[12] = (u32)kidx; o[13] = (u32)(kidx >> 32);
+}
+
+// The body of both tile kernels.  A tile of CTAS * K rows of T kangaroos is spread over CTAS CTAs; this one holds rows
+// rank * K .. rank * K + K - 1 in its shared memory (Cfg<T, K> layout) for all nRun jumps of the launch.  inverse(sTot, t)
+// turns the T thread totals in sTot into their inverses; every thread calls it, between two barriers.
+template <int T, int K, int CTAS, bool SYM, class Inverse>
+__device__ __forceinline__ void tile_body(const LaunchParams& p, u32 rank, Inverse inverse) {
   using C = Cfg<T, K>;
-  constexpr int TILE = C::TILE;
+  constexpr int TILE = T * K * CTAS;
   extern __shared__ uint4 smem[];
   uint8_t* sL = reinterpret_cast<uint8_t*>(smem) + C::LJ_OFF;
   uint4* sX = smem + C::S_X;
@@ -166,14 +247,14 @@ __global__ void __launch_bounds__(T, Cfg<T, K>::CTAS_PER_SM) jump_kernel(LaunchP
   uint4* sTot = smem + C::S_TOT;
   uint4* jt = smem + C::S_JT;
   const int t = threadIdx.x;
-  const int lane = t & 31;
   const u32 mlo = (u32)p.dpMask, mhi = (u32)(p.dpMask >> 32);
 
   for (int i = t; i < JT_WORDS; i += T) reinterpret_cast<u32*>(jt)[i] = p.jtab[i];
 
-  for (u32 tile = blockIdx.x; tile < p.numTiles; tile += gridDim.x) {
+  for (u32 tile = blockIdx.x / CTAS; tile < p.numTiles; tile += gridDim.x / CTAS) {   // the CTAs of a tile walk the same tiles
     __syncthreads();   // jump table visible; previous tile's shared state fully consumed
-    uint4* gsrc = p.state + (size_t)tile * (K * CHUNKS * T);
+    const u32 row0 = rank * K;   // this CTA's first row in the tile: slot tile * TILE + (row0 + g) * T + t
+    uint4* gsrc = p.state + (size_t)tile * (CTAS * K * CHUNKS * T) + (size_t)row0 * (CHUNKS * T);
 #pragma unroll
     for (int g = 0; g < K; g++) {
       sX[(g * 2 + 0) * T + t] = gsrc[(g * CHUNKS + 0) * T + t];
@@ -181,25 +262,18 @@ __global__ void __launch_bounds__(T, Cfg<T, K>::CTAS_PER_SM) jump_kernel(LaunchP
       sY[(g * 2 + 0) * T + t] = gsrc[(g * CHUNKS + 2) * T + t];
       sY[(g * 2 + 1) * T + t] = gsrc[(g * CHUNKS + 3) * T + t];
       sD[g * T + t] = gsrc[(g * CHUNKS + 4) * T + t];
-      if (SYM) sL[g * T + t] = p.aux[(size_t)tile * TILE + g * T + t];
+      if (SYM) sL[g * T + t] = p.aux[(size_t)tile * TILE + (row0 + g) * T + t];
     }
-    // prologue: forward chain of dx = x - jPx[x & 31]; sP[g] = product of the dx before g
+    // prologue: forward chain of dx; sP[g] = product of the dx before g
     u32 P[8];
     {
-      u32 x[8], jx[8], dx[8];
+      u32 x[8], dx[8];
 #pragma unroll 1
       for (int g = 0; g < K; g++) {
-        lds_fe(x, sX, (g * 2) * T + t, (g * 2 + 1) * T + t);
-        lds_jp4(jx, jt, jump_index<SYM>(x[0], SYM ? (u32)sL[g * T + t] : 0u, p.symRule));
-        fe_sub(dx, x, jx);
-        if (g == 0) {
-          u32 one[8]; fe_set_one(one);
-          sts_fe(sP, t, T + t, one);
-          fe_copy(P, dx);
-        } else {
-          sts_fe(sP, (g * 2) * T + t, (g * 2 + 1) * T + t, P);
-          fe_mul(P, P, dx);
-        }
+        const int i0 = (g * 2) * T + t, i1 = (g * 2 + 1) * T + t;
+        lds_fe(x, sX, i0, i1);
+        next_dx<SYM>(dx, x, SYM ? (u32)sL[g * T + t] : 0u, jt, p.symRule);
+        chain_dx(sP, i0, i1, P, dx, g == 0);
       }
       sts_fe(sTot, t, T + t, P);
     }
@@ -211,7 +285,7 @@ __global__ void __launch_bounds__(T, Cfg<T, K>::CTAS_PER_SM) jump_kernel(LaunchP
       if (p.prof && t == 0 && run > 0) atomicAdd(p.prof + 2, (unsigned long long)(tp1 - tp0));
       __syncthreads();
       long long ts0 = (p.prof && t == 0) ? clock64() : 0;
-      if (t < 32) tile_inverse<T, C::W>(sTot, lane, p.prof);
+      inverse(sTot, t);
       if (p.prof && t == 0) { atomicAdd(p.prof + 0, (unsigned long long)(clock64() - ts0)); atomicAdd(p.prof + 3, 1ull); }
       __syncthreads();
       tp0 = (p.prof && t == 0) ? clock64() : 0;
@@ -222,33 +296,17 @@ __global__ void __launch_bounds__(T, Cfg<T, K>::CTAS_PER_SM) jump_kernel(LaunchP
       for (int i = 0; i < K; i++) {
         const int g = backward ? (K - 1 - i) : i;
         const int i0 = (g * 2) * T + t, i1 = (g * 2 + 1) * T + t;
-        u32 x[8], y[8], jx[8], jy[8], dx[8], inv[8], s[8], rx[8], ry[8];
+        u32 x[8], pre[8], rx[8], ry[8], j;
         lds_fe(x, sX, i0, i1);
-        lds_fe(inv, sP, i0, i1);                 // prefix of this kangaroo
+        lds_fe(pre, sP, i0, i1);
         const u32 aux0 = SYM ? (u32)sL[g * T + t] : 0u;
-        const u32 j = jump_index<SYM>(x[0], aux0, p.symRule);
-        u32 aux1 = 0;
-        lds_jp4(jx, jt, j);
-        fe_sub(dx, x, jx);
-        fe_mul(inv, inv, I);                     // 1/dx
-        if (i != K - 1) fe_mul(I, I, dx);        // strip this dx from the running inverse
-        lds_fe(y, sY, i0, i1);
-        lds_jp4(jy, jt + 64, j);
-        fe_sub(s, y, jy);                        // dy
-        fe_mul(s, s, inv);                       // s = dy/dx
-        fe_sqr(rx, s);                           // s^2
-        fe_sub(rx, rx, jx);
-        fe_sub(rx, rx, x);                       // rx = s^2 - jx - x
-        fe_sub(ry, x, rx);
-        fe_mul(ry, ry, s);
-        fe_sub(ry, ry, y);                       // ry = s (x - rx) - y
+        const u32 neg = kangaroo_jump<SYM>(rx, ry, j, x, sY[i0], sY[i1], pre, I, i != K - 1, aux0, jt, p.symRule);
         uint4 dv = sD[g * T + t];
         u32 d[4] = {dv.x, dv.y, dv.z, dv.w};
         const uint4 jd = jt[128 + j];
         d128_add(d, jd.x, jd.y, jd.z, jd.w);
-        if (SYM) {                               // class switch (Check.cpp:551-556), see stream_body
-          const u32 neg = fe_gt_half_mask(ry);
-          fe_cneg(ry, neg);
+        u32 aux1 = 0;
+        if (SYM) {                               // signed 128-bit distance: negated after the add
           d128_cneg(d, neg);
           aux1 = sym_next_aux(aux0, j, neg, p.symRule);
           sL[g * T + t] = (uint8_t)aux1;
@@ -257,29 +315,16 @@ __global__ void __launch_bounds__(T, Cfg<T, K>::CTAS_PER_SM) jump_kernel(LaunchP
         sts_fe(sY, i0, i1, ry);
         sD[g * T + t] = make_uint4(d[0], d[1], d[2], d[3]);
         if (((rx[7] & mhi) | (rx[6] & mlo)) == 0u) {          // GPUCompute.h:96
-          const u64 kidx = (u64)tile * TILE + (u64)g * T + (u64)t;
+          const u64 kidx = (u64)tile * TILE + (u64)(row0 + g) * T + (u64)t;
           if (kidx < p.nKangaroos) {
             const u32 pos = atomicAdd(p.out, 1u);
-            if (pos < p.maxFound) {                           // GPUMath.h:173-188 record layout
-              u32* o = p.out + 1 + (size_t)pos * 14;
-#pragma unroll
-              for (int w = 0; w < 8; w++) o[w] = rx[w];
-              o[8] = d[0]; o[9] = d[1]; o[10] = d[2]; o[11] = d[3];
-              o[12] = (u32)kidx; o[13] = (u32)(kidx >> 32);
-            }
+            if (pos < p.maxFound) put_dp_record(p.out, pos, rx, d, kidx);
           }
         }
         if (!last) {                             // next jump's dx and prefix, accumulated in THIS order
-          lds_jp4(jx, jt, jump_index<SYM>(rx[0], aux1, p.symRule));
-          fe_sub(dx, rx, jx);
-          if (i == 0) {
-            u32 one[8]; fe_set_one(one);
-            sts_fe(sP, i0, i1, one);
-            fe_copy(P, dx);
-          } else {
-            sts_fe(sP, i0, i1, P);
-            fe_mul(P, P, dx);
-          }
+          u32 dx[8];
+          next_dx<SYM>(dx, rx, aux1, jt, p.symRule);
+          chain_dx(sP, i0, i1, P, dx, i == 0);
         }
       }
       if (!last) sts_fe(sTot, t, T + t, P);
@@ -294,30 +339,34 @@ __global__ void __launch_bounds__(T, Cfg<T, K>::CTAS_PER_SM) jump_kernel(LaunchP
       gdst[(g * CHUNKS + 2) * T + t] = sY[(g * 2 + 0) * T + t];
       gdst[(g * CHUNKS + 3) * T + t] = sY[(g * 2 + 1) * T + t];
       gdst[(g * CHUNKS + 4) * T + t] = sD[g * T + t];
-      if (SYM) p.aux[(size_t)tile * TILE + g * T + t] = sL[g * T + t];
+      if (SYM) p.aux[(size_t)tile * TILE + (row0 + g) * T + t] = sL[g * T + t];
     }
   }
 }
 
+// Resident tile kernel: a CTA of T threads owns a tile of T * K kangaroos; warp 0 inverts the tile product.
+template <int T, int K, bool SYM>
+__global__ void __launch_bounds__(T, Cfg<T, K>::CTAS_PER_SM) jump_kernel(LaunchParams p) {
+  tile_body<T, K, 1, SYM>(p, 0, [&](uint4* sTot, int t) {
+    if (t < 32) tile_inverse<T, Cfg<T, K>::W>(sTot, t & 31, p.prof);
+  });
+}
+
 // =====================================================================================================
-// Cluster tile kernel (KGX_MODE=tmem / KGX_KERNEL_TMEM; the selector keeps its name).  One tile of 1792 kangaroos (K = 14 rows
+// Cluster tile kernel (KGX_MODE=tmem / KGX_KERNEL_TMEM; the selector keeps its name).  One tile of 1792 kangaroos (14 rows
 // of T = 128) is shared by the two CTAs of a thread-block cluster, each holding 7 rows -- x, y, prefix products and distances
 // -- in its own shared memory (105 KB, so two CTAs fit on one SM).  The tile still takes ONE inverse per jump: each CTA
-// reduces its 128 thread totals to one product (tile_inverse's chain + butterfly), the two products meet through
-// distributed shared memory across a cluster barrier, both CTAs invert the same tile product and walk their own tree back.
-// That doubles the kangaroos per inverse of a 2-CTA-per-SM resident tile without needing more shared memory per SM.
-// Everything else -- arithmetic, fused pass -- is jump_kernel's (no symmetric instantiation).
+// reduces its 128 thread totals to one product (tile_reduce), the two products meet through distributed shared memory
+// across a cluster barrier, both CTAs invert the same tile product and walk their own tree back.  That doubles the
+// kangaroos per inverse of a 2-CTA-per-SM resident tile without needing more shared memory per SM.  Everything else is
+// tile_body (no symmetric instantiation).
 // =====================================================================================================
-struct CfgCl {
-  static constexpr int T = 128, K = 14, KH = 7, W = 4, TILE = T * K, CLUSTER = 2;   // KH rows per CTA
-  static constexpr int S_X = 0;
-  static constexpr int S_Y = S_X + KH * 2 * T;
-  static constexpr int S_P = S_Y + KH * 2 * T;
-  static constexpr int S_D = S_P + KH * 2 * T;
-  static constexpr int S_TOT = S_D + KH * T;
-  static constexpr int S_XCH = S_TOT + 2 * T;                      // 2 x 2 uint4: this CTA's product, double-buffered
-  static constexpr int S_JT = S_XCH + 4;
-  static constexpr int SMEM_BYTES = S_JT * 16 + JT_WORDS * 4;
+// A CTA's layout is Cfg<128, 7>'s, with the exchange slots (2 x 2 uint4: this CTA's product, double-buffered) where the
+// resident layout keeps its state bytes.
+struct CfgCl : Cfg<128, 7> {
+  static constexpr int CLUSTER = 2;
+  static constexpr int XCH_OFF = LJ_OFF;
+  static constexpr int SMEM_BYTES = XCH_OFF + 4 * 16;
 };
 
 // Called by every thread of both CTAs (it contains a cluster barrier).  Warp 0 turns the T totals of sTot into their
@@ -328,17 +377,7 @@ __device__ __noinline__ void cluster_tile_inverse(uint4* sTot, uint4* mine, cons
   const int lane = t & 31;
   u32 tw[W][8], c[W][8], v[8], sib[5][8];
   if (t < 32) {
-#pragma unroll
-    for (int w = 0; w < W; w++) lds_fe(tw[w], sTot, 32 * w + lane, T + 32 * w + lane);
-    fe_copy(c[0], tw[0]);
-#pragma unroll
-    for (int w = 1; w < W; w++) fe_mul(c[w], c[w - 1], tw[w]);
-    fe_copy(v, c[W - 1]);
-#pragma unroll
-    for (int l = 0; l < 5; l++) {
-      shfl_xor_fe(sib[l], v, 1 << l);
-      fe_mul(v, v, sib[l]);
-    }
+    tile_reduce<T, W>(v, tw, c, sib, sTot, lane);
     if (lane == 0) sts_fe(mine, 0, 1, v);         // product of this CTA's 128 totals
   }
   cooperative_groups::this_cluster().sync();      // release / acquire: both products are visible cluster-wide
@@ -348,149 +387,23 @@ __device__ __noinline__ void cluster_tile_inverse(uint4* sTot, uint4* mine, cons
     fe_mul(inv, v, pv);
     fe_inv(inv, inv);                             // 1 / tile product, identical in both CTAs
     fe_mul(inv, inv, pv);                         // -> 1 / this CTA's product
-#pragma unroll
-    for (int l = 4; l >= 0; l--) fe_mul(inv, inv, sib[l]);
-#pragma unroll
-    for (int w = W - 1; w >= 1; w--) {
-      u32 o[8];
-      fe_mul(o, inv, c[w - 1]);
-      sts_fe(sTot, 32 * w + lane, T + 32 * w + lane, o);
-      fe_mul(inv, inv, tw[w]);
-    }
-    sts_fe(sTot, lane, T + lane, inv);
+    tile_walk_back<T, W>(sTot, inv, tw, c, sib, lane);
   }
 }
 
 __global__ void __cluster_dims__(CfgCl::CLUSTER, 1, 1) __launch_bounds__(CfgCl::T, 2) jump_kernel_cluster(LaunchParams p) {
-  using C = CfgCl;
-  constexpr int T = C::T, KH = C::KH, TILE = C::TILE;
   extern __shared__ uint4 smem[];
-  uint4* sX = smem + C::S_X;
-  uint4* sY = smem + C::S_Y;
-  uint4* sP = smem + C::S_P;
-  uint4* sD = smem + C::S_D;
-  uint4* sTot = smem + C::S_TOT;
-  uint4* jt = smem + C::S_JT;
   cooperative_groups::cluster_group cluster = cooperative_groups::this_cluster();
   const u32 rank = cluster.block_rank();
-  uint4* xch = smem + C::S_XCH;
+  uint4* xch = smem + CfgCl::XCH_OFF / 16;
   const uint4* xchPeer = cluster.map_shared_rank(xch, rank ^ 1u);
-  const int t = threadIdx.x;
-  const u32 mlo = (u32)p.dpMask, mhi = (u32)(p.dpMask >> 32);
-
-  for (int i = t; i < JT_WORDS; i += T) reinterpret_cast<u32*>(jt)[i] = p.jtab[i];
-
   // Exchange slot of the next tile inverse.  It alternates on EVERY call, across tile boundaries too: a CTA can only write
   // a slot again after the cluster barrier of the call in between, which its partner passes only after reading that slot.
   u32 slot = 0;
-  const u32 nClusters = gridDim.x / C::CLUSTER;
-  for (u32 tile = blockIdx.x / C::CLUSTER; tile < p.numTiles; tile += nClusters) {   // both CTAs walk the same tiles
-    __syncthreads();
-    uint4* gsrc = p.state + (size_t)tile * (C::K * CHUNKS * T) + (size_t)rank * (KH * CHUNKS * T);   // rows KH*rank ..
-#pragma unroll
-    for (int g = 0; g < KH; g++) {
-      sX[(g * 2 + 0) * T + t] = gsrc[(g * CHUNKS + 0) * T + t];
-      sX[(g * 2 + 1) * T + t] = gsrc[(g * CHUNKS + 1) * T + t];
-      sY[(g * 2 + 0) * T + t] = gsrc[(g * CHUNKS + 2) * T + t];
-      sY[(g * 2 + 1) * T + t] = gsrc[(g * CHUNKS + 3) * T + t];
-      sD[g * T + t] = gsrc[(g * CHUNKS + 4) * T + t];
-    }
-    u32 P[8];
-    {   // prologue: forward chain of dx; sP[g] = product of the dx before g
-      u32 x[8], jx[8], dx[8];
-#pragma unroll 1
-      for (int g = 0; g < KH; g++) {
-        lds_fe(x, sX, (g * 2) * T + t, (g * 2 + 1) * T + t);
-        lds_jp4(jx, jt, x[0] & 31u);
-        fe_sub(dx, x, jx);
-        if (g == 0) {
-          u32 one[8]; fe_set_one(one);
-          sts_fe(sP, t, T + t, one);
-          fe_copy(P, dx);
-        } else {
-          sts_fe(sP, (g * 2) * T + t, (g * 2 + 1) * T + t, P);
-          fe_mul(P, P, dx);
-        }
-      }
-      sts_fe(sTot, t, T + t, P);
-    }
-    int backward = 1;
-    for (int run = 0; run < p.nRun; run++) {
-      __syncthreads();
-      cluster_tile_inverse<T, C::W>(sTot, xch + 2 * slot, xchPeer + 2 * slot, t);
-      slot ^= 1u;
-      __syncthreads();
-      u32 I[8];
-      lds_fe(I, sTot, t, T + t);
-      const bool last = (run == p.nRun - 1);
-#pragma unroll 1
-      for (int i = 0; i < KH; i++) {
-        const int g = backward ? (KH - 1 - i) : i;
-        const int i0 = (g * 2) * T + t, i1 = (g * 2 + 1) * T + t;
-        u32 x[8], y[8], jx[8], jy[8], dx[8], inv[8], s[8], rx[8], ry[8];
-        lds_fe(x, sX, i0, i1);
-        lds_fe(inv, sP, i0, i1);
-        const u32 j = x[0] & 31u;
-        lds_jp4(jx, jt, j);
-        fe_sub(dx, x, jx);
-        fe_mul(inv, inv, I);                     // 1/dx
-        if (i != KH - 1) fe_mul(I, I, dx);
-        lds_fe(y, sY, i0, i1);
-        lds_jp4(jy, jt + 64, j);
-        fe_sub(s, y, jy);
-        fe_mul(s, s, inv);
-        fe_sqr(rx, s);
-        fe_sub(rx, rx, jx);
-        fe_sub(rx, rx, x);
-        fe_sub(ry, x, rx);
-        fe_mul(ry, ry, s);
-        fe_sub(ry, ry, y);
-        uint4 dv = sD[g * T + t];
-        u32 d[4] = {dv.x, dv.y, dv.z, dv.w};
-        const uint4 jd = jt[128 + j];
-        d128_add(d, jd.x, jd.y, jd.z, jd.w);
-        sts_fe(sX, i0, i1, rx);
-        sts_fe(sY, i0, i1, ry);
-        sD[g * T + t] = make_uint4(d[0], d[1], d[2], d[3]);
-        if (((rx[7] & mhi) | (rx[6] & mlo)) == 0u) {
-          const u64 kidx = (u64)tile * TILE + (u64)(rank * KH + g) * T + (u64)t;
-          if (kidx < p.nKangaroos) {
-            const u32 pos = atomicAdd(p.out, 1u);
-            if (pos < p.maxFound) {
-              u32* o = p.out + 1 + (size_t)pos * 14;
-#pragma unroll
-              for (int w = 0; w < 8; w++) o[w] = rx[w];
-              o[8] = d[0]; o[9] = d[1]; o[10] = d[2]; o[11] = d[3];
-              o[12] = (u32)kidx; o[13] = (u32)(kidx >> 32);
-            }
-          }
-        }
-        if (!last) {
-          lds_jp4(jx, jt, rx[0] & 31u);
-          fe_sub(dx, rx, jx);
-          if (i == 0) {
-            u32 one[8]; fe_set_one(one);
-            sts_fe(sP, i0, i1, one);
-            fe_copy(P, dx);
-          } else {
-            sts_fe(sP, i0, i1, P);
-            fe_mul(P, P, dx);
-          }
-        }
-      }
-      if (!last) sts_fe(sTot, t, T + t, P);
-      backward ^= 1;
-    }
-    uint4* gdst = gsrc;
-#pragma unroll
-    for (int g = 0; g < KH; g++) {
-      gdst[(g * CHUNKS + 0) * T + t] = sX[(g * 2 + 0) * T + t];
-      gdst[(g * CHUNKS + 1) * T + t] = sX[(g * 2 + 1) * T + t];
-      gdst[(g * CHUNKS + 2) * T + t] = sY[(g * 2 + 0) * T + t];
-      gdst[(g * CHUNKS + 3) * T + t] = sY[(g * 2 + 1) * T + t];
-      gdst[(g * CHUNKS + 4) * T + t] = sD[g * T + t];
-    }
-  }
+  tile_body<CfgCl::T, CfgCl::K, CfgCl::CLUSTER, false>(p, rank, [&](uint4* sTot, int t) {
+    cluster_tile_inverse<CfgCl::T, CfgCl::W>(sTot, xch + 2 * slot, xchPeer + 2 * slot, t);
+    slot ^= 1u;
+  });
   cluster.sync();   // the other CTA may still read this CTA's exchange slot
 }
 
@@ -560,12 +473,10 @@ __device__ __noinline__ void emit_dp_from_state(u32* out, const u32 maxFound, co
   const u32 pos = atomicAdd(out, 1u);
   if (pos >= maxFound) return;                         // GPUEngine.cu:641-648: counted, not stored
   const uint4 x0 = sg[0], x1 = sg[T], dv = sg[4 * T];
-  u32 d[4] = {dv.x, dv.y, dv.z, dv.w};
+  u32 x[8], d[4] = {dv.x, dv.y, dv.z, dv.w};
   replay_window<SYM>(d, lg - (ptrdiff_t)runs * (ptrdiff_t)runStride, runStride, runs + 1, jt);
-  u32* o = out + 1 + (size_t)pos * 14;
-  o[0] = x0.x; o[1] = x0.y; o[2] = x0.z; o[3] = x0.w; o[4] = x1.x; o[5] = x1.y; o[6] = x1.z; o[7] = x1.w;
-  o[8] = d[0]; o[9] = d[1]; o[10] = d[2]; o[11] = d[3];
-  o[12] = (u32)kidx; o[13] = (u32)(kidx >> 32);
+  unpack8(x, x0, x1);
+  put_dp_record(out, pos, x, d, kidx);
 }
 
 // Folds the `runs` logged jumps of this thread's G kangaroos into their distance chunks.  st / lt: this thread's column
@@ -596,41 +507,23 @@ __device__ __noinline__ void stream_fold(uint4* st, const uint8_t* lt, const int
 template <int T, bool SYM>
 __device__ __forceinline__ bool stream_body(const KangLoad& cur, uint4* sg, uint4* pg, uint8_t* ag, uint8_t* lg, const uint4* jt, u32* I,
                                             u32* P, const u32 mlo, const u32 mhi, const int rule) {
-  u32 x[8], y[8], jx[8], jy[8], dx[8], inv[8], s[8], rx[8], ry[8];
+  u32 x[8], pre[8], dx[8], rx[8], ry[8], j;
   unpack8(x, cur.x0, cur.x1);
-  unpack8(inv, cur.p0, cur.p1);
-  const u32 j = jump_index<SYM>(x[0], cur.lj, rule);
+  unpack8(pre, cur.p0, cur.p1);
+  // I is stripped after the last kangaroo of a pass too: unused, but one branch fewer
+  const u32 neg = kangaroo_jump<SYM>(rx, ry, j, x, cur.y0, cur.y1, pre, I, true, cur.lj, jt, rule);
   u32 auxn = 0;
-  lds_jp4(jx, jt, j);
-  fe_sub(dx, x, jx);
-  fe_mul(inv, inv, I);                     // 1/dx
-  fe_mul(I, I, dx);                        // strip this dx from the running inverse (unused after the last one)
-  unpack8(y, cur.y0, cur.y1);
-  lds_jp4(jy, jt + 64, j);
-  fe_sub(s, y, jy);
-  fe_mul(s, s, inv);                       // s = dy/dx
-  fe_sqr(rx, s);
-  fe_sub(rx, rx, jx);
-  fe_sub(rx, rx, x);                       // rx = s^2 - jx - x
-  fe_sub(ry, x, rx);
-  fe_mul(ry, ry, s);
-  fe_sub(ry, ry, y);                       // ry = s (x - rx) - y
-  u32 lb = j;                              // jump-log byte (replay_jump): d += jD[j] happens in the fold
-  if (SYM) {                               // equivalence class switch (Check.cpp:551-556): y > (p-1)/2 -> (x, p - y), d -> -d
-    const u32 neg = fe_gt_half_mask(ry);
-    fe_cneg(ry, neg);
-    lb |= neg & 32u;                       // signed 128-bit distance: negated after the add
+  if (SYM) {
     auxn = sym_next_aux(cur.lj, j, neg, rule);
     ag[0] = (uint8_t)auxn;                 // lastJump / symClass
   }
-  lg[0] = (uint8_t)lb;
+  lg[0] = (uint8_t)(j | (neg & 32u));      // jump-log byte (replay_jump): the distance update happens in the fold
   sg[0] = make_uint4(rx[0], rx[1], rx[2], rx[3]);
   sg[T] = make_uint4(rx[4], rx[5], rx[6], rx[7]);
   sg[2 * T] = make_uint4(ry[0], ry[1], ry[2], ry[3]);
   sg[3 * T] = make_uint4(ry[4], ry[5], ry[6], ry[7]);
   // next jump's dx and prefix product, accumulated in THIS order (P starts at 1 for the first kangaroo of a pass)
-  lds_jp4(jx, jt, jump_index<SYM>(rx[0], auxn, rule));
-  fe_sub(dx, rx, jx);
+  next_dx<SYM>(dx, rx, auxn, jt, rule);
   pg[0] = make_uint4(P[0], P[1], P[2], P[3]);
   pg[T] = make_uint4(P[4], P[5], P[6], P[7]);
   fe_mul(P, P, dx);
@@ -648,14 +541,9 @@ __device__ __forceinline__ void stream_group_inverse(u32* I, const u32* P) {
   if (!WARPINV) { fe_inv(I, P); return; }
   u32 v[8], sib[5][8];
   fe_copy(v, P);
-#pragma unroll
-  for (int l = 0; l < 5; l++) {
-    shfl_xor_fe(sib[l], v, 1 << l);
-    fe_mul(v, v, sib[l]);
-  }
+  butterfly_up(v, sib);
   fe_inv(I, v);                                  // identical in all 32 lanes
-#pragma unroll
-  for (int l = 4; l >= 0; l--) fe_mul(I, I, sib[l]);       // -> 1 / (this lane's own product)
+  butterfly_down(I, sib);                        // -> 1 / (this lane's own product)
 }
 
 template <int T, int CTAS, bool WARPINV, bool SYM>
@@ -677,12 +565,11 @@ __global__ void __launch_bounds__(T, CTAS) stream_kernel(LaunchParams p) {
     u32 P[8];
     fe_set_one(P);
     {   // prologue: forward chain, pr[g] = product of the dx before g
-      u32 x[8], jx[8], dx[8];
+      u32 x[8], dx[8];
 #pragma unroll 1
       for (int g = 0; g < G; g++) {
         unpack8(x, st[(g * CHUNKS + 0) * T], st[(g * CHUNKS + 1) * T]);
-        lds_jp4(jx, jt, jump_index<SYM>(x[0], SYM ? (u32)au[(size_t)g * T] : 0u, p.symRule));
-        fe_sub(dx, x, jx);
+        next_dx<SYM>(dx, x, SYM ? (u32)au[(size_t)g * T] : 0u, jt, p.symRule);
         pr[(g * 2) * T] = make_uint4(P[0], P[1], P[2], P[3]); pr[(g * 2 + 1) * T] = make_uint4(P[4], P[5], P[6], P[7]);
         fe_mul(P, P, dx);
       }
@@ -746,40 +633,41 @@ __global__ void __launch_bounds__(T, CTAS) stream_kernel(LaunchParams p) {
 
 // ---- host AoS (kIdx order) <-> tile layout --------------------------------------------------------------
 // slot s -> tile = s / TILE, g = (s % TILE) / T, t = s % T.  Padding slots (s >= n) replicate kangaroo s % n
-// so that every tile is full of valid walkers; their DPs are dropped by the kidx < nKangaroos test.
-__global__ void pack_kernel(uint4* state, const uint4* px, const uint4* py, const uint4* d, u64 n, u64 nPadded, int T, int K, uint8_t* aux, int auxInit) {
+// so that every tile is full of valid walkers; their DPs are dropped by the kidx < nKangaroos test.  The state byte of
+// slot s (symmetric mode) is aux[s].
+// Chunk 0 of slot s in the [tile][g][CHUNKS][T] layout of T x K tiles; chunk c is at [c * T].
+template <class V>
+__device__ __forceinline__ V* slot_chunks(V* state, u64 s, int T, int K) {
   const int TILE = T * K;
+  const int r = (int)(s % TILE);
+  return state + (s / TILE) * (K * CHUNKS * T) + (r / T) * (CHUNKS * T) + r % T;
+}
+__global__ void pack_kernel(uint4* state, const uint4* px, const uint4* py, const uint4* d, u64 n, u64 nPadded, int T, int K, uint8_t* aux, int auxInit) {
   u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= nPadded) return;
   u64 src = s < n ? s : s % n;
-  u64 tile = s / TILE; int r = (int)(s % TILE); int g = r / T, t = r % T;
-  uint4* dst = state + tile * (K * CHUNKS * T);
-  dst[(g * CHUNKS + 0) * T + t] = px[2 * src];
-  dst[(g * CHUNKS + 1) * T + t] = px[2 * src + 1];
-  dst[(g * CHUNKS + 2) * T + t] = py[2 * src];
-  dst[(g * CHUNKS + 3) * T + t] = py[2 * src + 1];
-  dst[(g * CHUNKS + 4) * T + t] = d[src];
-  if (aux) aux[tile * TILE + (u64)g * T + t] = (uint8_t)auxInit;   // lastJump = NB_JUMP: none yet (GPUEngine.cu:413-416) / symClass = 0 (Kangaroo.cpp:345-347)
+  uint4* dst = slot_chunks(state, s, T, K);
+  dst[0] = px[2 * src];
+  dst[T] = px[2 * src + 1];
+  dst[2 * T] = py[2 * src];
+  dst[3 * T] = py[2 * src + 1];
+  dst[4 * T] = d[src];
+  if (aux) aux[s] = (uint8_t)auxInit;   // lastJump = NB_JUMP: none yet (GPUEngine.cu:413-416) / symClass = 0 (Kangaroo.cpp:345-347)
 }
 __global__ void unpack_kernel(const uint4* state, uint4* px, uint4* py, uint4* d, u64 n, int T, int K) {
-  const int TILE = T * K;
   u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= n) return;
-  u64 tile = s / TILE; int r = (int)(s % TILE); int g = r / T, t = r % T;
-  const uint4* src = state + tile * (K * CHUNKS * T);
-  px[2 * s] = src[(g * CHUNKS + 0) * T + t];
-  px[2 * s + 1] = src[(g * CHUNKS + 1) * T + t];
-  py[2 * s] = src[(g * CHUNKS + 2) * T + t];
-  py[2 * s + 1] = src[(g * CHUNKS + 3) * T + t];
-  d[s] = src[(g * CHUNKS + 4) * T + t];
+  const uint4* src = slot_chunks(state, s, T, K);
+  px[2 * s] = src[0];
+  px[2 * s + 1] = src[T];
+  py[2 * s] = src[2 * T];
+  py[2 * s + 1] = src[3 * T];
+  d[s] = src[4 * T];
 }
 struct PatchArgs { uint4 c[CHUNKS]; };
 __global__ void patch_kernel(uint4* state, u64 s, PatchArgs a, int T, int K, uint8_t* aux, int auxInit) {
-  const int TILE = T * K;
-  u64 tile = s / TILE; int r = (int)(s % TILE); int g = r / T, t = r % T;
-  uint4* dst = state + tile * (K * CHUNKS * T);
-  if (threadIdx.x < CHUNKS) dst[(g * CHUNKS + threadIdx.x) * T + t] = a.c[threadIdx.x];
-  if (aux && threadIdx.x == 0) aux[tile * TILE + (u64)g * T + t] = (uint8_t)auxInit;   // GPUEngine.cu:532-536
+  if (threadIdx.x < CHUNKS) slot_chunks(state, s, T, K)[threadIdx.x * T] = a.c[threadIdx.x];
+  if (aux && threadIdx.x == 0) aux[s] = (uint8_t)auxInit;   // GPUEngine.cu:532-536
 }
 
 // ---- SURVEY 8f/f1: device-side HashTable::Convert (HashTable.cpp:75-100) -------------------------------------------

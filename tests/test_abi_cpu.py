@@ -22,17 +22,24 @@ def test_header_symbols_are_exported():
     assert declared == set(_lib.EXPORTED_SYMBOLS)
 
 
+def kernel_table(src, sym):
+    """The entries of kgx_engine.cu's g_kernels table for the non-symmetric (sym = "false") or symmetric ("true") engine:
+    ("resident", "T,K") per KGX_RESIDENT (in table order; the first is the default geometry), ("stream", CTAS, inverse) per
+    KGX_STREAM and ("tmem",) for the cluster kernel's entry."""
+    table = re.search(r"g_kernels\[\]\s*=\s*\{(.*?)\n\};", src, re.S).group(1)
+    kernels = [("resident", "%s,%s" % (t, k)) for t, k in re.findall(
+        r"KGX_RESIDENT\(\s*(\d+)\s*,\s*(\d+)\s*,\s*%s\s*\)" % sym, table)]
+    for ctas, warp in re.findall(r"KGX_STREAM\(\s*(\d+)\s*,\s*(true|false)\s*,\s*%s\s*\)" % sym, table):
+        kernels.append(("stream", ctas, "warp" if warp == "true" else "thread"))
+    if re.search(r"\b%s\s*,\s*jump_kernel_cluster\b" % sym, table):      # the entry's sym field precedes its function
+        kernels.append(("tmem",))
+    return kernels
+
+
 def compiled_jump_kernels(src):
-    """The jump-kernel instantiations kgx_engine.cu launches in the non-symmetric engine: ("resident", "T,K") per KGX_CFG_ENTRY or
-    KGX_CFG_ENTRY_SYM (the first entry is the default geometry), ("stream", CTAS, inverse) per stream_kernel<128, CTAS, WARPINV,
-    false> launch, and the cluster kernel."""
-    geoms = re.findall(r"KGX_CFG_ENTRY(?:_SYM)?\(\s*(\d+)\s*,\s*(\d+)\s*\)", src)
-    kernels = {("resident", "%s,%s" % g) for g in geoms}
-    for ctas, warp in re.findall(r"stream_kernel<\s*128\s*,\s*(\d+)\s*,\s*(true|false)\s*,\s*false\s*>\s*<<<", src):
-        kernels.add(("stream", ctas, "warp" if warp == "true" else "thread"))
-    if re.search(r"jump_kernel_cluster\s*<<<", src):
-        kernels.add(("tmem",))
-    return kernels, "%s,%s" % geoms[0]
+    """The jump-kernel instantiations kgx_engine.cu launches in the non-symmetric engine, and its default tile geometry."""
+    kernels = kernel_table(src, "false")
+    return set(kernels), kernels[0][1]
 
 
 def variant_kernel(env, default_geometry):
@@ -47,12 +54,8 @@ def variant_kernel(env, default_geometry):
 
 
 def compiled_symmetric_jump_kernels(src):
-    """The instantiations the symmetric engine (kgx_set_symmetry) launches: ("resident", "T,K") per KGX_CFG_ENTRY_SYM and
-    ("stream", CTAS, inverse) per stream_kernel<128, CTAS, WARPINV, true> launch."""
-    kernels = {("resident", "%s,%s" % g) for g in re.findall(r"KGX_CFG_ENTRY_SYM\(\s*(\d+)\s*,\s*(\d+)\s*\)", src)}
-    for ctas, warp in re.findall(r"stream_kernel<\s*128\s*,\s*(\d+)\s*,\s*(true|false)\s*,\s*true\s*>\s*<<<", src):
-        kernels.add(("stream", ctas, "warp" if warp == "true" else "thread"))
-    return kernels
+    """The instantiations the symmetric engine (kgx_set_symmetry) launches."""
+    return set(kernel_table(src, "true"))
 
 
 def symmetric_variant_kernel(env, default_geometry):
@@ -87,8 +90,8 @@ def test_every_compiled_jump_kernel_has_a_gpu_test():
     assert compiled_symmetric_jump_kernels(src) == {("resident", "128,7"), ("stream", "2", "warp")}
     check_variants_cover(src, VARIANTS, SYM_VARIANTS)
     # the guard itself: one more geometry, one more symmetric geometry, or one variant fewer, must fail it
-    extra = src.replace("KGX_CFG_ENTRY(32, 12),", "KGX_CFG_ENTRY(32, 12), KGX_CFG_ENTRY(160, 3),")
-    extra_sym = src.replace("KGX_CFG_ENTRY(64, 7),", "KGX_CFG_ENTRY_SYM(64, 7),")
+    extra = src.replace("KGX_RESIDENT(32, 12, false),", "KGX_RESIDENT(32, 12, false), KGX_RESIDENT(160, 3, false),")
+    extra_sym = src.replace("KGX_RESIDENT(64, 7, false),", "KGX_RESIDENT(64, 7, false), KGX_RESIDENT(64, 7, true),")
     assert extra != src and extra_sym != src
     for bad_src in (extra, extra_sym):
         with pytest.raises(AssertionError):
@@ -134,7 +137,7 @@ def test_every_stream_instantiation_runs_multi_window_launches():
     assert adaptive_group_bounds(src) == (2, 128)
     check_log_variants_cover(src, LOG_VARIANTS, SYM_LOG_VARIANTS)
     # the guard itself: a 3-CTA symmetric stream kernel, or any one entry fewer in either list, must fail it
-    sym3 = src.replace("stream_kernel<128, 2, true, true>", "stream_kernel<128, 3, true, true>")
+    sym3 = src.replace("KGX_STREAM(2, true, true)", "KGX_STREAM(3, true, true)")
     assert sym3 != src
     with pytest.raises(AssertionError):
         check_log_variants_cover(sym3, LOG_VARIANTS, SYM_LOG_VARIANTS)

@@ -378,8 +378,10 @@ def long_walks_agree(monkeypatch, rule=None, sym_table=None, stream_runs=LONG_WA
 
 def test_stream_and_resident_agree_over_a_long_walk(monkeypatch):
     """Cross-validation at a scale the CPU oracle cannot reach: 1,048,576 kangaroos x 100 launches (6400 jumps each) on the
-    three independent kernel implementations (different memory layout, different batch-inverse topology; the tile kernels loop
-    over several tiles per CTA here) must end in bit-identical states and produce the same DP multiset."""
+    three kernels (different memory layout, different batch-inverse topology; the tile kernels loop over several tiles per
+    CTA here) must end in bit-identical states and produce the same DP multiset.  The per-kangaroo jump is one function
+    shared by all three, so the independent check of the arithmetic is the CPU oracle, which every variant is compared
+    against at smaller sizes."""
     long_walks_agree(monkeypatch)
 
 
