@@ -6,41 +6,9 @@
 //   export: d = biased - wildOffset (mod n) for odd kIdx, biased for even kIdx      (256-bit result)
 //   import: biased = (d mod n) + wildOffset (mod n) for odd kIdx, d mod n for even   (must fit in 128 bits)
 #pragma once
-#include "kgx_field.cuh"
+#include "kgx_curve.cuh"   // kOrder, sub256, add256, ge_order
 
 namespace kgx {
-
-__device__ __constant__ u64 kOrder[4] = {0xBFD25E8CD0364141ull, 0xBAAEDCE6AF48A03Bull, 0xFFFFFFFFFFFFFFFEull, 0xFFFFFFFFFFFFFFFFull};
-
-// r = a - b (mod 2^256); returns the borrow
-__device__ __forceinline__ u64 sub256(u64* r, const u64* a, const u64* b) {
-  u64 br = 0;
-#pragma unroll
-  for (int k = 0; k < 4; k++) {
-    const u64 t = a[k] - b[k];
-    const u64 b1 = a[k] < b[k];
-    r[k] = t - br;
-    br = b1 | (t < br);
-  }
-  return br;
-}
-// r = a + b (mod 2^256); returns the carry
-__device__ __forceinline__ u64 add256(u64* r, const u64* a, const u64* b) {
-  u64 c = 0;
-#pragma unroll
-  for (int k = 0; k < 4; k++) {
-    const u64 t = a[k] + b[k];
-    const u64 c1 = t < a[k];
-    r[k] = t + c;
-    c = c1 | (r[k] < t);
-  }
-  return c;
-}
-__device__ __forceinline__ bool ge_order(const u64* a) {
-#pragma unroll
-  for (int k = 3; k >= 0; k--) if (a[k] != kOrder[k]) return a[k] > kOrder[k];
-  return true;
-}
 
 // staging (AoS u32, kIdx order: x 8 words, y 8 words, biased d 4 words) -> records rec[n][12] (u64)
 __global__ void herd_export_kernel(const u32* __restrict__ px, const u32* __restrict__ py, const u32* __restrict__ d128,

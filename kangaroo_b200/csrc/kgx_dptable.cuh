@@ -4,7 +4,8 @@
 // with kgx_ingest.cpp's event mapping (kgx_ingest.cpp:68-83): 2^18 buckets h = x.bits64[2] & 0x3FFFF, one ENTRY {x, d} per
 // distinct x of a bucket, per-bucket nbItem / maxItem counted like the reference (maxItem 16 on the first Add of a bucket, +4
 // on every later Add -- stored or not -- that finds nbItem >= maxItem - 1), and work files that are byte for byte what
-// HashTable::SaveTable writes (buckets in order, entries sorted by unsigned (x.hi, x.lo)).
+// HashTable::SaveTable writes (buckets in order, entries sorted by unsigned (x.hi, x.lo)).  The file format is
+// kgx_workfile.h's; a save orders each chunk of whole buckets with kgx_bucketsort.cuh's sort.
 //
 // Layout (fixed capacity C entries, no growth):
 //   ent[C]      32-byte entries {x, d}, dense in insertion order; ent_h[C] their bucket
@@ -20,18 +21,18 @@
 //      the (h, x) index in place of its binary search.  Buckets never share an entry, so threads of different buckets only
 //      meet in the index, where an insert claims an empty slot with a CAS after its entry is written.
 //   4. the events, written at their arrival index, are compacted in arrival order; the first `cap` go back to the host.
-#include <cerrno>
 #include <cub/cub.cuh>
+#include "kgx_workfile.h"
+#include "kgx_bucketsort.cuh"
 
 namespace kgx_dpt {
 
+using kgx_wf::Entry;
+using kgx_wf::NBUCKET;
 typedef unsigned long long ull;
-constexpr uint32_t NBUCKET = 1u << 18;                  // HASH_SIZE (HashTable.h)
 constexpr uint64_t TYPE_BIT = 0x4000000000000000ull;    // b126 of the tagged distance: herd type (HashTable::CalcDistAndType)
 constexpr uint64_t SAVE_CHUNK = 1ull << 21;             // entries per device->host chunk of a save / host->device chunk of a load
-constexpr uint32_t HEADW = 0xFA6A8001u;                 // Kangaroo.h:120
 
-struct Entry { uint64_t x0, x1, d0, d1; };              // ENTRY {int128 x; int128 d}
 struct Res { ull count; uint32_t nsel; uint32_t bad; };
 struct Ranks { uint32_t n; uint32_t pre[KGX_DPT_MAX_RANKS + 1]; };
 
@@ -152,20 +153,6 @@ __global__ void k_save_select(const uint32_t* ent_h, uint64_t count, uint32_t b0
   if (h >= b0 && h < b1) idx[atomicAdd(cursor, 1u)] = (uint32_t)e;
 }
 
-__global__ void k_save_key(const Entry* ent, const uint32_t* ent_h, const uint32_t* idx, uint32_t n, int which, uint32_t b0, uint64_t* key) {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= n) return;
-  const uint32_t e = idx[t];
-  if (which == 0) key[t] = ent[e].x0;
-  else if (which == 1) key[t] = ent[e].x1;
-  else reinterpret_cast<uint32_t*>(key)[t] = ent_h[e] - b0;
-}
-
-__global__ void k_save_out(const Entry* ent, const uint32_t* idx, uint32_t n, Entry* out) {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t < n) out[t] = ent[idx[t]];
-}
-
 inline uint64_t slots_for(uint64_t capacity) { return capacity + capacity / 2 + 64; }
 inline uint64_t save_chunk_for(uint64_t capacity) { return capacity < SAVE_CHUNK ? (capacity ? capacity : 1) : SAVE_CHUNK; }
 
@@ -274,8 +261,6 @@ static int dpt_pinned(kgx_dptable* t) {
   return 0;
 }
 
-static int dpt_io_error() { return errno ? -errno : -EIO; }
-
 extern "C" {
 
 uint64_t kgx_dptable_bytes_for(uint64_t capacity) {
@@ -322,10 +307,7 @@ kgx_dptable* kgx_dptable_create(int dev, uint64_t capacity) {
   t->dev = dev; t->capacity = capacity; t->nslots = kgx_dpt::slots_for(capacity);
   t->chunk = kgx_dpt::save_chunk_for(capacity);
   const uint64_t c = t->chunk;
-  size_t tmpA = 0, tmpB = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tmpA, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)c, 0, 64);
-  cub::DeviceRadixSort::SortPairs(nullptr, tmpB, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)c, 0, 19);
-  t->sTmpBytes = tmpA > tmpB ? tmpA : tmpB;
+  t->sTmpBytes = kgx_wf::bucket_sort_scratch(c);
   bool ok = !dpt_alloc(t, (void**)&t->ent, sizeof(kgx_dpt::Entry) * capacity) && !dpt_alloc(t, (void**)&t->ent_h, 4ull * capacity) &&
             !dpt_alloc(t, (void**)&t->slots, 8ull * t->nslots) && !dpt_alloc(t, (void**)&t->nb, 4ull * kgx_dpt::NBUCKET) &&
             !dpt_alloc(t, (void**)&t->mx, 4ull * kgx_dpt::NBUCKET) && !dpt_alloc(t, (void**)&t->res, sizeof(kgx_dpt::Res)) &&
@@ -439,6 +421,7 @@ int kgx_dptable_save_work(kgx_dptable* t, const char* path, uint32_t dp_bits, co
                           const uint64_t keyx[4], const uint64_t keyy[4], uint64_t total_count, double total_time, uint64_t total_walk,
                           void* stream) {
   using namespace kgx_dpt;
+  using namespace kgx_wf;
   cudaStream_t st = (cudaStream_t)stream;
   DPT_CK(t, cudaSetDevice(t->dev));
   DPT_CK(t, cudaStreamSynchronize(st));                    // every add queued on this stream is in the table
@@ -454,13 +437,9 @@ int kgx_dptable_save_work(kgx_dptable* t, const char* path, uint32_t dp_bits, co
   }
   errno = 0;
   FILE* f = fopen(path, "wb");
-  if (!f) { const int e = dpt_io_error(); free(nbH); snprintf(t->err, sizeof t->err, "%s: %s", path, strerror(-e)); return e; }
+  if (!f) { const int e = io_error(); free(nbH); snprintf(t->err, sizeof t->err, "%s: %s", path, strerror(-e)); return e; }
   setvbuf(f, nullptr, _IOFBF, 1 << 22);
-  // Kangaroo::SaveHeader (Backup.cpp:368-394), type HEADW -- the header kgi_save_work_ex writes
-  const uint32_t head = HEADW, version = 0;
-  bool ok = fwrite(&head, 4, 1, f) == 1 && fwrite(&version, 4, 1, f) == 1 && fwrite(&dp_bits, 4, 1, f) == 1 &&
-            fwrite(range_start, 32, 1, f) == 1 && fwrite(range_end, 32, 1, f) == 1 && fwrite(keyx, 32, 1, f) == 1 &&
-            fwrite(keyy, 32, 1, f) == 1 && fwrite(&total_count, 8, 1, f) == 1 && fwrite(&total_time, 8, 1, f) == 1;
+  bool ok = write_header(f, make_header(dp_bits, range_start, range_end, keyx, keyy, total_count, total_time));
   int rc = 0;
   // HashTable::SaveTable (HashTable.cpp:375-396) in chunks of whole buckets: select, sort by (h, x.hi, x.lo), copy out
   uint32_t b0 = 0;
@@ -476,19 +455,12 @@ int kgx_dptable_save_work(kgx_dptable* t, const char* path, uint32_t dp_bits, co
     }
     if (m) {
       const uint32_t n = (uint32_t)m, B = 256, G = (n + B - 1) / B;
-      size_t tb = t->sTmpBytes;
-      int bits = 1;
-      while ((1u << bits) < b1 - b0) bits++;
+      uint32_t* order = nullptr;
       bool good = cudaMemsetAsync(t->sCursor, 0, 4, st) == cudaSuccess;
       k_save_select<<<(unsigned)((t->count + B - 1) / B), B, 0, st>>>(t->ent_h, t->count, b0, b1, t->sIdxA, t->sCursor);
-      k_save_key<<<G, B, 0, st>>>(t->ent, t->ent_h, t->sIdxA, n, 0, b0, t->sKeyA);
-      good = good && cub::DeviceRadixSort::SortPairs(t->sTmp, tb, t->sKeyA, t->sKeyB, t->sIdxA, t->sIdxB, (int)n, 0, 64, st) == cudaSuccess;
-      k_save_key<<<G, B, 0, st>>>(t->ent, t->ent_h, t->sIdxB, n, 1, b0, t->sKeyA);
-      good = good && cub::DeviceRadixSort::SortPairs(t->sTmp, tb, t->sKeyA, t->sKeyB, t->sIdxB, t->sIdxA, (int)n, 0, 64, st) == cudaSuccess;
-      k_save_key<<<G, B, 0, st>>>(t->ent, t->ent_h, t->sIdxA, n, 2, b0, t->sKeyA);
-      good = good && cub::DeviceRadixSort::SortPairs(t->sTmp, tb, (uint32_t*)t->sKeyA, (uint32_t*)t->sKeyB, t->sIdxA, t->sIdxB, (int)n, 0,
-                                                     bits, st) == cudaSuccess;
-      k_save_out<<<G, B, 0, st>>>(t->ent, t->sIdxB, n, t->sOut);
+      good = good && bucket_sort(t->ent, t->ent_h, t->sIdxA, n, b0, b1, t->sIdxA, t->sIdxB, t->sKeyA, t->sKeyB, t->sTmp, t->sTmpBytes, st,
+                                 &order) == cudaSuccess;
+      if (good) bucket_gather<<<G, B, 0, st>>>(t->ent, order, n, t->sOut);
       good = good && cudaMemcpyAsync(t->hostEnt, t->sOut, sizeof(Entry) * m, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
              cudaStreamSynchronize(st) == cudaSuccess;
       if (!good) {
@@ -499,8 +471,7 @@ int kgx_dptable_save_work(kgx_dptable* t, const char* path, uint32_t dp_bits, co
     }
     uint64_t off = 0;
     for (uint32_t b = b0; ok && b < b1; b++) {
-      ok = fwrite(&nbH[b], 4, 1, f) == 1 && fwrite(&mxH[b], 4, 1, f) == 1 &&
-           (nbH[b] == 0 || fwrite(t->hostEnt + off, sizeof(Entry), nbH[b], f) == nbH[b]);
+      ok = write_bucket(f, nbH[b], mxH[b], t->hostEnt + off);
       off += nbH[b];
     }
     b0 = b1;
@@ -508,8 +479,8 @@ int kgx_dptable_save_work(kgx_dptable* t, const char* path, uint32_t dp_bits, co
   free(nbH);
   ok = ok && fwrite(&total_walk, 8, 1, f) == 1;           // Backup.cpp:530-531 / 549-551
   ok = fflush(f) == 0 && ok;
-  int err = rc ? rc : (ok ? 0 : dpt_io_error());
-  if (fclose(f) != 0 && err == 0) err = dpt_io_error();
+  int err = rc ? rc : (ok ? 0 : io_error());
+  if (fclose(f) != 0 && err == 0) err = io_error();
   if (err < 0 && err != -3) snprintf(t->err, sizeof t->err, "%s: %s", path, strerror(-err));
   return err;
 }
@@ -518,6 +489,7 @@ int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, u
                           uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time, uint64_t* nb_walk,
                           uint64_t* walk_offset, void* stream) {
   using namespace kgx_dpt;
+  using namespace kgx_wf;
   cudaStream_t st = (cudaStream_t)stream;
   DPT_CK(t, cudaSetDevice(t->dev));
   DPT_CK(t, cudaStreamSynchronize(st));
@@ -525,14 +497,11 @@ int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, u
   if (dpt_pinned(t)) return -3;
   errno = 0;
   FILE* f = fopen(path, "rb");
-  if (!f) { const int e = dpt_io_error(); snprintf(t->err, sizeof t->err, "%s: %s", path, strerror(-e)); return e; }
+  if (!f) { const int e = io_error(); snprintf(t->err, sizeof t->err, "%s: %s", path, strerror(-e)); return e; }
   setvbuf(f, nullptr, _IOFBF, 1 << 22);
-  // Kangaroo::LoadWork (Backup.cpp:149-207)
-  uint32_t head = 0, version = 0, dp = 0;
-  uint64_t hdr[16], cnt = 0, walk = 0;
-  double tm = 0;
-  bool ok = fread(&head, 4, 1, f) == 1 && fread(&version, 4, 1, f) == 1 && head == HEADW;
-  ok = ok && fread(&dp, 4, 1, f) == 1 && fread(hdr, 32, 4, f) == 4 && fread(&cnt, 8, 1, f) == 1 && fread(&tm, 8, 1, f) == 1;
+  WorkHeader hd;                                          // Kangaroo::LoadWork (Backup.cpp:149-207)
+  uint64_t walk = 0, off = 0;
+  bool ok = read_header(f, hd);
   uint32_t* nbH = (uint32_t*)malloc(8ull * NBUCKET);
   if (!nbH) { fclose(f); snprintf(t->err, sizeof t->err, "out of host memory"); return -ENOMEM; }
   uint32_t* mxH = nbH + NBUCKET;
@@ -555,7 +524,7 @@ int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, u
     return true;
   };
   for (uint32_t h = 0; ok && h < NBUCKET; h++) {           // HashTable::LoadTable (HashTable.cpp:439-459)
-    ok = fread(&nbH[h], 4, 1, f) == 1 && fread(&mxH[h], 4, 1, f) == 1;
+    ok = read_bucket_head(f, nbH[h], mxH[h]);
     uint32_t left = ok ? nbH[h] : 0;
     total += left;
     if (ok && total > t->capacity) { rc = -ENOSPC; ok = false; break; }
@@ -569,13 +538,7 @@ int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, u
     }
   }
   ok = ok && flush();
-  ok = ok && fread(&walk, 8, 1, f) == 1;
-  long off = ok ? ftell(f) : -1;
-  if (ok && walk) {                                       // the kangaroo block must be all there (FetchWalks, Backup.cpp:211-223)
-    ok = off >= 0 && fseek(f, 0, SEEK_END) == 0;
-    const long end = ok ? ftell(f) : -1;
-    ok = ok && end >= off && (uint64_t)(end - off) / 96 >= walk;
-  }
+  ok = ok && fread(&walk, 8, 1, f) == 1 && walks_complete(f, walk, off);
   fclose(f);
   if (ok) {
     ok = cudaMemcpy(t->nb, nbH, 4ull * NBUCKET, cudaMemcpyHostToDevice) == cudaSuccess &&
@@ -593,15 +556,9 @@ int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, u
     dpt_reset(t, st);
     return rc ? rc : -EINVAL;
   }
-  if (dp_bits) *dp_bits = dp;
-  if (range_start) memcpy(range_start, hdr, 32);
-  if (range_end) memcpy(range_end, hdr + 4, 32);
-  if (keyx) memcpy(keyx, hdr + 8, 32);
-  if (keyy) memcpy(keyy, hdr + 12, 32);
-  if (total_count) *total_count = cnt;
-  if (total_time) *total_time = tm;
+  get_header(hd, dp_bits, range_start, range_end, keyx, keyy, total_count, total_time);
   if (nb_walk) *nb_walk = walk;
-  if (walk_offset) *walk_offset = (uint64_t)off;
+  if (walk_offset) *walk_offset = off;
   return 0;
 }
 

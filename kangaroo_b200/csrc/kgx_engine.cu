@@ -790,5 +790,6 @@ int kgx_bench_raw(int dev, int kind, int iters, float* ms, double* ops) {
 
 }  // extern "C"
 
+#include "kgx_bucketsort.cuh"  // work-file order for a block of buckets (the table's save and the merge)
 #include "kgx_dptable.cuh"   // the device-resident DP table (kgx_dptable_*)
 #include "kgx_worktool.cuh"  // work-file check and merge (kgx_work_*)

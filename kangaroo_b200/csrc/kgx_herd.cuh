@@ -4,34 +4,16 @@
 // the reference's 32x256-entry byte table walk this uses a 256-entry table of 2^i*G built on the device, Jacobian
 // mixed additions over the set bits of d, and ONE inversion per kangaroo.
 #pragma once
-#include "kgx_field.cuh"
+#include "kgx_curve.cuh"
 #include "kgx_kernel.cuh"
-#include "kgx_modinv.h"
 
 namespace kgx {
-
-__device__ __forceinline__ void fe_neg(u32* r, const u32* a) {
-  u32 z[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  fe_sub(r, z, a);
-}
-__device__ __forceinline__ void fe_dbl(u32* r, const u32* a) {   // 2a mod p
-  u32 n[8];
-  fe_neg(n, a);
-  fe_sub(r, a, n);
-}
-
-// a == 0 (mod p)?  fe_mul / fe_sub results live in [0, 2^256): the only representatives of 0 are 0 and p.
-__device__ __forceinline__ bool fe_is_zero_modp(const u32* a) {
-  const u32 orv = a[0] | a[1] | a[2] | a[3] | a[4] | a[5] | a[6] | a[7];
-  const u32 andv = a[2] & a[3] & a[4] & a[5] & a[6] & a[7];
-  return orv == 0u || (andv == 0xFFFFFFFFu && a[1] == 0xFFFFFFFEu && a[0] == 0xFFFFFC2Fu);
-}
 
 // tab[i] = 2^i * G (affine, 16 words each: x then y), i = 0..255.  One thread; 255 affine doublings.
 __global__ void herd_table_kernel(u32* tab) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  u32 x[8] = {0x16F81798u, 0x59F2815Bu, 0x2DCE28D9u, 0x029BFCDBu, 0xCE870B07u, 0x55A06295u, 0xF9DCBBACu, 0x79BE667Eu};
-  u32 y[8] = {0xFB10D4B8u, 0x9C47D08Fu, 0xA6855419u, 0xFD17B448u, 0x0E1108A8u, 0x5DA4FBFCu, 0x26A3C465u, 0x483ADA77u};
+  u32 x[8], y[8];
+  set_g(x, y);
   for (int i = 0; i < 256; i++) {
     for (int w = 0; w < 8; w++) { tab[i * 16 + w] = x[w]; tab[i * 16 + 8 + w] = y[w]; }
     // s = 3x^2 / 2y ; x' = s^2 - 2x ; y' = s (x - x') - y     (SECP256K1.cpp:438-466 DoubleDirect)
@@ -46,19 +28,6 @@ __global__ void herd_table_kernel(u32* tab) {
     fe_sub(ny, x, nx); fe_mul(ny, ny, s); fe_sub(ny, ny, y);
     // canonicalise (table entries are compared against nothing, but keep them in [0,p) like the reference)
     fe_copy(x, nx); fe_copy(y, ny);
-  }
-}
-
-// canonical residue: fe_mul / fe_sub leave values < 2^256 congruent mod p; subtract p once if needed
-// (subtracting p mod 2^256 == adding 0x1000003D1)
-__device__ __forceinline__ void fe_canon(u32* V) {
-  const u32 pm[8] = {0xFFFFFC2Fu, 0xFFFFFFFEu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
-  bool ge = true;
-  for (int w = 7; w >= 0; w--) { if (V[w] != pm[w]) { ge = V[w] > pm[w]; break; } }
-  if (ge) {
-    u64 acc = (u64)V[0] + 0x3D1u; V[0] = (u32)acc;
-    acc = (u64)V[1] + 1u + (acc >> 32); V[1] = (u32)acc;
-    for (int w = 2; w < 8; w++) { acc = (u64)V[w] + (acc >> 32); V[w] = (u32)acc; }
   }
 }
 
@@ -89,47 +58,9 @@ __global__ void herd_kernel(const u32* __restrict__ tab, const u32* __restrict__
     u32 qx[8], qy[8];
 #pragma unroll
     for (int w = 0; w < 8; w++) { qx[w] = q[w]; qy[w] = q[8 + w]; }
-    if (inf) {
-      fe_copy(X, qx); fe_copy(Y, qy); fe_set_one(Z); inf = false;
-      continue;
-    }
-    // mixed Jacobian + affine:  H = x2 Z^2 - X ; R = y2 Z^3 - Y ; X3 = R^2 - H^3 - 2 X H^2 ; Y3 = R (X H^2 - X3) - Y H^3 ; Z3 = Z H
-    u32 zz[8], u2[8], s2[8], h[8], r[8], hh[8], hhh[8], v[8], t[8];
-    fe_sqr(zz, Z);
-    fe_mul(u2, qx, zz);
-    fe_mul(s2, qy, zz); fe_mul(s2, s2, Z);
-    fe_sub(h, u2, X);
-    fe_sub(r, s2, Y);
-    if (fe_is_zero_modp(h)) {
-      // same x: the term equals the accumulator (double it) or its negative (sum = point at infinity).  Cannot happen
-      // between table terms for a scalar < n; happens for the key term when d*G == +-key (a wild kangaroo created on
-      // the key itself).  The reference's AddDirect (SECP256K1.cpp:238-262) would divide by zero -> garbage; here the
-      // group law is followed (VERDICT r1 weak #9).
-      if (!fe_is_zero_modp(r)) { inf = true; continue; }
-      // Jacobian doubling, a = 0: S = 4 X Y^2 ; M = 3 X^2 ; X' = M^2 - 2S ; Y' = M (S - X') - 8 Y^4 ; Z' = 2 Y Z
-      u32 yy[8], S[8], M[8], m2[8], y4[8], nx[8], ny[8], nz[8];
-      fe_sqr(yy, Y);
-      fe_mul(S, X, yy); fe_dbl(S, S); fe_dbl(S, S);
-      fe_sqr(m2, X); fe_dbl(M, m2); { u32 ng[8]; fe_neg(ng, m2); fe_sub(M, M, ng); }
-      fe_sqr(nx, M); fe_sub(nx, nx, S); fe_sub(nx, nx, S);
-      fe_sqr(y4, yy); fe_dbl(y4, y4); fe_dbl(y4, y4); fe_dbl(y4, y4);
-      fe_sub(ny, S, nx); fe_mul(ny, ny, M); fe_sub(ny, ny, y4);
-      fe_mul(nz, Y, Z); fe_dbl(nz, nz);
-      fe_copy(X, nx); fe_copy(Y, ny); fe_copy(Z, nz);
-      continue;
-    }
-    fe_sqr(hh, h);
-    fe_mul(hhh, hh, h);
-    fe_mul(v, X, hh);
-    fe_sqr(t, r);
-    fe_sub(t, t, hhh);
-    fe_sub(t, t, v); fe_sub(t, t, v);            // X3
-    fe_sub(v, v, t);
-    fe_mul(v, v, r);
-    fe_mul(hhh, hhh, Y);
-    fe_sub(Y, v, hhh);                           // Y3
-    fe_mul(Z, Z, h);                             // Z3
-    fe_copy(X, t);
+    // two table terms never share an x for a scalar < n; the key term does when d*G == +-key (a wild kangaroo created on
+    // the key itself), and jac_add_affine then follows the group law
+    jac_add_affine(X, Y, Z, inf, qx, qy);
   }
   if (inf) {
     // scalar 0 (tame) or d*G == -key (wild): the point at infinity has no affine form; store (0, 0) -- not on the curve,
@@ -159,30 +90,6 @@ __global__ void herd_kernel(const u32* __restrict__ tab, const u32* __restrict__
 }
 
 // ---- multi-key herd: moving the wild kangaroos of a solved key to other keys (kgx_retarget) ----------------------------
-// (x1, y1) += (x2, y2) in affine coordinates with one inverse; canonical result.  Same x: doubling when the points are
-// equal, the point at infinity (returns false, x1 / y1 then meaningless) when they are opposite -- the group law, as in
-// herd_kernel.
-__device__ bool affine_add(u32* x1, u32* y1, const u32* x2, const u32* y2) {
-  u32 num[8], den[8], s[8], t[8];
-  fe_sub(den, x2, x1);
-  fe_sub(num, y2, y1);
-  if (fe_is_zero_modp(den)) {
-    if (!fe_is_zero_modp(num)) return false;
-    // s = 3 x^2 / 2 y
-    fe_sqr(t, x1);
-    fe_dbl(num, t); fe_neg(s, t); fe_sub(num, num, s);
-    fe_dbl(den, y1);
-  }
-  modinv256(t, den);
-  fe_mul(s, num, t);
-  fe_sqr(t, s); fe_sub(t, t, x1); fe_sub(t, t, x2);     // x3 = s^2 - x1 - x2
-  fe_sub(num, x1, t); fe_mul(num, num, s); fe_sub(y1, num, y1);   // y3 = s (x1 - x3) - y1
-  fe_copy(x1, t);
-  fe_canon(x1);
-  fe_canon(y1);
-  return true;
-}
-
 // The destination list of one kgx_retarget travels as kernel parameters, copied at launch: the call returns without
 // waiting for the launch in flight and leaves no host buffer behind that the device still has to read.
 constexpr int RETARGET_CHUNK = 1024;

@@ -22,8 +22,7 @@
 #include "HashTable.h"               // reference header, found through -I$REF
 #include "SECPK1/SECP256k1.h"
 #include "../../include/kgx_ingest.h"
-
-#define HEADW_MAGIC 0xFA6A8001u      // Kangaroo.h:120
+#include "kgx_workfile.h"
 
 namespace {
 
@@ -274,19 +273,13 @@ int kgi_resolve_multi(kgi_table* t, const uint64_t d_old[2], const uint64_t d_ne
   return 0;
 }
 
-// a failed stdio call: -errno (EIO when the C library left errno at 0)
-static int io_error() { return errno ? -errno : -EIO; }
-
 int kgi_save_work_ex(kgi_table* t, const char* path, uint32_t dp_bits, const uint64_t range_start[4], const uint64_t range_end[4],
                      const uint64_t keyx[4], const uint64_t keyy[4], uint64_t total_count, double total_time, uint64_t total_walk) {
+  using namespace kgx_wf;
   errno = 0;
   FILE* f = fopen(path, "wb");
   if (!f) return io_error();
-  // Kangaroo::SaveHeader (Backup.cpp:368-394), type HEADW
-  const uint32_t head = HEADW_MAGIC, version = 0;
-  bool ok = fwrite(&head, 4, 1, f) == 1 && fwrite(&version, 4, 1, f) == 1 && fwrite(&dp_bits, 4, 1, f) == 1 &&
-            fwrite(range_start, 32, 1, f) == 1 && fwrite(range_end, 32, 1, f) == 1 && fwrite(keyx, 32, 1, f) == 1 &&
-            fwrite(keyy, 32, 1, f) == 1 && fwrite(&total_count, 8, 1, f) == 1 && fwrite(&total_time, 8, 1, f) == 1;
+  bool ok = write_header(f, make_header(dp_bits, range_start, range_end, keyx, keyy, total_count, total_time));
   if (ok) {
     t->ht->SaveTable(f, 0, HASH_SIZE, false);                     // HashTable.cpp:375-396 (ignores fwrite results: ferror below)
     ok = !ferror(f) && fwrite(&total_walk, 8, 1, f) == 1;         // Backup.cpp:530-531 / 549-551
@@ -305,35 +298,23 @@ int kgi_save_work(kgi_table* t, const char* path, uint32_t dp_bits, const uint64
 int kgi_load_work_ex(kgi_table* t, const char* path, uint32_t* dp_bits, uint64_t range_start[4], uint64_t range_end[4],
                      uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time, uint64_t* nb_walk,
                      uint64_t* walk_offset) {
+  using namespace kgx_wf;
   errno = 0;
   FILE* f = fopen(path, "rb");
   if (!f) return io_error();
-  // Kangaroo::LoadWork (Backup.cpp:149-207)
-  uint32_t head = 0, version = 0, dp = 0;
-  uint64_t hdr[16], cnt = 0, walk = 0; double tm = 0;
-  bool ok = fread(&head, 4, 1, f) == 1 && fread(&version, 4, 1, f) == 1 && head == HEADW_MAGIC;
-  ok = ok && fread(&dp, 4, 1, f) == 1 && fread(hdr, 32, 4, f) == 4 && fread(&cnt, 8, 1, f) == 1 && fread(&tm, 8, 1, f) == 1;
+  WorkHeader hd;                                                  // Kangaroo::LoadWork (Backup.cpp:149-207)
+  uint64_t walk = 0, off = 0;
+  bool ok = read_header(f, hd);
   if (ok) {
     t->ht->LoadTable(f);                                          // HashTable.cpp (Reset + per-bucket read; ignores fread results)
     ok = !ferror(f) && !feof(f) && fread(&walk, 8, 1, f) == 1;
   }
-  long off = ok ? ftell(f) : -1;
-  if (ok && walk) {                                               // the kangaroo block must be all there (FetchWalks, Backup.cpp:211-223)
-    ok = off >= 0 && fseek(f, 0, SEEK_END) == 0;
-    const long end = ok ? ftell(f) : -1;
-    ok = ok && end >= off && (uint64_t)(end - off) / 96 >= walk;
-  }
+  ok = ok && walks_complete(f, walk, off);
   fclose(f);
   if (!ok) { t->ht->Reset(); return -EINVAL; }
-  if (dp_bits) *dp_bits = dp;
-  if (range_start) memcpy(range_start, hdr, 32);
-  if (range_end) memcpy(range_end, hdr + 4, 32);
-  if (keyx) memcpy(keyx, hdr + 8, 32);
-  if (keyy) memcpy(keyy, hdr + 12, 32);
-  if (total_count) *total_count = cnt;
-  if (total_time) *total_time = tm;
+  get_header(hd, dp_bits, range_start, range_end, keyx, keyy, total_count, total_time);
   if (nb_walk) *nb_walk = walk;
-  if (walk_offset) *walk_offset = (uint64_t)off;
+  if (walk_offset) *walk_offset = off;
   return 0;
 }
 

@@ -1,10 +1,10 @@
 // kgx_testhooks.cuh -- device side of the kgx_test_field hook (include/kgx.h): one primitive per thread, applied to operands
 // copied in from the host, so that the tests can feed the branch-free field / distance / jump-rule primitives of
-// kgx_field.cuh, kgx_herd.cuh and kgx_kernel.cuh the boundary values that random walks never produce.
+// kgx_field.cuh, kgx_curve.cuh and kgx_kernel.cuh the boundary values that random walks never produce.
 #pragma once
 #include "../../include/kgx.h"   // KGX_TF_* op codes
 #include "kgx_kernel.cuh"
-#include "kgx_herd.cuh"
+#include "kgx_curve.cuh"
 
 namespace kgx {
 

@@ -15,24 +15,27 @@
 // equal keys; one scan keeps the first entry of every run of equal (h, x) -- the earliest input's, as the reference's
 // pairwise merges do -- and classifies each later one against it: equal tagged d = a duplicate ("Dead kangaroo"), else a
 // collision returned to the host.  The kept entries are compacted, counted per bucket and written with maxItem = nbItem
-// rounded up to a multiple of 4 (HashTable.cpp:204-209).
-#include <cerrno>
+// rounded up to a multiple of 4 (HashTable.cpp:204-209).  The file format is kgx_workfile.h's, the block sort
+// kgx_bucketsort.cuh's (shared with the device table's save) and the group law kgx_curve.cuh's (shared with herd creation).
 #include <vector>
 #include <algorithm>
 #include <string>
 #include <thrust/iterator/counting_iterator.h>
+#include "kgx_workfile.h"
+#include "kgx_bucketsort.cuh"
+#include "kgx_curve.cuh"
 
 namespace kgx_wt {
 
 using ::u32;
 using ::u64;
+using kgx_wf::Entry;
+using kgx_wf::NBUCKET;
 typedef unsigned long long ull;
 constexpr int COMB_W = 32, COMB_J = 15, COMB_WORDS = COMB_W * COMB_J * 16;   // 480 affine points, 16 words each
 constexpr int CHECK_THREADS = 128, GROUP = 8;                                 // entries per thread share one inverse
-constexpr uint32_t NBUCKET = 1u << 18, HEADW = 0xFA6A8001u;
 constexpr uint64_t DEFAULT_CHUNK = 1ull << 21, DEFAULT_BLOCK = 1ull << 22;
 
-struct Entry { uint64_t x0, x1, d0, d1; };
 struct Coll { uint32_t h, seq; uint64_t d_first[2], d_other[2]; };
 struct MergeRes { ull dup, ncoll; };
 
@@ -40,8 +43,8 @@ struct MergeRes { ull dup, ncoll; };
 __global__ void wt_comb_kernel(u32* tab) {
   const int w = threadIdx.x;
   if (w >= COMB_W) return;
-  u32 bx[8] = {0x16F81798u, 0x59F2815Bu, 0x2DCE28D9u, 0x029BFCDBu, 0xCE870B07u, 0x55A06295u, 0xF9DCBBACu, 0x79BE667Eu};
-  u32 by[8] = {0xFB10D4B8u, 0x9C47D08Fu, 0xA6855419u, 0xFD17B448u, 0x0E1108A8u, 0x5DA4FBFCu, 0x26A3C465u, 0x483ADA77u};
+  u32 bx[8], by[8];
+  kgx::set_g(bx, by);
   for (int i = 0; i < 4 * w; i++) {                 // 2^(4w) * G
     u32 cx[8], cy[8];
     fe_copy(cx, bx); fe_copy(cy, by);
@@ -56,44 +59,6 @@ __global__ void wt_comb_kernel(u32* tab) {
   }
 }
 
-// (X, Y, Z) += (qx, qy) in Jacobian + affine coordinates, infinity as a flag.  Same x: a doubling when the points are equal,
-// the point at infinity when they are opposite (the group law, as herd_kernel).
-__device__ __forceinline__ void wt_madd(u32* X, u32* Y, u32* Z, bool& inf, const u32* qx, const u32* qy) {
-  using namespace kgx;
-  if (inf) { fe_copy(X, qx); fe_copy(Y, qy); fe_set_one(Z); inf = false; return; }
-  u32 zz[8], u2[8], s2[8], h[8], r[8], hh[8], hhh[8], v[8], t[8];
-  fe_sqr(zz, Z);
-  fe_mul(u2, qx, zz);
-  fe_mul(s2, qy, zz); fe_mul(s2, s2, Z);
-  fe_sub(h, u2, X);
-  fe_sub(r, s2, Y);
-  if (fe_is_zero_modp(h)) {
-    if (!fe_is_zero_modp(r)) { inf = true; return; }
-    u32 yy[8], S[8], M[8], m2[8], y4[8], nx[8], ny[8], nz[8];
-    fe_sqr(yy, Y);
-    fe_mul(S, X, yy); fe_dbl(S, S); fe_dbl(S, S);
-    fe_sqr(m2, X); fe_dbl(M, m2); { u32 ng[8]; fe_neg(ng, m2); fe_sub(M, M, ng); }
-    fe_sqr(nx, M); fe_sub(nx, nx, S); fe_sub(nx, nx, S);
-    fe_sqr(y4, yy); fe_dbl(y4, y4); fe_dbl(y4, y4); fe_dbl(y4, y4);
-    fe_sub(ny, S, nx); fe_mul(ny, ny, M); fe_sub(ny, ny, y4);
-    fe_mul(nz, Y, Z); fe_dbl(nz, nz);
-    fe_copy(X, nx); fe_copy(Y, ny); fe_copy(Z, nz);
-    return;
-  }
-  fe_sqr(hh, h);
-  fe_mul(hhh, hh, h);
-  fe_mul(v, X, hh);
-  fe_sqr(t, r);
-  fe_sub(t, t, hhh);
-  fe_sub(t, t, v); fe_sub(t, t, v);
-  fe_sub(v, v, t);
-  fe_mul(v, v, r);
-  fe_mul(hhh, hhh, Y);
-  fe_sub(Y, v, hhh);
-  fe_mul(Z, Z, h);
-  fe_copy(X, t);
-}
-
 // m * G for a 128-bit m (4 words) from the comb in shared memory, lowest window first
 __device__ __forceinline__ void wt_comb_mul(const u32* sc, const u32* m, u32* X, u32* Y, u32* Z, bool& inf) {
   inf = true;
@@ -102,7 +67,7 @@ __device__ __forceinline__ void wt_comb_mul(const u32* sc, const u32* m, u32* X,
     const u32 nib = (m[w >> 3] >> (4 * (w & 7))) & 15u;
     if (nib) {
       const u32* q = sc + (w * COMB_J + nib - 1) * 16;
-      wt_madd(X, Y, Z, inf, q, q + 8);
+      kgx::jac_add_affine(X, Y, Z, inf, q, q + 8);
     }
   }
 }
@@ -138,7 +103,7 @@ __global__ void __launch_bounds__(CHECK_THREADS) wt_check_entries_kernel(const u
       bool f;
       wt_comb_mul(sc, m, X[g], Y, Z[g], f);
       if (neg && !f) { u32 t[8]; fe_neg(t, Y); fe_copy(Y, t); }
-      if (wild && !kinf) wt_madd(X[g], Y, Z[g], f, K, K + 8);
+      if (wild && !kinf) jac_add_affine(X[g], Y, Z[g], f, K, K + 8);
       inf[g] = f;
       if (!f) fe_mul(run, run, Z[g]);
     }
@@ -187,29 +152,28 @@ __global__ void __launch_bounds__(CHECK_THREADS) wt_check_walks_kernel(const u32
   using namespace kgx;
   __shared__ u32 sc[COMB_WORDS];
   wt_load_comb(sc, comb);
-  const u32 N[8] = {0xD0364141u, 0xBFD25E8Cu, 0xAF48A03Bu, 0xBAAEDCE6u, 0xFFFFFFFEu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     const u32* r = recs + i * 24;
-    u32 x[8], y[8], d[8];
-    for (int k = 0; k < 8; k++) { x[k] = r[k]; y[k] = r[8 + k]; d[k] = r[16 + k]; }
+    u32 x[8], y[8];
+    for (int k = 0; k < 8; k++) { x[k] = r[k]; y[k] = r[8 + k]; }
+    const u64* r64 = reinterpret_cast<const u64*>(r);
+    u64 d[4] = {r64[8], r64[9], r64[10], r64[11]};
     int kind = 0;
-    bool lt = false;                                    // d < n ?
-    for (int k = 7; k >= 0; k--) if (d[k] != N[k]) { lt = d[k] < N[k]; break; }
-    if (lt) {
-      u32 nd[8];                                        // n - d
-      u64 br = 0;
-      for (int k = 0; k < 8; k++) { const u64 s = (u64)N[k] - d[k] - br; nd[k] = (u32)s; br = (s >> 32) & 1; }
-      bool dle = true;                                  // d <= n - d ?
-      for (int k = 7; k >= 0; k--) if (d[k] != nd[k]) { dle = d[k] < nd[k]; break; }
-      const u32* m = dle ? d : nd;
-      if ((m[4] | m[5] | m[6] | m[7]) == 0) {
+    if (!ge_order(d)) {
+      u64 nd[4];                                        // n - d
+      const u64 nn[4] = {kOrder[0], kOrder[1], kOrder[2], kOrder[3]};
+      sub256(nd, nn, d);
+      const bool dle = ge256(nd, d);                    // d <= n - d ?
+      const u64* m = dle ? d : nd;
+      if ((m[2] | m[3]) == 0) {
+        const u32 mw[4] = {(u32)m[0], (u32)(m[0] >> 32), (u32)m[1], (u32)(m[1] >> 32)};
         u32 X[8], Y[8], Z[8];
         bool f;
-        wt_comb_mul(sc, m, X, Y, Z, f);
+        wt_comb_mul(sc, mw, X, Y, Z, f);
         if (!dle && !f) { u32 t[8]; fe_neg(t, Y); fe_copy(Y, t); }
         if (!f && wt_proj_eq(X, Y, Z, x, y)) kind = 1;
         else {
-          if (!kinf) wt_madd(X, Y, Z, f, K, K + 8);
+          if (!kinf) jac_add_affine(X, Y, Z, f, K, K + 8);
           if (!f && wt_proj_eq(X, Y, Z, x, y)) kind = 2;
         }
       }
@@ -238,20 +202,6 @@ __global__ void wt_on_curve_kernel(const u32* key, int* ok) {
 }
 
 // ---- merge ----
-__global__ void wt_merge_key(const Entry* ent, const uint32_t* hs, const uint32_t* idx, uint32_t n, int which, uint32_t b0, uint64_t* key) {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= n) return;
-  const uint32_t e = idx ? idx[t] : t;
-  if (which == 0) key[t] = ent[e].x0;
-  else if (which == 1) key[t] = ent[e].x1;
-  else reinterpret_cast<uint32_t*>(key)[t] = hs[e] - b0;
-}
-
-__global__ void wt_iota(uint32_t* v, uint32_t n) {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t < n) v[t] = t;
-}
-
 // ord: the block's entries in (h, x) order, input order among equals.  keep[i] = first of its run; later entries are
 // duplicates or collisions against that first one.  nb[h - b0] counts the kept entries of each bucket.
 __global__ void wt_merge_scan(const Entry* ent, const uint32_t* hs, const uint32_t* ord, uint32_t n, uint32_t b0, uint8_t* keep,
@@ -275,11 +225,6 @@ __global__ void wt_merge_scan(const Entry* ent, const uint32_t* hs, const uint32
   coll[c] = Coll{h, i, {w.d0, w.d1}, {v.d0, v.d1}};
 }
 
-__global__ void wt_gather(const Entry* ent, const uint32_t* idx, uint32_t n, Entry* out) {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t < n) out[t] = ent[idx[t]];
-}
-
 }  // namespace kgx_wt
 
 static char g_wt_err[512] = "";
@@ -295,19 +240,6 @@ static char g_wt_err[512] = "";
   } while (0)
 
 namespace kgx_wt {
-
-struct Header {
-  uint32_t head = 0, version = 0, dp = 0;
-  uint64_t rs[4], re[4], kx[4], ky[4];
-  uint64_t count = 0;
-  double time = 0;
-};
-
-static bool read_header(FILE* f, Header& h) {
-  return fread(&h.head, 4, 1, f) == 1 && h.head == HEADW && fread(&h.version, 4, 1, f) == 1 && fread(&h.dp, 4, 1, f) == 1 &&
-         fread(h.rs, 32, 1, f) == 1 && fread(h.re, 32, 1, f) == 1 && fread(h.kx, 32, 1, f) == 1 && fread(h.ky, 32, 1, f) == 1 &&
-         fread(&h.count, 8, 1, f) == 1 && fread(&h.time, 8, 1, f) == 1;
-}
 
 // device scratch that lives for one call: freed on every return path
 struct DevBufs {
@@ -358,16 +290,11 @@ static int key_setup(DevBufs& B, const uint64_t kx[4], const uint64_t ky[4], con
   WT_CK(cudaStreamSynchronize(st));
   if (!K || !*ok) return 0;
   // s = (n - start mod n) mod n
-  static const uint64_t N[4] = {0xBFD25E8CD0364141ull, 0xBAAEDCE6AF48A03Bull, 0xFFFFFFFFFFFFFFFEull, 0xFFFFFFFFFFFFFFFFull};
-  uint64_t a[4], s[4];
+  using kgx::kOrderHost;
+  u64 a[4], s[4] = {0, 0, 0, 0};
   memcpy(a, rs, 32);
-  auto ge = [](const uint64_t* x, const uint64_t* y) { for (int k = 3; k >= 0; k--) if (x[k] != y[k]) return x[k] > y[k]; return true; };
-  auto sub = [](uint64_t* r, const uint64_t* x, const uint64_t* y) {
-    unsigned __int128 br = 0;
-    for (int k = 0; k < 4; k++) { const unsigned __int128 t = (unsigned __int128)x[k] - y[k] - br; r[k] = (uint64_t)t; br = (t >> 64) & 1; }
-  };
-  if (ge(a, N)) sub(a, a, N);
-  if ((a[0] | a[1] | a[2] | a[3]) == 0) memset(s, 0, 32); else sub(s, N, a);
+  if (kgx::ge256(a, kOrderHost)) kgx::sub256(a, a, kOrderHost);
+  if (a[0] | a[1] | a[2] | a[3]) kgx::sub256(s, kOrderHost, a);
   if (B.dev(&tab, 256 * 16 * 4) || B.dev(&scal, 32) || B.dev(K, 64) || B.dev(&ky_, 64)) return -3;
   WT_CK(cudaMemcpyAsync(scal, s, 32, cudaMemcpyHostToDevice, st));
   kgx::herd_table_kernel<<<1, 32, 0, st>>>(tab);
@@ -447,11 +374,11 @@ int kgx_work_check(int dev, const char* path, uint64_t chunk, kgx_work_check_inf
   if (chunk >= 0x40000000ull) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_work_check: chunk of %llu entries (at most 2^30-1)", (unsigned long long)chunk); return -1; }
   errno = 0;
   FILE* f = fopen(path, "rb");
-  if (!f) { const int e = errno ? errno : EIO; snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", path, strerror(e)); return -e; }
+  if (!f) { const int e = kgx_wf::io_error(); snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", path, strerror(-e)); return e; }
   struct Closer { FILE* f; ~Closer() { fclose(f); } } closer{f};
   setvbuf(f, nullptr, _IOFBF, 1 << 22);
-  Header hd;
-  if (!read_header(f, hd)) { snprintf(g_wt_err, sizeof g_wt_err, "%s is not a HEADW work file", path); return -1; }
+  kgx_wf::WorkHeader hd;
+  if (!kgx_wf::read_header(f, hd)) { snprintf(g_wt_err, sizeof g_wt_err, "%s is not a HEADW work file", path); return -1; }
   info->dp_bits = hd.dp;
   DevBufs B;
   cudaStream_t st;
@@ -534,7 +461,7 @@ int kgx_work_check(int dev, const char* path, uint64_t chunk, kgx_work_check_inf
   bool okr = true;
   for (uint32_t h = 0; okr && h < NBUCKET; h++) {      // HashTable::LoadTable order; buckets may span chunks
     uint32_t nb = 0, mx = 0;
-    okr = fread(&nb, 4, 1, f) == 1 && fread(&mx, 4, 1, f) == 1;
+    okr = kgx_wf::read_bucket_head(f, nb, mx);
     uint32_t done_in_bucket = 0;
     while (okr && done_in_bucket < nb) {
       if (fill == 0 && drain(cur)) return -3;           // the buffer is free once its previous chunk was counted
@@ -584,15 +511,15 @@ int kgx_work_merge(int dev, const char* const* paths, uint32_t n_paths, const ch
   if (set_device(dev)) return -3;
   std::vector<FILE*> fs(n_paths, nullptr);
   struct Closer { std::vector<FILE*>& v; ~Closer() { for (FILE* f : v) if (f) fclose(f); } } closer{fs};
-  std::vector<Header> hd(n_paths);
+  std::vector<kgx_wf::WorkHeader> hd(n_paths);
   DevBufs B;
   // Merge.cpp:56-143: every input is checked before anything is written
   for (uint32_t i = 0; i < n_paths; i++) {
     errno = 0;
     fs[i] = fopen(paths[i], "rb");
-    if (!fs[i]) { const int e = errno ? errno : EIO; snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", paths[i], strerror(e)); return -e; }
+    if (!fs[i]) { const int e = kgx_wf::io_error(); snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", paths[i], strerror(-e)); return e; }
     setvbuf(fs[i], nullptr, _IOFBF, 1 << 22);
-    if (!read_header(fs[i], hd[i])) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s is not a HEADW work file", paths[i]); return -1; }
+    if (!kgx_wf::read_header(fs[i], hd[i])) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s is not a HEADW work file", paths[i]); return -1; }
     if (hd[i].version != hd[0].version) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: cannot merge workfile of different version (%s)", paths[i]); return -1; }
     int ok = 0;
     if (key_setup(B, hd[i].kx, hd[i].ky, hd[i].rs, 0, &ok, nullptr, nullptr)) return -3;
@@ -613,11 +540,9 @@ int kgx_work_merge(int dev, const char* const* paths, uint32_t n_paths, const ch
   uint8_t* keep;
   MergeRes* dRes;
   Coll* dColl;
-  size_t tA = 0, tB = 0, tC = 0;
-  WT_CK(cub::DeviceRadixSort::SortPairs(nullptr, tA, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)C, 0, 64));
-  WT_CK(cub::DeviceRadixSort::SortPairs(nullptr, tB, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)C, 0, 19));
+  size_t tC = 0;
   WT_CK(cub::DeviceSelect::Flagged(nullptr, tC, (uint32_t*)nullptr, (uint8_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)C));
-  const size_t tmpBytes = std::max(tA, std::max(tB, tC));
+  const size_t tmpBytes = std::max(kgx_wf::bucket_sort_scratch(C), tC);
   void* dTmp;
   if (B.host(&hIn, 32 * C) || B.dev(&dIn, 32 * C) || B.dev(&dOut, 32 * C) || B.host(&hOut, 32 * C) || B.host(&hH, 4 * C) ||
       B.dev(&dH, 4 * C) || B.dev(&idxA, 4 * C) || B.dev(&idxB, 4 * C) || B.dev(&dNsel, 4) || B.dev(&dNb, 4ull * NBUCKET) ||
@@ -627,16 +552,13 @@ int kgx_work_merge(int dev, const char* const* paths, uint32_t n_paths, const ch
   std::vector<Coll> hColl;
   errno = 0;
   FILE* out = fopen(tmp_path, "wb");
-  if (!out) { const int e = errno ? errno : EIO; snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: Cannot open %s for writing: %s", tmp_path, strerror(e)); return -e; }
+  if (!out) { const int e = kgx_wf::io_error(); snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: Cannot open %s for writing: %s", tmp_path, strerror(-e)); return e; }
   setvbuf(out, nullptr, _IOFBF, 1 << 22);
-  uint32_t dp = hd[0].dp;
-  uint64_t cnt = 0;
-  double tm = 0;
-  for (uint32_t i = 0; i < n_paths; i++) { dp = std::min(dp, hd[i].dp); cnt += hd[i].count; tm += hd[i].time; }
-  const uint32_t version = 0;                         // Kangaroo::SaveHeader, Backup.cpp:368-394
-  bool okw = fwrite(&HEADW, 4, 1, out) == 1 && fwrite(&version, 4, 1, out) == 1 && fwrite(&dp, 4, 1, out) == 1 &&
-             fwrite(hd[0].rs, 32, 1, out) == 1 && fwrite(hd[0].re, 32, 1, out) == 1 && fwrite(hd[0].kx, 32, 1, out) == 1 &&
-             fwrite(hd[0].ky, 32, 1, out) == 1 && fwrite(&cnt, 8, 1, out) == 1 && fwrite(&tm, 8, 1, out) == 1;
+  kgx_wf::WorkHeader oh = hd[0];                      // the first input's range and key, written as version 0
+  oh.count = 0;
+  oh.time = 0;
+  for (uint32_t i = 0; i < n_paths; i++) { oh.dp = std::min(oh.dp, hd[i].dp); oh.count += hd[i].count; oh.time += hd[i].time; }
+  bool okw = kgx_wf::write_header(out, oh);
   int rc = 0;
   uint64_t fill = 0;
   uint32_t b0 = 0;
@@ -645,27 +567,20 @@ int kgx_work_merge(int dev, const char* const* paths, uint32_t n_paths, const ch
     const uint32_t n = (uint32_t)fill, T = 256, G = (n + T - 1) / T;
     WT_CK(cudaMemsetAsync(dNb, 0, 4ull * (b1 - b0)));
     if (n) {
-      int bits = 1;
-      while ((1u << bits) < b1 - b0) bits++;
-      size_t tb;
       WT_CK(cudaMemcpyAsync(dIn, hIn, 32ull * n, cudaMemcpyHostToDevice));
       WT_CK(cudaMemcpyAsync(dH, hH, 4ull * n, cudaMemcpyHostToDevice));
       WT_CK(cudaMemsetAsync(dRes, 0, sizeof(MergeRes)));
-      wt_iota<<<G, T>>>(idxA, n);
-      wt_merge_key<<<G, T>>>(dIn, dH, nullptr, n, 0, b0, keyA);
-      tb = tmpBytes; WT_CK(cub::DeviceRadixSort::SortPairs(dTmp, tb, keyA, keyB, idxA, idxB, (int)n, 0, 64));
-      wt_merge_key<<<G, T>>>(dIn, dH, idxB, n, 1, b0, keyA);
-      tb = tmpBytes; WT_CK(cub::DeviceRadixSort::SortPairs(dTmp, tb, keyA, keyB, idxB, idxA, (int)n, 0, 64));
-      wt_merge_key<<<G, T>>>(dIn, dH, idxA, n, 2, b0, keyA);
-      tb = tmpBytes; WT_CK(cub::DeviceRadixSort::SortPairs(dTmp, tb, (uint32_t*)keyA, (uint32_t*)keyB, idxA, idxB, (int)n, 0, bits));
-      wt_merge_scan<<<G, T>>>(dIn, dH, idxB, n, b0, keep, dNb, dRes, dColl);
-      tb = tmpBytes; WT_CK(cub::DeviceSelect::Flagged(dTmp, tb, idxB, keep, idxA, dNsel, (int)n));
+      uint32_t* ord;                                    // the legacy default stream, as every other call of the merge
+      WT_CK(kgx_wf::bucket_sort(dIn, dH, nullptr, n, b0, b1, idxA, idxB, keyA, keyB, dTmp, tmpBytes, 0, &ord));
+      wt_merge_scan<<<G, T>>>(dIn, dH, ord, n, b0, keep, dNb, dRes, dColl);
+      size_t tb = tmpBytes;
+      WT_CK(cub::DeviceSelect::Flagged(dTmp, tb, ord, keep, idxA, dNsel, (int)n));
       WT_CK(cudaGetLastError());
       MergeRes r;
       uint32_t nk = 0;
       WT_CK(cudaMemcpy(&r, dRes, sizeof r, cudaMemcpyDeviceToHost));
       WT_CK(cudaMemcpy(&nk, dNsel, 4, cudaMemcpyDeviceToHost));
-      wt_gather<<<(nk + T - 1) / T, T>>>(dIn, idxA, nk, dOut);
+      kgx_wf::bucket_gather<<<(nk + T - 1) / T, T>>>(dIn, idxA, nk, dOut);
       WT_CK(cudaGetLastError());
       WT_CK(cudaMemcpy(hOut, dOut, 32ull * nk, cudaMemcpyDeviceToHost));
       WT_CK(cudaMemcpy(hNb, dNb, 4ull * (b1 - b0), cudaMemcpyDeviceToHost));
@@ -683,8 +598,8 @@ int kgx_work_merge(int dev, const char* const* paths, uint32_t n_paths, const ch
     }
     uint64_t off = 0;
     for (uint32_t b = b0; okw && b < b1; b++) {
-      const uint32_t nb = hNb[b - b0], md = (nb + 3) & ~3u;
-      okw = fwrite(&nb, 4, 1, out) == 1 && fwrite(&md, 4, 1, out) == 1 && (nb == 0 || fwrite(hOut + off, 32, nb, out) == nb);
+      const uint32_t nb = hNb[b - b0];
+      okw = kgx_wf::write_bucket(out, nb, (nb + 3) & ~3u, hOut + off);
       off += nb;
       info->entries += nb;
     }
@@ -698,7 +613,7 @@ int kgx_work_merge(int dev, const char* const* paths, uint32_t n_paths, const ch
     uint64_t sum = 0;
     for (uint32_t i = 0; i < n_paths; i++) {
       uint32_t mx;
-      if (fread(&nbs[i], 4, 1, fs[i]) != 1 || fread(&mx, 4, 1, fs[i]) != 1) {
+      if (!kgx_wf::read_bucket_head(fs[i], nbs[i], mx)) {
         snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: the table of %s is cut short", paths[i]);
         rc = -1;
         break;
@@ -726,13 +641,13 @@ int kgx_work_merge(int dev, const char* const* paths, uint32_t n_paths, const ch
   const uint64_t zero = 0;                              // the kangaroo count: 0, so that loaders of -ws files take the result
   okw = okw && fwrite(&zero, 8, 1, out) == 1;
   okw = fflush(out) == 0 && okw;
-  const int ioerr = errno ? errno : EIO;
+  const int ioerr = kgx_wf::io_error();
   okw = (fclose(out) == 0) && okw;
-  if (rc == 0 && !okw) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s: %s", tmp_path, strerror(ioerr)); rc = -ioerr; }
+  if (rc == 0 && !okw) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s: %s", tmp_path, strerror(-ioerr)); rc = ioerr; }
   if (rc) { remove(tmp_path); return rc; }
-  info->dp_bits = dp;
-  info->total_count = cnt;
-  info->total_time = tm;
+  info->dp_bits = oh.dp;
+  info->total_count = oh.count;
+  info->total_time = oh.time;
   info->n_listed = (uint32_t)hColl.size();
   for (size_t k = 0; k < hColl.size(); k++) {
     coll[k].h = hColl[k].h;

@@ -4,8 +4,10 @@ The table is the reference's own `class HashTable` (HashTable.{h,cpp}, compiled 
 kangaroo_b200/csrc/build_ingest.sh); the library adds the batched, bucket-sharded multi-threaded insert that replaces the
 single-mutex loop of Kangaroo::SolveKeyGPU (Kangaroo.cpp:594-612) when the DP records of all GPUs arrive on rank 0.
 No Python-side fallback: without the library DPTable() raises."""
+import collections
 import ctypes
 import os
+import struct
 
 import numpy as np
 
@@ -68,6 +70,23 @@ def load_library():
 
 def _limbs4(v):
     return (ctypes.c_uint64 * 4)(*[(int(v) >> (64 * k)) & _M64 for k in range(4)])
+
+
+def _save_args(dp_bits, range_start, range_end, pubkey, total_count, total_time, total_walk):
+    """the header arguments of kgi_save_work_ex / kgx_dptable_save_work"""
+    return (int(dp_bits), _limbs4(range_start), _limbs4(range_end), _limbs4(pubkey[0]), _limbs4(pubkey[1]), int(total_count),
+            float(total_time), int(total_walk))
+
+
+def _load_work_ex(fn, handle, path, *extra):
+    """kgi_load_work_ex / kgx_dptable_load_work (extra: their trailing arguments) -> (return code, WorkInfo)"""
+    dp, cnt, tm = ctypes.c_uint32(0), ctypes.c_uint64(0), ctypes.c_double(0)
+    rs, re_, kx, ky = (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)()
+    walk, off = ctypes.c_uint64(0), ctypes.c_uint64(0)
+    rc = fn(handle, os.fsencode(path), ctypes.byref(dp), rs, re_, kx, ky, ctypes.byref(cnt), ctypes.byref(tm), ctypes.byref(walk),
+            ctypes.byref(off), *extra)
+    val = lambda a: sum(int(a[k]) << (64 * k) for k in range(4))
+    return rc, WorkInfo(path, dp.value, val(rs), val(re_), (val(kx), val(ky)), cnt.value, tm.value, walk.value, off.value)
 
 
 class DPTable:
@@ -159,8 +178,8 @@ class DPTable:
 
     def save_work(self, path, dp_bits, range_start, range_end, pubkey, total_count=0, total_time=0.0, total_walk=0):
         """Header + table (+ the kangaroo count: the caller appends total_walk x 96-byte records right after)."""
-        rc = self._lib.kgi_save_work_ex(self._h, os.fsencode(path), int(dp_bits), _limbs4(range_start), _limbs4(range_end),
-                                        _limbs4(pubkey[0]), _limbs4(pubkey[1]), int(total_count), float(total_time), int(total_walk))
+        rc = self._lib.kgi_save_work_ex(self._h, os.fsencode(path),
+                                        *_save_args(dp_bits, range_start, range_end, pubkey, total_count, total_time, total_walk))
         if rc != 0:
             raise RuntimeError("kgi_save_work: cannot write %s: %s" % (path, os.strerror(-rc)))
 
@@ -174,15 +193,10 @@ class DPTable:
     def load_work_ex(self, path):
         """Kangaroo::LoadWork (Backup.cpp:149-207): the table into this DPTable -> WorkInfo (header, nbLoadedWalk and the
         offset of the kangaroo block)."""
-        dp, cnt, tm = ctypes.c_uint32(0), ctypes.c_uint64(0), ctypes.c_double(0)
-        rs, re_, kx, ky = (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)()
-        walk, off = ctypes.c_uint64(0), ctypes.c_uint64(0)
-        rc = self._lib.kgi_load_work_ex(self._h, os.fsencode(path), ctypes.byref(dp), rs, re_, kx, ky, ctypes.byref(cnt),
-                                        ctypes.byref(tm), ctypes.byref(walk), ctypes.byref(off))
+        rc, info = _load_work_ex(self._lib.kgi_load_work_ex, self._h, path)
         if rc != 0:
             raise RuntimeError("kgi_load_work: %s is not a complete HEADW work file" % path)
-        val = lambda a: sum(int(a[k]) << (64 * k) for k in range(4))
-        return WorkInfo(path, dp.value, val(rs), val(re_), (val(kx), val(ky)), cnt.value, tm.value, walk.value, off.value)
+        return info
 
 
 class TableFull(RuntimeError):
@@ -271,25 +285,20 @@ class DeviceDPTable:
         return self.add(buf.data_ptr() - rank * n * DP40_BYTES, counts, n, stream) if n else []
 
     def save_work(self, path, dp_bits, range_start, range_end, pubkey, total_count=0, total_time=0.0, total_walk=0, stream=0):
-        rc = self._lib.kgx_dptable_save_work(self._h, os.fsencode(path), int(dp_bits), _limbs4(range_start), _limbs4(range_end),
-                                             _limbs4(pubkey[0]), _limbs4(pubkey[1]), int(total_count), float(total_time), int(total_walk),
+        rc = self._lib.kgx_dptable_save_work(self._h, os.fsencode(path),
+                                             *_save_args(dp_bits, range_start, range_end, pubkey, total_count, total_time, total_walk),
                                              ctypes.c_void_p(int(stream)))
         if rc != 0:
             raise RuntimeError("kgx_dptable_save_work: cannot write %s: %s" % (path, self._err()))
 
     def load_work_ex(self, path, stream=0):
         """DPTable.load_work_ex into the device table; a file of more entries than the capacity raises TableFull"""
-        dp, cnt, tm = ctypes.c_uint32(0), ctypes.c_uint64(0), ctypes.c_double(0)
-        rs, re_, kx, ky = (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)(), (ctypes.c_uint64 * 4)()
-        walk, off = ctypes.c_uint64(0), ctypes.c_uint64(0)
-        rc = self._lib.kgx_dptable_load_work(self._h, os.fsencode(path), ctypes.byref(dp), rs, re_, kx, ky, ctypes.byref(cnt),
-                                             ctypes.byref(tm), ctypes.byref(walk), ctypes.byref(off), ctypes.c_void_p(int(stream)))
+        rc, info = _load_work_ex(self._lib.kgx_dptable_load_work, self._h, path, ctypes.c_void_p(int(stream)))
         if rc == -28:                                            # -ENOSPC
             raise TableFull(self._err())
         if rc != 0:
             raise RuntimeError("kgx_dptable_load_work: %s" % self._err())
-        val = lambda a: sum(int(a[k]) << (64 * k) for k in range(4))
-        return WorkInfo(path, dp.value, val(rs), val(re_), (val(kx), val(ky)), cnt.value, tm.value, walk.value, off.value)
+        return info
 
     def _host(self):
         if self._resolver is None:
@@ -303,17 +312,26 @@ class DeviceDPTable:
         return self._host().resolve_multi(d_old, d_new, keys, range_start)
 
 
+class WorkHeader(collections.namedtuple("WorkHeader", "dp_bits range_start range_end key total_count total_time")):
+    """The header's six fields as a tuple, and the file's version as the attribute `version` (outside the tuple, so the header
+    still unpacks and compares as those six fields)"""
+
+    def __new__(cls, dp_bits, range_start, range_end, key, total_count, total_time, version=0):
+        self = super().__new__(cls, dp_bits, range_start, range_end, key, total_count, total_time)
+        self.version = version
+        return self
+
+
 def read_work_header(path):
-    """The fixed 156-byte HEADW header (Backup.cpp:368-394) without the table -> (dp_bits, range_start, range_end,
-    (key x, key y), total_count, total_time).  Needs no library."""
-    import struct
+    """The fixed 156-byte HEADW header (Backup.cpp:368-394) without the table -> WorkHeader (dp_bits, range_start, range_end,
+    (key x, key y), total_count, total_time; .version).  Needs no library."""
     with open(path, "rb") as f:
         raw = f.read(156)
     if len(raw) != 156 or struct.unpack_from("<I", raw)[0] != 0xFA6A8001:
         raise RuntimeError("%s is not a HEADW work file" % path)
     val = lambda o: int.from_bytes(raw[o:o + 32], "little")
-    return (struct.unpack_from("<I", raw, 8)[0], val(12), val(44), (val(76), val(108)),
-            struct.unpack_from("<Q", raw, 140)[0], struct.unpack_from("<d", raw, 148)[0])
+    return WorkHeader(struct.unpack_from("<I", raw, 8)[0], val(12), val(44), (val(76), val(108)), struct.unpack_from("<Q", raw, 140)[0],
+                      struct.unpack_from("<d", raw, 148)[0], struct.unpack_from("<I", raw, 4)[0])
 
 
 class WorkInfo:

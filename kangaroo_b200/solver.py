@@ -869,8 +869,8 @@ def _resume_header(path):
     hdr = None
     if int(os.environ.get("RANK", "0")) == 0:
         from .ingest import read_work_header
-        dp, start, end, pub, _, _ = read_work_header(path)
-        hdr = (dp, start, end, pub)
+        h = read_work_header(path)
+        hdr = (h.dp_bits, h.range_start, h.range_end, h.key)
     if world > 1:
         import torch
         import torch.distributed as dist

@@ -19,10 +19,10 @@ import sys
 
 from . import ecmath as ec
 from ._lib import load_library
+from .ingest import _limbs4, read_work_header
 
 HEADW = 0xFA6A8001
 TYPE_BIT = 1 << 126                    # b126 of a tagged distance: the herd (HashTable::CalcDistAndType)
-_M64 = (1 << 64) - 1
 
 
 class CheckInfo(ctypes.Structure):
@@ -48,10 +48,6 @@ class Collision(ctypes.Structure):
 
 def _err(lib):
     return lib.kgx_work_last_error().decode()
-
-
-def _limbs4(v):
-    return (ctypes.c_uint64 * 4)(*[(int(v) >> (64 * k)) & _M64 for k in range(4)])
 
 
 def is_work_file(path):
@@ -159,26 +155,19 @@ def validate(paths):
             raise ValueError("%s is a directory: partitioned work files are not supported" % p)
         if not is_work_file(p):
             raise ValueError("MergeWork: %s is not a HEADW work file" % p)
-        with open(p, "rb") as f:
-            version = struct.unpack("<I", f.read(8)[4:])[0]
-        dp, start, end, key, _, _ = read_header(p)
-        x, y = key
+        h = read_work_header(p)
+        x, y = h.key
         if not (x < ec.P and y < ec.P and (y * y - x * x * x - 7) % ec.P == 0):
             raise ValueError("MergeWork: key of %s does not lie on elliptic curve" % p)
         if first is None:
-            first = (version, start, end, key)
+            first = h
             continue
-        if version != first[0]:
+        if h.version != first.version:
             raise ValueError("MergeWork: cannot merge workfile of different version (%s)" % p)
-        if (start, end) != first[1:3]:
+        if (h.range_start, h.range_end) != (first.range_start, first.range_end):
             raise ValueError("MergeWork: File range differs (%s, %s)" % (paths[0], p))
-        if key != first[3]:
+        if h.key != first.key:
             raise ValueError("MergeWork: key differs, multiple keys not yet supported (%s, %s)" % (paths[0], p))
-
-
-def read_header(path):
-    from .ingest import read_work_header
-    return read_work_header(path)
 
 
 def merge(paths, dest, device=0, block_entries=0, out=print):
@@ -188,8 +177,9 @@ def merge(paths, dest, device=0, block_entries=0, out=print):
     tmp = dest + ".tmp"
     res = merge_files(paths, tmp, device=device, block_entries=block_entries)
     for p in paths:
-        out("File %s: [DP%d]" % (p, read_header(p)[0]))
-    dp, start, end, pub, _, _ = read_header(tmp)
+        out("File %s: [DP%d]" % (p, read_work_header(p).dp_bits))
+    h = read_work_header(tmp)
+    start, pub = h.range_start, h.key
     key = ec.add(pub, ec.neg(ec.mul(start))) if start else pub          # Kangaroo::InitSearchKey
     unresolved, priv = 0, None
     cross = [c for c in res.collision_list if (c[1][1] ^ c[2][1]) & (TYPE_BIT >> 64)]

@@ -13,6 +13,8 @@ import sys
 import numpy as np
 import pytest
 
+from tests.worktool_util import Work
+
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden")
@@ -125,15 +127,8 @@ def digest(path):
 
 def table_entries(path):
     """(h, x0, x1, d0, d1) of every entry of a work file's table (a small file: parsed in Python)"""
-    raw = open(path, "rb").read()
-    o, out = 156, []
-    for h in range(NB):
-        nb = int.from_bytes(raw[o:o + 4], "little")
-        o += 8
-        e = np.frombuffer(raw, dtype=np.uint64, count=4 * nb, offset=o).reshape(nb, 4)
-        out += [(h,) + tuple(int(v) for v in row) for row in e]
-        o += 32 * nb
-    return out
+    m64 = (1 << 64) - 1
+    return [(h, x & m64, x >> 64, d & m64, d >> 64) for h, bucket in enumerate(Work.read(path).table) for x, d in bucket]
 
 
 def as_recs(entries, rng, kidx0=0):
@@ -182,11 +177,8 @@ def test_batches_match_the_host_table_and_the_saves_are_identical(tmp_path):
     h, d = p.saves(tmp_path)
     assert open(h, "rb").read() == open(d, "rb").read()
     # the saved buckets carry the reference's maxItem: the hot bucket's went past 16 several times
-    raw = open(d, "rb").read()
-    o = 156
-    for b in range(hot):
-        o += 8 + 32 * int.from_bytes(raw[o:o + 4], "little")
-    nb, mx = int.from_bytes(raw[o:o + 4], "little"), int.from_bytes(raw[o + 4:o + 8], "little")
+    w = Work.read(d)
+    nb, mx = len(w.table[hot]), w.maxitem[hot]
     assert nb >= 103 and mx > nb and (mx - 16) % 4 == 0             # (a random record of another batch may share the bucket)
     p.close()
 

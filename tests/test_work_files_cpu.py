@@ -38,6 +38,7 @@ def test_reference_written_work_file_loads_with_its_kangaroos(tmp_path):
     assert w.nb_walk == 1024                                              # one CPU thread: CPU_GRP_SIZE kangaroos
     assert os.path.getsize(path) == w.walk_offset + 96 * w.nb_walk
     assert read_work_header(path) == (w.dp_bits, w.range_start, w.range_end, w.key, w.total_count, w.total_time)
+    assert read_work_header(path).version == 0                            # Kangaroo::SaveHeader writes version 0
     key = ec.add(pub, ec.neg(ec.mul(g.START)))                            # Kangaroo::InitSearchKey: P - start*G
     recs = w.walks()
     for i in list(range(8)) + list(range(1016, 1024)) + [101, 502, 777]:
