@@ -129,6 +129,20 @@ int kgx_create_herd_multi(kgx_engine* e, const uint64_t* scalars, const uint64_t
                           const uint16_t* targets, int first_type);
 int kgx_retarget(kgx_engine* e, uint32_t from, const uint16_t* to, uint32_t n_to);
 int kgx_targets(kgx_engine* e, uint16_t* out);
+/* --- checkpoint and resume of a multi-key herd (the solver's batch work files).
+ * kgx_snapshot_begin on a herd with a key table also copies the targets, device to device in stream order with the state, so a
+ *     kgx_retarget queued after it does not show in the snapshot.
+ * _snapshot_export_targets: targets [first, first+count) of the pending snapshot (kIdx order) to dst (host memory); call it
+ *     before the kgx_snapshot_export chunk that releases the snapshot.  Fails when the snapshot was taken without a key table.
+ * _import_multi: kgx_import with a key table (keys: n_keys x 8 limbs, 1 <= n_keys <= KGX_MAX_KEYS) and a target per record
+ *     (targets: count entries, each below n_keys): verify != 0 checks wild record i against keys[targets[i]] + d*G and tame ones
+ *     against d*G, on the device.  On success the engine holds the key table and targets[0..count) as kgx_create_herd_multi
+ *     leaves them (kgx_retarget and kgx_targets work); kangaroos count..n-1 keep their state and targets, so a partial import
+ *     needs a herd of kgx_create_herd_multi with the same keys first.  Fails in symmetric mode; with mismatches nothing
+ *     changes, key table and targets included. --- */
+int kgx_snapshot_export_targets(kgx_engine* e, uint64_t first, uint64_t count, uint16_t* dst);
+int kgx_import_multi(kgx_engine* e, const uint64_t wild_offset[2], const void* recs, uint64_t count, const uint64_t* keys,
+                     uint32_t n_keys, const uint16_t* targets, int verify, uint64_t* mismatches);
 
 /* --- GPUEngine::callKernel (GPUEngine.cu:540-557): zero the DP count, start NB_RUN jumps, asynchronous --- */
 int kgx_launch_async(kgx_engine* e);
@@ -217,12 +231,21 @@ int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, u
  *     time, the merged table (maxItem = nbItem rounded up to 4), then a kangaroo count of 0.  Inputs without a kangaroo count
  *     are accepted.  The inputs stream through the device in blocks of whole buckets of at most block_entries entries over
  *     all inputs (0 = 2^22); a bucket larger than that is refused and tmp_path removed.  The first `cap` collisions, ordered by
- *     bucket then x, go to coll. --- */
+ *     bucket then x, go to coll.  A batch work file (kgx_workfile.h) is refused.
+ * A batch work file (_check reads it too: each kangaroo against its own target key K_t = keys[t] - start*G, each wild table
+ *     entry accepted when it matches any key of the block, info->n_keys = the block's keys):
+ * _batch_block_bytes / _batch_block: the block that follows the records of a file with nb_walk kangaroos whose records end
+ *     at byte `offset`; keys: n_keys x 8 limbs (public x, y), solved: n_keys flags, privs: n_keys x 4 limbs (read where
+ *     solved), targets: nb_walk key indices in file order.  Plain host code, no device needed.
+ * _batch_read: 1 = `path` holds a batch block: *n_keys, *nb_walk, *offset and, where non-NULL, keys / solved / privs /
+ *     targets (sized as above) are filled; 0 = a plain HEADW file; -1 = not a HEADW file, or a block cut short or damaged,
+ *     reason in kgx_work_last_error(); -errno when the file cannot be opened.  No device needed. --- */
 typedef struct {
   uint32_t dp_bits, has_walk_count;
   uint64_t entries, wrong_entries;
   uint64_t walks, walks_tame, walks_wild, wrong_walks;
   uint32_t n_wrong_entries_listed, n_wrong_walks_listed;
+  uint32_t n_keys, reserved;   /* keys of a batch work file's block; 0 for a plain HEADW file */
 } kgx_work_check_info;
 typedef struct {
   uint32_t dp_bits, blocks;
@@ -244,6 +267,11 @@ int kgx_work_check_records(int dev, int kind, const void* recs, const uint32_t* 
 int kgx_work_comb(int dev, uint64_t* out);
 int kgx_work_merge(int dev, const char* const* paths, uint32_t n_paths, const char* tmp_path, uint64_t block_entries,
                    kgx_work_merge_info* info, kgx_work_collision* coll, uint32_t cap);
+uint64_t kgx_batch_block_bytes(uint32_t n_keys, uint64_t nb_walk);
+int kgx_batch_block(const uint64_t* keys, const uint8_t* solved, const uint64_t* privs, uint32_t n_keys, const uint16_t* targets,
+                    uint64_t nb_walk, uint64_t offset, void* out);
+int kgx_batch_read(const char* path, uint32_t* n_keys, uint64_t* nb_walk, uint64_t* offset, uint64_t* keys, uint8_t* solved,
+                   uint64_t* privs, uint16_t* targets);
 
 /* Debug (KGX_PROF=1 in the environment at kgx_create): phase cycle counters summed over warp 0 of every CTA:
  * out = {serial section, modular inverse alone, parallel phase, tile-steps}; resets them. -1 when disabled. */

@@ -47,6 +47,9 @@ _SIGS = {
     "kgx_snapshot_read": (ctypes.c_int, [ctypes.c_void_p, _u64p, _u64p, _u64p]),
     "kgx_snapshot_export": (ctypes.c_int, [ctypes.c_void_p, _u64p, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_void_p]),
     "kgx_import": (ctypes.c_int, [ctypes.c_void_p, _u64p, ctypes.c_void_p, ctypes.c_uint64, _u64p, _u64p, ctypes.c_int, _u64p]),
+    "kgx_snapshot_export_targets": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_uint64, ctypes.c_uint64, _u16p]),
+    "kgx_import_multi": (ctypes.c_int, [ctypes.c_void_p, _u64p, ctypes.c_void_p, ctypes.c_uint64, _u64p, ctypes.c_uint32, _u16p, ctypes.c_int,
+                                        _u64p]),
     "kgx_launch_async": (ctypes.c_int, [ctypes.c_void_p]),
     "kgx_collect": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(Item), ctypes.c_uint32, ctypes.POINTER(ctypes.c_uint32),
                                    ctypes.POINTER(ctypes.c_uint32), ctypes.c_int, ctypes.c_int]),
@@ -85,6 +88,11 @@ _SIGS = {
     "kgx_work_comb": (ctypes.c_int, [ctypes.c_int, _u64p]),
     "kgx_work_merge": (ctypes.c_int, [ctypes.c_int, ctypes.POINTER(ctypes.c_char_p), ctypes.c_uint32, ctypes.c_char_p, ctypes.c_uint64,
                                       ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32]),
+    "kgx_batch_block_bytes": (ctypes.c_uint64, [ctypes.c_uint32, ctypes.c_uint64]),
+    "kgx_batch_block": (ctypes.c_int, [_u64p, ctypes.POINTER(ctypes.c_uint8), _u64p, ctypes.c_uint32, _u16p, ctypes.c_uint64, ctypes.c_uint64,
+                                       ctypes.c_void_p]),
+    "kgx_batch_read": (ctypes.c_int, [ctypes.c_char_p, ctypes.POINTER(ctypes.c_uint32), _u64p, _u64p, _u64p, ctypes.POINTER(ctypes.c_uint8),
+                                      _u64p, _u16p]),
 }
 EXPORTED_SYMBOLS = sorted(_SIGS)
 

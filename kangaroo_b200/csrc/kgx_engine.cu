@@ -94,6 +94,8 @@ struct kgx_engine {
   u32* rtDelta = nullptr;         // keyCap x 16 words: keys[to[j]] - keys[from] of the retarget in stream order
   u32* rtTo = nullptr;            // keyCap: to[j] | infinity flag
   u32 nKeys = 0, keyCap = 0;      // nKeys == 0: no key table (a herd of kgx_create_herd or kgx_upload)
+  uint16_t* snapTargets = nullptr; // n: the targets of the pending snapshot (kgx_snapshot_begin on a herd with a key table)
+  bool snapHasTargets = false;
   int firstType = 0;
   float lastMs = 0.f;
   unsigned long long* prof = nullptr;   // KGX_PROF=1: phase cycle counters
@@ -152,7 +154,7 @@ void kgx_destroy(kgx_engine* e) {
   if (e->stream) cudaStreamSynchronize(e->stream);
   cudaFree(e->dp40); cudaFree(e->herdTab); cudaFree(e->state); cudaFree(e->pre); cudaFree(e->jlog); cudaFree(e->slab[0]); cudaFree(e->slab[1]); cudaFree(e->jtab);
   cudaFree(e->stgX); cudaFree(e->stgY); cudaFree(e->stgD); cudaFree(e->aux); cudaFree(e->herdRecs);
-  cudaFree(e->keys); cudaFree(e->targets); cudaFree(e->rtDelta); cudaFree(e->rtTo);
+  cudaFree(e->keys); cudaFree(e->targets); cudaFree(e->rtDelta); cudaFree(e->rtTo); cudaFree(e->snapTargets);
   if (e->slabPinned) cudaFreeHost(e->slabPinned);
   for (int i = 0; i < 2; i++) { if (e->evStart[i]) cudaEventDestroy(e->evStart[i]); if (e->evStop[i]) cudaEventDestroy(e->evStop[i]); }
   if (e->evSnap) cudaEventDestroy(e->evSnap);
@@ -280,7 +282,7 @@ uint64_t kgx_num_kangaroos(kgx_engine* e) { return e->n; }
 int kgx_kernel_kind(kgx_engine* e) { return e->kind; }
 uint64_t kgx_memory_bytes(kgx_engine* e) {
   return e->stateBytes + (e->pre ? e->nPadded * 32 : 0) + (e->jlog ? e->nPadded * LOG_RUNS : 0) + 2 * e->slabBytes + JT_WORDS * 4 +
-         (e->targets ? e->n * 2 : 0) + (u64)e->keyCap * (64 + 64 + 4);
+         (e->targets ? e->n * 4 : 0) + (u64)e->keyCap * (64 + 64 + 4);
 }
 uint32_t kgx_max_found(kgx_engine* e) { return e->maxFound; }
 float kgx_last_launch_ms(kgx_engine* e) { return e->lastMs; }
@@ -400,9 +402,12 @@ int kgx_snapshot_begin(kgx_engine* e) {
   unpack_kernel<<<blocks, 256, 0, e->stream>>>(e->state, e->stgX, e->stgY, e->stgD, e->n, e->T, e->K);
   e->launches++;
   CK(e, cudaGetLastError());
+  // the targets of a multi-key herd, in the same stream order: a kgx_retarget queued after this call changes e->targets only
+  if (e->nKeys) CK(e, cudaMemcpyAsync(e->snapTargets, e->targets, e->n * 2, cudaMemcpyDeviceToDevice, e->stream));
   CK(e, cudaEventRecord(e->evSnap, e->stream));
   e->snapPending = true;
   e->snapConverted = false;
+  e->snapHasTargets = e->nKeys != 0;
   return 0;
 }
 
@@ -444,16 +449,63 @@ int kgx_snapshot_export(kgx_engine* e, const uint64_t wild_offset[2], uint64_t f
   return 0;
 }
 
+int kgx_snapshot_export_targets(kgx_engine* e, uint64_t first, uint64_t count, uint16_t* dst) {
+  CK(e, cudaSetDevice(e->dev));
+  if (!e->snapPending) { snprintf(e->err, sizeof e->err, "kgx_snapshot_export_targets: no snapshot pending"); return -1; }
+  if (!e->snapHasTargets) { snprintf(e->err, sizeof e->err, "kgx_snapshot_export_targets: the snapshot's herd has no key table (kgx_create_herd_multi)"); return -1; }
+  if (first > e->n || count > e->n - first) { snprintf(e->err, sizeof e->err, "kgx_snapshot_export_targets: range [%llu, +%llu) outside the herd", (unsigned long long)first, (unsigned long long)count); return -1; }
+  CK(e, cudaStreamWaitEvent(e->copyStream, e->evSnap, 0));
+  if (count) CK(e, cudaMemcpyAsync(dst, e->snapTargets + first, count * 2, cudaMemcpyDeviceToHost, e->copyStream));
+  CK(e, cudaStreamSynchronize(e->copyStream));
+  return 0;
+}
+
+// The device key table of a multi-key herd, grown to n_keys, and the per-kangaroo targets (kgx_create_herd_multi,
+// kgx_import_multi).  The snapshot's copy of the targets is allocated with them: kgx_snapshot_begin allocates nothing.
+static int ensure_key_table(kgx_engine* e, uint32_t n_keys) {
+  if (n_keys > e->keyCap) {
+    cudaFree(e->keys); cudaFree(e->rtDelta); cudaFree(e->rtTo);
+    e->keys = e->rtDelta = e->rtTo = nullptr;
+    e->keyCap = 0;
+    CK(e, cudaMalloc(&e->keys, (size_t)n_keys * 64));
+    CK(e, cudaMalloc(&e->rtDelta, (size_t)n_keys * 64));
+    CK(e, cudaMalloc(&e->rtTo, (size_t)n_keys * 4));
+    e->keyCap = n_keys;
+  }
+  if (!e->targets) CK(e, cudaMalloc(&e->targets, e->n * 2));
+  if (!e->snapTargets) CK(e, cudaMalloc(&e->snapTargets, e->n * 2));
+  // load the retarget kernels now: kgx_retarget must not be the first launch of a kernel, which can wait for the device
+  cudaFuncAttributes fa;
+  CK(e, cudaFuncGetAttributes(&fa, retarget_delta_kernel));
+  CK(e, cudaFuncGetAttributes(&fa, retarget_kernel));
+  return 0;
+}
+
 // Replace kangaroos 0..count-1 by `count` work-file records (host memory), in stream order after the launch in flight.
 // Nothing changes when a record's biased distance does not fit in 128 bits (error) or, with verify != 0, when any position
-// differs from d*G (tame) / key + d*G (wild): *mismatches then says how many do (0 = imported).
-int kgx_import(kgx_engine* e, const uint64_t wild_offset[2], const void* recs, uint64_t count, const uint64_t keyx[4],
-               const uint64_t keyy[4], int verify, uint64_t* mismatches) {
+// differs from d*G (tame) / key + d*G (wild): *mismatches then says how many do (0 = imported).  keys: n_keys x 8 limbs;
+// targets NULL: one key; else wild record i is checked against keys[targets[i]], and on success the key table and the
+// targets of kangaroos 0..count-1 are installed (kgx_import_multi).
+static int import_records(kgx_engine* e, const char* what, const uint64_t wild_offset[2], const void* recs, uint64_t count,
+                          const uint64_t* keys, uint32_t n_keys, const uint16_t* targets, int verify, uint64_t* mismatches) {
   CK(e, cudaSetDevice(e->dev));
   if (mismatches) *mismatches = 0;
-  if (e->symmetry) { snprintf(e->err, sizeof e->err, "kgx_import: not available in symmetric mode (signed distances)"); return -1; }
-  if (e->snapPending) { snprintf(e->err, sizeof e->err, "kgx_import: snapshot pending (export it first)"); return -1; }
-  if (count > e->n) { snprintf(e->err, sizeof e->err, "kgx_import: %llu records for a herd of %llu", (unsigned long long)count, (unsigned long long)e->n); return -1; }
+  if (e->symmetry) { snprintf(e->err, sizeof e->err, "%s: not available in symmetric mode (signed distances)", what); return -1; }
+  if (e->snapPending) { snprintf(e->err, sizeof e->err, "%s: snapshot pending (export it first)", what); return -1; }
+  if (count > e->n) { snprintf(e->err, sizeof e->err, "%s: %llu records for a herd of %llu", what, (unsigned long long)count, (unsigned long long)e->n); return -1; }
+  if (targets) {
+    if (n_keys == 0 || n_keys > KGX_MAX_KEYS) { snprintf(e->err, sizeof e->err, "%s: n_keys must be in [1, %d]", what, KGX_MAX_KEYS); return -1; }
+    for (u64 i = 0; i < count; i++)
+      if (targets[i] >= n_keys) {
+        snprintf(e->err, sizeof e->err, "%s: target %u of record %llu is not below n_keys = %u", what, targets[i], (unsigned long long)i, n_keys);
+        return -1;
+      }
+    if (count < e->n && !e->nKeys) {
+      snprintf(e->err, sizeof e->err, "%s: %llu records for a herd of %llu without a key table (kgx_create_herd_multi first)", what,
+               (unsigned long long)count, (unsigned long long)e->n);
+      return -1;
+    }
+  }
   if (count == 0) return 0;
   if (verify && !e->herdTab) {
     CK(e, cudaMalloc(&e->herdTab, 256 * 16 * 4));
@@ -464,6 +516,7 @@ int kgx_import(kgx_engine* e, const uint64_t wild_offset[2], const void* recs, u
   if (!e->herdRecs) CK(e, cudaMalloc(&e->herdRecs, e->n * 96));
   if (ensure_staging(e)) return -1;
   u32 *scal = nullptr, *vx = nullptr, *vy = nullptr, *dKey = nullptr;
+  uint16_t* dTg = nullptr;
   unsigned long long* flags = nullptr;     // [0] lowest out-of-range index (~0 = none), [1] mismatches
   auto body = [&]() -> int {
     CK(e, cudaMalloc(&scal, count * 32));
@@ -481,11 +534,13 @@ int kgx_import(kgx_engine* e, const uint64_t wild_offset[2], const void* recs, u
     if (verify) {
       CK(e, cudaMalloc(&vx, count * 32));
       CK(e, cudaMalloc(&vy, count * 32));
-      CK(e, cudaMalloc(&dKey, 64));
-      uint64_t key[8];
-      memcpy(key, keyx, 32); memcpy(key + 4, keyy, 32);
-      CK(e, cudaMemcpyAsync(dKey, key, 64, cudaMemcpyHostToDevice, e->stream));
-      herd_kernel<<<(u32)((count + 127) / 128), 128, 0, e->stream>>>(e->herdTab, scal, dKey, nullptr, 0, count, vx, vy, 0, nullptr);
+      CK(e, cudaMalloc(&dKey, (size_t)n_keys * 64));
+      CK(e, cudaMemcpyAsync(dKey, keys, (size_t)n_keys * 64, cudaMemcpyHostToDevice, e->stream));
+      if (targets) {
+        CK(e, cudaMalloc(&dTg, count * 2));
+        CK(e, cudaMemcpyAsync(dTg, targets, count * 2, cudaMemcpyHostToDevice, e->stream));
+      }
+      herd_kernel<<<(u32)((count + 127) / 128), 128, 0, e->stream>>>(e->herdTab, scal, dKey, dTg, 0, count, vx, vy, 0, nullptr);
       e->launches++;
       CK(e, cudaGetLastError());
       herd_compare_kernel<<<4 * e->sms, 256, 0, e->stream>>>(reinterpret_cast<u32*>(e->stgX), reinterpret_cast<u32*>(e->stgY), vx, vy, count, flags + 1);
@@ -501,16 +556,34 @@ int kgx_import(kgx_engine* e, const uint64_t wild_offset[2], const void* recs, u
     }
     if (mismatches) *mismatches = res[1];
     if (res[1]) return 0;
+    if (targets) {                         // verified: install the key table and the targets, as kgx_create_herd_multi does
+      if (ensure_key_table(e, n_keys)) return -1;
+      CK(e, cudaMemcpyAsync(e->keys, keys, (size_t)n_keys * 64, cudaMemcpyHostToDevice, e->stream));
+      CK(e, cudaMemcpyAsync(e->targets, targets, count * 2, cudaMemcpyHostToDevice, e->stream));
+    }
     pack_kernel<<<(u32)((e->nPadded + 255) / 256), 256, 0, e->stream>>>(e->state, e->stgX, e->stgY, e->stgD, e->n, e->nPadded, e->T, e->K, e->aux, aux_init(e));
     e->launches++;
     CK(e, cudaGetLastError());
     CK(e, cudaStreamSynchronize(e->stream));
+    if (targets) { e->nKeys = n_keys; e->firstType = 0; }
     return 0;
   };
   const int rc = body();
-  cudaFree(scal); cudaFree(vx); cudaFree(vy); cudaFree(dKey); cudaFree(flags);
+  cudaFree(scal); cudaFree(vx); cudaFree(vy); cudaFree(dKey); cudaFree(dTg); cudaFree(flags);
   free_staging(e);
   return rc;
+}
+
+int kgx_import(kgx_engine* e, const uint64_t wild_offset[2], const void* recs, uint64_t count, const uint64_t keyx[4],
+               const uint64_t keyy[4], int verify, uint64_t* mismatches) {
+  uint64_t key[8];
+  memcpy(key, keyx, 32); memcpy(key + 4, keyy, 32);
+  return import_records(e, "kgx_import", wild_offset, recs, count, key, 1, nullptr, verify, mismatches);
+}
+
+int kgx_import_multi(kgx_engine* e, const uint64_t wild_offset[2], const void* recs, uint64_t count, const uint64_t* keys,
+                     uint32_t n_keys, const uint16_t* targets, int verify, uint64_t* mismatches) {
+  return import_records(e, "kgx_import_multi", wild_offset, recs, count, keys, n_keys, targets, verify, mismatches);
 }
 
 int kgx_patch(kgx_engine* e, uint64_t kidx, const uint64_t px[4], const uint64_t py[4], const uint64_t d[2]) {
@@ -546,20 +619,7 @@ static int create_herd(kgx_engine* e, const char* what, const uint64_t* scalars,
   auto body = [&]() -> int {      // CK returns from the lambda, so the scratch buffers are always released below
     CK(e, cudaMalloc(&dScal, e->n * 32));
     if (targets) {
-      if (n_keys > e->keyCap) {
-        cudaFree(e->keys); cudaFree(e->rtDelta); cudaFree(e->rtTo);
-        e->keys = e->rtDelta = e->rtTo = nullptr;
-        e->keyCap = 0;
-        CK(e, cudaMalloc(&e->keys, (size_t)n_keys * 64));
-        CK(e, cudaMalloc(&e->rtDelta, (size_t)n_keys * 64));
-        CK(e, cudaMalloc(&e->rtTo, (size_t)n_keys * 4));
-        e->keyCap = n_keys;
-      }
-      if (!e->targets) CK(e, cudaMalloc(&e->targets, e->n * 2));
-      // load the retarget kernels now: kgx_retarget must not be the first launch of a kernel, which can wait for the device
-      cudaFuncAttributes fa;
-      CK(e, cudaFuncGetAttributes(&fa, retarget_delta_kernel));
-      CK(e, cudaFuncGetAttributes(&fa, retarget_kernel));
+      if (ensure_key_table(e, n_keys)) return -1;
       CK(e, cudaMemcpyAsync(e->keys, keys, (size_t)n_keys * 64, cudaMemcpyHostToDevice, e->stream));
       CK(e, cudaMemcpyAsync(e->targets, targets, e->n * 2, cudaMemcpyHostToDevice, e->stream));
     } else {

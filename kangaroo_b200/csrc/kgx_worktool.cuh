@@ -145,10 +145,12 @@ __device__ __forceinline__ bool wt_proj_eq(const u32* X, const u32* Y, const u32
 }
 
 // Walk records (96 bytes: x[4], y[4], d[4] limbs): res[i] = 1 tame OK, 2 wild OK, 0 wrong; cnt = {tame, wild, wrong}.
-// bad[i] = 1 when wrong.  d >= n or min(d, n - d) >= 2^128 is wrong: engine distances are 128-bit.
+// bad[i] = 1 when wrong.  d >= n or min(d, n - d) >= 2^128 is wrong: engine distances are 128-bit.  K: the key table (16 words
+// per key), kinfs[k] = key k is the point at infinity; record i is checked against key tg[i] (a batch file's targets), or key
+// 0 when tg is null.
 __global__ void __launch_bounds__(CHECK_THREADS) wt_check_walks_kernel(const u32* __restrict__ comb, const u32* __restrict__ recs,
-                                                                      uint64_t n, const u32* __restrict__ K, int kinf, uint8_t* res,
-                                                                      uint8_t* bad, ull* cnt) {
+                                                                      uint64_t n, const u32* __restrict__ K, const int* __restrict__ kinfs,
+                                                                      const uint16_t* __restrict__ tg, uint8_t* res, uint8_t* bad, ull* cnt) {
   using namespace kgx;
   __shared__ u32 sc[COMB_WORDS];
   wt_load_comb(sc, comb);
@@ -173,7 +175,8 @@ __global__ void __launch_bounds__(CHECK_THREADS) wt_check_walks_kernel(const u32
         if (!dle && !f) { u32 t[8]; fe_neg(t, Y); fe_copy(Y, t); }
         if (!f && wt_proj_eq(X, Y, Z, x, y)) kind = 1;
         else {
-          if (!kinf) jac_add_affine(X, Y, Z, f, K, K + 8);
+          const u32 t = tg ? tg[i] : 0u;
+          if (!kinfs[t]) jac_add_affine(X, Y, Z, f, K + 16 * t, K + 16 * t + 8);
           if (!f && wt_proj_eq(X, Y, Z, x, y)) kind = 2;
         }
       }
@@ -184,10 +187,13 @@ __global__ void __launch_bounds__(CHECK_THREADS) wt_check_walks_kernel(const u32
   }
 }
 
-// key checks: ok[0] = key (x, y) on the curve; K = key + s*G (s = -start mod n, 8 words) is left to herd_kernel
-__global__ void wt_on_curve_kernel(const u32* key, int* ok) {
+// key checks: *ok (set to 1 by the caller) is cleared when one of the n keys (x, y) is off the curve; K = key + s*G (s = -start
+// mod n, 8 words) is left to herd_kernel
+__global__ void wt_on_curve_kernel(const u32* keys, uint32_t n, int* ok) {
   using namespace kgx;
-  if (threadIdx.x || blockIdx.x) return;
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const u32* key = keys + 16 * i;
   u32 l[8], r[8], s[8], seven[8] = {7, 0, 0, 0, 0, 0, 0, 0};
   fe_sqr(l, key + 8);
   fe_sqr(r, key);
@@ -198,7 +204,92 @@ __global__ void wt_on_curve_kernel(const u32* key, int* ok) {
   bool canon = true;                                    // coordinates must be below p, as the reference's EC() check reads them
   u32 t[8];
   for (int c = 0; c < 2; c++) { fe_copy(t, key + 8 * c); fe_canon(t); for (int k = 0; k < 8; k++) canon = canon && t[k] == key[8 * c + k]; }
-  *ok = fe_is_zero_modp(l) && canon;
+  if (!(fe_is_zero_modp(l) && canon)) atomicAnd(ok, 0);
+}
+
+// Table entries of a batch file: as wt_check_entries_kernel, one entry per thread, but a wild entry is OK when S = +-|d|*G
+// plus any of the n_keys keys K (16 words each; kinfs[k]: K is the point at infinity, then S itself) passes the test.  S is
+// made affine once; then every key costs one affine addition, whose inverses are batched over KB keys at a time (a key
+// with K = +-S counts as no match).  The scan stops at the first key that matches.
+constexpr int KB = 8;
+__global__ void __launch_bounds__(CHECK_THREADS) wt_check_entries_multi_kernel(const u32* __restrict__ comb, const Entry* __restrict__ ent,
+                                                                              const uint32_t* __restrict__ hs, uint64_t n,
+                                                                              const u32* __restrict__ K, const int* __restrict__ kinfs,
+                                                                              uint32_t n_keys, uint8_t* bad, ull* nbad) {
+  using namespace kgx;
+  __shared__ u32 sc[COMB_WORDS];
+  wt_load_comb(sc, comb);
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const Entry e = ent[i];
+  const uint32_t h = hs[i];
+  auto match = [&](u32* x) { fe_canon(x); return (x[4] & 0x3FFFFu) == h && (((u64)x[1] << 32) | x[0]) == e.x0 && (((u64)x[3] << 32) | x[2]) == e.x1; };
+  const bool wild = (e.d1 >> 62) & 1, neg = e.d1 >> 63;
+  const u32 m[4] = {(u32)e.d0, (u32)(e.d0 >> 32), (u32)e.d1, (u32)(e.d1 >> 32) & 0x3FFFFFFFu};
+  u32 X[8], Y[8], Z[8];
+  bool f, ok = false;
+  wt_comb_mul(sc, m, X, Y, Z, f);
+  if (!f) {
+    u32 zi[8], z2[8];
+    modinv256(zi, Z);
+    fe_sqr(z2, zi);
+    fe_mul(X, X, z2);
+    fe_mul(z2, z2, zi);
+    fe_mul(Y, Y, z2);
+    fe_canon(X);
+    fe_canon(Y);
+    if (neg) { u32 t[8]; fe_neg(t, Y); fe_copy(Y, t); fe_canon(Y); }
+    if (!wild) {
+      u32 x[8];
+      fe_copy(x, X);
+      ok = match(x);
+    } else {
+#pragma unroll 1
+      for (uint32_t k0 = 0; k0 < n_keys && !ok; k0 += KB) {
+        u32 acc[KB][8], run[8];
+        fe_set_one(run);
+#pragma unroll
+        for (int j = 0; j < KB; j++) {            // prefix products of x_K - x_S (1 in place of a zero or a missing key)
+          u32 dx[8];
+          const uint32_t k = k0 + j;
+          fe_set_one(dx);
+          if (k < n_keys && !kinfs[k]) {
+            fe_sub(dx, K + 16 * k, X);
+            if (fe_is_zero_modp(dx)) fe_set_one(dx);
+          }
+          fe_mul(run, run, dx);
+          fe_copy(acc[j], run);
+        }
+        u32 inv[8];
+        modinv256(inv, run);
+#pragma unroll
+        for (int j = KB - 1; j >= 0; j--) {
+          const uint32_t k = k0 + j;
+          u32 dx[8], di[8];
+          fe_set_one(dx);
+          bool use = false;
+          if (k < n_keys && !kinfs[k]) {
+            fe_sub(dx, K + 16 * k, X);
+            use = !fe_is_zero_modp(dx);
+            if (!use) fe_set_one(dx);
+          }
+          if (j > 0) fe_mul(di, inv, acc[j - 1]); else fe_copy(di, inv);   // 1 / dx
+          fe_mul(inv, inv, dx);
+          if (k < n_keys && kinfs[k]) { u32 x[8]; fe_copy(x, X); ok = ok || match(x); }
+          if (!use) continue;
+          u32 lam[8], x3[8], t[8];
+          fe_sub(lam, K + 16 * k + 8, Y);
+          fe_mul(lam, lam, di);
+          fe_sqr(x3, lam);
+          fe_sub(x3, x3, X);
+          fe_sub(t, x3, K + 16 * k);
+          ok = ok || match(t);
+        }
+      }
+    }
+  }
+  bad[i] = !ok;
+  if (!ok) atomicAdd(nbad, 1ull);
 }
 
 // ---- merge ----
@@ -283,8 +374,10 @@ static int key_setup(DevBufs& B, const uint64_t kx[4], const uint64_t ky[4], con
   if (B.dev(&dKey, 64) || B.dev(&dOk, 4)) return -3;
   uint64_t key[8];
   memcpy(key, kx, 32); memcpy(key + 4, ky, 32);
+  const int one = 1;
   WT_CK(cudaMemcpyAsync(dKey, key, 64, cudaMemcpyHostToDevice, st));
-  wt_on_curve_kernel<<<1, 32, 0, st>>>(dKey, dOk);
+  WT_CK(cudaMemcpyAsync(dOk, &one, 4, cudaMemcpyHostToDevice, st));
+  wt_on_curve_kernel<<<1, 32, 0, st>>>(dKey, 1, dOk);
   WT_CK(cudaGetLastError());
   WT_CK(cudaMemcpyAsync(ok, dOk, 4, cudaMemcpyDeviceToHost, st));
   WT_CK(cudaStreamSynchronize(st));
@@ -307,6 +400,60 @@ static int key_setup(DevBufs& B, const uint64_t kx[4], const uint64_t ky[4], con
   bool z = true;
   for (int k = 0; k < 8; k++) z = z && kh[k] == 0;
   *kinf = z;                                            // herd_kernel stores the point at infinity as (0, 0)
+  return 0;
+}
+
+// A batch file's keys (n x 8 limbs, public x, y) -> *ok = all on the curve; K (n x 16 words on the device) = key - start*G,
+// kinfs[k] = K is the point at infinity.  herd_kernel makes odd slots wild, so key k is computed in slot 2k + 1.
+static int keys_setup(DevBufs& B, const std::vector<uint64_t>& keys, uint32_t n, const uint64_t rs[4], cudaStream_t st, int* ok,
+                      u32** K, int** kinfs) {
+  u32 *dKeys, *tab, *scal, *px, *py;
+  uint16_t* tg;
+  int* dOk;
+  if (B.dev(&dKeys, 64ull * n) || B.dev(&dOk, 4) || B.dev(&tab, 256 * 16 * 4) || B.dev(&scal, 64ull * n) || B.dev(&px, 64ull * n) ||
+      B.dev(&py, 64ull * n) || B.dev(&tg, 4ull * n) || B.dev(K, 64ull * n) || B.dev(kinfs, 4ull * n))
+    return -3;
+  const int one = 1;
+  WT_CK(cudaMemcpyAsync(dKeys, keys.data(), 64ull * n, cudaMemcpyHostToDevice, st));
+  WT_CK(cudaMemcpyAsync(dOk, &one, 4, cudaMemcpyHostToDevice, st));
+  wt_on_curve_kernel<<<(n + 127) / 128, 128, 0, st>>>(dKeys, n, dOk);
+  WT_CK(cudaGetLastError());
+  WT_CK(cudaMemcpyAsync(ok, dOk, 4, cudaMemcpyDeviceToHost, st));
+  WT_CK(cudaStreamSynchronize(st));
+  if (!*ok) return 0;
+  using kgx::kOrderHost;
+  u64 a[4], s[4] = {0, 0, 0, 0};
+  memcpy(a, rs, 32);
+  if (kgx::ge256(a, kOrderHost)) kgx::sub256(a, a, kOrderHost);
+  if (a[0] | a[1] | a[2] | a[3]) kgx::sub256(s, kOrderHost, a);
+  std::vector<uint64_t> hs(8ull * n);
+  std::vector<uint16_t> ht(2ull * n);
+  for (uint32_t k = 0; k < n; k++) {
+    memcpy(&hs[8ull * k], s, 32); memcpy(&hs[8ull * k + 4], s, 32);
+    ht[2 * k] = ht[2 * k + 1] = (uint16_t)k;
+  }
+  WT_CK(cudaMemcpyAsync(scal, hs.data(), 64ull * n, cudaMemcpyHostToDevice, st));
+  WT_CK(cudaMemcpyAsync(tg, ht.data(), 4ull * n, cudaMemcpyHostToDevice, st));
+  kgx::herd_table_kernel<<<1, 32, 0, st>>>(tab);
+  kgx::herd_kernel<<<(2 * n + 127) / 128, 128, 0, st>>>(tab, scal, dKeys, tg, 0, 2ull * n, px, py, 0, nullptr);
+  WT_CK(cudaGetLastError());
+  std::vector<uint32_t> hx(16ull * n), hy(16ull * n), hk(16ull * n);
+  std::vector<int> hinf(n);
+  WT_CK(cudaMemcpyAsync(hx.data(), px, 64ull * n, cudaMemcpyDeviceToHost, st));
+  WT_CK(cudaMemcpyAsync(hy.data(), py, 64ull * n, cudaMemcpyDeviceToHost, st));
+  WT_CK(cudaStreamSynchronize(st));
+  for (uint32_t k = 0; k < n; k++) {
+    bool z = true;
+    for (int w = 0; w < 8; w++) {
+      hk[16ull * k + w] = hx[16ull * k + 8 + w];
+      hk[16ull * k + 8 + w] = hy[16ull * k + 8 + w];
+      z = z && hk[16ull * k + w] == 0 && hk[16ull * k + 8 + w] == 0;
+    }
+    hinf[k] = z;                                        // herd_kernel stores the point at infinity as (0, 0)
+  }
+  WT_CK(cudaMemcpyAsync(*K, hk.data(), 64ull * n, cudaMemcpyHostToDevice, st));
+  WT_CK(cudaMemcpyAsync(*kinfs, hinf.data(), 4ull * n, cudaMemcpyHostToDevice, st));
+  WT_CK(cudaStreamSynchronize(st));
   return 0;
 }
 
@@ -353,7 +500,11 @@ int kgx_work_check_records(int dev, int walks, const void* recs, const uint32_t*
   WT_CK(cudaMemcpy(dRec, recs, n * (walks ? 96 : 32), cudaMemcpyHostToDevice));
   WT_CK(cudaMemset(cnt, 0, 24));
   if (walks) {
-    wt_check_walks_kernel<<<(unsigned)std::min<uint64_t>((n + 127) / 128, 4096), 128>>>(comb, (const u32*)dRec, n, K, kinf, dRes, dBad, cnt);
+    int* dKinf;
+    if (B.dev(&dKinf, 4)) return -3;
+    WT_CK(cudaMemcpy(dKinf, &kinf, 4, cudaMemcpyHostToDevice));
+    wt_check_walks_kernel<<<(unsigned)std::min<uint64_t>((n + 127) / 128, 4096), 128>>>(comb, (const u32*)dRec, n, K, dKinf, nullptr, dRes,
+                                                                                         dBad, cnt);
   } else {
     uint32_t* dH;
     if (B.dev(&dH, 4 * n)) return -3;
@@ -389,11 +540,38 @@ int kgx_work_check(int dev, const char* path, uint64_t chunk, kgx_work_check_inf
   if (key_setup(B, hd.kx, hd.ky, hd.rs, st, &ok, &K, &kinf)) return -3;
   if (!ok) { snprintf(g_wt_err, sizeof g_wt_err, "CheckWorkFile: key1 does not lie on elliptic curve"); return -1; }
   if (build_comb(B, &comb, st)) return -3;
+  int* Kinfs;                                           // per key of K: the point at infinity
+  if (B.dev(&Kinfs, 4)) return -3;
+  WT_CK(cudaMemcpyAsync(Kinfs, &kinf, 4, cudaMemcpyHostToDevice, st));
+  // a batch file: every key of its block, and every kangaroo's target
+  kgx_wf::BatchInfo bi;
+  std::vector<uint64_t> bkeys;
+  std::vector<uint16_t> btg;
+  {
+    FILE* g = fopen(path, "rb");
+    if (!g) { const int e = kgx_wf::io_error(); snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", path, strerror(-e)); return e; }
+    char berr[256] = "";
+    int bf = kgx_wf::batch_find(g, bi, berr, sizeof berr);
+    if (bf == 1) {
+      bkeys.resize(8ull * bi.n_keys);
+      btg.resize(bi.nb_walk);
+      if (kgx_wf::batch_read(g, bi, bkeys.data(), nullptr, nullptr, btg.data(), berr, sizeof berr)) bf = -1;
+    }
+    fclose(g);
+    if (bf < 0) { snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", path, berr); return -1; }
+    if (bf == 1) {
+      if (keys_setup(B, bkeys, bi.n_keys, hd.rs, st, &ok, &K, &Kinfs)) return -3;
+      if (!ok) { snprintf(g_wt_err, sizeof g_wt_err, "CheckWorkFile: a key of the batch block does not lie on elliptic curve"); return -1; }
+      info->n_keys = bi.n_keys;
+    }
+  }
+  const bool batch = info->n_keys != 0;
   // two buffers: the host fills one from disk while the device checks the other
   const uint64_t wchunk = chunk / 3 ? chunk / 3 : 1;    // walks per chunk: 96-byte records in the 32-byte entries' room
   Entry *hEnt[2], *dEnt[2];
   uint32_t *hH[2], *dH[2], *dSel[2], *hSel[2], *dNsel[2], *hNsel[2];
   uint8_t *dBad[2], *dRes[2];
+  uint16_t* dTg[2] = {nullptr, nullptr};
   ull *dCnt[2], *hCnt[2];
   std::vector<uint32_t> hIdx[2];
   size_t selTmp = 0;
@@ -405,7 +583,7 @@ int kgx_work_check(int dev, const char* path, uint64_t chunk, kgx_work_check_inf
     if (B.host(&hEnt[b], 32 * chunk) || B.dev(&dEnt[b], 32 * chunk) || B.host(&hH[b], 4 * chunk) || B.dev(&dH[b], 4 * chunk) ||
         B.dev(&dBad[b], chunk) || B.dev(&dRes[b], chunk) || B.dev(&dNsel[b], 4) ||
         B.host(&hSel[b], 4ull * (cap + 1)) || B.host(&hNsel[b], 4) || B.dev(&dCnt[b], 24) || B.host(&hCnt[b], 24) ||
-        B.dev(&dTmp[b], selTmp) || B.dev(&dSel[b], 4 * chunk))
+        B.dev(&dTmp[b], selTmp) || B.dev(&dSel[b], 4 * chunk) || (batch && B.dev(&dTg[b], 2 * wchunk)))
       return -3;
     hIdx[b].resize(chunk);
     WT_CK(cudaEventCreateWithFlags(&done[b], cudaEventDisableTiming));
@@ -419,11 +597,16 @@ int kgx_work_check(int dev, const char* path, uint64_t chunk, kgx_work_check_inf
     if (kind == 0) {
       WT_CK(cudaMemcpyAsync(dEnt[b], hEnt[b], 32 * n, cudaMemcpyHostToDevice, st));
       WT_CK(cudaMemcpyAsync(dH[b], hH[b], 4 * n, cudaMemcpyHostToDevice, st));
-      wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS, 0, st>>>(comb, dEnt[b], dH[b], n, K, kinf, dBad[b], dCnt[b]);
+      if (batch)
+        wt_check_entries_multi_kernel<<<(unsigned)((n + CHECK_THREADS - 1) / CHECK_THREADS), CHECK_THREADS, 0, st>>>(
+            comb, dEnt[b], dH[b], n, K, Kinfs, bi.n_keys, dBad[b], dCnt[b]);
+      else
+        wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS, 0, st>>>(comb, dEnt[b], dH[b], n, K, kinf, dBad[b], dCnt[b]);
     } else {
       WT_CK(cudaMemcpyAsync(dEnt[b], hEnt[b], 96 * n, cudaMemcpyHostToDevice, st));
-      wt_check_walks_kernel<<<(unsigned)std::min<uint64_t>((n + 127) / 128, 4096), 128, 0, st>>>(comb, (const u32*)dEnt[b], n, K, kinf,
-                                                                                                   dRes[b], dBad[b], dCnt[b]);
+      if (batch) WT_CK(cudaMemcpyAsync(dTg[b], btg.data() + first, 2 * n, cudaMemcpyHostToDevice, st));
+      wt_check_walks_kernel<<<(unsigned)std::min<uint64_t>((n + 127) / 128, 4096), 128, 0, st>>>(comb, (const u32*)dEnt[b], n, K, Kinfs,
+                                                                                                   dTg[b], dRes[b], dBad[b], dCnt[b]);
     }
     WT_CK(cudaGetLastError());
     size_t tb = selTmp;
@@ -520,6 +703,11 @@ int kgx_work_merge(int dev, const char* const* paths, uint32_t n_paths, const ch
     if (!fs[i]) { const int e = kgx_wf::io_error(); snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", paths[i], strerror(-e)); return e; }
     setvbuf(fs[i], nullptr, _IOFBF, 1 << 22);
     if (!kgx_wf::read_header(fs[i], hd[i])) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s is not a HEADW work file", paths[i]); return -1; }
+    uint32_t nk = 0;                                    // batch work files (--batch-keys) are not merged
+    if (kgx_batch_read(paths[i], &nk, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr) == 1) {
+      snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s is a batch work file (%u keys): merging batch files is not supported", paths[i], nk);
+      return -1;
+    }
     if (hd[i].version != hd[0].version) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: cannot merge workfile of different version (%s)", paths[i]); return -1; }
     int ok = 0;
     if (key_setup(B, hd[i].kx, hd[i].ky, hd[i].rs, 0, &ok, nullptr, nullptr)) return -3;
@@ -656,6 +844,34 @@ int kgx_work_merge(int dev, const char* const* paths, uint32_t n_paths, const ch
     memcpy(coll[k].d_other, hColl[k].d_other, 16);
   }
   return 0;
+}
+
+uint64_t kgx_batch_block_bytes(uint32_t n_keys, uint64_t nb_walk) { return kgx_wf::batch_block_bytes(n_keys, nb_walk); }
+
+int kgx_batch_block(const uint64_t* keys, const uint8_t* solved, const uint64_t* privs, uint32_t n_keys, const uint16_t* targets,
+                    uint64_t nb_walk, uint64_t offset, void* out) {
+  if (n_keys == 0 || n_keys > kgx_wf::BATCH_MAX_KEYS) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_batch_block: n_keys must be in [1, %u]", kgx_wf::BATCH_MAX_KEYS); return -1; }
+  for (uint64_t i = 0; i < nb_walk; i++)
+    if (targets[i] >= n_keys) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_batch_block: target %u of kangaroo %llu is not below n_keys = %u", targets[i], (unsigned long long)i, n_keys); return -1; }
+  kgx_wf::batch_encode(keys, solved, privs, n_keys, targets, nb_walk, offset, static_cast<uint8_t*>(out));
+  return 0;
+}
+
+int kgx_batch_read(const char* path, uint32_t* n_keys, uint64_t* nb_walk, uint64_t* offset, uint64_t* keys, uint8_t* solved,
+                   uint64_t* privs, uint16_t* targets) {
+  errno = 0;
+  FILE* f = fopen(path, "rb");
+  if (!f) { const int e = kgx_wf::io_error(); snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", path, strerror(-e)); return e; }
+  kgx_wf::BatchInfo bi;
+  char err[256] = "";
+  int rc = kgx_wf::batch_find(f, bi, err, sizeof err);
+  if (rc == 1 && (keys || solved || privs || targets) && kgx_wf::batch_read(f, bi, keys, solved, privs, targets, err, sizeof err)) rc = -1;
+  fclose(f);
+  if (rc < 0) { snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", path, err); return -1; }
+  if (n_keys) *n_keys = bi.n_keys;
+  if (nb_walk) *nb_walk = bi.nb_walk;
+  if (offset) *offset = bi.offset;
+  return rc;
 }
 
 }  // extern "C"

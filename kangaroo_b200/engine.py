@@ -187,7 +187,8 @@ class GPUEngine:
         return ax, ay, ad
 
     def SnapshotBegin(self):
-        """Asynchronous GetKangaroos (checkpoint path): snapshot after the launch in flight, do not block."""
+        """Asynchronous GetKangaroos (checkpoint path): snapshot after the launch in flight, do not block.  A multi-key herd's
+        targets are snapshotted with it (SnapshotExportTargets)."""
         self._ck(self._lib.kgx_snapshot_begin(self._h), "SnapshotBegin")
 
     def SnapshotRead(self):
@@ -225,6 +226,29 @@ class GPUEngine:
         bad = ctypes.c_uint64(0)
         self._ck(self._lib.kgx_import(self._h, _p(self._wo()), a.ctypes.data_as(ctypes.c_void_p), a.size // 96, _p(kx), _p(ky),
                                       int(bool(verify)), ctypes.byref(bad)), "ImportKangaroos")
+        return int(bad.value)
+
+    def SnapshotExportTargets(self, first, count, dst=None):
+        """Targets [first, first+count) of the snapshot taken by SnapshotBegin on a multi-key herd (kIdx order, uint16), as
+        kgx_targets showed them at the snapshot.  Call it before the SnapshotExport chunk that releases the snapshot."""
+        out = np.empty(count, dtype=np.uint16) if dst is None else dst
+        assert out.dtype == np.uint16 and out.flags.c_contiguous and out.size >= count
+        self._ck(self._lib.kgx_snapshot_export_targets(self._h, int(first), int(count), out.ctypes.data_as(_u16p)), "SnapshotExportTargets")
+        return out
+
+    def ImportKangaroosMulti(self, recs, keys, targets, verify=True):
+        """ImportKangaroos for a multi-key herd: keys = list of (x, y) points (the key table), targets = one key index per
+        record; wild record i is verified against keys[targets[i]] + d*G.  On success the engine holds the key table and the
+        targets of kangaroos 0..len(recs)-1 (Retarget / Targets work); the rest of the herd keeps its state and targets.
+        Returns the number of records that fail verification (then nothing changes)."""
+        a = np.ascontiguousarray(np.frombuffer(recs, dtype=np.uint8) if not isinstance(recs, np.ndarray) else recs.view(np.uint8).reshape(-1))
+        assert a.size % 96 == 0
+        kt = np.ascontiguousarray(np.hstack([_limbs([k[0] for k in keys], 4), _limbs([k[1] for k in keys], 4)]))
+        tg = np.ascontiguousarray(targets, dtype=np.uint16)
+        assert tg.shape == (a.size // 96,)
+        bad = ctypes.c_uint64(0)
+        self._ck(self._lib.kgx_import_multi(self._h, _p(self._wo()), a.ctypes.data_as(ctypes.c_void_p), a.size // 96, _p(kt), len(keys),
+                                            tg.ctypes.data_as(_u16p), int(bool(verify)), ctypes.byref(bad)), "ImportKangaroosMulti")
         return int(bad.value)
 
     def SetKangaroosRaw(self, ax, ay, ad):

@@ -32,6 +32,10 @@ follow over the next steps (Solver._save_start).  The end-of-run save does the s
 with the launch in flight when the loop stops.  Kangaroos re-created at step k are re-created after the snapshot, so the
 file holds them dead: a resumed run finds them again.  A save goes to FILE.tmp, is fsynced and renamed over FILE; a failed
 save removes FILE.tmp and the run goes on.  On --resume only rank 0 reads the file.
+
+--batch-keys saves and resumes through the same path with --batch-save FILE, --batch-save-interval SECS and --batch-resume
+FILE: the work file of the cut followed by a batch block with every key, its solved flag and every kangaroo's target
+(BatchSolver, kgx_workfile.h).
 """
 import argparse
 import contextlib
@@ -368,7 +372,10 @@ class Solver:
         self._save_stats.append(self._save_steps)
         if self.rank == 0:
             nwalk = self.herd.total if kangaroos else 0
-            self._work.put(("begin", self.jumps, self.time_offset + time.time() - self.t_start, nwalk, time.perf_counter()))
+            self._work.put(("begin", self.jumps, self.time_offset + time.time() - self.t_start, nwalk, time.perf_counter(),
+                            self._cut(kangaroos)))
+        else:
+            self._cut(kangaroos)                               # every rank takes part (--batch-keys: the targets' gather)
         self._save_progress(chunks)
 
     def _save_progress(self, chunks):
@@ -391,7 +398,7 @@ class Solver:
         """ingest thread: one piece of a scheduled work file (jobs arrive in file order)"""
         kind = job[0]
         if kind == "begin":
-            count, total_time, nwalk, t0 = job[1:]
+            count, total_time, nwalk, t0, self._wf_cut = job[1:]
             self._wf = WorkFile(self.save_path, t0)
             if self.table_msg is not None:
                 self._wf.err = "the DP table lacks DPs of the launches this file would count (%s)" % self.table_msg
@@ -404,12 +411,21 @@ class Solver:
             finally:
                 self._chunk_pool.put(buf)
         else:
+            self._end_file(self._wf, self._wf_cut)
             self._finish(self._wf, scheduled=True)
             self._wf = None
 
     def _write_table(self, wf, count, total_time, nwalk):
         wf.begin(lambda tmp: self.dpt.save(tmp, self.dp_bits, self.start, self.end, self.pub, total_count=count,
                                            total_time=total_time, total_walk=nwalk))
+
+    def _cut(self, kangaroos):
+        """every rank, first step of a save: what a file of this cut holds beyond the table and the records (rank 0: passed to
+        _end_file with the file's last job)"""
+        return None
+
+    def _end_file(self, wf, cut):
+        """ingest thread: the file's table and records are written; append what follows them"""
 
     def _finish(self, wf, scheduled):
         """ingest thread: close a work file -> its error or None.  scheduled: begun by _save_start (not the full table's save)"""
@@ -456,6 +472,7 @@ class Solver:
         if self.save_path and self._wf is None:
             wf = WorkFile(self.save_path, time.perf_counter())
             self._write_table(wf, jumps_before, self.time_offset + time.time() - self.t_start, 0)
+            self._end_file(wf, self._cut(kangaroos=False))
             self.full_saved = (self.save_path, jumps_before, self._finish(wf, scheduled=False))
 
     def _ingest(self, events):
@@ -715,11 +732,19 @@ def class_privs(start, priv_rep, neg):
     return (2 * start - priv_rep) % ORDER if neg else priv_rep
 
 
+# Batch work files (--batch-save / --batch-resume): the single-key file of the cut (table, kangaroo records; header key = input
+# key 0, wild distances relative to each wild's own target) followed by the batch block (kgx_workfile.h: the keys, their solved
+# flags and private keys, every kangaroo's target).  The order that keeps a cut consistent: the keys rank 0 announces solved
+# at step k are retargeted on every rank at step k, before the snapshot a save decided at step k takes, and a save's solved
+# flags are the keys announced up to the step that took its snapshot.  So a file shows a key solved exactly when the wilds of
+# it were moved on before the snapshot; a key found but not yet announced is written unsolved, with its wilds still on it.
 class BatchSolver(Solver):
-    """--batch-keys.  pubs: every public key of the input.  After run(), rank 0 holds priv[i] (None: not found)."""
+    """--batch-keys.  pubs: every public key of the input.  After run(), rank 0 holds priv[i] (None: not found).
+    save_work / save_interval: --batch-save / --batch-save-interval; resume: --batch-resume FILE with resume_block its batch
+    block (worktool.BatchBlock, from batch_resume_file: the targets on rank 0 only)."""
 
     def __init__(self, start, end, pubs, dp_bits, grid=None, max_found=1 << 17, seed=None, ingest_threads=0, dp_table="host",
-                 dp_table_capacity=None):
+                 dp_table_capacity=None, save_work="", save_interval=0.0, resume=None, resume_block=None):
         self.pubs = list(pubs)
         if not 1 <= len(self.pubs) <= MAX_KEYS:
             raise ValueError("--batch-keys takes 1 to %d keys, not %d" % (MAX_KEYS, len(self.pubs)))
@@ -729,10 +754,100 @@ class BatchSolver(Solver):
         # a key listed twice, or the negative of another, is searched once, as the first of its class: kgi_resolve_multi
         # reports the first matching key, so the later ones would never be hit
         self.rep, self.neg = key_classes(self.keys)
-        self.live = [i for i, k in enumerate(self.keys) if k is not None and self.rep[i] == i]
+        self.announced = set()              # every rank: classes (their first key) announced solved, those of the file included
+        self._resume_block = resume_block
+        if resume_block is not None:
+            for i, done in enumerate(resume_block.solved):
+                if done:
+                    self.priv[i] = resume_block.privs[i]
+                    self.announced.add(self.rep[i])
+        self.live = [i for i, k in enumerate(self.keys) if k is not None and self.rep[i] == i and i not in self.announced]
         super().__init__(start, end, self.pubs[0], dp_bits, grid, max_found, seed, ingest_threads, dp_table=dp_table,
-                         dp_table_capacity=dp_table_capacity)
+                         dp_table_capacity=dp_table_capacity, save_work=save_work, save_interval=save_interval,
+                         save_kangaroos=bool(save_work), resume=resume)
         self.key_table = DPTable.key_table(self.keys)
+
+    def _resume(self, path):
+        """Solver._resume with the targets: rank 0 loads the table and sends every rank its records and their targets; each
+        rank imports its slice verified against each record's own target key.  The wilds of keys the file shows solved then
+        move on to the live keys (the spread rule, as a retarget would have moved them); kangaroos the file lacks keep the
+        fresh herd spread over the live keys."""
+        torch = self.torch
+        info = torch.zeros(4, dtype=torch.int64, device="cuda")
+        if self.rank == 0:
+            w = self.dps.load_work_ex(path)
+            info.copy_(torch.tensor([w.nb_walk, w.walk_offset, w.total_count, 0], dtype=torch.int64))
+            self.time_offset = w.total_time
+        if self.dist is not None:
+            self.dist.broadcast(info, 0)
+        nb_walk, offset, count, _ = (int(v) for v in info.cpu().tolist())
+        self.jumps = count
+        off = self.herd.offsets[self.rank]
+        take = max(0, min(self.eng.nbKangaroo, nb_walk - off))
+        if self.rank == 0:
+            tg = self._resume_block.targets
+            print("Resume %s: %d DPs, count 2^%.2f, %d kangaroos in the file for %d in the herd, %d of %d keys solved in the file, "
+                  "%d keys left to search" % (path, len(self.dps), np.log2(max(count, 1)), nb_walk, self.herd.total,
+                                              sum(self._resume_block.solved), len(self.keys), len(self.live)), flush=True)
+            if nb_walk > self.herd.total:
+                print("Warning: %d unhandled kangaroos" % (nb_walk - self.herd.total), flush=True)
+        if self.dist is not None:                               # the targets, as bytes (NCCL has no 16-bit integers)
+            t = torch.zeros(2 * max(nb_walk, 1), dtype=torch.uint8, device="cuda")
+            if self.rank == 0 and nb_walk:
+                t[:2 * nb_walk].copy_(torch.from_numpy(tg.view(np.uint8)))
+            self.dist.broadcast(t, 0)
+            tg = t.cpu().numpy().view(np.uint16)
+        mine = np.ascontiguousarray(tg[off:off + take])
+
+        def read(first, cnt):                                   # rank 0 only
+            return np.fromfile(path, dtype=np.uint8, count=cnt * WALK_BYTES, offset=offset + first * WALK_BYTES)
+
+        t0 = time.perf_counter()
+        recs = self.herd.scatter(nb_walk, read)
+        bad = self.eng.ImportKangaroosMulti(recs, [k or (0, 0) for k in self.keys], mine, verify=True) if take else 0
+        if self.dist is not None:
+            t = torch.tensor([bad], dtype=torch.int64, device="cuda")
+            self.dist.all_reduce(t)
+            bad = int(t.item())
+        if bad:
+            raise RuntimeError("%s: %d kangaroos are not at d*G (tame) / key[target] + d*G (wild): the file belongs to other keys "
+                               "or another range" % (path, bad))
+        self.targets[:take] = mine
+        if self.live:
+            wild = self.targets[WILD::2]
+            for idx in sorted(set(np.unique(wild).tolist()) - set(self.live)):
+                self.eng.Retarget(idx, self.live)
+                self.targets = retarget_targets(self.targets, idx, self.live)
+        if take:
+            print("rank %d: %d kangaroos imported and verified in %.2f s" % (self.rank, take, time.perf_counter() - t0), flush=True)
+
+    def _cut(self, kangaroos):
+        """every rank: the snapshot's targets, gathered to rank 0 in rank order -> rank 0: the batch block of the cut"""
+        targets = np.zeros(0, dtype=np.uint16)
+        if kangaroos:
+            targets = self.eng.SnapshotExportTargets(0, self.eng.nbKangaroo)
+            if self.dist is not None:                            # as bytes, padded to the largest herd
+                torch, width = self.torch, 2 * max(self.herd.sizes)
+                t = torch.zeros(width, dtype=torch.uint8, device="cuda")
+                t[:2 * targets.size].copy_(torch.from_numpy(targets.view(np.uint8)))
+                bufs = [torch.empty(width, dtype=torch.uint8, device="cuda") for _ in range(self.world)] if self.rank == 0 else None
+                self.dist.gather(t, bufs, dst=0)
+                if self.rank == 0:
+                    targets = np.concatenate([b.cpu().numpy().view(np.uint16)[:n] for b, n in zip(bufs, self.herd.sizes)])
+        if self.rank != 0:
+            return None
+        from .worktool import BatchBlock
+        solved = [p is not None and (k is None or self.rep[i] in self.announced) for i, (k, p) in enumerate(zip(self.keys, self.priv))]
+        return BatchBlock(self.pubs, solved, [p if done else None for p, done in zip(self.priv, solved)], targets)
+
+    def _end_file(self, wf, cut):
+        if cut is None or wf.f is None or wf.err is not None:
+            return
+        from .worktool import batch_block
+        try:
+            wf.append(memoryview(batch_block(cut, wf.f.tell())))
+        except (OSError, ValueError) as e:
+            wf.err = str(e)
 
     def _create_herd(self, sc, d128):
         self.targets = assign_targets(self.eng.nbKangaroo, self.live or [0])         # host mirror of the engine's targets
@@ -772,6 +887,7 @@ class BatchSolver(Solver):
     def _solved(self, solved):
         """every rank moves the wilds of each solved key to the live ones (a reset kangaroo starts at its current key)"""
         for idx in solved:
+            self.announced.add(idx)
             self.live.remove(idx)
             if self.live:
                 self.eng.Retarget(idx, self.live)                        # stream order: after launch i+1, before the resets
@@ -785,10 +901,11 @@ class BatchSolver(Solver):
         return super().run(max_steps, verbose)
 
 
-def _run_batch(start, end, pubs, dp, grid, a):
+def _run_batch(start, end, pubs, dp, grid, a, block=None):
     t0 = time.perf_counter()
     s = BatchSolver(start, end, pubs, dp, grid, seed=a.seed, ingest_threads=a.ingest_threads, dp_table=a.dp_table,
-                    dp_table_capacity=a.dp_table_capacity)
+                    dp_table_capacity=a.dp_table_capacity, save_work=a.batch_save, save_interval=a.batch_save_interval,
+                    resume=a.batch_resume or None, resume_block=block)
     t_setup = time.perf_counter() - t0
     if s.rank == 0:
         print("Range width: 2^%d  kangaroos/GPU: %d  GPUs: %d  dp: %d  %s  keys: %d in one run" %
@@ -827,11 +944,11 @@ def report(s, a):
     if s.table_stopped:
         print(table_message(s, a))
         return 1
-    if a.save_work and s.save_error is None:
+    if s.save_path and s.save_error is None:
         mb, dt_save = s.saves[-1]
-        print("work file written: %s (%.1f MB in %.2f s, count 2^%.2f)" % (a.save_work, mb, dt_save, np.log2(max(s.jumps, 1))))
-    elif a.save_work:
-        print("work file NOT written: %s: %s" % (a.save_work, s.save_error))
+        print("work file written: %s (%.1f MB in %.2f s, count 2^%.2f)" % (s.save_path, mb, dt_save, np.log2(max(s.jumps, 1))))
+    elif s.save_path:
+        print("work file NOT written: %s: %s" % (s.save_path, s.save_error))
         return 1
     return 0
 
@@ -856,7 +973,7 @@ def table_message(s, a):
     elif s.last_saved:
         msg += (" The last work file written, %s, is a consistent cut from before the table stopped; resume it with "
                 "--dp-table host or a larger --dp-table-capacity" % s.last_saved)
-    elif a.save_work:
+    elif s.save_path:
         msg += " No work file was written."
     elif what == "full":
         msg += " Use --dp-table host or a larger --dp-table-capacity (with --save-work, the run writes a resumable file first)."
@@ -884,6 +1001,53 @@ def _resume_header(path):
     return hdr
 
 
+def batch_resume_file(path):
+    """--batch-resume: rank 0 reads the file's header and batch block and sends every rank (dp, start, end, block) with the
+    block's targets left on rank 0, or the reason the file cannot be resumed (a string)"""
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    res = None
+    if int(os.environ.get("RANK", "0")) == 0:
+        from .ingest import read_work_header
+        from .worktool import read_batch
+        try:
+            h = read_work_header(path)
+            block = read_batch(path)
+            if block is None:
+                res = ("%s is a plain HEADW work file (no batch block): resume it with --resume, without --batch-keys" % path)
+            else:
+                res = (h.dp_bits, h.range_start, h.range_end, block)
+        except (OSError, RuntimeError, ValueError) as e:
+            res = "cannot resume %s: %s" % (path, e)
+    if world > 1:
+        import torch
+        import torch.distributed as dist
+        from .worktool import BatchBlock
+        local = int(os.environ.get("LOCAL_RANK", "0"))
+        torch.cuda.set_device(local)
+        if not dist.is_initialized():
+            dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+        box = [res if isinstance(res, str) or res is None else
+               res[:3] + (BatchBlock(res[3].pubs, res[3].solved, res[3].privs, np.zeros(0, np.uint16), res[3].offset),)]
+        dist.broadcast_object_list(box, 0)
+        if int(os.environ.get("RANK", "0")) != 0:
+            res = box[0]
+    return res
+
+
+def config_difference(start, end, pubs, f_start, f_end, f_pubs):
+    """the first difference between a config (range, keys in order) and a batch work file's, or None"""
+    if start != f_start:
+        return "the config's range start 0x%X is not the file's 0x%X" % (start, f_start)
+    if end != f_end:
+        return "the config's range end 0x%X is not the file's 0x%X" % (end, f_end)
+    for i, (p, q) in enumerate(zip(pubs, f_pubs)):
+        if p != q:
+            return "key #%d differs: the config has 04%064X%064X, the file 04%064X%064X" % (i, p[0], p[1], q[0], q[1])
+    if len(pubs) != len(f_pubs):
+        return "the config lists %d keys, the file %d" % (len(pubs), len(f_pubs))
+    return None
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("config", nargs="?", help="range start, end and public keys (optional with --resume)")
@@ -908,17 +1072,41 @@ def main(argv=None):
     ap.add_argument("--batch-keys", action="store_true",
                     help="solve every key of the config in one run: one tame herd and one DP table shared by all keys, the "
                          "wild kangaroos spread over the unsolved ones")
+    ap.add_argument("--batch-save", default="", metavar="FILE",
+                    help="--batch-keys only: write a batch work file (a HEADW work file with every rank's herd, then every key, "
+                         "its solved flag and every kangaroo's target key) at the end, and with --batch-save-interval while running")
+    ap.add_argument("--batch-save-interval", type=float, default=0.0, metavar="SECS",
+                    help="also save every SECS seconds (0 = at the end only)")
+    ap.add_argument("--batch-resume", default="", metavar="FILE",
+                    help="--batch-keys only: continue a batch run from FILE; the keys, range and dp come from the file (a config, "
+                         "if given, must list the same range and keys in the same order)")
     a = ap.parse_args(argv)
     if a.batch_keys and (a.resume or a.save_work or a.save_interval or a.save_kangaroos):
         ap.error("--batch-keys cannot be combined with --save-work, --save-interval, --save-kangaroos or --resume "
                  "(a work file carries one key)")
-    if a.batch_keys and not a.config:
+    if (a.batch_save or a.batch_save_interval or a.batch_resume) and not a.batch_keys:
+        ap.error("--batch-save, --batch-save-interval and --batch-resume need --batch-keys")
+    if a.batch_save_interval and not a.batch_save:
+        ap.error("--batch-save-interval needs --batch-save FILE")
+    if a.batch_keys and not a.config and not a.batch_resume:
         ap.error("--batch-keys needs a config file")
     if a.dp_table_capacity is not None and a.dp_table != "device":
         ap.error("--dp-table-capacity needs --dp-table device")
     if a.dp_table_capacity is not None and not 0 < a.dp_table_capacity < (1 << 32) - 1:
         ap.error("--dp-table-capacity must be 1 .. 2^32-2 entries, not %d" % a.dp_table_capacity)
-    if a.resume:
+    block = None
+    if a.batch_resume:
+        res = batch_resume_file(a.batch_resume)
+        if isinstance(res, str):
+            ap.error("--batch-resume: " + res)
+        file_dp, start, end, block = res
+        pubs = block.pubs
+        if a.config:
+            diff = config_difference(*ec.parse_config(a.config), start, end, pubs)
+            if diff:
+                ap.error("--batch-resume: the config does not match %s: %s" % (a.batch_resume, diff))
+        dp = a.dp if a.dp is not None else file_dp
+    elif a.resume:
         file_dp, start, end, pub = _resume_header(a.resume)
         pubs = [pub]
         if a.config:
@@ -936,7 +1124,7 @@ def main(argv=None):
     if a.batch_keys and len(pubs) > MAX_KEYS:
         ap.error("--batch-keys takes at most %d keys, the config has %d" % (MAX_KEYS, len(pubs)))
     grid = tuple(int(v) for v in a.grid.split(",")) if a.grid else None
-    rc = _run_batch(start, end, pubs, dp, grid, a) if a.batch_keys else 0
+    rc = _run_batch(start, end, pubs, dp, grid, a, block) if a.batch_keys else 0
     for i, pub in enumerate([] if a.batch_keys else pubs):
         s = Solver(start, end, pub, dp, grid, seed=a.seed, ingest_threads=a.ingest_threads, save_work=a.save_work,
                    save_interval=a.save_interval, save_kangaroos=a.save_kangaroos, resume=a.resume or None, dp_table=a.dp_table,

@@ -5,11 +5,16 @@
     python -m kangaroo_b200.worktool merge --dir DIR -o DEST [--device N]
 
 `check` recomputes every stored DP (d*G, or key - start*G + d*G for a wild one) and every kangaroo on the GPU
-(libkgx.so, kgx_work_check) and exits 1 when anything is wrong.  `merge` combines files of the same key and range in the order
+(libkgx.so, kgx_work_check) and exits 1 when anything is wrong.  It also takes the solver's batch work files (--batch-keys
+--batch-save): every kangaroo is checked against its own target key, every wild DP against all keys of the file.  `merge` combines files of the same key and range in the order
 given (the entry of the earlier file wins at equal x) with kgx_work_merge, resolves every tame/wild collision with the
 solver's resolver (the reference's CheckKey, build/libkgx_ingest.so), and either prints the key and writes nothing, or writes
 DEST through DEST.tmp, fsync and rename.  The merged file ends with a kangaroo count of 0, so the solver's --resume and the
-reference's -i take it; they start fresh herds.  There is no CPU path: without a device both commands fail."""
+reference's -i take it; they start fresh herds.  Batch work files are not merged.  There is no CPU path: without a device both
+commands fail.
+
+The batch block of a batch work file (its layout: kgx_workfile.h) is written and read here, through libkgx.so's
+kgx_batch_block / kgx_batch_read, which the device check uses too; neither needs a device."""
 import argparse
 import ctypes
 import math
@@ -17,11 +22,14 @@ import os
 import struct
 import sys
 
+import numpy as np
+
 from . import ecmath as ec
 from ._lib import load_library
 from .ingest import _limbs4, read_work_header
 
 HEADW = 0xFA6A8001
+_u64p = ctypes.POINTER(ctypes.c_uint64)
 TYPE_BIT = 1 << 126                    # b126 of a tagged distance: the herd (HashTable::CalcDistAndType)
 
 
@@ -30,7 +38,7 @@ class CheckInfo(ctypes.Structure):
     _fields_ = [("dp_bits", ctypes.c_uint32), ("has_walk_count", ctypes.c_uint32), ("entries", ctypes.c_uint64),
                 ("wrong_entries", ctypes.c_uint64), ("walks", ctypes.c_uint64), ("walks_tame", ctypes.c_uint64),
                 ("walks_wild", ctypes.c_uint64), ("wrong_walks", ctypes.c_uint64), ("n_wrong_entries_listed", ctypes.c_uint32),
-                ("n_wrong_walks_listed", ctypes.c_uint32)]
+                ("n_wrong_walks_listed", ctypes.c_uint32), ("n_keys", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
 
 
 class MergeInfo(ctypes.Structure):
@@ -57,6 +65,70 @@ def is_work_file(path):
     with open(path, "rb") as f:
         raw = f.read(4)
     return len(raw) == 4 and struct.unpack("<I", raw)[0] == HEADW
+
+
+class BatchBlock:
+    """The batch block of a batch work file: pubs [(x, y)] in input order, solved (bool per key), privs (int, or None when
+    unsolved), targets (uint16 per kangaroo, file order), offset (byte where the block starts = where the records end)."""
+
+    def __init__(self, pubs, solved, privs, targets, offset=0):
+        self.pubs, self.solved, self.privs, self.offset = list(pubs), [bool(v) for v in solved], list(privs), int(offset)
+        self.targets = np.ascontiguousarray(targets, dtype=np.uint16)
+
+    @property
+    def n_keys(self):
+        return len(self.pubs)
+
+    @property
+    def nb_walk(self):
+        return int(self.targets.size)
+
+
+def _limbs(vals, n):
+    return np.array([[(int(v) >> (64 * k)) & 0xFFFFFFFFFFFFFFFF for k in range(n)] for v in vals], dtype=np.uint64).reshape(len(vals), n)
+
+
+def _val(row):
+    return sum(int(v) << (64 * k) for k, v in enumerate(row))
+
+
+def batch_block(block, offset):
+    """kgx_batch_block: the bytes that follow the kangaroo records of a batch work file whose records end at byte `offset`"""
+    lib = load_library()
+    n = block.n_keys
+    keys = np.ascontiguousarray(np.hstack([_limbs([p[0] for p in block.pubs], 4), _limbs([p[1] for p in block.pubs], 4)]))
+    privs = np.ascontiguousarray(_limbs([(p or 0) if s else 0 for p, s in zip(block.privs, block.solved)], 4))
+    solved = np.ascontiguousarray(block.solved, dtype=np.uint8)
+    out = np.empty(int(lib.kgx_batch_block_bytes(n, block.nb_walk)), dtype=np.uint8)
+    rc = lib.kgx_batch_block(keys.ctypes.data_as(_u64p), solved.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8)), privs.ctypes.data_as(_u64p), n,
+                             block.targets.ctypes.data_as(ctypes.POINTER(ctypes.c_uint16)), block.nb_walk, int(offset),
+                             out.ctypes.data_as(ctypes.c_void_p))
+    if rc != 0:
+        raise ValueError(_err(lib))
+    return out
+
+
+def read_batch(path):
+    """kgx_batch_read -> BatchBlock, or None for a plain HEADW file.  Not a HEADW file, or a batch block cut short or damaged:
+    ValueError; a file that cannot be opened: OSError."""
+    lib = load_library()
+    nk, nw, off = ctypes.c_uint32(0), ctypes.c_uint64(0), ctypes.c_uint64(0)
+    rc = lib.kgx_batch_read(os.fsencode(path), ctypes.byref(nk), ctypes.byref(nw), ctypes.byref(off), None, None, None, None)
+    if rc == 0:
+        return None
+    if rc == 1:
+        n = nk.value
+        keys, privs = np.zeros((n, 8), dtype=np.uint64), np.zeros((n, 4), dtype=np.uint64)
+        solved, targets = np.zeros(n, dtype=np.uint8), np.zeros(nw.value, dtype=np.uint16)
+        rc = lib.kgx_batch_read(os.fsencode(path), ctypes.byref(nk), ctypes.byref(nw), ctypes.byref(off), keys.ctypes.data_as(_u64p),
+                                solved.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8)), privs.ctypes.data_as(_u64p),
+                                targets.ctypes.data_as(ctypes.POINTER(ctypes.c_uint16)))
+        if rc == 1:
+            return BatchBlock([(_val(k[:4]), _val(k[4:])) for k in keys], solved, [_val(p) if s else None for p, s in zip(privs, solved)],
+                              targets, off.value)
+    if rc == -1:
+        raise ValueError(_err(lib))
+    raise OSError(-rc, "%s: %s" % (path, os.strerror(-rc)))
 
 
 class CheckResult:
@@ -91,7 +163,6 @@ def check(path, device=0, chunk=0, cap=16):
 def check_records(kind, recs, hs, key, range_start, device=0):
     """kgx_work_check_records: kind 0 = (n, 4) uint64 table entries with their buckets hs, kind 1 = (n, 12) uint64 kangaroo
     records -> per-record uint8 results (entries: 1 = wrong; kangaroos: 0 wrong, 1 tame, 2 wild)"""
-    import numpy as np
     recs = np.ascontiguousarray(recs, dtype=np.uint64)
     n = recs.shape[0]
     out = np.zeros(n, dtype=np.uint8)
@@ -231,6 +302,8 @@ def main(argv=None):
             r = check(a.file, device=a.device)
             pct = 100.0 * (1.0 - r.wrong_entries / r.entries) if r.entries else 100.0
             print("[%.3f%% OK]" % pct)
+            if r.n_keys:
+                print("Batch work file: %d keys (every kangaroo checked against its own target key)" % r.n_keys)
             print("DP: %d" % r.entries)
             print("DP Wrong: %d" % r.wrong_entries)
             for h, i in r.wrong_entry_positions:
