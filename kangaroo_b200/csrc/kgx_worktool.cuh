@@ -209,8 +209,10 @@ __global__ void wt_on_curve_kernel(const u32* keys, uint32_t n, int* ok) {
 
 // Table entries of a batch file: as wt_check_entries_kernel, one entry per thread, but a wild entry is OK when S = +-|d|*G
 // plus any of the n_keys keys K (16 words each; kinfs[k]: K is the point at infinity, then S itself) passes the test.  S is
-// made affine once; then every key costs one affine addition, whose inverses are batched over KB keys at a time (a key
-// with K = +-S counts as no match).  The scan stops at the first key that matches.
+// made affine once; then every key costs one affine addition, whose inverses are batched over KB keys at a time.  The group
+// law is followed as in wt_check_entries_kernel: S at infinity (|d| = 0) gives K itself; K = S is a doubling, whose slope
+// 3 x_S^2 / 2 y_S takes the key's place in the batched inverse; K = -S gives infinity, no match (its factor is 1, so that
+// it leaves the other keys' inverses intact).  The scan stops at the first key that matches.
 constexpr int KB = 8;
 __global__ void __launch_bounds__(CHECK_THREADS) wt_check_entries_multi_kernel(const u32* __restrict__ comb, const Entry* __restrict__ ent,
                                                                               const uint32_t* __restrict__ hs, uint64_t n,
@@ -229,7 +231,11 @@ __global__ void __launch_bounds__(CHECK_THREADS) wt_check_entries_multi_kernel(c
   u32 X[8], Y[8], Z[8];
   bool f, ok = false;
   wt_comb_mul(sc, m, X, Y, Z, f);
-  if (!f) {
+  if (f && wild) {                                  // S at infinity: S + K = K
+#pragma unroll 1
+    for (uint32_t k = 0; k < n_keys && !ok; k++)
+      if (!kinfs[k]) { u32 x[8]; fe_copy(x, K + 16 * k); ok = match(x); }
+  } else if (!f) {
     u32 zi[8], z2[8];
     modinv256(zi, Z);
     fe_sqr(z2, zi);
@@ -244,19 +250,27 @@ __global__ void __launch_bounds__(CHECK_THREADS) wt_check_entries_multi_kernel(c
       fe_copy(x, X);
       ok = match(x);
     } else {
+      // key k's factor in the batched inverse -> 0: no addition (a missing key, K at infinity or K = -S; factor 1),
+      // 1: an addition (x_K - x_S), 2: a doubling, K = S (2 y_S)
+      auto factor = [&](uint32_t k, u32* dx) -> int {
+        fe_set_one(dx);
+        if (k >= n_keys || kinfs[k]) return 0;
+        fe_sub(dx, K + 16 * k, X);
+        if (!fe_is_zero_modp(dx)) return 1;
+        u32 dy[8];
+        fe_sub(dy, K + 16 * k + 8, Y);
+        if (fe_is_zero_modp(dy)) { fe_dbl(dx, Y); return 2; }
+        fe_set_one(dx);
+        return 0;
+      };
 #pragma unroll 1
       for (uint32_t k0 = 0; k0 < n_keys && !ok; k0 += KB) {
         u32 acc[KB][8], run[8];
         fe_set_one(run);
 #pragma unroll
-        for (int j = 0; j < KB; j++) {            // prefix products of x_K - x_S (1 in place of a zero or a missing key)
+        for (int j = 0; j < KB; j++) {            // prefix products of the factors
           u32 dx[8];
-          const uint32_t k = k0 + j;
-          fe_set_one(dx);
-          if (k < n_keys && !kinfs[k]) {
-            fe_sub(dx, K + 16 * k, X);
-            if (fe_is_zero_modp(dx)) fe_set_one(dx);
-          }
+          factor(k0 + j, dx);
           fe_mul(run, run, dx);
           fe_copy(acc[j], run);
         }
@@ -266,19 +280,19 @@ __global__ void __launch_bounds__(CHECK_THREADS) wt_check_entries_multi_kernel(c
         for (int j = KB - 1; j >= 0; j--) {
           const uint32_t k = k0 + j;
           u32 dx[8], di[8];
-          fe_set_one(dx);
-          bool use = false;
-          if (k < n_keys && !kinfs[k]) {
-            fe_sub(dx, K + 16 * k, X);
-            use = !fe_is_zero_modp(dx);
-            if (!use) fe_set_one(dx);
-          }
+          const int add = factor(k, dx);
           if (j > 0) fe_mul(di, inv, acc[j - 1]); else fe_copy(di, inv);   // 1 / dx
           fe_mul(inv, inv, dx);
           if (k < n_keys && kinfs[k]) { u32 x[8]; fe_copy(x, X); ok = ok || match(x); }
-          if (!use) continue;
+          if (!add) continue;
           u32 lam[8], x3[8], t[8];
-          fe_sub(lam, K + 16 * k + 8, Y);
+          if (add == 2) {                                 // 3 x_S^2
+            u32 ng[8];
+            fe_sqr(t, X);
+            fe_dbl(lam, t); fe_neg(ng, t); fe_sub(lam, lam, ng);
+          } else {
+            fe_sub(lam, K + 16 * k + 8, Y);
+          }
           fe_mul(lam, lam, di);
           fe_sqr(x3, lam);
           fe_sub(x3, x3, X);
@@ -678,7 +692,7 @@ int kgx_work_check(int dev, const char* path, uint64_t chunk, kgx_work_check_inf
       first += k;
     }
   }
-  if (drain(0) || drain(1)) return -3;
+  if (drain(cur) || drain(cur ^ 1)) return -3;         // the older chunk first: wrong records are listed in file order
   info->n_wrong_entries_listed = nwe;
   info->n_wrong_walks_listed = nww;
   return 0;
