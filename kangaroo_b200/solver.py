@@ -726,6 +726,15 @@ def key_classes(keys):
     return rep, neg
 
 
+def class_members(rep):
+    """the keys of every class, from key_classes' rep -> {first key of the class: [its keys in input order]}; built once, so
+    that claiming a class visits its own keys and not every key of the input"""
+    members = {}
+    for i, r in enumerate(rep):
+        members.setdefault(r, []).append(i)
+    return members
+
+
 def class_privs(start, priv_rep, neg):
     """the private key of a key of the class solved with priv_rep: keyToSearch = priv - start*G, so the negative of a key
     has priv 2*start - priv_rep"""
@@ -754,6 +763,7 @@ class BatchSolver(Solver):
         # a key listed twice, or the negative of another, is searched once, as the first of its class: kgi_resolve_multi
         # reports the first matching key, so the later ones would never be hit
         self.rep, self.neg = key_classes(self.keys)
+        self.members = class_members(self.rep)
         self.announced = set()              # every rank: classes (their first key) announced solved, those of the file included
         self._resume_block = resume_block
         if resume_block is not None:
@@ -877,9 +887,8 @@ class BatchSolver(Solver):
             r = self.rep[idx]
             if self.priv[r] is None:
                 self.priv[r] = class_privs(self.start, priv, self.neg[idx])
-                for i in range(len(self.keys)):                 # the other keys of its class
-                    if self.rep[i] == r:
-                        self.priv[i] = class_privs(self.start, self.priv[r], self.neg[i])
+                for i in self.members[r]:                       # the other keys of its class
+                    self.priv[i] = class_privs(self.start, self.priv[r], self.neg[i])
                 self._announce.append(r)
             else:
                 resets.append((rk, kidx))

@@ -120,6 +120,48 @@ def test_truncated_or_damaged_batch_block_is_refused(tmp_path):
         batch_block(BatchBlock(PUBS[:2], [False, False], [None, None], [0, 2]), 0)
 
 
+def test_batch_block_round_trip_at_65535_keys(tmp_path):
+    """The key limit: 65535 keys with solved flags and private keys at the high indices, an odd number of kangaroos (the
+    targets' padding) whose targets cover every key 0..65534, byte patterns that a byte swap or a truncation to 8 bits changes.
+    The reader does not check the records or the points, so both are plain patterns here."""
+    n_keys, nb_walk = 65535, 2 * 65535 + 3
+    rng = np.random.default_rng(12)
+    pubs = [(int(a) | (1 << 200), int(b) << 3) for a, b in zip(rng.integers(1, 1 << 62, size=n_keys), rng.integers(1, 1 << 62, size=n_keys))]
+    hi = [255, 256, 257, 511, 512, 4095, 4096, 65279, 65280, 65528, 65533, 65534]
+    solved = [i in hi or i % 997 == 3 for i in range(n_keys)]
+    privs = [(0xA5 << 248) | (i << 16) | 0x5A if s else None for i, s in enumerate(solved)]
+    targets = np.empty(nb_walk, dtype=np.uint16)
+    targets[0::2] = rng.integers(0, n_keys, size=(nb_walk + 1) // 2)
+    targets[1:2 * n_keys:2] = np.arange(n_keys)                           # every key is some wild's target
+    targets[-2:] = [0x0100, 65534]
+    plain = headw(START, END, PUBS[0], [(i, ~i & 0xFFFF, i) for i in range(nb_walk)])
+    block = batch_block(BatchBlock(pubs, solved, privs, targets), len(plain)).tobytes()
+    pad = 8 - (2 * nb_walk) % 8
+    assert pad == 6 and len(block) == 24 + n_keys * 104 + 2 * nb_walk + pad + 16
+    assert block[24 + n_keys * 104 + 2 * nb_walk:][:pad] == b"\0" * pad
+    path = tmp_path / "max.work"
+    path.write_bytes(plain + block)
+    got = read_batch(str(path))
+    assert got.n_keys == n_keys and got.nb_walk == nb_walk and got.offset == len(plain)
+    assert got.pubs == pubs and got.solved == solved and got.privs == privs
+    assert np.array_equal(got.targets, targets) and set(np.unique(got.targets).tolist()) == set(range(n_keys))
+    for i in hi:
+        assert got.privs[i] == (0xA5 << 248) | (i << 16) | 0x5A and got.pubs[i] == pubs[i]
+
+    # the block of 65536 keys, with every size consistent (the footer, the targets): the reader refuses it on the key count
+    raw = plain + block
+    at = len(plain) + 24 + n_keys * 104
+    big = bytearray(raw[:at] + raw[at - 104:at] + raw[at:])
+    big[len(plain) + 8:len(plain) + 12] = struct.pack("<I", n_keys + 1)
+    assert len(big) - len(plain) == 24 + (n_keys + 1) * 104 + 2 * nb_walk + pad + 16
+    p = tmp_path / "over.work"
+    p.write_bytes(bytes(big))
+    with pytest.raises(ValueError, match="65536 keys"):
+        read_batch(str(p))
+    with pytest.raises(ValueError, match="n_keys must be in \\[1, 65535\\]"):
+        batch_block(BatchBlock(pubs + [pubs[0]], solved + [False], privs + [None], targets), len(plain))
+
+
 # ---- flags ---------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("extra", [["--batch-save", "w.work"], ["--batch-save-interval", "5"], ["--batch-resume", "w.work"]])
 def test_batch_flags_need_batch_keys(extra, capsys):

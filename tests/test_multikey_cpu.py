@@ -59,6 +59,44 @@ def test_equal_and_opposite_keys_share_one_search():
             assert class_privs(start, privs[rep[i]], neg[i]) == privs[i]
 
 
+def test_class_members_claim_the_same_keys_as_a_scan_at_65535_keys():
+    """BatchSolver._claim gives every key of a solved class its private key through class_members, built once, in place of a
+    scan over all keys per class.  At 65535 keys, with keys listed twice, three times and negated mixed in (points stand in as
+    (x, y) pairs: key_classes looks only at x and y), both give the same private keys for every class."""
+    from kangaroo_b200.solver import BatchSolver, class_members
+    n, p = 65535, ec.P
+    rng = np.random.default_rng(11)
+    xs = [int(v) for v in rng.integers(1, 1 << 62, size=n)]
+    keys = [(x, x + 1) for x in xs]
+    for i in range(300, n, 257):                                         # a copy of an earlier key, or its negative
+        j = int(rng.integers(0, i))
+        keys[i] = keys[j] if i % 2 else (keys[j][0], p - keys[j][1])
+    keys[n - 1] = keys[n - 2] = (keys[5][0], p - keys[5][1])             # one class across the whole input
+    keys[4000] = None                                                     # the point at infinity: a class of its own
+    rep, neg = key_classes(keys)
+    members = class_members(rep)
+    assert sorted(i for m in members.values() for i in m) == list(range(n))
+    assert all(rep[i] == r for r, m in members.items() for i in m) and all(m == sorted(m) for m in members.values())
+    multi = [r for r, m in members.items() if len(m) > 1]
+    assert len(multi) > 100 and any(neg[i] for r in multi for i in members[r]) and members[5] == [5, n - 2, n - 1]
+
+    start = 0x3447F65ABC9F46F736A95F87B044829C8A0129D56782D635CD00000000000000
+    s = BatchSolver.__new__(BatchSolver)                                 # _claim's state only: no engine
+    s.start, s.rep, s.neg, s.members = start, rep, neg, members
+    s.priv, s._announce = [None] * n, []
+    hits = [(i, start + 1000 + i, 0, 2 * i + 1) for i in range(n)]       # a hit on every key, its class solved by the first
+    resets = []
+    s._claim(hits, resets)
+    assert s._announce == sorted(members) and len(resets) == n - len(members)
+    scan, rep_a = [None] * n, np.asarray(rep)                            # the scan over all keys, per class
+    for r in multi + [int(v) for v in rng.choice(sorted(members), 40, replace=False)]:
+        scan[r] = start + 1000 + r
+        for i in np.flatnonzero(rep_a == r).tolist():
+            scan[i] = class_privs(start, scan[r], neg[i])
+        assert [s.priv[i] for i in members[r]] == [scan[i] for i in members[r]], r
+    assert s.priv[n - 1] == (2 * start - (start + 1005)) % ec.N
+
+
 def test_wilds_are_spread_evenly_over_the_live_keys():
     for n, live in [(2 * 4096, list(range(64))), (12288, [0, 3, 4, 9, 10]), (1000, [7]), (130, list(range(100)))]:
         t = assign_targets(n, live)
