@@ -231,7 +231,7 @@ int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, u
  *     time, the merged table (maxItem = nbItem rounded up to 4), then a kangaroo count of 0.  Inputs without a kangaroo count
  *     are accepted.  The inputs stream through the device in blocks of whole buckets of at most block_entries entries over
  *     all inputs (0 = 2^22); a bucket larger than that is refused and tmp_path removed.  The first `cap` collisions, ordered by
- *     bucket then x, go to coll.  A batch work file (kgx_workfile.h) is refused.
+ *     bucket then x, go to coll.  A batch work file (kgx_workfile.h) is refused: kgx_work_merge_batch merges those.
  * A batch work file (_check reads it too: each kangaroo against its own target key K_t = keys[t] - start*G, each wild table
  *     entry accepted when it matches any key of the block, info->n_keys = the block's keys):
  * _batch_block_bytes / _batch_block: the block that follows the records of a file with nb_walk kangaroos whose records end
@@ -272,6 +272,37 @@ int kgx_batch_block(const uint64_t* keys, const uint8_t* solved, const uint64_t*
                     uint64_t nb_walk, uint64_t offset, void* out);
 int kgx_batch_read(const char* path, uint32_t* n_keys, uint64_t* nb_walk, uint64_t* offset, uint64_t* keys, uint8_t* solved,
                    uint64_t* privs, uint16_t* targets);
+/* --- merging batch work files: kgx_work_merge for files of many keys, every tame/wild collision resolved on the device.
+ * _merge_batch: n_paths >= 2 batch work files of the same range, version and key list (same keys in the same order).  Refused
+ *     before anything is written (-1, reason in kgx_work_last_error()): a plain HEADW file among them, another key count or
+ *     order, another range or version, a range start not below the group order n, a key off the curve, a recorded private key
+ *     that is not below n or does not give its public key, two inputs recording different private keys for one key, more keys
+ *     than cap_keys.  The table is merged as kgx_work_merge merges the same files without their batch blocks (same blocks, same
+ *     bytes; no collision is listed: info->n_listed = 0), and every collision of a block is resolved on the device before the
+ *     next block, as kgi_resolve_multi resolves it against the keys K = key - start*G: the first key in input order that
+ *     +-Td +-Wd * G hits.  In bucket then x order, a collision on a key not yet solved solves it and the keys listed before as
+ *     the same point or its negative (the solver's classes: priv, or 2*start - priv for the negative); one on a key solved in an
+ *     input or earlier in the merge changes nothing.  tmp_path gets the merged table, a kangaroo count of 0 and a batch block
+ *     with every key, no kangaroo, solved = solved in an input or by the merge, privs as recorded or found.  binfo: the counts;
+ *     keys[k] (n_keys entries): status 0 = unsolved, 1 = solved in an input (priv recorded), 2 = solved by this merge (priv, and
+ *     h, d_first, d_other of the collision that solved its class).
+ * _resolve: the merge's resolver on n collisions in host memory (d_first, d_other: n x 2 limbs of tagged distances) against
+ *     n_keys (1..KGX_MAX_KEYS) keys K (n_keys x 8 limbs, keyToSearch = key - start*G, the point at infinity as (0, 0)) and a
+ *     range start below n: key_out[i] = kgi_resolve_multi's key index for collision i, or 0xFFFFFFFF when it gives none (same
+ *     herd included), priv_out (n x 4 limbs) = its private key (0 with no key). --- */
+typedef struct {
+  uint32_t n_keys, solved_in_inputs, solved_by_merge, left;
+  uint64_t same_herd, no_key, already_solved, solving;   /* collisions by outcome; they sum to info->collisions */
+} kgx_batch_merge_info;
+typedef struct {
+  uint32_t status, h;
+  uint64_t priv[4];
+  uint64_t d_first[2], d_other[2];
+} kgx_batch_key_result;
+int kgx_work_merge_batch(int dev, const char* const* paths, uint32_t n_paths, const char* tmp_path, uint64_t block_entries,
+                         kgx_work_merge_info* info, kgx_batch_merge_info* binfo, kgx_batch_key_result* keys, uint32_t cap_keys);
+int kgx_work_resolve(int dev, const uint64_t* d_first, const uint64_t* d_other, uint64_t n, const uint64_t* keys, uint32_t n_keys,
+                     const uint64_t range_start[4], uint32_t* key_out, uint64_t* priv_out);
 
 /* Debug (KGX_PROF=1 in the environment at kgx_create): phase cycle counters summed over warp 0 of every CTA:
  * out = {serial section, modular inverse alone, parallel phase, tile-steps}; resets them. -1 when disabled. */

@@ -88,6 +88,10 @@ _SIGS = {
     "kgx_work_comb": (ctypes.c_int, [ctypes.c_int, _u64p]),
     "kgx_work_merge": (ctypes.c_int, [ctypes.c_int, ctypes.POINTER(ctypes.c_char_p), ctypes.c_uint32, ctypes.c_char_p, ctypes.c_uint64,
                                       ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32]),
+    "kgx_work_merge_batch": (ctypes.c_int, [ctypes.c_int, ctypes.POINTER(ctypes.c_char_p), ctypes.c_uint32, ctypes.c_char_p, ctypes.c_uint64,
+                                            ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32]),
+    "kgx_work_resolve": (ctypes.c_int, [ctypes.c_int, _u64p, _u64p, ctypes.c_uint64, _u64p, ctypes.c_uint32, _u64p,
+                                        ctypes.POINTER(ctypes.c_uint32), _u64p]),
     "kgx_batch_block_bytes": (ctypes.c_uint64, [ctypes.c_uint32, ctypes.c_uint64]),
     "kgx_batch_block": (ctypes.c_int, [_u64p, ctypes.POINTER(ctypes.c_uint8), _u64p, ctypes.c_uint32, _u16p, ctypes.c_uint64, ctypes.c_uint64,
                                        ctypes.c_void_p]),

@@ -125,7 +125,7 @@ __host__ __device__ __forceinline__ u64 sub256(u64* r, const u64* a, const u64* 
   return br;
 }
 // r = a + b (mod 2^256); returns the carry
-__device__ __forceinline__ u64 add256(u64* r, const u64* a, const u64* b) {
+__host__ __device__ __forceinline__ u64 add256(u64* r, const u64* a, const u64* b) {
   u64 c = 0;
 #pragma unroll
   for (int k = 0; k < 4; k++) {

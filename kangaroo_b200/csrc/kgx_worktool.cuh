@@ -15,7 +15,8 @@
 // equal keys; one scan keeps the first entry of every run of equal (h, x) -- the earliest input's, as the reference's
 // pairwise merges do -- and classifies each later one against it: equal tagged d = a duplicate ("Dead kangaroo"), else a
 // collision returned to the host.  The kept entries are compacted, counted per bucket and written with maxItem = nbItem
-// rounded up to a multiple of 4 (HashTable.cpp:204-209).  The file format is kgx_workfile.h's, the block sort
+// rounded up to a multiple of 4 (HashTable.cpp:204-209).  Batch work files merge through the same blocks, each block's
+// collisions resolved against every key on the device (wt_resolve_kernel).  The file format is kgx_workfile.h's, the block sort
 // kgx_bucketsort.cuh's (shared with the device table's save) and the group law kgx_curve.cuh's (shared with herd creation).
 #include <vector>
 #include <algorithm>
@@ -330,6 +331,126 @@ __global__ void wt_merge_scan(const Entry* ent, const uint32_t* hs, const uint32
   coll[c] = Coll{h, i, {w.d0, w.d1}, {v.d0, v.d1}};
 }
 
+// ---- batch merge: every tame/wild collision resolved against all keys (kgi_resolve_multi's result, on the device) ----
+// kgi_resolve_multi tries the four candidates +-Td +-Wd of Kangaroo::CheckKey against every key K and its negative and
+// reports the first key in input order that one of them hits.  With t = |Td| and w = |Wd| (both < 2^126) the candidates are
+// +-m1 and +-m2, m1 = t + w and m2 = |t - w| (< 2^127), so the keys hit are those whose x is the x of m1*G or of m2*G, and
+// the sign of y gives s = +-m with s*G = K; the private key is s + start (mod n).  m = 0 gives the point at infinity, which the
+// host stores as (0, 0), as the key table stores a key at infinity; no point of the curve has x = 0, so (0, 0) matches those
+// keys only.
+constexpr uint32_t NO_KEY = 0xFFFFFFFFu;
+struct Hit { uint32_t h, seq, key, reserved; uint64_t priv[4], d_first[2], d_other[2]; };
+struct Start { u64 v[4]; };                            // the range start, below n
+
+__device__ __forceinline__ int wt_cmp8(const u32* a, const u32* b) {
+  for (int w = 7; w >= 0; w--) if (a[w] != b[w]) return a[w] < b[w] ? -1 : 1;
+  return 0;
+}
+
+// The first key (input order) that is (x, y) or its negative -> its index (NO_KEY: none), neg = it is -(x, y).  kx: the
+// n keys' x, 8 words each, ascending, equal x in input order; ki: their indices; K: 16 words per key, by index.
+__device__ uint32_t wt_find_key(const u32* kx, const uint32_t* ki, const u32* K, uint32_t n, const u32* x, const u32* y, bool& neg) {
+  using namespace kgx;
+  uint32_t lo = 0, hi = n;
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (wt_cmp8(kx + 8ull * mid, x) < 0) lo = mid + 1; else hi = mid;
+  }
+  u32 ny[8];
+  fe_neg(ny, y);
+  fe_canon(ny);
+  for (; lo < n && wt_cmp8(kx + 8ull * lo, x) == 0; lo++) {
+    const uint32_t k = ki[lo];
+    if (wt_cmp8(K + 16ull * k + 8, y) == 0) { neg = false; return k; }
+    if (wt_cmp8(K + 16ull * k + 8, ny) == 0) { neg = true; return k; }
+  }
+  return NO_KEY;
+}
+
+// One collision per thread.  out_key / out_priv (optional): every collision's key (NO_KEY: none, same-herd included) and
+// private key.  solved (optional): the merge's classification, cnt = {same herd, no key, key already solved, hit} and every
+// hit on an unsolved key appended to hits.  The two points share one inverse.
+__global__ void __launch_bounds__(CHECK_THREADS) wt_resolve_kernel(const u32* __restrict__ comb, const Coll* __restrict__ coll, uint32_t n,
+                                                                  const u32* __restrict__ kx, const uint32_t* __restrict__ ki,
+                                                                  const u32* __restrict__ K, uint32_t n_keys, Start start,
+                                                                  uint32_t* out_key, u64* out_priv, const uint8_t* solved, ull* cnt,
+                                                                  Hit* hits) {
+  using namespace kgx;
+  __shared__ u32 sc[COMB_WORDS];
+  wt_load_comb(sc, comb);
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const Coll c = coll[i];
+  const u64 M = 0x3FFFFFFFFFFFFFFFull;
+  const bool cross = ((c.d_first[1] ^ c.d_other[1]) >> 62) & 1;
+  uint32_t key = NO_KEY;
+  u64 priv[4] = {0, 0, 0, 0};
+  if (cross) {                                         // a tame/wild pair
+    const u64 a[2] = {c.d_first[0], c.d_first[1] & M}, b[2] = {c.d_other[0], c.d_other[1] & M};
+    u64 m[2][2];
+    m[0][0] = a[0] + b[0];
+    m[0][1] = a[1] + b[1] + (m[0][0] < a[0]);
+    const bool age = a[1] != b[1] ? a[1] > b[1] : a[0] >= b[0];
+    const u64* p = age ? a : b;
+    const u64* q = age ? b : a;
+    m[1][0] = p[0] - q[0];
+    m[1][1] = p[1] - q[1] - (p[0] < q[0]);
+    u32 X[2][8], Y[2][8], Z[2][8];
+    bool inf[2];
+    for (int j = 0; j < 2; j++) {
+      const u32 mw[4] = {(u32)m[j][0], (u32)(m[j][0] >> 32), (u32)m[j][1], (u32)(m[j][1] >> 32)};
+      wt_comb_mul(sc, mw, X[j], Y[j], Z[j], inf[j]);
+    }
+    u32 zi[2][8], t[8];                                  // 1/Z of each finite point, from one inverse
+    if (!inf[0] && !inf[1]) {
+      fe_mul(t, Z[0], Z[1]);
+      modinv256(t, t);
+      fe_mul(zi[0], t, Z[1]);
+      fe_mul(zi[1], t, Z[0]);
+    } else {
+      for (int j = 0; j < 2; j++) if (!inf[j]) modinv256(zi[j], Z[j]);
+    }
+    bool neg = false;
+    int hit = -1;
+    for (int j = 0; j < 2; j++) {
+      u32 x[8] = {0, 0, 0, 0, 0, 0, 0, 0}, y[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+      if (!inf[j]) {
+        fe_sqr(t, zi[j]);
+        fe_mul(x, X[j], t);
+        fe_mul(t, t, zi[j]);
+        fe_mul(y, Y[j], t);
+        fe_canon(x);
+        fe_canon(y);
+      }
+      bool ng = false;
+      const uint32_t k = wt_find_key(kx, ki, K, n_keys, x, y, ng);
+      if (k < key) { key = k; neg = ng; hit = j; }
+    }
+    if (hit >= 0) {                                      // s = +-m, priv = s + start (mod n)
+      u64 s[4] = {m[hit][0], m[hit][1], 0, 0};
+      if (neg && (s[0] | s[1])) { const u64 nn[4] = {kOrder[0], kOrder[1], kOrder[2], kOrder[3]}; sub256(s, nn, s); }
+      const u64 cy = add256(priv, s, start.v);
+      if (cy || ge_order(priv)) { const u64 nn[4] = {kOrder[0], kOrder[1], kOrder[2], kOrder[3]}; sub256(priv, priv, nn); }
+    }
+  }
+  if (out_key) {
+    out_key[i] = key;
+    for (int w = 0; w < 4; w++) out_priv[4ull * i + w] = priv[w];
+  }
+  if (!solved) return;
+  if (!cross) atomicAdd(&cnt[0], 1ull);
+  else if (key == NO_KEY) atomicAdd(&cnt[1], 1ull);
+  else if (solved[key]) atomicAdd(&cnt[2], 1ull);
+  else {
+    const ull slot = atomicAdd(&cnt[3], 1ull);
+    Hit& o = hits[slot];
+    o.h = c.h; o.seq = c.seq; o.key = key; o.reserved = 0;
+    for (int w = 0; w < 4; w++) o.priv[w] = priv[w];
+    o.d_first[0] = c.d_first[0]; o.d_first[1] = c.d_first[1];
+    o.d_other[0] = c.d_other[0]; o.d_other[1] = c.d_other[1];
+  }
+}
+
 }  // namespace kgx_wt
 
 static char g_wt_err[512] = "";
@@ -479,6 +600,183 @@ static int build_comb(DevBufs& B, u32** comb, cudaStream_t st) {
 }
 
 static unsigned check_blocks(uint64_t n) { return (unsigned)((n + CHECK_THREADS * GROUP - 1) / (CHECK_THREADS * GROUP)); }
+
+// wt_find_key's index of n keys (hk: 16 words per key, x then y, by index): *kx = their x in ascending order, equal x in input
+// order, *ki = the key indices in that order, both on the device; order (host) = the same indices
+static int key_index(DevBufs& B, const std::vector<uint32_t>& hk, uint32_t n, u32** kx, uint32_t** ki, std::vector<uint32_t>& order) {
+  order.resize(n);
+  for (uint32_t k = 0; k < n; k++) order[k] = k;
+  auto less = [&hk](uint32_t a, uint32_t b) {
+    for (int w = 7; w >= 0; w--) if (hk[16ull * a + w] != hk[16ull * b + w]) return hk[16ull * a + w] < hk[16ull * b + w];
+    return false;
+  };
+  std::stable_sort(order.begin(), order.end(), less);
+  std::vector<uint32_t> sx(8ull * n);
+  for (uint32_t j = 0; j < n; j++) memcpy(&sx[8ull * j], &hk[16ull * order[j]], 32);
+  if (B.dev(kx, 32ull * n) || B.dev(ki, 4ull * n)) return -3;
+  WT_CK(cudaMemcpy(*kx, sx.data(), 32ull * n, cudaMemcpyHostToDevice));
+  WT_CK(cudaMemcpy(*ki, order.data(), 4ull * n, cudaMemcpyHostToDevice));
+  return 0;
+}
+
+// (a + b) mod n and (a - b) mod n for a, b < n
+static void add_mod_n(u64* r, const u64* a, const u64* b) {
+  if (kgx::add256(r, a, b) || kgx::ge256(r, kgx::kOrderHost)) kgx::sub256(r, r, kgx::kOrderHost);
+}
+static void sub_mod_n(u64* r, const u64* a, const u64* b) {
+  u64 t[4];
+  if (kgx::sub256(t, a, b)) kgx::add256(t, t, kgx::kOrderHost);
+  memcpy(r, t, 32);
+}
+
+// *bad = the first key k with solved[k] whose priv[k] * G is not its public key (x, y: keys, 8 limbs per key), or -1; herd_kernel
+// makes even slots tame, so the j-th solved key is computed in slot 2j
+static int privs_check(DevBufs& B, const std::vector<uint64_t>& keys, const std::vector<uint8_t>& solved, const std::vector<uint64_t>& privs,
+                       uint32_t n, int64_t* bad) {
+  *bad = -1;
+  std::vector<uint32_t> sel;
+  for (uint32_t k = 0; k < n; k++) if (solved[k]) sel.push_back(k);
+  if (sel.empty()) return 0;
+  const uint64_t m = sel.size();
+  u32 *tab, *scal, *px, *py;
+  if (B.dev(&tab, 256 * 16 * 4) || B.dev(&scal, 64 * m) || B.dev(&px, 64 * m) || B.dev(&py, 64 * m)) return -3;
+  std::vector<uint64_t> hs(8 * m, 0);
+  for (uint64_t j = 0; j < m; j++) memcpy(&hs[8 * j], &privs[4ull * sel[j]], 32);
+  WT_CK(cudaMemcpy(scal, hs.data(), 64 * m, cudaMemcpyHostToDevice));
+  kgx::herd_table_kernel<<<1, 32>>>(tab);
+  kgx::herd_kernel<<<(unsigned)((2 * m + 127) / 128), 128>>>(tab, scal, tab, nullptr, 0, 2 * m, px, py, 0, nullptr);
+  WT_CK(cudaGetLastError());
+  std::vector<uint64_t> hx(8 * m), hy(8 * m);
+  WT_CK(cudaMemcpy(hx.data(), px, 64 * m, cudaMemcpyDeviceToHost));
+  WT_CK(cudaMemcpy(hy.data(), py, 64 * m, cudaMemcpyDeviceToHost));
+  for (uint64_t j = 0; j < m && *bad < 0; j++)
+    if (memcmp(&hx[8 * j], &keys[8ull * sel[j]], 32) || memcmp(&hy[8 * j], &keys[8ull * sel[j] + 4], 32)) *bad = sel[j];
+  return 0;
+}
+
+// The merge proper, after every input was checked (fs: the inputs, positioned after their headers hd): writes tmp_path (the
+// header, the merged table, a kangaroo count of 0, then whatever tail(out) writes) and fills info but n_listed.  on_coll(n, dColl)
+// gets each block's n > 0 collisions on the device (legacy default stream), before the next block is read; its nonzero
+// result ends the merge with that code.  On failure tmp_path is removed.
+template <class OnColl, class Tail>
+static int merge_stream(DevBufs& B, std::vector<FILE*>& fs, const char* const* paths, const std::vector<kgx_wf::WorkHeader>& hd,
+                        uint32_t n_paths, const char* tmp_path, uint64_t block_entries, kgx_work_merge_info* info, OnColl on_coll,
+                        Tail tail) {
+  const uint64_t C = block_entries;
+  Entry *hIn, *dIn, *dOut, *hOut;
+  uint32_t *hH, *dH, *idxA, *idxB, *dNsel, *dNb, *hNb;
+  uint64_t *keyA, *keyB;
+  uint8_t* keep;
+  MergeRes* dRes;
+  Coll* dColl;
+  size_t tC = 0;
+  WT_CK(cub::DeviceSelect::Flagged(nullptr, tC, (uint32_t*)nullptr, (uint8_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)C));
+  const size_t tmpBytes = std::max(kgx_wf::bucket_sort_scratch(C), tC);
+  void* dTmp;
+  if (B.host(&hIn, 32 * C) || B.dev(&dIn, 32 * C) || B.dev(&dOut, 32 * C) || B.host(&hOut, 32 * C) || B.host(&hH, 4 * C) ||
+      B.dev(&dH, 4 * C) || B.dev(&idxA, 4 * C) || B.dev(&idxB, 4 * C) || B.dev(&dNsel, 4) || B.dev(&dNb, 4ull * NBUCKET) ||
+      B.host(&hNb, 4ull * NBUCKET) || B.dev(&keyA, 8 * C) || B.dev(&keyB, 8 * C) || B.dev(&keep, C) || B.dev(&dRes, sizeof(MergeRes)) ||
+      B.dev(&dColl, sizeof(Coll) * C) || B.dev(&dTmp, tmpBytes))
+    return -3;
+  errno = 0;
+  FILE* out = fopen(tmp_path, "wb");
+  if (!out) { const int e = kgx_wf::io_error(); snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: Cannot open %s for writing: %s", tmp_path, strerror(-e)); return e; }
+  setvbuf(out, nullptr, _IOFBF, 1 << 22);
+  kgx_wf::WorkHeader oh = hd[0];                      // the first input's range and key, written as version 0
+  oh.count = 0;
+  oh.time = 0;
+  for (uint32_t i = 0; i < n_paths; i++) { oh.dp = std::min(oh.dp, hd[i].dp); oh.count += hd[i].count; oh.time += hd[i].time; }
+  bool okw = kgx_wf::write_header(out, oh);
+  int rc = 0;
+  uint64_t fill = 0;
+  uint32_t b0 = 0;
+  // one block: entries of buckets [b0, b1) in hIn (bucket by bucket, inputs in order within a bucket) -> the merged buckets
+  auto flush = [&](uint32_t b1) -> int {
+    const uint32_t n = (uint32_t)fill, T = 256, G = (n + T - 1) / T;
+    WT_CK(cudaMemsetAsync(dNb, 0, 4ull * (b1 - b0)));
+    if (n) {
+      WT_CK(cudaMemcpyAsync(dIn, hIn, 32ull * n, cudaMemcpyHostToDevice));
+      WT_CK(cudaMemcpyAsync(dH, hH, 4ull * n, cudaMemcpyHostToDevice));
+      WT_CK(cudaMemsetAsync(dRes, 0, sizeof(MergeRes)));
+      uint32_t* ord;                                    // the legacy default stream, as every other call of the merge
+      WT_CK(kgx_wf::bucket_sort(dIn, dH, nullptr, n, b0, b1, idxA, idxB, keyA, keyB, dTmp, tmpBytes, 0, &ord));
+      wt_merge_scan<<<G, T>>>(dIn, dH, ord, n, b0, keep, dNb, dRes, dColl);
+      size_t tb = tmpBytes;
+      WT_CK(cub::DeviceSelect::Flagged(dTmp, tb, ord, keep, idxA, dNsel, (int)n));
+      WT_CK(cudaGetLastError());
+      MergeRes r;
+      uint32_t nk = 0;
+      WT_CK(cudaMemcpy(&r, dRes, sizeof r, cudaMemcpyDeviceToHost));
+      WT_CK(cudaMemcpy(&nk, dNsel, 4, cudaMemcpyDeviceToHost));
+      kgx_wf::bucket_gather<<<(nk + T - 1) / T, T>>>(dIn, idxA, nk, dOut);
+      WT_CK(cudaGetLastError());
+      WT_CK(cudaMemcpy(hOut, dOut, 32ull * nk, cudaMemcpyDeviceToHost));
+      WT_CK(cudaMemcpy(hNb, dNb, 4ull * (b1 - b0), cudaMemcpyDeviceToHost));
+      info->duplicates += r.dup;
+      info->collisions += r.ncoll;
+      if (r.ncoll) {
+        const int e = on_coll((uint32_t)r.ncoll, dColl);
+        if (e) return e;
+      }
+    } else {
+      memset(hNb, 0, 4ull * (b1 - b0));
+    }
+    uint64_t off = 0;
+    for (uint32_t b = b0; okw && b < b1; b++) {
+      const uint32_t nb = hNb[b - b0];
+      okw = kgx_wf::write_bucket(out, nb, (nb + 3) & ~3u, hOut + off);
+      off += nb;
+      info->entries += nb;
+    }
+    info->blocks++;
+    b0 = b1;
+    fill = 0;
+    return 0;
+  };
+  std::vector<uint32_t> nbs(n_paths);
+  for (uint32_t h = 0; rc == 0 && okw && h < NBUCKET; h++) {
+    uint64_t sum = 0;
+    for (uint32_t i = 0; i < n_paths; i++) {
+      uint32_t mx;
+      if (!kgx_wf::read_bucket_head(fs[i], nbs[i], mx)) {
+        snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: the table of %s is cut short", paths[i]);
+        rc = -1;
+        break;
+      }
+      sum += nbs[i];
+    }
+    if (rc) break;
+    if (sum > C) {
+      snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: bucket %u holds %llu entries over the inputs, more than a merge block (%llu)", h,
+               (unsigned long long)sum, (unsigned long long)C);
+      rc = -1;
+      break;
+    }
+    if (fill + sum > C && (rc = flush(h)) != 0) break;
+    for (uint32_t i = 0; i < n_paths && rc == 0; i++) {
+      if (nbs[i] && fread(hIn + fill, 32, nbs[i], fs[i]) != nbs[i]) {
+        snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: the table of %s is cut short", paths[i]);
+        rc = -1;
+      }
+      for (uint32_t q = 0; q < nbs[i]; q++) hH[fill + q] = h;
+      fill += nbs[i];
+    }
+  }
+  if (rc == 0 && okw) rc = flush(NBUCKET);
+  const uint64_t zero = 0;                              // the kangaroo count: 0, so that loaders of -ws files take the result
+  okw = okw && fwrite(&zero, 8, 1, out) == 1;
+  okw = okw && tail(out);
+  okw = fflush(out) == 0 && okw;
+  const int ioerr = kgx_wf::io_error();
+  okw = (fclose(out) == 0) && okw;
+  if (rc == 0 && !okw) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s: %s", tmp_path, strerror(-ioerr)); rc = ioerr; }
+  if (rc) { remove(tmp_path); return rc; }
+  info->dp_bits = oh.dp;
+  info->total_count = oh.count;
+  info->total_time = oh.time;
+  return 0;
+}
+
 
 }  // namespace kgx_wt
 
@@ -735,121 +1033,19 @@ int kgx_work_merge(int dev, const char* const* paths, uint32_t n_paths, const ch
       return -1;
     }
   }
-  const uint64_t C = block_entries;
-  Entry *hIn, *dIn, *dOut, *hOut;
-  uint32_t *hH, *dH, *idxA, *idxB, *dNsel, *dNb, *hNb;
-  uint64_t *keyA, *keyB;
-  uint8_t* keep;
-  MergeRes* dRes;
-  Coll* dColl;
-  size_t tC = 0;
-  WT_CK(cub::DeviceSelect::Flagged(nullptr, tC, (uint32_t*)nullptr, (uint8_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)C));
-  const size_t tmpBytes = std::max(kgx_wf::bucket_sort_scratch(C), tC);
-  void* dTmp;
-  if (B.host(&hIn, 32 * C) || B.dev(&dIn, 32 * C) || B.dev(&dOut, 32 * C) || B.host(&hOut, 32 * C) || B.host(&hH, 4 * C) ||
-      B.dev(&dH, 4 * C) || B.dev(&idxA, 4 * C) || B.dev(&idxB, 4 * C) || B.dev(&dNsel, 4) || B.dev(&dNb, 4ull * NBUCKET) ||
-      B.host(&hNb, 4ull * NBUCKET) || B.dev(&keyA, 8 * C) || B.dev(&keyB, 8 * C) || B.dev(&keep, C) || B.dev(&dRes, sizeof(MergeRes)) ||
-      B.dev(&dColl, sizeof(Coll) * C) || B.dev(&dTmp, tmpBytes))
-    return -3;
   std::vector<Coll> hColl;
-  errno = 0;
-  FILE* out = fopen(tmp_path, "wb");
-  if (!out) { const int e = kgx_wf::io_error(); snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: Cannot open %s for writing: %s", tmp_path, strerror(-e)); return e; }
-  setvbuf(out, nullptr, _IOFBF, 1 << 22);
-  kgx_wf::WorkHeader oh = hd[0];                      // the first input's range and key, written as version 0
-  oh.count = 0;
-  oh.time = 0;
-  for (uint32_t i = 0; i < n_paths; i++) { oh.dp = std::min(oh.dp, hd[i].dp); oh.count += hd[i].count; oh.time += hd[i].time; }
-  bool okw = kgx_wf::write_header(out, oh);
-  int rc = 0;
-  uint64_t fill = 0;
-  uint32_t b0 = 0;
-  // one block: entries of buckets [b0, b1) in hIn (bucket by bucket, inputs in order within a bucket) -> the merged buckets
-  auto flush = [&](uint32_t b1) -> int {
-    const uint32_t n = (uint32_t)fill, T = 256, G = (n + T - 1) / T;
-    WT_CK(cudaMemsetAsync(dNb, 0, 4ull * (b1 - b0)));
-    if (n) {
-      WT_CK(cudaMemcpyAsync(dIn, hIn, 32ull * n, cudaMemcpyHostToDevice));
-      WT_CK(cudaMemcpyAsync(dH, hH, 4ull * n, cudaMemcpyHostToDevice));
-      WT_CK(cudaMemsetAsync(dRes, 0, sizeof(MergeRes)));
-      uint32_t* ord;                                    // the legacy default stream, as every other call of the merge
-      WT_CK(kgx_wf::bucket_sort(dIn, dH, nullptr, n, b0, b1, idxA, idxB, keyA, keyB, dTmp, tmpBytes, 0, &ord));
-      wt_merge_scan<<<G, T>>>(dIn, dH, ord, n, b0, keep, dNb, dRes, dColl);
-      size_t tb = tmpBytes;
-      WT_CK(cub::DeviceSelect::Flagged(dTmp, tb, ord, keep, idxA, dNsel, (int)n));
-      WT_CK(cudaGetLastError());
-      MergeRes r;
-      uint32_t nk = 0;
-      WT_CK(cudaMemcpy(&r, dRes, sizeof r, cudaMemcpyDeviceToHost));
-      WT_CK(cudaMemcpy(&nk, dNsel, 4, cudaMemcpyDeviceToHost));
-      kgx_wf::bucket_gather<<<(nk + T - 1) / T, T>>>(dIn, idxA, nk, dOut);
-      WT_CK(cudaGetLastError());
-      WT_CK(cudaMemcpy(hOut, dOut, 32ull * nk, cudaMemcpyDeviceToHost));
-      WT_CK(cudaMemcpy(hNb, dNb, 4ull * (b1 - b0), cudaMemcpyDeviceToHost));
-      info->duplicates += r.dup;
-      info->collisions += r.ncoll;
-      if (r.ncoll) {
+  const int rc = merge_stream(
+      B, fs, paths, hd, n_paths, tmp_path, block_entries, info,
+      [&](uint32_t n, const Coll* dColl) -> int {
         const size_t c0 = hColl.size();
-        hColl.resize(c0 + r.ncoll);
-        WT_CK(cudaMemcpy(hColl.data() + c0, dColl, sizeof(Coll) * r.ncoll, cudaMemcpyDeviceToHost));
+        hColl.resize(c0 + n);
+        WT_CK(cudaMemcpy(hColl.data() + c0, dColl, sizeof(Coll) * n, cudaMemcpyDeviceToHost));
         std::sort(hColl.begin() + c0, hColl.end(), [](const Coll& a, const Coll& b) { return a.h != b.h ? a.h < b.h : a.seq < b.seq; });
         if (hColl.size() > cap) hColl.resize(cap);
-      }
-    } else {
-      memset(hNb, 0, 4ull * (b1 - b0));
-    }
-    uint64_t off = 0;
-    for (uint32_t b = b0; okw && b < b1; b++) {
-      const uint32_t nb = hNb[b - b0];
-      okw = kgx_wf::write_bucket(out, nb, (nb + 3) & ~3u, hOut + off);
-      off += nb;
-      info->entries += nb;
-    }
-    info->blocks++;
-    b0 = b1;
-    fill = 0;
-    return 0;
-  };
-  std::vector<uint32_t> nbs(n_paths);
-  for (uint32_t h = 0; rc == 0 && okw && h < NBUCKET; h++) {
-    uint64_t sum = 0;
-    for (uint32_t i = 0; i < n_paths; i++) {
-      uint32_t mx;
-      if (!kgx_wf::read_bucket_head(fs[i], nbs[i], mx)) {
-        snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: the table of %s is cut short", paths[i]);
-        rc = -1;
-        break;
-      }
-      sum += nbs[i];
-    }
-    if (rc) break;
-    if (sum > C) {
-      snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: bucket %u holds %llu entries over the inputs, more than a merge block (%llu)", h,
-               (unsigned long long)sum, (unsigned long long)C);
-      rc = -1;
-      break;
-    }
-    if (fill + sum > C && (rc = flush(h)) != 0) break;
-    for (uint32_t i = 0; i < n_paths && rc == 0; i++) {
-      if (nbs[i] && fread(hIn + fill, 32, nbs[i], fs[i]) != nbs[i]) {
-        snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: the table of %s is cut short", paths[i]);
-        rc = -1;
-      }
-      for (uint32_t q = 0; q < nbs[i]; q++) hH[fill + q] = h;
-      fill += nbs[i];
-    }
-  }
-  if (rc == 0 && okw) rc = flush(NBUCKET);
-  const uint64_t zero = 0;                              // the kangaroo count: 0, so that loaders of -ws files take the result
-  okw = okw && fwrite(&zero, 8, 1, out) == 1;
-  okw = fflush(out) == 0 && okw;
-  const int ioerr = kgx_wf::io_error();
-  okw = (fclose(out) == 0) && okw;
-  if (rc == 0 && !okw) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s: %s", tmp_path, strerror(-ioerr)); rc = ioerr; }
-  if (rc) { remove(tmp_path); return rc; }
-  info->dp_bits = oh.dp;
-  info->total_count = oh.count;
-  info->total_time = oh.time;
+        return 0;
+      },
+      [](FILE*) { return true; });
+  if (rc) return rc;
   info->n_listed = (uint32_t)hColl.size();
   for (size_t k = 0; k < hColl.size(); k++) {
     coll[k].h = hColl[k].h;
@@ -886,6 +1082,182 @@ int kgx_batch_read(const char* path, uint32_t* n_keys, uint64_t* nb_walk, uint64
   if (nb_walk) *nb_walk = bi.nb_walk;
   if (offset) *offset = bi.offset;
   return rc;
+}
+
+int kgx_work_resolve(int dev, const uint64_t* d_first, const uint64_t* d_other, uint64_t n, const uint64_t* keys, uint32_t n_keys,
+                     const uint64_t range_start[4], uint32_t* key_out, uint64_t* priv_out) {
+  using namespace kgx_wt;
+  if (n_keys == 0 || n_keys > kgx_wf::BATCH_MAX_KEYS) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_work_resolve: n_keys must be in [1, %u]", kgx_wf::BATCH_MAX_KEYS); return -1; }
+  if (n >= 0x80000000ull) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_work_resolve: %llu collisions (at most 2^31-1)", (unsigned long long)n); return -1; }
+  if (kgx::ge256(range_start, kgx::kOrderHost)) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_work_resolve: the range start is not below n"); return -1; }
+  if (set_device(dev)) return -3;
+  DevBufs B;
+  u32 *comb, *kx, *K;
+  uint32_t *ki, *dKey;
+  std::vector<uint32_t> order, hk(16ull * n_keys);
+  memcpy(hk.data(), keys, 64ull * n_keys);
+  if (build_comb(B, &comb, 0) || key_index(B, hk, n_keys, &kx, &ki, order) || B.dev(&K, 64ull * n_keys)) return -3;
+  WT_CK(cudaMemcpy(K, keys, 64ull * n_keys, cudaMemcpyHostToDevice));
+  if (n == 0) return 0;
+  Coll* dColl;
+  u64* dPriv;
+  if (B.dev(&dColl, sizeof(Coll) * n) || B.dev(&dKey, 4 * n) || B.dev(&dPriv, 32 * n)) return -3;
+  std::vector<Coll> hc(n);
+  for (uint64_t i = 0; i < n; i++) hc[i] = Coll{0, (uint32_t)i, {d_first[2 * i], d_first[2 * i + 1]}, {d_other[2 * i], d_other[2 * i + 1]}};
+  WT_CK(cudaMemcpy(dColl, hc.data(), sizeof(Coll) * n, cudaMemcpyHostToDevice));
+  Start st;
+  memcpy(st.v, range_start, 32);
+  wt_resolve_kernel<<<(unsigned)((n + CHECK_THREADS - 1) / CHECK_THREADS), CHECK_THREADS>>>(comb, dColl, (uint32_t)n, kx, ki, K, n_keys, st, dKey,
+                                                                                           dPriv, nullptr, nullptr, nullptr);
+  WT_CK(cudaGetLastError());
+  WT_CK(cudaMemcpy(key_out, dKey, 4 * n, cudaMemcpyDeviceToHost));
+  WT_CK(cudaMemcpy(priv_out, dPriv, 32 * n, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int kgx_work_merge_batch(int dev, const char* const* paths, uint32_t n_paths, const char* tmp_path, uint64_t block_entries,
+                         kgx_work_merge_info* info, kgx_batch_merge_info* binfo, kgx_batch_key_result* keys_out, uint32_t cap_keys) {
+  using namespace kgx_wt;
+  memset(info, 0, sizeof *info);
+  memset(binfo, 0, sizeof *binfo);
+  if (n_paths < 2) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: at least two work files are needed, %u given", n_paths); return -1; }
+  if (block_entries == 0) block_entries = DEFAULT_BLOCK;
+  if (block_entries >= 0x40000000ull) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_work_merge_batch: block of %llu entries (at most 2^30-1)", (unsigned long long)block_entries); return -1; }
+  if (set_device(dev)) return -3;
+  std::vector<FILE*> fs(n_paths, nullptr);
+  struct Closer { std::vector<FILE*>& v; ~Closer() { for (FILE* f : v) if (f) fclose(f); } } closer{fs};
+  std::vector<kgx_wf::WorkHeader> hd(n_paths);
+  DevBufs B;
+  // every input is checked before anything is written: the HEADW part as kgx_work_merge checks it, then the batch blocks
+  uint32_t n = 0;
+  std::vector<uint64_t> keys, ki, privs, pi;             // the first input's keys; privs: the union of the recorded ones
+  std::vector<uint8_t> solved, si;
+  for (uint32_t i = 0; i < n_paths; i++) {
+    errno = 0;
+    fs[i] = fopen(paths[i], "rb");
+    if (!fs[i]) { const int e = kgx_wf::io_error(); snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", paths[i], strerror(-e)); return e; }
+    setvbuf(fs[i], nullptr, _IOFBF, 1 << 22);
+    if (!kgx_wf::read_header(fs[i], hd[i])) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s is not a HEADW work file", paths[i]); return -1; }
+    uint32_t nk = 0;
+    const int bf = kgx_batch_read(paths[i], &nk, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+    if (bf < 0) return bf;
+    if (bf == 0) {
+      snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s is a plain HEADW work file: batch work files merge only with batch work files", paths[i]);
+      return -1;
+    }
+    if (hd[i].version != hd[0].version) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: cannot merge workfile of different version (%s)", paths[i]); return -1; }
+    if (memcmp(hd[i].rs, hd[0].rs, 32) || memcmp(hd[i].re, hd[0].re, 32)) {
+      snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: File range differs (%s, %s)", paths[0], paths[i]);
+      return -1;
+    }
+    if (i == 0) n = nk;
+    if (nk != n) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s holds %u keys, %s %u: the key lists differ", paths[i], nk, paths[0], n); return -1; }
+    ki.assign(8ull * n, 0); pi.assign(4ull * n, 0); si.assign(n, 0);
+    const int rb = kgx_batch_read(paths[i], nullptr, nullptr, nullptr, ki.data(), si.data(), pi.data(), nullptr);
+    if (rb < 0) return rb;
+    if (i == 0) { keys = ki; privs.assign(4ull * n, 0); solved.assign(n, 0); }
+    for (uint32_t k = 0; k < n; k++) {
+      if (memcmp(&ki[8ull * k], &keys[8ull * k], 64)) {
+        snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: key #%u of %s differs from key #%u of %s: the key lists differ", k, paths[i], k, paths[0]);
+        return -1;
+      }
+      if (!si[k]) continue;
+      if (kgx::ge256(&pi[4ull * k], kgx::kOrderHost)) {
+        snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: the private key of key #%u in %s is not below the group order", k, paths[i]);
+        return -1;
+      }
+      if (solved[k] && memcmp(&pi[4ull * k], &privs[4ull * k], 32)) {
+        snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: two inputs record different private keys for key #%u (%s, %s)", k, paths[i],
+                 paths[0]);
+        return -1;
+      }
+      solved[k] = 1;
+      memcpy(&privs[4ull * k], &pi[4ull * k], 32);
+    }
+  }
+  if (kgx::ge256(hd[0].rs, kgx::kOrderHost)) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: the range start of %s is not below the group order", paths[0]); return -1; }
+  if (n > cap_keys) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_work_merge_batch: %u keys, room for %u results", n, cap_keys); return -1; }
+  int ok = 0;
+  u32* K;
+  int* kinfs;
+  if (keys_setup(B, keys, n, hd[0].rs, 0, &ok, &K, &kinfs)) return -3;
+  if (!ok) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: a key of %s does not lie on elliptic curve", paths[0]); return -1; }
+  int64_t bad = -1;
+  if (privs_check(B, keys, solved, privs, n, &bad)) return -3;
+  if (bad >= 0) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: the private key recorded for key #%lld does not give its public key", (long long)bad); return -1; }
+  // K on the host, its index on the device; keys with the same x (the same point or its negative) form one class
+  std::vector<uint32_t> hk(16ull * n), order, pos(n);
+  WT_CK(cudaMemcpy(hk.data(), K, 64ull * n, cudaMemcpyDeviceToHost));
+  u32* kx;
+  uint32_t* kidx;
+  if (key_index(B, hk, n, &kx, &kidx, order)) return -3;
+  for (uint32_t j = 0; j < n; j++) pos[order[j]] = j;
+  std::vector<kgx_batch_key_result> res(n);
+  memset(res.data(), 0, sizeof(kgx_batch_key_result) * n);
+  for (uint32_t k = 0; k < n; k++)
+    if (solved[k]) { res[k].status = 1; memcpy(res[k].priv, &privs[4ull * k], 32); binfo->solved_in_inputs++; }
+  u32* comb;
+  uint8_t* dSolved;
+  ull* dCnt;
+  Hit* dHits;
+  const uint64_t C = block_entries;
+  if (build_comb(B, &comb, 0) || B.dev(&dSolved, n) || B.dev(&dCnt, 32) || B.dev(&dHits, sizeof(Hit) * C)) return -3;
+  WT_CK(cudaMemcpy(dSolved, solved.data(), n, cudaMemcpyHostToDevice));
+  Start st;
+  memcpy(st.v, hd[0].rs, 32);
+  std::vector<Hit> hits;
+  auto on_coll = [&](uint32_t nc, const Coll* dColl) -> int {
+    WT_CK(cudaMemset(dCnt, 0, 32));
+    wt_resolve_kernel<<<(nc + CHECK_THREADS - 1) / CHECK_THREADS, CHECK_THREADS>>>(comb, dColl, nc, kx, kidx, K, n, st, nullptr, nullptr,
+                                                                                   dSolved, dCnt, dHits);
+    WT_CK(cudaGetLastError());
+    ull cnt[4];
+    WT_CK(cudaMemcpy(cnt, dCnt, 32, cudaMemcpyDeviceToHost));
+    binfo->same_herd += cnt[0];
+    binfo->no_key += cnt[1];
+    binfo->already_solved += cnt[2];
+    if (!cnt[3]) return 0;
+    hits.resize(cnt[3]);
+    WT_CK(cudaMemcpy(hits.data(), dHits, sizeof(Hit) * cnt[3], cudaMemcpyDeviceToHost));
+    std::sort(hits.begin(), hits.end(), [](const Hit& a, const Hit& b) { return a.h != b.h ? a.h < b.h : a.seq < b.seq; });
+    for (const Hit& t : hits) {
+      if (solved[t.key]) { binfo->already_solved++; continue; }
+      binfo->solving++;
+      // the hit key is the first of its class; the others get priv (the same point) or 2 * start - priv (its negative)
+      u64 neg[4], s2[4];
+      add_mod_n(s2, hd[0].rs, hd[0].rs);
+      sub_mod_n(neg, s2, t.priv);
+      for (uint32_t j = pos[t.key]; j < n && !memcmp(&hk[16ull * order[j]], &hk[16ull * t.key], 32); j++) {
+        const uint32_t k = order[j];
+        if (solved[k]) continue;
+        solved[k] = 1;
+        kgx_batch_key_result& r = res[k];
+        r.status = 2;
+        r.h = t.h;
+        memcpy(r.priv, memcmp(&hk[16ull * k + 8], &hk[16ull * t.key + 8], 32) ? neg : t.priv, 32);
+        memcpy(r.d_first, t.d_first, 16);
+        memcpy(r.d_other, t.d_other, 16);
+        memcpy(&privs[4ull * k], r.priv, 32);
+        binfo->solved_by_merge++;
+      }
+    }
+    WT_CK(cudaMemcpy(dSolved, solved.data(), n, cudaMemcpyHostToDevice));
+    return 0;
+  };
+  auto tail = [&](FILE* out) -> bool {                  // the batch block: every key, no kangaroo
+    const long off = ftell(out);
+    if (off < 0) return false;
+    std::vector<uint8_t> blk(kgx_wf::batch_block_bytes(n, 0));
+    const uint16_t no_target = 0;
+    kgx_wf::batch_encode(keys.data(), solved.data(), privs.data(), n, &no_target, 0, (uint64_t)off, blk.data());
+    return fwrite(blk.data(), 1, blk.size(), out) == blk.size();
+  };
+  const int rc = merge_stream(B, fs, paths, hd, n_paths, tmp_path, block_entries, info, on_coll, tail);
+  if (rc) return rc;
+  binfo->n_keys = n;
+  binfo->left = n - binfo->solved_in_inputs - binfo->solved_by_merge;
+  memcpy(keys_out, res.data(), sizeof(kgx_batch_key_result) * n);
+  return 0;
 }
 
 }  // extern "C"

@@ -10,8 +10,10 @@
 given (the entry of the earlier file wins at equal x) with kgx_work_merge, resolves every tame/wild collision with the
 solver's resolver (the reference's CheckKey, build/libkgx_ingest.so), and either prints the key and writes nothing, or writes
 DEST through DEST.tmp, fsync and rename.  The merged file ends with a kangaroo count of 0, so the solver's --resume and the
-reference's -i take it; they start fresh herds.  Batch work files are not merged.  There is no CPU path: without a device both
-commands fail.
+reference's -i take it; they start fresh herds.  Batch work files (the same keys in the same order and the same range) are
+merged with kgx_work_merge_batch, which resolves every tame/wild collision against all keys on the device; DEST is always
+written, with a batch block that records every key solved in an input or by the merge, so that --batch-resume continues from
+it.  There is no CPU path: without a device both commands fail.
 
 The batch block of a batch work file (its layout: kgx_workfile.h) is written and read here, through libkgx.so's
 kgx_batch_block / kgx_batch_read, which the device check uses too; neither needs a device."""
@@ -46,6 +48,19 @@ class MergeInfo(ctypes.Structure):
     _fields_ = [("dp_bits", ctypes.c_uint32), ("blocks", ctypes.c_uint32), ("entries", ctypes.c_uint64),
                 ("duplicates", ctypes.c_uint64), ("collisions", ctypes.c_uint64), ("total_count", ctypes.c_uint64),
                 ("total_time", ctypes.c_double), ("n_listed", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+class BatchMergeInfo(ctypes.Structure):
+    """kgx_batch_merge_info"""
+    _fields_ = [("n_keys", ctypes.c_uint32), ("solved_in_inputs", ctypes.c_uint32), ("solved_by_merge", ctypes.c_uint32),
+                ("left", ctypes.c_uint32), ("same_herd", ctypes.c_uint64), ("no_key", ctypes.c_uint64),
+                ("already_solved", ctypes.c_uint64), ("solving", ctypes.c_uint64)]
+
+
+class BatchKeyResult(ctypes.Structure):
+    """kgx_batch_key_result"""
+    _fields_ = [("status", ctypes.c_uint32), ("h", ctypes.c_uint32), ("priv", ctypes.c_uint64 * 4), ("d_first", ctypes.c_uint64 * 2),
+                ("d_other", ctypes.c_uint64 * 2)]
 
 
 class Collision(ctypes.Structure):
@@ -207,6 +222,55 @@ def merge_files(paths, tmp_path, device=0, block_entries=0, cap=1 << 20):
     return MergeResult(info, [(c.h, (c.d_first[0], c.d_first[1]), (c.d_other[0], c.d_other[1])) for c in coll[:info.n_listed]])
 
 
+class BatchMergeResult(MergeResult):
+    """MergeResult of kgx_work_merge_batch (collision_list is empty) with the counts of kgx_batch_merge_info and, per key,
+    status (0 unsolved, 1 solved in an input, 2 solved by the merge), priv (int or None) and, for status 2, the collision
+    (h, d_first, d_other) that solved it"""
+
+    def __init__(self, info, binfo, keys):
+        super().__init__(info, [])
+        for name, _ in BatchMergeInfo._fields_:
+            setattr(self, name, getattr(binfo, name))
+        self.status = [k.status for k in keys]
+        self.privs = [_val(k.priv) if k.status else None for k in keys]
+        self.solved_by = [(k.h, _val(k.d_first), _val(k.d_other)) if k.status == 2 else None for k in keys]
+
+
+def merge_batch_files(paths, tmp_path, device=0, block_entries=0):
+    """kgx_work_merge_batch: batch work files merged in order into tmp_path -> BatchMergeResult.  Refusals raise ValueError
+    and leave no tmp_path."""
+    lib = load_library()
+    first = read_batch(paths[0])
+    if first is None:
+        raise ValueError("MergeWork: %s is a plain HEADW work file: batch work files merge only with batch work files" % paths[0])
+    arr = (ctypes.c_char_p * len(paths))(*[os.fsencode(p) for p in paths])
+    info, binfo = MergeInfo(), BatchMergeInfo()
+    keys = (BatchKeyResult * first.n_keys)()
+    rc = lib.kgx_work_merge_batch(int(device), arr, len(paths), os.fsencode(tmp_path), int(block_entries), ctypes.byref(info),
+                                  ctypes.byref(binfo), keys, first.n_keys)
+    if rc == -1:
+        raise ValueError(_err(lib))
+    if rc != 0:
+        raise RuntimeError("kgx_work_merge_batch: " + _err(lib))
+    return BatchMergeResult(info, binfo, keys[:binfo.n_keys])
+
+
+def resolve(d_first, d_other, keys, range_start, device=0):
+    """kgx_work_resolve: collisions (two lists of tagged distances) against keys K = key - start*G (a list of (x, y), None for
+    the point at infinity) -> [(key index, private key) or None], as kgi_resolve_multi gives them"""
+    lib = load_library()
+    n = len(d_first)
+    kt = np.ascontiguousarray(np.hstack([_limbs([0 if k is None else k[0] for k in keys], 4),
+                                         _limbs([0 if k is None else k[1] for k in keys], 4)]))
+    a, b = np.ascontiguousarray(_limbs(d_first, 2)), np.ascontiguousarray(_limbs(d_other, 2))
+    idx, priv = np.zeros(n, dtype=np.uint32), np.zeros((n, 4), dtype=np.uint64)
+    rc = lib.kgx_work_resolve(int(device), a.ctypes.data_as(_u64p), b.ctypes.data_as(_u64p), n, kt.ctypes.data_as(_u64p), len(keys),
+                              _limbs4(range_start), idx.ctypes.data_as(ctypes.POINTER(ctypes.c_uint32)), priv.ctypes.data_as(_u64p))
+    if rc != 0:
+        raise (ValueError if rc == -1 else RuntimeError)("kgx_work_resolve: " + _err(lib))
+    return [None if i == 0xFFFFFFFF else (int(i), _val(p)) for i, p in zip(idx.tolist(), priv)]
+
+
 def dir_inputs(dirname):
     """Kangaroo::MergeDir's inputs (Merge.cpp:255-315): every regular HEADW file of the directory, largest first (equal sizes
     by name, so that the order does not depend on the directory's listing)"""
@@ -241,9 +305,65 @@ def validate(paths):
             raise ValueError("MergeWork: key differs, multiple keys not yet supported (%s, %s)" % (paths[0], p))
 
 
+def validate_batch(paths, blocks):
+    """kgx_work_merge_batch's refusals that need no device (blocks: read_batch of every path): a plain file among batch
+    files, another range or version, another key count or order, two inputs with different private keys for one key ->
+    ValueError"""
+    for p, b in zip(paths, blocks):
+        if b is None:
+            raise ValueError("MergeWork: %s is a plain HEADW work file: batch work files merge only with batch work files" % p)
+    h0, b0 = read_work_header(paths[0]), blocks[0]
+    for p, b in zip(paths[1:], blocks[1:]):
+        h = read_work_header(p)
+        if h.version != h0.version:
+            raise ValueError("MergeWork: cannot merge workfile of different version (%s)" % p)
+        if (h.range_start, h.range_end) != (h0.range_start, h0.range_end):
+            raise ValueError("MergeWork: File range differs (%s, %s)" % (paths[0], p))
+        if b.n_keys != b0.n_keys:
+            raise ValueError("MergeWork: %s holds %d keys, %s %d: the key lists differ" % (p, b.n_keys, paths[0], b0.n_keys))
+        for k, (q, q0) in enumerate(zip(b.pubs, b0.pubs)):
+            if q != q0:
+                raise ValueError("MergeWork: key #%d of %s differs from key #%d of %s: the key lists differ" % (k, p, k, paths[0]))
+    for k in range(b0.n_keys):
+        recorded = {b.privs[k] for b in blocks if b.solved[k]}
+        if len(recorded) > 1:
+            raise ValueError("MergeWork: two inputs record different private keys for key #%d" % k)
+
+
+def merge_batch(paths, blocks, dest, device=0, block_entries=0, out=print):
+    """Merge batch work files into dest (always written, through DEST.tmp, fsync and rename) -> (0, {key index: private key}
+    of the keys the merge solved)"""
+    validate_batch(paths, blocks)
+    tmp = dest + ".tmp"
+    res = merge_batch_files(paths, tmp, device=device, block_entries=block_entries)
+    with open(tmp, "rb+") as f:
+        os.fsync(f.fileno())
+    os.replace(tmp, dest)
+    for p in paths:
+        out("File %s: [DP%d]" % (p, read_work_header(p).dp_bits))
+    found = {}
+    for i, (st, priv) in enumerate(zip(res.status, res.privs)):
+        if st == 2:
+            found[i] = priv
+            out("Key#%2d Pub:  0x%064X\n       Priv: 0x%X" % (i, blocks[0].pubs[i][0], priv))
+    out("Keys: %d, %d solved in the inputs, %d solved by the merge, %d left" %
+        (res.n_keys, res.solved_in_inputs, res.solved_by_merge, res.left))
+    out("Collisions: %d (%d solved a key, %d on a key already solved, %d on no key, %d same-herd)" %
+        (res.collisions, res.solving, res.already_solved, res.no_key, res.same_herd))
+    out("Dead kangaroo: %d" % (res.duplicates + res.same_herd))
+    out("Total f1+f2: DP count 2^%.2f" % (math.log2(res.entries) if res.entries else float("-inf")))
+    out("Merged %d batch files into %s: %d entries, %d duplicates" % (len(paths), dest, res.entries, res.duplicates))
+    return 0, found
+
+
 def merge(paths, dest, device=0, block_entries=0, out=print):
     """Merge `paths` (in order) into dest -> (exit code, private key or None).  A solved key removes DEST.tmp and writes no
-    file (Merge.cpp:218-229); otherwise DEST.tmp is synced and renamed over dest."""
+    file (Merge.cpp:218-229); otherwise DEST.tmp is synced and renamed over dest.  Batch work files go to merge_batch, which
+    returns the keys it solved instead of a private key."""
+    if len(paths) >= 2 and all(is_work_file(p) for p in paths):
+        blocks = [read_batch(p) for p in paths]
+        if any(b is not None for b in blocks):
+            return merge_batch(paths, blocks, dest, device=device, block_entries=block_entries, out=out)
     validate(paths)
     tmp = dest + ".tmp"
     res = merge_files(paths, tmp, device=device, block_entries=block_entries)
@@ -292,7 +412,7 @@ def main(argv=None):
     c.add_argument("--device", type=int, default=0)
     m = sub.add_parser("merge", help="merge work files of the same key and range on the GPU (-wm / -wmdir)")
     m.add_argument("files", nargs="*")
-    m.add_argument("--dir", default=None, help="merge every HEADW file of DIR, largest first (-wmdir)")
+    m.add_argument("--dir", default=None, help="merge every HEADW file of DIR, largest first (-wmdir); batch work files too")
     m.add_argument("-o", "--output", required=True, metavar="DEST")
     m.add_argument("--device", type=int, default=0)
     m.add_argument("--block-entries", type=int, default=0, help="entries per device block, summed over the inputs (0 = 2^22)")
