@@ -209,6 +209,32 @@ int kgx_dptable_save_work(kgx_dptable* t, const char* path, uint32_t dp_bits, co
 int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, uint64_t range_start[4], uint64_t range_end[4],
                           uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time, uint64_t* nb_walk,
                           uint64_t* walk_offset, void* stream);
+/* --- the sharded DP table: rank r of W holds the buckets [floor(r*2^18/W), floor((r+1)*2^18/W)) in a table of its own GPU.
+ * _create_range: kgx_dptable_create for the buckets [lo, hi) only (lo < hi <= 2^18): _add skips a record of another bucket
+ *     as malformed (-1), _save_work writes the other buckets empty, _load_work loads the range and walks past the rest.
+ * _piece_bytes: the bytes of the table's piece of a work file, the nbItem, maxItem and entries of its buckets:
+ *     8 * (hi - lo) + 32 * count.
+ * _save_range: the piece written at byte `offset` of the existing file `path` (no header, no kangaroo count; the rest of
+ *     the file is left as it is), after the work queued on `stream`, then flushed and fsynced.  The pieces of the W shards at
+ *     offsets 156, 156 + piece 0, ... make the table of the file the single table writes for the same records.
+ * _load_range: _load_work with a limit: more than max_entries entries in the range fail with -ENOSPC, and an empty table.
+ *     The header arguments and the kangaroo count and offset are the file's, as _load_work returns them. --- */
+kgx_dptable* kgx_dptable_create_range(int dev, uint64_t capacity, uint32_t lo, uint32_t hi);
+uint64_t     kgx_dptable_piece_bytes(kgx_dptable* t);
+int kgx_dptable_save_range(kgx_dptable* t, const char* path, uint64_t offset, void* stream);
+int kgx_dptable_load_range(kgx_dptable* t, const char* path, uint32_t* dp_bits, uint64_t range_start[4], uint64_t range_end[4],
+                           uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time, uint64_t* nb_walk,
+                           uint64_t* walk_offset, uint64_t max_entries, void* stream);
+/* --- kgx_dp_partition (kgx_partition.cuh): n 40-byte DP records of kgx_convert_dps (device memory) grouped by the rank of W
+ *     (1 .. KGX_DPT_MAX_RANKS) that owns their bucket, each group in input order (a stable partition), into out: packed when
+ *     stride = 0, else group r at record r * stride (stride >= n).  recs and out need 4-byte alignment only (kgx_convert_dps's
+ *     records follow its u32 count).  counts (device memory, W + 1 entries): the records of each
+ *     group, then the malformed ones (h >= 2^18), which are left out.  scratch: device memory of at least
+ *     kgx_dp_partition_scratch_bytes(n, W) bytes.  Stream-ordered on `stream`, the call does not wait.  -1: bad arguments;
+ *     -3: a CUDA error. --- */
+uint64_t kgx_dp_partition_scratch_bytes(uint32_t n, uint32_t world);
+int kgx_dp_partition(const void* recs, uint32_t n, uint32_t world, uint64_t stride, void* out, uint32_t* counts, void* scratch,
+                     uint64_t scratch_bytes, void* stream);
 
 /* --- work-file tools on one GPU (kgx_worktool.cuh): the reference's -wcheck and -wm / -wmdir for HEADW files.  Without a
  *     device every call fails (-3); there is no CPU path.  Errors: a negative value, text in kgx_work_last_error().

@@ -80,6 +80,14 @@ _SIGS = {
                                              ctypes.c_double, ctypes.c_uint64, ctypes.c_void_p]),
     "kgx_dptable_load_work": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_uint32), _u64p, _u64p, _u64p, _u64p,
                                              _u64p, ctypes.POINTER(ctypes.c_double), _u64p, _u64p, ctypes.c_void_p]),
+    "kgx_dptable_create_range": (ctypes.c_void_p, [ctypes.c_int, ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint32]),
+    "kgx_dptable_piece_bytes": (ctypes.c_uint64, [ctypes.c_void_p]),
+    "kgx_dptable_save_range": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_uint64, ctypes.c_void_p]),
+    "kgx_dptable_load_range": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_uint32), _u64p, _u64p, _u64p, _u64p,
+                                              _u64p, ctypes.POINTER(ctypes.c_double), _u64p, _u64p, ctypes.c_uint64, ctypes.c_void_p]),
+    "kgx_dp_partition_scratch_bytes": (ctypes.c_uint64, [ctypes.c_uint32, ctypes.c_uint32]),
+    "kgx_dp_partition": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint64, ctypes.c_void_p, ctypes.c_void_p,
+                                        ctypes.c_void_p, ctypes.c_uint64, ctypes.c_void_p]),
     "kgx_work_last_error": (ctypes.c_char_p, []),
     "kgx_work_check": (ctypes.c_int, [ctypes.c_int, ctypes.c_char_p, ctypes.c_uint64, ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint32),
                                       _u64p, ctypes.c_uint32]),

@@ -6,6 +6,8 @@
 // on every later Add -- stored or not -- that finds nbItem >= maxItem - 1), and work files that are byte for byte what
 // HashTable::SaveTable writes (buckets in order, entries sorted by unsigned (x.hi, x.lo)).  The file format is
 // kgx_workfile.h's; a save orders each chunk of whole buckets with kgx_bucketsort.cuh's sort.
+// A table may hold a range of buckets only (kgx_dptable_create_range): one shard of the sharded table, which saves and loads
+// its range as a piece of a work file at an offset.
 //
 // Layout (fixed capacity C entries, no growth):
 //   ent[C]      32-byte entries {x, d}, dense in insertion order; ent_h[C] their bucket
@@ -63,15 +65,16 @@ __device__ __forceinline__ void index_insert(ull* slots, uint64_t nslots, uint64
     if (++p == nslots) p = 0;
 }
 
-__global__ void k_keys(const uint8_t* recs, uint64_t stride, Ranks R, uint32_t n, uint32_t* keys, uint32_t* vals,
-                       uint8_t* evFlag, Res* res) {
+__global__ void k_keys(const uint8_t* recs, uint64_t stride, Ranks R, uint32_t n, uint32_t lo, uint32_t hi, uint32_t* keys,
+                       uint32_t* vals, uint8_t* evFlag, Res* res) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const uint32_t h = (uint32_t)(record(recs, stride, R, i, rank_of(R, i))[0] >> 32);
-  keys[i] = h < NBUCKET ? h : NBUCKET;
+  const bool in = h >= lo && h < hi;                    // [lo, hi): the table's buckets, all 2^18 but in a shard
+  keys[i] = in ? h : NBUCKET;
   vals[i] = i;
   evFlag[i] = 0;
-  if (h >= NBUCKET) res->bad = 1;                       // skipped, like kgx_ingest.cpp's workers; the call returns -1
+  if (!in) res->bad = 1;                                // skipped, like kgx_ingest.cpp's workers; the call returns -1
 }
 
 // one thread per bucket present in the call: HashTable::Add(h, x, d) for each of its records in arrival order
@@ -162,6 +165,7 @@ static char g_dpt_create_err[256] = "";
 
 struct kgx_dptable {
   int dev = 0;
+  uint32_t lo = 0, hi = kgx_dpt::NBUCKET;                 // the buckets the table holds (a shard of the sharded table: a range)
   uint64_t capacity = 0, nslots = 0, count = 0;           // count: host mirror of res->count after the last call
   kgx_dpt::Entry* ent = nullptr;
   uint32_t* ent_h = nullptr;
@@ -285,6 +289,16 @@ void kgx_dptable_destroy(kgx_dptable* t) {
   delete t;
 }
 
+kgx_dptable* kgx_dptable_create_range(int dev, uint64_t capacity, uint32_t lo, uint32_t hi) {
+  if (lo >= hi || hi > kgx_dpt::NBUCKET) {
+    snprintf(g_dpt_create_err, sizeof g_dpt_create_err, "kgx_dptable_create_range: buckets [%u, %u) are not a range of [0, 2^18)", lo, hi);
+    return nullptr;
+  }
+  kgx_dptable* t = kgx_dptable_create(dev, capacity);
+  if (t) { t->lo = lo; t->hi = hi; }
+  return t;
+}
+
 kgx_dptable* kgx_dptable_create(int dev, uint64_t capacity) {
   int cnt = 0;
   cudaError_t s = cudaGetDeviceCount(&cnt);
@@ -391,7 +405,7 @@ int kgx_dptable_add(kgx_dptable* t, const void* recs, const uint32_t* counts, ui
   const uint8_t* rp = static_cast<const uint8_t*>(recs);
   DPT_CK(t, cudaMemsetAsync(&t->res->nsel, 0, 8, st));
   const uint32_t B = 256, G = (n + B - 1) / B;
-  k_keys<<<G, B, 0, st>>>(rp, stride, R, n, t->keyIn, t->valIn, t->evFlag, t->res);
+  k_keys<<<G, B, 0, st>>>(rp, stride, R, n, t->lo, t->hi, t->keyIn, t->valIn, t->evFlag, t->res);
   DPT_CK(t, cudaGetLastError());
   size_t tb = t->cubTmpBytes;
   DPT_CK(t, cub::DeviceRadixSort::SortPairs(t->cubTmp, tb, t->keyIn, t->keyOut, t->valIn, t->valOut, (int)n, 0, 19, st));
@@ -417,17 +431,15 @@ int kgx_dptable_add(kgx_dptable* t, const void* recs, const uint32_t* counts, ui
   return t->resHost->bad ? -1 : 0;
 }
 
-int kgx_dptable_save_work(kgx_dptable* t, const char* path, uint32_t dp_bits, const uint64_t range_start[4], const uint64_t range_end[4],
-                          const uint64_t keyx[4], const uint64_t keyy[4], uint64_t total_count, double total_time, uint64_t total_walk,
-                          void* stream) {
+// The buckets [b0, b1) of the table, each nbItem, maxItem and its entries (HashTable::SaveTable, HashTable.cpp:375-396), to f
+// in chunks of whole buckets: select, sort by (h, x.hi, x.lo), copy out.  -> 0, -3 on a CUDA error (text in t->err), or 1
+// when a write failed (errno tells).
+static int dpt_write_buckets(kgx_dptable* t, FILE* f, uint32_t b0, uint32_t b1, cudaStream_t st) {
   using namespace kgx_dpt;
   using namespace kgx_wf;
-  cudaStream_t st = (cudaStream_t)stream;
-  DPT_CK(t, cudaSetDevice(t->dev));
-  DPT_CK(t, cudaStreamSynchronize(st));                    // every add queued on this stream is in the table
   if (dpt_pinned(t)) return -3;
   uint32_t* nbH = (uint32_t*)malloc(8ull * NBUCKET);
-  if (!nbH) { snprintf(t->err, sizeof t->err, "out of host memory"); return -ENOMEM; }
+  if (!nbH) { snprintf(t->err, sizeof t->err, "out of host memory"); return -3; }
   uint32_t* mxH = nbH + NBUCKET;
   if (cudaMemcpy(nbH, t->nb, 4ull * NBUCKET, cudaMemcpyDeviceToHost) != cudaSuccess ||
       cudaMemcpy(mxH, t->mx, 4ull * NBUCKET, cudaMemcpyDeviceToHost) != cudaSuccess) {
@@ -435,18 +447,13 @@ int kgx_dptable_save_work(kgx_dptable* t, const char* path, uint32_t dp_bits, co
     snprintf(t->err, sizeof t->err, "kgx_dptable_save_work: bucket counters: %s", cudaGetErrorString(cudaGetLastError()));
     return -3;
   }
-  errno = 0;
-  FILE* f = fopen(path, "wb");
-  if (!f) { const int e = io_error(); free(nbH); snprintf(t->err, sizeof t->err, "%s: %s", path, strerror(-e)); return e; }
-  setvbuf(f, nullptr, _IOFBF, 1 << 22);
-  bool ok = write_header(f, make_header(dp_bits, range_start, range_end, keyx, keyy, total_count, total_time));
+  bool ok = true;
   int rc = 0;
-  // HashTable::SaveTable (HashTable.cpp:375-396) in chunks of whole buckets: select, sort by (h, x.hi, x.lo), copy out
-  uint32_t b0 = 0;
-  while (ok && rc == 0 && b0 < NBUCKET) {
+  const uint32_t end = b1;
+  while (ok && rc == 0 && b0 < end) {
     uint64_t m = 0;
-    uint32_t b1 = b0;
-    while (b1 < NBUCKET && (m + nbH[b1] <= t->chunk || b1 == b0)) m += nbH[b1++];
+    b1 = b0;
+    while (b1 < end && (m + nbH[b1] <= t->chunk || b1 == b0)) m += nbH[b1++];
     if (m > t->chunk) {                                   // one bucket larger than a chunk
       snprintf(t->err, sizeof t->err, "kgx_dptable_save_work: bucket %u holds %llu entries, more than a save chunk (%llu)", b0,
                (unsigned long long)m, (unsigned long long)t->chunk);
@@ -477,6 +484,25 @@ int kgx_dptable_save_work(kgx_dptable* t, const char* path, uint32_t dp_bits, co
     b0 = b1;
   }
   free(nbH);
+  return rc ? rc : (ok ? 0 : 1);
+}
+
+int kgx_dptable_save_work(kgx_dptable* t, const char* path, uint32_t dp_bits, const uint64_t range_start[4], const uint64_t range_end[4],
+                          const uint64_t keyx[4], const uint64_t keyy[4], uint64_t total_count, double total_time, uint64_t total_walk,
+                          void* stream) {
+  using namespace kgx_dpt;
+  using namespace kgx_wf;
+  cudaStream_t st = (cudaStream_t)stream;
+  DPT_CK(t, cudaSetDevice(t->dev));
+  DPT_CK(t, cudaStreamSynchronize(st));                    // every add queued on this stream is in the table
+  if (dpt_pinned(t)) return -3;
+  errno = 0;
+  FILE* f = fopen(path, "wb");
+  if (!f) { const int e = io_error(); snprintf(t->err, sizeof t->err, "%s: %s", path, strerror(-e)); return e; }
+  setvbuf(f, nullptr, _IOFBF, 1 << 22);
+  bool ok = write_header(f, make_header(dp_bits, range_start, range_end, keyx, keyy, total_count, total_time));
+  int rc = ok ? dpt_write_buckets(t, f, 0, NBUCKET, st) : 0;   // every bucket: those out of a shard's range are empty
+  if (rc == 1) { ok = false; rc = 0; }
   ok = ok && fwrite(&total_walk, 8, 1, f) == 1;           // Backup.cpp:530-531 / 549-551
   ok = fflush(f) == 0 && ok;
   int err = rc ? rc : (ok ? 0 : io_error());
@@ -485,16 +511,39 @@ int kgx_dptable_save_work(kgx_dptable* t, const char* path, uint32_t dp_bits, co
   return err;
 }
 
-int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, uint64_t range_start[4], uint64_t range_end[4],
-                          uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time, uint64_t* nb_walk,
-                          uint64_t* walk_offset, void* stream) {
-  using namespace kgx_dpt;
+uint64_t kgx_dptable_piece_bytes(kgx_dptable* t) { return 8ull * (t->hi - t->lo) + sizeof(kgx_dpt::Entry) * t->count; }
+
+int kgx_dptable_save_range(kgx_dptable* t, const char* path, uint64_t offset, void* stream) {
   using namespace kgx_wf;
   cudaStream_t st = (cudaStream_t)stream;
   DPT_CK(t, cudaSetDevice(t->dev));
   DPT_CK(t, cudaStreamSynchronize(st));
+  errno = 0;
+  FILE* f = fopen(path, "r+b");                           // the file exists: its header and the other pieces stay
+  if (!f) { const int e = io_error(); snprintf(t->err, sizeof t->err, "%s: %s", path, strerror(-e)); return e; }
+  setvbuf(f, nullptr, _IOFBF, 1 << 22);
+  bool ok = fseeko(f, (off_t)offset, SEEK_SET) == 0;
+  int rc = ok ? dpt_write_buckets(t, f, t->lo, t->hi, st) : 0;
+  if (rc == 1) { ok = false; rc = 0; }
+  ok = ok && fflush(f) == 0 && fsync(fileno(f)) == 0;
+  int err = rc ? rc : (ok ? 0 : io_error());
+  if (fclose(f) != 0 && err == 0) err = io_error();
+  if (err < 0 && err != -3) snprintf(t->err, sizeof t->err, "%s: %s", path, strerror(-err));
+  return err;
+}
+
+// HashTable::LoadTable (HashTable.cpp:439-459) of the table's buckets [lo, hi): the others are walked past.  More than
+// max_entries entries in the range: -ENOSPC and an empty table, like any failed load.
+static int dpt_load(kgx_dptable* t, const char* path, uint64_t max_entries, uint32_t* dp_bits, uint64_t range_start[4],
+                    uint64_t range_end[4], uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time,
+                    uint64_t* nb_walk, uint64_t* walk_offset, cudaStream_t st) {
+  using namespace kgx_dpt;
+  using namespace kgx_wf;
+  DPT_CK(t, cudaSetDevice(t->dev));
+  DPT_CK(t, cudaStreamSynchronize(st));
   if (dpt_reset(t, st)) return -3;                         // HashTable::LoadTable starts with Reset()
   if (dpt_pinned(t)) return -3;
+  if (max_entries > t->capacity) max_entries = t->capacity;
   errno = 0;
   FILE* f = fopen(path, "rb");
   if (!f) { const int e = io_error(); snprintf(t->err, sizeof t->err, "%s: %s", path, strerror(-e)); return e; }
@@ -523,11 +572,16 @@ int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, u
     staged = 0;
     return true;
   };
-  for (uint32_t h = 0; ok && h < NBUCKET; h++) {           // HashTable::LoadTable (HashTable.cpp:439-459)
+  for (uint32_t h = 0; ok && h < NBUCKET; h++) {
     ok = read_bucket_head(f, nbH[h], mxH[h]);
+    if (ok && (h < t->lo || h >= t->hi)) {                 // another shard's bucket
+      ok = nbH[h] == 0 || fseeko(f, (off_t)nbH[h] * (off_t)sizeof(Entry), SEEK_CUR) == 0;
+      nbH[h] = mxH[h] = 0;
+      continue;
+    }
     uint32_t left = ok ? nbH[h] : 0;
     total += left;
-    if (ok && total > t->capacity) { rc = -ENOSPC; ok = false; break; }
+    if (ok && total > max_entries) { rc = -ENOSPC; ok = false; break; }
     while (ok && left) {
       if (staged == t->chunk && !flush()) { ok = false; break; }
       const uint32_t k = (uint32_t)std::min<uint64_t>(left, t->chunk - staged);
@@ -549,7 +603,9 @@ int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, u
   }
   free(nbH);
   if (!ok) {
-    if (rc == -ENOSPC)
+    if (rc == -ENOSPC && max_entries < t->capacity)
+      snprintf(t->err, sizeof t->err, "%s: buckets [%u, %u) hold more than %llu entries", path, t->lo, t->hi, (unsigned long long)max_entries);
+    else if (rc == -ENOSPC)
       snprintf(t->err, sizeof t->err, "%s holds more than the table's capacity of %llu entries", path, (unsigned long long)t->capacity);
     else if (rc == 0)
       snprintf(t->err, sizeof t->err, "%s is not a complete HEADW work file", path);
@@ -560,6 +616,20 @@ int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, u
   if (nb_walk) *nb_walk = walk;
   if (walk_offset) *walk_offset = off;
   return 0;
+}
+
+int kgx_dptable_load_work(kgx_dptable* t, const char* path, uint32_t* dp_bits, uint64_t range_start[4], uint64_t range_end[4],
+                          uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time, uint64_t* nb_walk,
+                          uint64_t* walk_offset, void* stream) {
+  return dpt_load(t, path, t->capacity, dp_bits, range_start, range_end, keyx, keyy, total_count, total_time, nb_walk, walk_offset,
+                  (cudaStream_t)stream);
+}
+
+int kgx_dptable_load_range(kgx_dptable* t, const char* path, uint32_t* dp_bits, uint64_t range_start[4], uint64_t range_end[4],
+                           uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time, uint64_t* nb_walk,
+                           uint64_t* walk_offset, uint64_t max_entries, void* stream) {
+  return dpt_load(t, path, max_entries, dp_bits, range_start, range_end, keyx, keyy, total_count, total_time, nb_walk, walk_offset,
+                  (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -195,3 +195,82 @@ def decode_dp40(buf):
         mag = d & ((1 << 126) - 1)
         out.append((kidx, h, x, -mag if d >> 127 else mag, ktype))
     return out
+
+
+# ---- the sharded DP table (--dp-table sharded): every rank's records to the ranks that own their buckets ----------------------
+NBUCKET = 1 << 18        # HASH_SIZE: the buckets of a DP table, h = x.bits64[2] & 0x3FFFF
+
+
+def owner_ranges(world):
+    """[(lo, hi)] per rank: rank r of W owns the buckets [floor(r*2^18/W), floor((r+1)*2^18/W))"""
+    return [(r * NBUCKET // world, (r + 1) * NBUCKET // world) for r in range(world)]
+
+
+def owner_of(h, world):
+    """the rank that owns bucket h (h < 2^18), as kgx_partition.cuh computes it: the last r with floor(r*2^18/W) <= h"""
+    return ((h + 1) * world - 1) // NBUCKET
+
+
+class DPExchange:
+    """The sharded table's exchange, beside DPGather: each rank's 40-byte DP records go to the ranks that own their buckets.
+
+        partition : kgx_dp_partition groups this rank's records by owner (stable), group r at record r*max_found
+        counts    : all_gather of every rank's W + 1 counts (its groups, then its malformed records): every rank learns what it
+                    receives, and cap = the largest count rounded up to 256 records
+        payload   : one equal-split all_to_all_single of cap records per (source, destination) pair into a [W][cap] buffer
+
+    A shard receives source rank 0's records first, then rank 1's, ..., each in the order its source produced them: restricted to
+    one bucket, the order the single table sees.  step() returns (records from each source, cap, receive buffer, malformed
+    records of this rank); the buffer is rewritten by the next step.
+
+    engine: kangaroo_b200.GPUEngine, or None with partition_fn for the CPU (gloo) tests: partition_fn(n) -> (uint8 tensor of W
+    groups of max_found records, W + 1 counts as an int32 tensor)."""
+
+    def __init__(self, engine, dist, rank, world, torch, device=None, max_found=None, partition_fn=None):
+        self.eng, self.dist, self.rank, self.world, self.torch = engine, dist, rank, world, torch
+        self.device = device if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.max_found = max_found if max_found is not None else engine.maxFound
+        self._partition = partition_fn if partition_fn is not None else self._engine_partition
+        self._send = self._recv = self._scratch = self._counts = None
+        self.total_exchanged = 0
+
+    def _engine_partition(self, n):
+        """this launch's converted records grouped by owner on the device (torch's stream)"""
+        import ctypes
+        torch, W = self.torch, self.world
+        lib = self.eng._lib
+        if self._send is None:
+            self._send = torch.empty(W * self.max_found * DP40_BYTES, dtype=torch.uint8, device=self.device)
+            self._counts = torch.empty(W + 1, dtype=torch.int32, device=self.device)
+            nb = int(lib.kgx_dp_partition_scratch_bytes(self.max_found, W))
+            self._scratch = torch.empty(nb, dtype=torch.uint8, device=self.device)
+        src = self.eng.convert_dps_device_ptr() + 4
+        rc = lib.kgx_dp_partition(ctypes.c_void_p(src), int(n), W, self.max_found, ctypes.c_void_p(self._send.data_ptr()),
+                                  ctypes.c_void_p(self._counts.data_ptr()), ctypes.c_void_p(self._scratch.data_ptr()),
+                                  self._scratch.numel(), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+        if rc != 0:
+            raise RuntimeError("kgx_dp_partition failed (%d)" % rc)
+        return self._send, self._counts
+
+    def step(self, n_found):
+        torch, W, R = self.torch, self.world, DP40_BYTES
+        n = min(int(n_found), self.max_found)
+        send, counts = self._partition(n)
+        if W == 1:
+            c = [int(v) for v in counts.cpu().tolist()]
+            res = [c[0]], c[0], send, c[1]
+        else:
+            allc = torch.empty(W * (W + 1), dtype=torch.int32, device=self.device)
+            self.dist.all_gather_into_tensor(allc, counts)
+            m = allc.cpu().view(W, W + 1).tolist()                          # m[source][destination], then malformed
+            cap = min(max(ROUND, (max(max(row[:W]) for row in m) + ROUND - 1) // ROUND * ROUND), self.max_found)
+            if self._recv is None:
+                self._recv = torch.empty(W * self.max_found * R, dtype=torch.uint8, device=self.device)
+            payload = send.view(W, self.max_found * R)[:, :cap * R].reshape(-1)   # [W][cap]: a copy unless cap = max_found
+            recv = self._recv[:W * cap * R]
+            self.dist.all_to_all_single(recv, payload)
+            res = [m[s][self.rank] for s in range(W)], cap, recv, m[self.rank][W]
+        if self.device.type == "cuda":
+            torch.cuda.current_stream().synchronize()   # the engine's record buffer is recycled by the launch after next
+        self.total_exchanged += sum(res[0])
+        return res

@@ -207,15 +207,20 @@ class DeviceDPTable:
     """The rank-0 DP table in the memory of one GPU (libkgx.so, kgx_dptable_*): DPTable's add / __len__ / save_work /
     load_work_ex with exactly its results for the same records in the same order, inserted by CUDA kernels straight from device
     memory.  Its capacity (entries) is fixed at creation; an add that could pass it raises TableFull and changes nothing.
-    resolve / resolve_multi are the host table's (kgi_resolve: the reference's CheckKey), on a DPTable that holds no entry."""
+    resolve / resolve_multi are the host table's (kgi_resolve: the reference's CheckKey), on a DPTable that holds no entry.
+    buckets=(lo, hi): a shard of the sharded table, holding the buckets [lo, hi) only (kgx_dptable_create_range)."""
 
-    def __init__(self, capacity, device=None, max_events=4096):
+    def __init__(self, capacity, device=None, max_events=4096, buckets=None):
         from ._lib import load_library as load_engine
         self._lib = load_engine()
         self.device = int(device if device is not None else 0)
-        self._h = ctypes.c_void_p(self._lib.kgx_dptable_create(self.device, int(capacity)))
+        if buckets is None:
+            self._h = ctypes.c_void_p(self._lib.kgx_dptable_create(self.device, int(capacity)))
+        else:
+            self._h = ctypes.c_void_p(self._lib.kgx_dptable_create_range(self.device, int(capacity), int(buckets[0]), int(buckets[1])))
         if not self._h:
             raise RuntimeError(self._lib.kgx_dptable_last_error(None).decode())
+        self.buckets = (0, 1 << 18) if buckets is None else (int(buckets[0]), int(buckets[1]))
         self.capacity = int(capacity)
         self._ev = (Event * max_events)()
         self._cap = max_events
@@ -298,6 +303,26 @@ class DeviceDPTable:
             raise TableFull(self._err())
         if rc != 0:
             raise RuntimeError("kgx_dptable_load_work: %s" % self._err())
+        return info
+
+    def piece_bytes(self):
+        """the size of this table's piece of a work file: its buckets' nbItem, maxItem and entries"""
+        return int(self._lib.kgx_dptable_piece_bytes(self._h))
+
+    def save_piece(self, path, offset, stream=0):
+        """write this table's piece at byte `offset` of the existing file `path` (flushed and fsynced)"""
+        rc = self._lib.kgx_dptable_save_range(self._h, os.fsencode(path), int(offset), ctypes.c_void_p(int(stream)))
+        if rc != 0:
+            raise RuntimeError("kgx_dptable_save_range: cannot write %s: %s" % (path, self._err()))
+
+    def load_piece(self, path, max_entries, stream=0):
+        """load_work_ex of this table's buckets only; more than max_entries entries in them raise TableFull"""
+        rc, info = _load_work_ex(self._lib.kgx_dptable_load_range, self._h, path, ctypes.c_uint64(int(max_entries)),
+                                 ctypes.c_void_p(int(stream)))
+        if rc == -28:                                            # -ENOSPC
+            raise TableFull(self._err())
+        if rc != 0:
+            raise RuntimeError("kgx_dptable_load_range: %s" % self._err())
         return info
 
     def _host(self):

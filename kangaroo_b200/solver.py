@@ -19,6 +19,10 @@ With --dp-table device, rank 0's table is ingest.DeviceDPTable in its GPU's memo
 records are copied device to device into a staging buffer and inserted from there by the ingest thread on its own stream, no
 host copy of them.  Its capacity is fixed; a full table stops the run (with --save-work, after writing the table it holds).
 
+With --dp-table sharded, every rank holds the device table of the buckets it owns and inserts them on an ingest thread of its
+own: the records go to their owners (dist.DPExchange) in place of the gather, and a per-step block from every rank brings rank
+0 the hits to claim (Solver._shard_round).  A full shard stops the run with the normal end-of-run save.
+
   single GPU :  python -m kangaroo_b200.solver in.txt --dp 12
   N GPUs     :  torchrun --nproc-per-node N -m kangaroo_b200.solver in.txt --dp 12
 
@@ -38,11 +42,13 @@ FILE: the work file of the cut followed by a batch block with every key, its sol
 (BatchSolver, kgx_workfile.h).
 """
 import argparse
+import collections
 import contextlib
 import ctypes
 import functools
 import os
 import queue
+import struct
 import sys
 import threading
 import time
@@ -51,7 +57,7 @@ import numpy as np
 
 from . import ecmath as ec
 from .engine import GPUEngine, NB_JUMP, NB_RUN, WILD, random_herd_arrays
-from .dist import DPGather, HerdGather, SlabView, DP40_BYTES, WALK_BYTES
+from .dist import DPExchange, DPGather, HerdGather, SlabView, DP40_BYTES, WALK_BYTES, owner_ranges
 from .ingest import DPTable, DeviceDPTable, TableFull, EV_RESET, EV_COLLISION
 
 ORDER = ec.N
@@ -81,6 +87,84 @@ def default_table_capacity(free_bytes, margin=DP_TABLE_MARGIN):
     while cap > 0 and DeviceDPTable.bytes_for(cap) > room:
         cap = cap * 63 // 64
     return int(min(cap, (1 << 32) - 2))
+
+
+def shard_headroom(world, max_found):
+    """--dp-table sharded: the entries a shard keeps free.  A step brings a shard at most world * max_found records, and a run
+    stopped at step k still inserts the launch in flight at its end, so a rank stops the run at the step where its bound plus
+    two steps' records would pass its capacity."""
+    return 2 * world * max_found
+
+
+def sharded_capacity_error(capacity, world, max_found=1 << 17):
+    """why --dp-table-capacity cannot be a shard's capacity on `world` ranks, or None"""
+    if capacity is not None and capacity <= shard_headroom(world, max_found):
+        return ("--dp-table sharded: a shard of capacity %d entries cannot hold the %d records two steps may bring on %d GPUs "
+                "(2 x GPUs x %d); give more than %d" % (capacity, shard_headroom(world, max_found), world, max_found,
+                                                        shard_headroom(world, max_found)))
+    return None
+
+
+# The per-step block of --dp-table sharded: every rank's report to rank 0, all gathered, a fixed number of int64 words.
+#   0 hits, 1 resets, 2 shard entries, 3 stop (0 no, 1 shard full, 2 insert failed), 4 work-file piece size (-1 none),
+#   5 piece written (0 no news, 1 ok, 2 failed), 6 busy (ingest work or reports outstanding), 7 herd chunks every rank moves
+#   after this round (rank 0's block, in the end-of-run drain; the control broadcast carries them during the run),
+#   then the stop message, the piece's error (BLOCK_MSG words of UTF-8 each), hits (key index, private key in 4 words, rank,
+#   kIdx) and resets (rank, kIdx).  Hits and resets over the caps wait for the next step.
+BLOCK_MSG = 32
+BLOCK_HITS = MAX_SOLVED
+BLOCK_WORDS = 8 + 2 * BLOCK_MSG + 7 * BLOCK_HITS + 2 * MAX_RESETS
+_M64 = (1 << 64) - 1
+
+
+def _msg_words(text):
+    raw = text.encode("utf-8", "replace")[:8 * BLOCK_MSG - 1]
+    return np.frombuffer(raw.ljust(8 * BLOCK_MSG, b"\0"), np.int64)
+
+
+def encode_block(hits, resets, count, stop=0, msg="", size=-1, done=0, err="", busy=0, chunks=0):
+    """-> (int64 array of BLOCK_WORDS, hits over the cap, resets over the cap)"""
+    b = np.zeros(BLOCK_WORDS, np.int64)
+    h, r = hits[:BLOCK_HITS], resets[:MAX_RESETS]
+    b[:8] = [len(h), len(r), count, stop, size, done, busy, chunks]
+    b[8:8 + BLOCK_MSG] = _msg_words(msg)
+    b[8 + BLOCK_MSG:8 + 2 * BLOCK_MSG] = _msg_words(err)
+    o = 8 + 2 * BLOCK_MSG
+    for i, (idx, priv, rk, kidx) in enumerate(h):
+        row = [idx] + [(priv >> (64 * k)) & _M64 for k in range(4)] + [rk, kidx]
+        b[o + 7 * i:o + 7 * i + 7] = np.array(row, np.uint64).view(np.int64)
+    o += 7 * BLOCK_HITS
+    for i, (rk, kidx) in enumerate(r):
+        b[o + 2 * i:o + 2 * i + 2] = [rk, kidx]
+    return b, hits[len(h):], resets[len(r):]
+
+
+def decode_block(b):
+    """encode_block's array -> dict(hits, resets, count, stop, msg, size, done, err, busy, chunks)"""
+    b = np.asarray(b, np.int64)
+    nh, nr = int(b[0]), int(b[1])
+    text = lambda w: w.tobytes().rstrip(b"\0").decode("utf-8", "replace")
+    o = 8 + 2 * BLOCK_MSG
+    hits = []
+    for i in range(nh):
+        w = [int(v) for v in b[o + 7 * i:o + 7 * i + 7].view(np.uint64)]
+        hits.append((w[0], sum(w[1 + k] << (64 * k) for k in range(4)), w[5], w[6]))
+    o += 7 * BLOCK_HITS
+    resets = [(int(b[o + 2 * i]), int(b[o + 2 * i + 1])) for i in range(nr)]
+    return dict(hits=hits, resets=resets, count=int(b[2]), stop=int(b[3]), msg=text(b[8:8 + BLOCK_MSG]), size=int(b[4]),
+                done=int(b[5]), err=text(b[8 + BLOCK_MSG:8 + 2 * BLOCK_MSG]), busy=int(b[6]), chunks=int(b[7]))
+
+
+def piece_offsets(sizes):
+    """where each shard's piece of a work file starts (after the 156-byte header), then where the table ends"""
+    return [156 + sum(sizes[:r]) for r in range(len(sizes) + 1)]
+
+
+def work_header(dp_bits, range_start, range_end, pub, total_count, total_time):
+    """the 156-byte HEADW header (Backup.cpp:368-394) the tables write"""
+    v = lambda x: int(x).to_bytes(32, "little")
+    return (struct.pack("<III", 0xFA6A8001, 0, int(dp_bits)) + v(range_start) + v(range_end) + v(pub[0]) + v(pub[1]) +
+            struct.pack("<Qd", int(total_count), float(total_time)))
 
 
 def create_jump_table(range_power):
@@ -148,14 +232,15 @@ class DeviceTable:
     take; the table's per-add scratch is reserved up front, so the table needs no allocation while it runs."""
     label = "device table"
 
-    def __init__(self, torch, n_records, device, capacity, wait_copy):
-        """wait_copy: the records' source is rewritten unordered with torch's stream (the engine's own buffer, on one GPU)"""
+    def __init__(self, torch, n_records, device, capacity, wait_copy, buckets=None):
+        """wait_copy: the records' source is rewritten unordered with torch's stream (the engine's own buffer, on one GPU).
+        buckets: (lo, hi) of a shard (ShardedTable)"""
         self.torch, self._wait_copy = torch, wait_copy
         self._bufs = [torch.empty(n_records * DP40_BYTES, dtype=torch.uint8, device=torch.device("cuda", device)) for _ in range(3)]
         self._back = self._bufs.pop()
         if not capacity:
             capacity = default_table_capacity(torch.cuda.mem_get_info(device)[0] - scratch_bytes(n_records))
-        self.dps = DeviceDPTable(capacity, device=device)
+        self.dps = DeviceDPTable(capacity, device=device, buckets=buckets)
         self.dps.reserve(n_records)
         self._stream = torch.cuda.Stream(device=device)
         self._i = 0
@@ -187,6 +272,16 @@ class DeviceTable:
         else:
             self._stream.wait_event(ev)                     # the records' copy into the staging buffer
         return self.dps.add(buf.data_ptr(), counts, stride, self._stream.cuda_stream)
+
+
+class ShardedTable(DeviceTable):
+    """--dp-table sharded: this rank's shard, a DeviceDPTable of the buckets the rank owns, fed what DPExchange brought it.
+    Its capacity is the shard's; save_piece writes its piece of a work file at an offset."""
+    label = "sharded table"
+
+    def __init__(self, torch, n_records, device, capacity, buckets):
+        super().__init__(torch, n_records, device, capacity, False, buckets)
+        self.save_piece = functools.partial(self.dps.save_piece, stream=self._stream.cuda_stream)
 
 
 class WorkFile:
@@ -268,16 +363,21 @@ class Solver:
         self.rng = np.random.Generator(np.random.PCG64((seed if seed is not None else int(time.time())) * 1000 + self.rank))
         sc, d128 = random_herd_arrays(n, self.range_power, self.wdiv2, self.rng)
         self._create_herd(sc, d128)
-        self.gather = DPGather(self.eng, self.dist, self.rank, self.world, torch, wire="dp40") if self.world > 1 else None
+        self.sharded = dp_table == "sharded"
+        self.gather = (DPGather(self.eng, self.dist, self.rank, self.world, torch, wire="dp40") if self.world > 1 and not self.sharded
+                       else None)
         # rank 0's table stopped taking records: "full" (TableFull) or "error" (any other failure of an insert), with its message
         self.table_msg, self.table_kind, self.table_stopped = None, None, False
+        self.shard_msg, self.shard_stop, self.exchange = None, False, None   # --dp-table sharded (_init_shard)
         self.last_saved = None              # rank 0: path of the last save that succeeded
         self.full_saved = None              # rank 0: (path, count, error or None) of the save a full table made
         self.parked = 0                     # rank 0: steps whose records waited in host RAM behind a save
         self.found = None                   # rank 0: the private key, once found
         self._announce = []                 # rank 0: keys solved, not yet in a control broadcast
         self.dpt = self.dps = None          # rank 0: HostTable / DeviceTable, and the table it holds
-        if self.rank == 0:
+        if self.sharded:
+            self._init_shard(max_found, dp_table_capacity)
+        elif self.rank == 0:
             self.dpt = (DeviceTable(torch, self.world * max_found, self.local, dp_table_capacity, self.gather is None)
                         if dp_table == "device" else HostTable(torch, self.world * max_found, ingest_threads))
             self.dps = self.dpt.dps
@@ -287,7 +387,7 @@ class Solver:
         self._acc_hits, self._acc_resets = [], []
         self._wf = None                     # ingest thread: the scheduled work file being written
         self._thread = None
-        if self.rank == 0:
+        if self.rank == 0 or self.sharded:
             self._thread = threading.Thread(target=self._ingest_loop, daemon=True)
             self._thread.start()
         self._ctrl = torch.zeros(5 + MAX_SOLVED + 2 * MAX_RESETS, dtype=torch.int64, device="cuda")
@@ -318,6 +418,146 @@ class Solver:
     def _create_herd(self, sc, d128):
         self.eng.CreateHerdRaw(sc, d128, self.key)
 
+    # -- --dp-table sharded ---------------------------------------------------------------------------------------------
+    # Every rank holds the shard of the buckets it owns (dist.owner_ranges) and runs an ingest thread of its own, one step
+    # behind like rank 0's.  Per step: DPExchange brings each rank the records of its buckets; each rank's main thread then
+    # sends every rank its block (encode_block: hits, resets, its shard's entries, a stop flag, its work-file piece's news), and
+    # rank 0 claims the hits of all of them before the control broadcast.  A work file of the cut decided at step k: each rank's
+    # ingest thread, right behind step k+1's records, reports its piece's size; once every size is in, every rank knows the
+    # offsets and its ingest thread writes its piece there; rank 0 writes the header first and the kangaroos after the last
+    # piece, and renames the file once every rank reported its piece written.
+    def _init_shard(self, max_found, capacity):
+        torch = self.torch
+        err = sharded_capacity_error(capacity, self.world, max_found)
+        if err:
+            raise ValueError(err)
+        self.buckets = owner_ranges(self.world)[self.rank]
+        self.headroom = shard_headroom(self.world, max_found)
+        self.dpt = ShardedTable(torch, self.world * max_found, self.local, capacity, self.buckets)
+        self.dps = self.dpt.dps
+        if self.dps.capacity <= self.headroom:
+            raise RuntimeError(sharded_capacity_error(self.dps.capacity, self.world, max_found))
+        self.exchange = DPExchange(self.eng, self.dist, self.rank, self.world, torch, max_found=max_found)
+        caps = [self.dps.capacity]
+        if self.dist is not None:
+            t = torch.tensor([self.dps.capacity], dtype=torch.int64, device="cuda")
+            g = torch.empty(self.world, dtype=torch.int64, device="cuda")
+            self.dist.all_gather_into_tensor(g, t)
+            caps = [int(v) for v in g.cpu().tolist()]
+        self.shard_caps = caps
+        self.dpt.info = ("dp table: sharded over %d GPUs, %d entries in all (rank 0: buckets [%d, %d), %d entries, %.2f GB)" %
+                         (self.world, sum(caps), self.buckets[0], self.buckets[1], caps[0], self.dps.memory_bytes() / 1e9))
+        self.shard_total = 0                # entries of all shards, as the last blocks reported them
+        self.shard_msg = None               # rank 0: why a full shard stopped the run
+        self.shard_stop = False             # every rank: a shard is full, the run ends with the normal end-of-run save
+        self._handed = collections.deque()  # records of the steps handed to the ingest thread and not yet inserted
+        self._handed_done = 0
+        self._ingested = 0                  # ingest thread: steps inserted; _shard_count: the shard's entries after them
+        self._shard_count = 0
+        self._piece_q = queue.Queue()       # ingest thread -> main: ("size", bytes) / ("done", error or None) of a piece
+        self._offsets_q = queue.Queue()     # main -> ingest thread: the offsets of every piece of the file being written
+        self._pieces_result = queue.Queue() # rank 0, main -> ingest thread: every piece written (None) or the first error
+        self._pieces_open = 0               # pieces queued on this rank whose "done" no block has carried yet
+        self._sizes, self._pstat = {}, {}
+
+    def _shard_round(self, drain=False):
+        """every rank, once per step (and in the end-of-run drain): the blocks of all ranks.  -> (hits, resets) of every rank on
+        rank 0, ([], []) elsewhere; and whether any rank still has work or news outstanding"""
+        torch = self.torch
+        hits, resets = self._harvest()
+        done = self._ingested
+        while self._handed_done < done:
+            self._handed.popleft()
+            self._handed_done += 1
+        count = self._shard_count
+        bound = count + sum(self._handed)
+        stop, msg = 0, ""
+        if self.table_msg is not None:
+            stop, msg = 2, "shard %d: %s" % (self.rank, self.table_msg)
+        elif not drain and bound + self.headroom > self.dps.capacity:
+            stop, msg = 1, ("shard %d of %d (buckets [%d, %d)) holds up to %d entries of its capacity %d, and the next two steps "
+                            "may bring %d" % (self.rank, self.world, self.buckets[0], self.buckets[1], bound, self.dps.capacity,
+                                              self.headroom))
+        size, pdone, perr = -1, 0, ""
+        if not self._piece_q.empty():
+            kind, v = self._piece_q.get()
+            if kind == "size":
+                size = v
+            else:
+                pdone, perr = (1, "") if v is None else (2, v)
+                self._pieces_open -= 1
+        busy = int(self._pending > 0 or self._pieces_open > 0 or self._saving)
+        chunks = 0                                      # the drain moves herd chunks as rank 0's writer frees buffers
+        if drain and self.rank == 0 and self._saving:
+            chunks = min(len(self._save_left), self._chunk_pool.qsize())
+        blk, self._acc_hits, self._acc_resets = encode_block(hits, resets, count, stop, msg, size, pdone, perr, busy, chunks)
+        busy |= int(len(self._acc_hits) > 0 or len(self._acc_resets) > 0)
+        blk[6] = busy
+        if self.dist is not None:
+            mine = torch.from_numpy(blk).to("cuda")
+            allb = torch.empty(self.world * BLOCK_WORDS, dtype=torch.int64, device="cuda")
+            self.dist.all_gather_into_tensor(allb, mine)
+            blocks = [decode_block(b) for b in allb.cpu().numpy().reshape(self.world, BLOCK_WORDS)]
+        else:
+            blocks = [decode_block(blk)]
+        for r, b in enumerate(blocks):
+            if b["size"] >= 0:
+                self._sizes[r] = b["size"]
+            if b["done"]:
+                self._pstat[r] = b["err"] if b["done"] == 2 else None
+        if len(self._sizes) == self.world:              # every piece's size: the offsets (the same on every rank)
+            self._offsets_q.put(piece_offsets([self._sizes[r] for r in range(self.world)]))
+            self._sizes = {}
+        if len(self._pstat) == self.world:              # every piece written or failed
+            if self.rank == 0:
+                errs = ["rank %d: %s" % (r, self._pstat[r]) for r in range(self.world) if self._pstat[r] is not None]
+                self._pieces_result.put("; ".join(errs) if errs else None)
+            self._pstat = {}
+        self.shard_total = sum(b["count"] for b in blocks)
+        self._shard_busy = any(b["busy"] for b in blocks)
+        self._drain_chunks = blocks[0]["chunks"]
+        if self.rank != 0:
+            return [], []
+        for r, b in enumerate(blocks):
+            if b["stop"] == 2 and self.table_msg is None:
+                self.table_msg, self.table_kind = b["msg"], "error"
+            elif b["stop"] == 1 and self.shard_msg is None:
+                self.shard_msg = b["msg"]
+        return [h for b in blocks for h in b["hits"]], [rk for b in blocks for rk in b["resets"]]
+
+    def _shard_drain(self):
+        """every rank, after the loop: blocks go round until every rank's records are inserted, its hits reported and the
+        save in progress done: its herd chunks moved, as rank 0's writer frees buffers (that writer waits for the pieces'
+        offsets, which only these rounds bring), and its pieces written"""
+        while True:
+            if (self._pending or self._pieces_open or self._saving) and self._done.empty() and self._piece_q.empty():
+                time.sleep(0.002)
+            hits, _ = self._shard_round(drain=True)
+            if self.rank == 0:
+                self._claim(hits, [])
+            if self._drain_chunks:
+                self._save_progress(self._drain_chunks)
+            if not self._shard_busy:
+                return
+
+    def _write_piece(self, err):
+        """ingest thread, behind the cut's records: this shard's piece of the file -> the offset where the table ends"""
+        self._piece_q.put(("size", self.dps.piece_bytes()))
+        offsets = self._offsets_q.get()
+        if err is None and self.table_msg is not None:
+            err = "the DP table lacks DPs of the launches this file would count (%s)" % self.table_msg
+        if err is None:
+            try:
+                self.dpt.save_piece(self.save_path + ".tmp", offsets[self.rank])
+            except RuntimeError as e:
+                err = str(e)
+        self._piece_q.put(("done", err))
+        return offsets[-1]
+
+    def table_entries(self):
+        """entries of the DP table (every shard's, as last reported, with --dp-table sharded)"""
+        return self.shard_total if self.sharded else len(self.dps)
+
     # -- work files ------------------------------------------------------------------------------------------------
     def _resume(self, path):
         """Kangaroo::LoadWork + FetchWalks (Backup.cpp:149-231): rank 0 loads the table; rank r takes the file's kangaroos
@@ -325,8 +565,8 @@ class Solver:
         file lacks keep the fresh random herd made above.  Only rank 0 reads the file; it sends every rank its records."""
         torch = self.torch
         info = torch.zeros(4, dtype=torch.int64, device="cuda")
+        w = self._load_table(path)
         if self.rank == 0:
-            w = self.dps.load_work_ex(path)
             info.copy_(torch.tensor([w.nb_walk, w.walk_offset, w.total_count, 0], dtype=torch.int64))
             self.time_offset = w.total_time
         if self.dist is not None:
@@ -336,7 +576,7 @@ class Solver:
         take = max(0, min(self.eng.nbKangaroo, nb_walk - self.herd.offsets[self.rank]))
         if self.rank == 0:
             print("Resume %s: %d DPs, count 2^%.2f, %d kangaroos in the file for %d in the herd" %
-                  (path, len(self.dps), np.log2(max(count, 1)), nb_walk, self.herd.total), flush=True)
+                  (path, self.table_entries(), np.log2(max(count, 1)), nb_walk, self.herd.total), flush=True)
             if nb_walk > self.herd.total:
                 print("Warning: %d unhandled kangaroos" % (nb_walk - self.herd.total), flush=True)   # Kangaroo.cpp FectchKangaroos
 
@@ -356,6 +596,37 @@ class Solver:
         if take:
             print("rank %d: %d kangaroos imported and verified in %.2f s" % (self.rank, take, time.perf_counter() - t0), flush=True)
 
+    def _load_table(self, path):
+        """the file's table into rank 0's table -> its WorkInfo on rank 0, None elsewhere.  --dp-table sharded: every rank
+        loads its buckets; a shard the file's entries would leave less than the stop headroom refuses the run on every rank,
+        before the first step."""
+        if not self.sharded:
+            return self.dps.load_work_ex(path) if self.rank == 0 else None
+        torch = self.torch
+        limit = self.dps.capacity - self.headroom
+        w, err = None, None
+        try:
+            w = self.dps.load_piece(path, limit)
+        except TableFull as e:
+            err = e
+        flags = [1 if err is not None else 0, len(self.dps)]
+        if self.dist is not None:
+            t = torch.tensor(flags, dtype=torch.int64, device="cuda")
+            g = torch.empty(2 * self.world, dtype=torch.int64, device="cuda")
+            self.dist.all_gather_into_tensor(g, t)
+            flags = [int(v) for v in g.cpu().tolist()]
+        refused = [r for r in range(self.world) if flags[2 * r]]
+        if refused:
+            r = refused[0]
+            lo, hi = owner_ranges(self.world)[r]
+            raise RuntimeError("--dp-table sharded: %s: buckets [%d, %d) of shard %d hold more than its capacity %d less the stop "
+                               "headroom %d (%d entries); resume it on more GPUs, with a larger --dp-table-capacity or "
+                               "--dp-table host" % (path, lo, hi, r, self.shard_caps[r], self.headroom,
+                                                    self.shard_caps[r] - self.headroom))
+        self.shard_total = sum(flags[1::2])
+        self._shard_count = len(self.dps)
+        return w
+
     def _export(self, first, count, dst):
         self.eng.SnapshotExport(first, count, dst.data_ptr())
 
@@ -370,12 +641,16 @@ class Solver:
         self._save_left = list(range(len(self.herd.plan))) if kangaroos else []
         self._save_steps = []                                  # times of the steps that moved this save
         self._save_stats.append(self._save_steps)
+        if self.sharded:
+            self._pieces_open += 1                             # every rank writes its piece of the table
         if self.rank == 0:
             nwalk = self.herd.total if kangaroos else 0
             self._work.put(("begin", self.jumps, self.time_offset + time.time() - self.t_start, nwalk, time.perf_counter(),
                             self._cut(kangaroos)))
         else:
             self._cut(kangaroos)                               # every rank takes part (--batch-keys: the targets' gather)
+            if self.sharded:
+                self._work.put(("piece",))
         self._save_progress(chunks)
 
     def _save_progress(self, chunks):
@@ -400,10 +675,14 @@ class Solver:
         if kind == "begin":
             count, total_time, nwalk, t0, self._wf_cut = job[1:]
             self._wf = WorkFile(self.save_path, t0)
-            if self.table_msg is not None:
+            if self.sharded:
+                self._begin_sharded(self._wf, count, total_time, nwalk)
+            elif self.table_msg is not None:
                 self._wf.err = "the DP table lacks DPs of the launches this file would count (%s)" % self.table_msg
             else:
                 self._write_table(self._wf, count, total_time, nwalk)
+        elif kind == "piece":
+            self._write_piece(None)
         elif kind == "chunk":
             buf, nbytes = job[1], job[2]
             try:
@@ -412,8 +691,29 @@ class Solver:
                 self._chunk_pool.put(buf)
         else:
             self._end_file(self._wf, self._wf_cut)
+            if self.sharded:                                   # the other ranks' pieces: written, or the first error
+                err = self._pieces_result.get()
+                if err is not None and self._wf.err is None:
+                    self._wf.err = err
             self._finish(self._wf, scheduled=True)
             self._wf = None
+
+    def _begin_sharded(self, wf, count, total_time, nwalk):
+        """rank 0's ingest thread: FILE.tmp with the header (a new file: no other rank writes before every size is in, which
+        needs this rank's), this shard's piece, then the kangaroo count after the last piece"""
+        try:
+            with open(wf.tmp, "wb") as f:
+                f.write(work_header(self.dp_bits, self.start, self.end, self.pub, count, total_time))
+        except OSError as e:
+            wf.err = str(e)
+        end = self._write_piece(wf.err)
+        if wf.err is None:
+            try:
+                wf.f = open(wf.tmp, "r+b")
+                wf.f.seek(end)
+                wf.f.write(struct.pack("<Q", int(nwalk)))
+            except OSError as e:
+                wf.err = str(e)
 
     def _write_table(self, wf, count, total_time, nwalk):
         wf.begin(lambda tmp: self.dpt.save(tmp, self.dp_bits, self.start, self.end, self.pub, total_count=count,
@@ -455,15 +755,21 @@ class Solver:
                   (path, mb, secs, len(st), 1e3 * max(st or [0]), 1e3 * float(np.median(self._step_times[-64:] or [0]))), flush=True)
 
     # -- rank 0: ingest -------------------------------------------------------------------------------------------
-    def _events(self, batch, jumps_before):
+    def _events(self, batch, jumps_before, malformed=0):
         """the table's events for one step's records"""
         if self.table_msg is not None:                  # the run is stopping: later steps' DPs are not inserted
             return []
         try:
-            return self.dpt.insert(batch)
+            ev = self.dpt.insert(batch)
         except TableFull as e:
-            self._on_full(str(e), jumps_before)
+            if self.sharded:                            # the stop rule keeps a shard from filling: an error if it does
+                self.table_msg, self.table_kind = str(e), "full"
+            else:
+                self._on_full(str(e), jumps_before)
             return []
+        if malformed:
+            raise RuntimeError("kgx_dp_partition: %d malformed DP records (h >= 2^18)" % malformed)
+        return ev
 
     def _on_full(self, msg, jumps_before):
         """ingest thread: the table cannot take this step's records.  With --save-work, and no save open, the table is written
@@ -510,11 +816,14 @@ class Solver:
                     if self.table_msg is None:          # leaving the main thread waiting for this step's result
                         self.table_msg, self.table_kind = "%s: %s" % (type(e).__name__, e), "error"
                     res = [], []
+                if self.sharded:                        # the count first: the main thread's bound may only overestimate
+                    self._shard_count = len(self.dps)
+                    self._ingested += 1
                 self._done.put(res)
             else:
                 self._write(job)
 
-    def _submit(self, counts, stride, src, jumps_before):
+    def _submit(self, counts, stride, src, jumps_before, malformed=0):
         """hand one step's records (counts[r] of rank r at src[r*stride*40:], device memory) to the ingest thread.  At most
         one older step may still be in that thread, reading the other staging buffer.  While a save keeps it busy, further
         steps are parked in host RAM instead of waiting: the step loop never waits for the disk, and the backlog takes no GPU
@@ -524,10 +833,14 @@ class Solver:
             self.parked += 1
         while not park and self._pending >= 2:
             self._take()
-        self._work.put(("dps", self.dpt.stage(counts, stride, src, park), jumps_before))
+        if self.sharded:
+            self._handed.append(sum(counts))
+        self._work.put(("dps", self.dpt.stage(counts, stride, src, park), jumps_before, malformed))
         self._pending += 1
 
     def _writes_pending(self):
+        if self.sharded:                                # an ingest thread waits for the offsets of its piece meanwhile
+            return self._saving or self._pieces_open > 0 or (self.rank == 0 and len(self._save_stats) > 0)
         return self._saving or len(self._save_stats) > 0
 
     def _take(self):
@@ -579,13 +892,19 @@ class Solver:
             self._save_start(self.save_kangaroos, self._chunks_next)     # behind launch i+1's DPs: the cut
         elif self._saving:
             self._save_progress(self._chunks_next)
+        if self.sharded:
+            hits, resets = self._shard_round()
         if self.rank == 0:
-            hits, resets = self._harvest()
+            if not self.sharded:
+                hits, resets = self._harvest()
             self._claim(hits, resets)
             solved, self._announce = self._announce[:MAX_SOLVED], self._announce[MAX_SOLVED:]
             self.table_stopped = self.table_msg is not None
+            self.shard_stop = self.sharded and self.shard_msg is not None
         save_next = (may_save and self.save_interval > 0 and self.rank == 0 and not self._saving and
                      time.time() - self._last_save >= self.save_interval)
+        if self.sharded:                                                 # one file at a time: its pieces share FILE.tmp
+            save_next = save_next and not self._save_stats
         # herd chunks the next step may move: only into pinned buffers the writer has already freed, so a step never waits for
         # the disk (rank 0 decides, every rank follows)
         chunks = min(SAVE_CHUNKS_PER_STEP, self._chunk_pool.qsize()) if self.rank == 0 else 0
@@ -593,15 +912,17 @@ class Solver:
         if self.dist is not None:
             if self.rank == 0:
                 resets = resets[:MAX_RESETS]
-                c = [int(self.table_stopped), len(resets), int(save_next), chunks, len(solved)] + solved + \
+                c = [2 if self.shard_stop and not self.table_stopped else int(self.table_stopped), len(resets), int(save_next), chunks,
+                     len(solved)] + solved + \
                     [v for rk in resets for v in rk]
                 self._ctrl[:len(c)].copy_(torch.tensor(c, dtype=torch.int64))
             self.dist.broadcast(self._ctrl, 0)
             c = self._ctrl.cpu().tolist()
-            self.table_stopped, save_next, chunks, ns = bool(c[0]), bool(c[2]), c[3], c[4]
+            self.table_stopped, save_next, chunks, ns = c[0] == 1, bool(c[2]), c[3], c[4]
+            self.shard_stop = c[0] == 2
             solved = c[5:5 + ns]
             resets = [(c[5 + ns + 2 * i], c[6 + ns + 2 * i]) for i in range(c[1])]
-        self.stop = self._solved(solved) or self.table_stopped          # (--batch-keys: retargets, before the resets below)
+        self.stop = self._solved(solved) or self.table_stopped or self.shard_stop   # (--batch-keys: retargets, before the resets)
         self._chunks_next = chunks
         if save_next and not self.stop:
             if self.save_kangaroos:
@@ -618,7 +939,10 @@ class Solver:
         jumps_before = self.jumps
         self.jumps += self.eng.nbKangaroo * NB_RUN * self.world
         res = None
-        if self.gather is not None:
+        if self.sharded:
+            counts, cap, recv, bad = self.exchange.step(cnt)                # every rank: the records of its buckets
+            self._submit(counts, cap, recv, jumps_before, bad)
+        elif self.gather is not None:
             res = self.gather.step_flat(cnt)                             # rank 0: (counts, cap, device tensor [world*cap*40])
         elif cnt:
             ptr = self.eng.convert_dps_device_ptr()
@@ -647,11 +971,13 @@ class Solver:
             if verbose and self.rank == 0 and (s % 64 == 63 or self.stop):
                 dt = time.time() - t0
                 print("[%6.1fs] 2^%.2f jumps  %.0f MJump/s  %d DPs  dead %d  %s %.1f ms/step" %
-                      (dt, np.log2(max(self.jumps, 1)), (self.jumps - self.jumps0) / dt / 1e6, len(self.dps), self.same_herd,
+                      (dt, np.log2(max(self.jumps, 1)), (self.jumps - self.jumps0) / dt / 1e6, self.table_entries(), self.same_herd,
                        self.dpt.label, 1e3 * self.t_ingest / steps), flush=True)
             if self.stop:
                 break
-        if self._saving:                                        # a save still moving its herd: finish it first
+        if self.sharded:                                        # a save in progress: finish it first
+            self._shard_drain()
+        elif self._saving:                                      # a save still moving its herd: finish it first
             self._save_progress(len(self._save_left))
         if self.save_path and not self.table_stopped:
             # end-of-run cut: the launch still in flight is collected, its DPs go into the table before it is written
@@ -661,8 +987,10 @@ class Solver:
         else:
             self.eng.sync()
         t1 = time.time()
-        if self.save_path and not self.table_stopped:
-            self._save_start(self.save_kangaroos, len(self.herd.plan) if self.save_kangaroos else 0)
+        if self.save_path and not self.table_stopped:           # (sharded: the drain below moves the herd chunks)
+            self._save_start(self.save_kangaroos, len(self.herd.plan) if self.save_kangaroos and not self.sharded else 0)
+        if self.sharded:
+            self._shard_drain()
         if self.rank == 0:                                      # drain: the last steps' records may still be in the ingest thread
             self._claim(*self._harvest(wait_all=True))
             self._report_saves(block_for=len(self._save_stats))
@@ -784,8 +1112,8 @@ class BatchSolver(Solver):
         fresh herd spread over the live keys."""
         torch = self.torch
         info = torch.zeros(4, dtype=torch.int64, device="cuda")
+        w = self._load_table(path)
         if self.rank == 0:
-            w = self.dps.load_work_ex(path)
             info.copy_(torch.tensor([w.nb_walk, w.walk_offset, w.total_count, 0], dtype=torch.int64))
             self.time_offset = w.total_time
         if self.dist is not None:
@@ -797,7 +1125,7 @@ class BatchSolver(Solver):
         if self.rank == 0:
             tg = self._resume_block.targets
             print("Resume %s: %d DPs, count 2^%.2f, %d kangaroos in the file for %d in the herd, %d of %d keys solved in the file, "
-                  "%d keys left to search" % (path, len(self.dps), np.log2(max(count, 1)), nb_walk, self.herd.total,
+                  "%d keys left to search" % (path, self.table_entries(), np.log2(max(count, 1)), nb_walk, self.herd.total,
                                               sum(self._resume_block.solved), len(self.keys), len(self.live)), flush=True)
             if nb_walk > self.herd.total:
                 print("Warning: %d unhandled kangaroos" % (nb_walk - self.herd.total), flush=True)
@@ -930,7 +1258,7 @@ def _run_batch(start, end, pubs, dp, grid, a, block=None):
         rc |= solved < len(pubs)
         print("Batch: %d/%d keys solved, %d jumps (2^%.2f) in total, %.3f sqrt(N) jumps per key (N = 2^%d), %d DPs" %
               (solved, len(pubs), s.jumps, np.log2(max(s.jumps, 1)), s.jumps / len(pubs) / 2.0 ** (s.range_power / 2),
-               s.range_power, len(s.dps)), flush=True)
+               s.range_power, s.table_entries()), flush=True)
     t_results = time.perf_counter() - t0
     t0 = time.perf_counter()
     s.close()
@@ -949,7 +1277,10 @@ def report(s, a):
     print("Solver rate: %.0f MJump/s steady state (after the first 32 steps), %.0f MJump/s over all %d steps (%.2f s); "
           "rank-0 %s %.2f ms/step; %d DPs; %d dead kangaroos re-created" %
           (s.steady_rate / 1e6, (s.jumps - s.jumps0) / s.elapsed / 1e6, s.steps, s.elapsed, s.dpt.label,
-           1e3 * s.t_ingest / max(s.steps, 1), len(s.dps), s.same_herd))
+           1e3 * s.t_ingest / max(s.steps, 1), s.table_entries(), s.same_herd))
+    if s.shard_stop and not s.table_stopped:
+        print("DP table shard full, run stopped: %s.  Resume the work file with a larger --dp-table-capacity, on more GPUs or with "
+              "--dp-table host" % s.shard_msg)
     if s.table_stopped:
         print(table_message(s, a))
         return 1
@@ -1071,13 +1402,17 @@ def main(argv=None):
     ap.add_argument("--save-kangaroos", action="store_true", help="save every rank's herd with the table (-ws)")
     ap.add_argument("--resume", default="", metavar="FILE",
                     help="continue from a work file (-i): range, key and dp come from the file unless given")
-    ap.add_argument("--dp-table", choices=("host", "device"), default="host",
-                    help="where rank 0 keeps the DP table: host = the reference's HashTable in host RAM, inserted by "
+    ap.add_argument("--dp-table", choices=("host", "device", "sharded"), default="host",
+                    help="where the DP table is kept: host = the reference's HashTable in rank 0's host RAM, inserted by "
                          "--ingest-threads workers; device = a hash table with the same results in rank 0's GPU memory, inserted "
-                         "by CUDA kernels straight from the gathered records (fixed capacity: a full table stops the run)")
+                         "by CUDA kernels straight from the gathered records (fixed capacity: a full table stops the run); "
+                         "sharded = the device table split by bucket over every rank's GPU, each rank inserting the records of its "
+                         "buckets (a full shard stops the run with the normal end-of-run work file; every rank writes its piece of "
+                         "a work file into FILE.tmp itself, so FILE's directory must be one file system for all ranks)")
     ap.add_argument("--dp-table-capacity", type=int, default=None, metavar="ENTRIES",
                     help="--dp-table device: entries the table holds, 48 bytes of GPU memory each (default: what fits in rank "
-                         "0's free GPU memory after the engine, less %d GiB)" % (DP_TABLE_MARGIN >> 30))
+                         "0's free GPU memory after the engine, less %d GiB); --dp-table sharded: entries of each GPU's shard "
+                         "(default: the same rule on each GPU)" % (DP_TABLE_MARGIN >> 30))
     ap.add_argument("--batch-keys", action="store_true",
                     help="solve every key of the config in one run: one tame herd and one DP table shared by all keys, the "
                          "wild kangaroos spread over the unsolved ones")
@@ -1099,10 +1434,12 @@ def main(argv=None):
         ap.error("--batch-save-interval needs --batch-save FILE")
     if a.batch_keys and not a.config and not a.batch_resume:
         ap.error("--batch-keys needs a config file")
-    if a.dp_table_capacity is not None and a.dp_table != "device":
-        ap.error("--dp-table-capacity needs --dp-table device")
+    if a.dp_table_capacity is not None and a.dp_table not in ("device", "sharded"):
+        ap.error("--dp-table-capacity needs --dp-table device or sharded")
     if a.dp_table_capacity is not None and not 0 < a.dp_table_capacity < (1 << 32) - 1:
         ap.error("--dp-table-capacity must be 1 .. 2^32-2 entries, not %d" % a.dp_table_capacity)
+    if a.dp_table == "sharded" and sharded_capacity_error(a.dp_table_capacity, int(os.environ.get("WORLD_SIZE", "1"))):
+        ap.error(sharded_capacity_error(a.dp_table_capacity, int(os.environ.get("WORLD_SIZE", "1"))))
     block = None
     if a.batch_resume:
         res = batch_resume_file(a.batch_resume)
