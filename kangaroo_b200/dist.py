@@ -120,6 +120,30 @@ class HerdGather:
         self.chunk_records = int(chunk)
         self.plan = [(r, first, min(self.chunk_records, n - first)) for r, n in enumerate(self.sizes) for first in range(0, n, self.chunk_records)]
         self._buf = None
+        # gloo's send / recv take host tensors only: under gloo every chunk crosses through a host buffer of the same size
+        self._staged = dist is not None and world > 1 and dist.get_backend() == "gloo"
+        self._host = None
+
+    def _host_view(self, nbytes):
+        if self._host is None:
+            self._host = self.torch.empty(self.chunk_records * WALK_BYTES, dtype=self.torch.uint8,
+                                          pin_memory=self.device.type == "cuda")
+        return self._host[:nbytes]
+
+    def _send(self, view, dst):
+        if self._staged:
+            h = self._host_view(view.numel())
+            h.copy_(view)
+            view = h
+        self.dist.send(view, dst=dst)
+
+    def _recv(self, view, src):
+        if self._staged:
+            h = self._host_view(view.numel())
+            self.dist.recv(h, src=src)
+            view.copy_(h)
+        else:
+            self.dist.recv(view, src=src)
 
     def chunk(self, j, export):
         """Move chunk j of the plan to rank 0.  export(first, count, dst) writes this rank's records [first, first+count)
@@ -135,9 +159,9 @@ class HerdGather:
             export(first, count, view)
         if r != 0:
             if self.rank == r:
-                self.dist.send(view, dst=0)
+                self._send(view, 0)
             else:
-                self.dist.recv(view, src=r)
+                self._recv(view, r)
             if self.device.type == "cuda":
                 self.torch.cuda.current_stream().synchronize()   # the next export rewrites the buffer from another stream
         return view if self.rank == 0 else None
@@ -160,9 +184,9 @@ class HerdGather:
                 view.copy_(self.torch.from_numpy(read(self.offsets[r] + first, count)))
             if r != 0:
                 if self.rank == 0:
-                    self.dist.send(view, dst=r)
+                    self._send(view, r)
                 else:
-                    self.dist.recv(view, src=0)
+                    self._recv(view, 0)
                 if self.device.type == "cuda":
                     self.torch.cuda.current_stream().synchronize()
             if self.rank == r:

@@ -72,6 +72,24 @@ DP_TABLE_MARGIN = 4 << 30 # --dp-table device without a capacity: rank 0's free 
                           # and torch's allocator.  Nothing else grows on the GPU: steps queued behind a save wait in host RAM
 
 
+def init_dist():
+    """torch.distributed for a multi-GPU run (WORLD_SIZE > 1), started once per process -> the module.  The backend comes from
+    KGX_DIST_BACKEND: nccl (the default, one GPU per rank) or gloo, which lets several ranks share one GPU (the tests run a
+    multi-rank solver on one GPU that way).  The collectives stay on CUDA tensors either way; HerdGather stages its
+    point-to-point chunks through host memory under gloo."""
+    import torch
+    import torch.distributed as dist
+    local = int(os.environ.get("LOCAL_RANK", "0"))
+    torch.cuda.set_device(local)
+    if not dist.is_initialized():
+        backend = os.environ.get("KGX_DIST_BACKEND", "nccl")
+        if backend == "nccl":
+            dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+        else:
+            dist.init_process_group(backend)
+    return dist
+
+
 def scratch_bytes(n_records):
     """GPU memory of the device table's per-add scratch for adds of up to n_records records (kgx_dptable_reserve), rounded up"""
     m = 1024
@@ -341,12 +359,7 @@ class Solver:
         self.world = int(os.environ.get("WORLD_SIZE", "1"))
         self.local = int(os.environ.get("LOCAL_RANK", "0"))
         torch.cuda.set_device(self.local)
-        self.dist = None
-        if self.world > 1:
-            import torch.distributed as dist
-            if not dist.is_initialized():
-                dist.init_process_group("nccl", device_id=torch.device("cuda", self.local))
-            self.dist = dist
+        self.dist = init_dist() if self.world > 1 else None
         self.start, self.end, self.pub, self.dp_bits = start, end, pub, dp_bits
         width = end - start
         self.range_power = width.bit_length()                         # Kangaroo::InitRange (:877-890)
@@ -392,8 +405,12 @@ class Solver:
             self._thread.start()
         self._ctrl = torch.zeros(5 + MAX_SOLVED + 2 * MAX_RESETS, dtype=torch.int64, device="cuda")
         self.jumps = 0
-        self.same_herd = 0
-        self.resets_done = 0
+        self.same_herd = 0                  # every rank: kangaroos listed to re-create by the control broadcasts
+        self.resets_done = 0                # every rank: kangaroos of its herd re-created
+        self.resets_reported = 0            # rank 0: dead kangaroos the table reported during the run, and the most in one step
+        self.resets_most = 0
+        self.recreated = 0                  # after run(): kangaroos re-created on every rank
+        self._reset_backlog = []            # rank 0: resets past MAX_RESETS of a broadcast, sent first in the next one
         self.t_ingest = 0.0
         self.stop = False
         self.save_path, self.save_interval, self.save_kangaroos = save_work, float(save_interval), bool(save_kangaroos)
@@ -448,6 +465,7 @@ class Solver:
         self.dpt.info = ("dp table: sharded over %d GPUs, %d entries in all (rank 0: buckets [%d, %d), %d entries, %.2f GB)" %
                          (self.world, sum(caps), self.buckets[0], self.buckets[1], caps[0], self.dps.memory_bytes() / 1e9))
         self.shard_total = 0                # entries of all shards, as the last blocks reported them
+        self.shard_hits = [0] * self.world  # rank 0: collisions resolved to a key on each shard
         self.shard_msg = None               # rank 0: why a full shard stopped the run
         self.shard_stop = False             # every rank: a shard is full, the run ends with the normal end-of-run save
         self._handed = collections.deque()  # records of the steps handed to the ingest thread and not yet inserted
@@ -519,6 +537,7 @@ class Solver:
         if self.rank != 0:
             return [], []
         for r, b in enumerate(blocks):
+            self.shard_hits[r] += len(b["hits"])
             if b["stop"] == 2 and self.table_msg is None:
                 self.table_msg, self.table_kind = b["msg"], "error"
             elif b["stop"] == 1 and self.shard_msg is None:
@@ -898,6 +917,8 @@ class Solver:
             if not self.sharded:
                 hits, resets = self._harvest()
             self._claim(hits, resets)
+            self.resets_reported += len(resets)
+            self.resets_most = max(self.resets_most, len(resets))
             solved, self._announce = self._announce[:MAX_SOLVED], self._announce[MAX_SOLVED:]
             self.table_stopped = self.table_msg is not None
             self.shard_stop = self.sharded and self.shard_msg is not None
@@ -908,10 +929,13 @@ class Solver:
         # herd chunks the next step may move: only into pinned buffers the writer has already freed, so a step never waits for
         # the disk (rank 0 decides, every rank follows)
         chunks = min(SAVE_CHUNKS_PER_STEP, self._chunk_pool.qsize()) if self.rank == 0 else 0
-        # control word: table stopped + save flag + chunks + keys solved + kangaroos to re-create, back to their owners
+        # control word: table stopped + save flag + chunks + keys solved + kangaroos to re-create, back to their owners.  Resets
+        # past MAX_RESETS wait for the next step's broadcast, ahead of that step's own (a kangaroo listed twice meanwhile is
+        # re-created twice: harmless)
         if self.dist is not None:
             if self.rank == 0:
-                resets = resets[:MAX_RESETS]
+                resets = self._reset_backlog + resets
+                resets, self._reset_backlog = resets[:MAX_RESETS], resets[MAX_RESETS:]
                 c = [2 if self.shard_stop and not self.table_stopped else int(self.table_stopped), len(resets), int(save_next), chunks,
                      len(solved)] + solved + \
                     [v for rk in resets for v in rk]
@@ -994,6 +1018,11 @@ class Solver:
         if self.rank == 0:                                      # drain: the last steps' records may still be in the ingest thread
             self._claim(*self._harvest(wait_all=True))
             self._report_saves(block_for=len(self._save_stats))
+        self.recreated = self.resets_done
+        if self.dist is not None:                               # the kangaroos every rank re-created, for rank 0's report
+            t = self.torch.tensor([self.resets_done], dtype=self.torch.int64, device="cuda")
+            self.dist.all_reduce(t)
+            self.recreated = int(t.item())
         self.elapsed = t1 - t0
         self.steps = steps
         self.steady_rate = ((self.jumps - self.steady[1]) / (t1 - self.steady[0]) if self.steady and steps > 64
@@ -1275,9 +1304,11 @@ def report(s, a):
     """rank 0, after the run: the rate line, then why the table stopped the run or where the work file went -> 1 when the
     table stopped the run or the work file was not written, else 0"""
     print("Solver rate: %.0f MJump/s steady state (after the first 32 steps), %.0f MJump/s over all %d steps (%.2f s); "
-          "rank-0 %s %.2f ms/step; %d DPs; %d dead kangaroos re-created" %
+          "rank-0 %s %.2f ms/step; %d DPs; %d dead kangaroos re-created (%d reported by the table, at most %d in one step)" %
           (s.steady_rate / 1e6, (s.jumps - s.jumps0) / s.elapsed / 1e6, s.steps, s.elapsed, s.dpt.label,
-           1e3 * s.t_ingest / max(s.steps, 1), s.table_entries(), s.same_herd))
+           1e3 * s.t_ingest / max(s.steps, 1), s.table_entries(), s.recreated, s.resets_reported, s.resets_most))
+    if s.sharded:
+        print("Hits resolved per shard: %s" % " ".join(str(v) for v in s.shard_hits))
     if s.shard_stop and not s.table_stopped:
         print("DP table shard full, run stopped: %s.  Resume the work file with a larger --dp-table-capacity, on more GPUs or with "
               "--dp-table host" % s.shard_msg)
@@ -1329,12 +1360,7 @@ def _resume_header(path):
         h = read_work_header(path)
         hdr = (h.dp_bits, h.range_start, h.range_end, h.key)
     if world > 1:
-        import torch
-        import torch.distributed as dist
-        local = int(os.environ.get("LOCAL_RANK", "0"))
-        torch.cuda.set_device(local)
-        if not dist.is_initialized():
-            dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+        dist = init_dist()
         box = [hdr]
         dist.broadcast_object_list(box, 0)
         hdr = box[0]
@@ -1359,13 +1385,8 @@ def batch_resume_file(path):
         except (OSError, RuntimeError, ValueError) as e:
             res = "cannot resume %s: %s" % (path, e)
     if world > 1:
-        import torch
-        import torch.distributed as dist
         from .worktool import BatchBlock
-        local = int(os.environ.get("LOCAL_RANK", "0"))
-        torch.cuda.set_device(local)
-        if not dist.is_initialized():
-            dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+        dist = init_dist()
         box = [res if isinstance(res, str) or res is None else
                res[:3] + (BatchBlock(res[3].pubs, res[3].solved, res[3].privs, np.zeros(0, np.uint16), res[3].offset),)]
         dist.broadcast_object_list(box, 0)

@@ -166,14 +166,11 @@ def test_batch_resume_finishes_the_keys(stopped_run, table, tmp_path):
 
 @needs_ingest
 def test_batch_resume_with_the_config_and_on_two_gpus(stopped_run):
-    import torch
     path, _ = stopped_run
     rc, out = solver([CFG64, "--batch-keys", "--batch-resume", path, "--seed", "5", "--grid", "32,128", "--max-steps", "2"])
     assert resume_line(out)[1] == 32 * 128 * 128 and "imported and verified" in out, out[-3000:]
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
-    rc, out = solver(["--batch-keys", "--batch-resume", path, "--seed", "5", "--grid", "16,128"],
-                     prefix=[sys.executable, "-m", "torch.distributed.run", "--nproc-per-node", "2"])
+    from tests.ranks_util import solver_on                              # two GPUs, or two ranks sharing one over gloo
+    rc, out = solver_on(2, ["--batch-keys", "--batch-resume", path, "--seed", "5", "--grid", "16,128"])
     assert rc == 0, out[-3000:]
     assert privs(out) == dict(enumerate(ANSWERS)), out[-3000:]
     assert out.count("kangaroos imported and verified") == 2

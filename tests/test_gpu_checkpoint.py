@@ -222,14 +222,11 @@ def test_reference_program_resumes_a_solver_file(tmp_path):
 
 @needs_ingest
 def test_two_gpu_checkpoint_resumes_on_one_gpu(tmp_path):
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
+    """two GPUs, or two ranks sharing one over gloo"""
+    from tests.ranks_util import solver_on
     work = str(tmp_path / "two.work")
-    p = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nproc-per-node", "2", "-m", "kangaroo_b200.solver",
-                        os.path.join(GOLD, "in56.txt"), "--max-steps", "4", "--save-work", work] + COMMON,
-                       capture_output=True, text=True, timeout=900, cwd=ROOT)
-    assert os.path.exists(work), (p.stdout + p.stderr)[-2000:]
+    rc, out = solver_on(2, [os.path.join(GOLD, "in56.txt"), "--max-steps", "4", "--save-work", work] + COMMON)
+    assert os.path.exists(work), out[-2000:]
     out = solver(["--resume", work, "--grid", "16,32", "--seed", "2"])
     assert "%d kangaroos imported and verified" % (2 * 8 * 32 * 128) in out, out[-2000:]
     assert "Priv: 0x3447F65ABC9F46F736A95F87B044829C8A0129D56782D635CD612C0F05F3DA03" in out, out[-2000:]

@@ -298,11 +298,9 @@ def test_solver_device_table_batch_keys():
 
 @needs_ingest
 def test_solver_device_table_on_two_gpus():
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
-    rc, out = solver([os.path.join(GOLD, "in56.txt"), "--dp", "8", "--grid", "32,128", "--seed", "8"] + DEV,
-                     prefix=[sys.executable, "-m", "torch.distributed.run", "--nproc-per-node", "2"])
+    """two GPUs, or two ranks sharing one over gloo"""
+    from tests.ranks_util import solver_on
+    rc, out = solver_on(2, [os.path.join(GOLD, "in56.txt"), "--dp", "8", "--grid", "32,128", "--seed", "8"] + DEV)
     assert rc == 0 and PRIV56 in out and "GPUs: 2" in out, out[-3000:]
 
 

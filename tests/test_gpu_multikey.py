@@ -226,11 +226,9 @@ def test_batch_solves_a_key_listed_twice_and_its_negative(tmp_path):
 
 @needs_ingest
 def test_batch_on_two_gpus():
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
-    rc, out = solver([os.path.join(GOLD, "in56_64keys.txt"), "--batch-keys", "--dp", "8", "--grid", "32,128", "--seed", "5"],
-                     prefix=[sys.executable, "-m", "torch.distributed.run", "--nproc-per-node", "2"])
+    """two GPUs, or two ranks sharing one over gloo"""
+    from tests.ranks_util import solver_on
+    rc, out = solver_on(2, [os.path.join(GOLD, "in56_64keys.txt"), "--batch-keys", "--dp", "8", "--grid", "32,128", "--seed", "5"])
     assert rc == 0, out[-3000:]
     assert privs(out) == dict(enumerate(ANSWERS)), out[-3000:]
     assert batch_jumps(out)[:2] == (64, 64)

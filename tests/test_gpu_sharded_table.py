@@ -14,6 +14,7 @@ import pytest
 from kangaroo_b200 import worktool as wt
 from tests import dptable_model as dm
 from tests import shard_model as sm
+from tests.ranks_util import solver_on
 from tests.worktool_util import NB, ROOT
 
 pytestmark = pytest.mark.gpu
@@ -177,13 +178,6 @@ def solver(args, timeout=900, prefix=None):
 
 
 SH = ["--dp-table", "sharded"]
-TORCHRUN2 = [sys.executable, "-m", "torch.distributed.run", "--nproc-per-node", "2"]
-
-
-def two_gpus():
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
 
 
 @needs_ingest
@@ -275,26 +269,26 @@ def test_resume_file_too_large_for_the_shard_is_refused(tmp_path):
     assert "imported and verified" not in out and "MJump/s" not in out
 
 
-# ---- 4: two GPUs ------------------------------------------------------------------------------------------------------------
+# ---- 4: two ranks: two GPUs, or two ranks sharing one over gloo (tests/ranks_util.py) ----------------------------------------
 @needs_ingest
 def test_two_shards_solve_and_their_files_cross_tables(tmp_path):
-    two_gpus()
-    rc, out = solver([os.path.join(GOLD, "puzzle110_window56.txt"), "--dp", "8", "--grid", "32,128", "--seed", "11"] + SH,
-                     prefix=TORCHRUN2)
+    rc, out = solver_on(2, [os.path.join(GOLD, "puzzle110_window56.txt"), "--dp", "8", "--grid", "32,128", "--seed", "11",
+                            "--dp-table-capacity", str(1 << 24)] + SH)
     assert rc == 0 and "Priv: 0x35C0D7234DF7DEB0F20CF7062444" in out and "GPUs: 2" in out, out[-3000:]
-    rc, out = solver([os.path.join(GOLD, "in56_64keys.txt"), "--batch-keys", "--dp", "8", "--grid", "32,128", "--seed", "3"] + SH,
-                     prefix=TORCHRUN2)
+    rc, out = solver_on(2, [os.path.join(GOLD, "in56_64keys.txt"), "--batch-keys", "--dp", "8", "--grid", "32,128", "--seed", "3",
+                            "--dp-table-capacity", str(1 << 25)] + SH)
     batch_ok(rc, out)
     cfg = os.path.join(GOLD, "in56.txt")
     sh, host = str(tmp_path / "sh.work"), str(tmp_path / "host.work")
-    rc, out = solver([cfg, "--max-steps", "40", "--save-work", sh, "--save-interval", "0.05"] + COMMON + SH, prefix=TORCHRUN2)
+    rc, out = solver_on(2, [cfg, "--max-steps", "40", "--save-work", sh, "--save-interval", "0.05", "--dp-table-capacity",
+                            str(1 << 22)] + COMMON + SH)
     assert os.path.exists(sh) and "SaveWork" in out, out[-3000:]
     r = wt.check(sh)
     assert r.ok and r.walks == 2 * 8 * 32 * 128
     rc, out = solver(["--resume", sh, "--grid", "16,32", "--seed", "2"])
     assert "imported and verified" in out and PRIV56 in out, out[-2000:]
     solver([cfg, "--max-steps", "4", "--save-work", host] + COMMON)
-    rc, out = solver(["--resume", host, "--grid", "16,32", "--seed", "2"] + SH, prefix=TORCHRUN2)
+    rc, out = solver_on(2, ["--resume", host, "--grid", "16,32", "--seed", "2", "--dp-table-capacity", str(1 << 24)] + SH)
     assert "imported and verified" in out and PRIV56 in out, out[-3000:]
     from kangaroo_b200.ingest import DeviceDPTable
     t = DeviceDPTable(1 << 22)
