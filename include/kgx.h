@@ -181,7 +181,7 @@ uint64_t kgx_kernel_launches(kgx_engine* e);
  *     skipped (the others inserted, as kgi_add); -2 when count + records > capacity: nothing inserted, reason in
  *     kgx_dptable_last_error; -3 on a CUDA error.
  * _reserve: allocates now the per-call scratch of adds of up to n_records records (about 70 bytes per record) and of `cap`
- *     events, which adds otherwise grow on demand; a caller that sizes the table to the free memory reserves first.
+ *     events (136 bytes each, for both kinds of add), which adds otherwise grow on demand; a caller that sizes the table to the free memory reserves first.
  * _save_work / _load_work: kgi_save_work_ex / kgi_load_work_ex on this table (same header arguments and results, same
  *     bytes; the entries move in bounded chunks through pinned memory), after the work queued on `stream`.  A load that
  *     holds more entries than the capacity fails with -ENOSPC and leaves the table empty, like any failed load. --- */
@@ -193,6 +193,29 @@ typedef struct {                     /* = kgi_event (include/kgx_ingest.h) */
 #define KGX_DPT_EV_RESET     1
 #define KGX_DPT_EV_COLLISION 2
 #define KGX_DPT_MAX_RANKS    256
+/* --- the collision resolver on one GPU (kgx_resolver.cuh): kgi_resolve_multi's result without the host.
+ * _create: keys K = key - start*G (n_keys x 8 limbs, x then y; the point at infinity as (0, 0); 1 <= n_keys <= KGX_MAX_KEYS)
+ *     and a range start below the group order n.  Builds the fixed-base comb and the keys' index by x once, on device dev,
+ *     and waits for them.  NULL on bad arguments or a CUDA error, reason in kgx_resolver_last_error(NULL).
+ * _run: n collisions in device memory, pairs = n x 4 limbs {d_first[2], d_other[2]} of tagged distances (either order) ->
+ *     key_out[i] (device, n entries) = the first key in input order that one of the four candidates +-Td +-Wd * G hits (the
+ *     key or its negative), KGX_NO_KEY when none does or both distances are of one herd; priv_out (device, n x 4 limbs) = its
+ *     private key, (+-m + start) mod n, 0 with no key.  Stream-ordered on `stream` (NULL = the legacy default stream), no
+ *     allocation, no synchronisation.  -1: too many collisions; -3: a CUDA error, text in kgx_resolver_last_error(r).
+ * _destroy frees the resolver after the runs queued on it. --- */
+typedef struct kgx_resolver kgx_resolver;
+#define KGX_NO_KEY 0xFFFFFFFFu
+kgx_resolver* kgx_resolver_create(int dev, const uint64_t* keys, uint32_t n_keys, const uint64_t range_start[4]);
+void          kgx_resolver_destroy(kgx_resolver* r);
+const char*   kgx_resolver_last_error(kgx_resolver* r);
+int           kgx_resolver_run(kgx_resolver* r, const void* pairs, uint32_t n, uint32_t* key_out, uint64_t* priv_out, void* stream);
+/* An event of kgx_dptable_add_resolve: the event of kgx_dptable_add, then for a collision event the resolver's key index and
+ * private key, KGX_NO_KEY and 0 for any other event. */
+typedef struct {
+  kgx_dp_event ev;
+  uint32_t key, reserved;
+  uint64_t priv[4];
+} kgx_dp_event_key;
 kgx_dptable* kgx_dptable_create(int dev, uint64_t capacity);
 void         kgx_dptable_destroy(kgx_dptable* t);
 const char*  kgx_dptable_last_error(kgx_dptable* t);
@@ -203,6 +226,10 @@ uint64_t     kgx_dptable_bytes_for(uint64_t capacity);
 int          kgx_dptable_reserve(kgx_dptable* t, uint32_t n_records, uint32_t cap);
 int kgx_dptable_add(kgx_dptable* t, const void* recs, const uint32_t* counts, uint32_t n_ranks, uint64_t stride, kgx_dp_event* ev,
                     uint32_t cap, uint32_t* n_ev, void* stream);
+/* _add_resolve: kgx_dptable_add (same inserts, events, counts and return codes) with the first `cap` events resolved by r on the
+ *     same stream before the one copy of them to the host: ev gets kgx_dp_event_key records.  r must be on the table's device. */
+int kgx_dptable_add_resolve(kgx_dptable* t, const void* recs, const uint32_t* counts, uint32_t n_ranks, uint64_t stride, kgx_resolver* r,
+                            kgx_dp_event_key* ev, uint32_t cap, uint32_t* n_ev, void* stream);
 int kgx_dptable_save_work(kgx_dptable* t, const char* path, uint32_t dp_bits, const uint64_t range_start[4], const uint64_t range_end[4],
                           const uint64_t keyx[4], const uint64_t keyy[4], uint64_t total_count, double total_time, uint64_t total_walk,
                           void* stream);
@@ -315,7 +342,8 @@ int kgx_batch_read(const char* path, uint32_t* n_keys, uint64_t* nb_walk, uint64
  * _resolve: the merge's resolver on n collisions in host memory (d_first, d_other: n x 2 limbs of tagged distances) against
  *     n_keys (1..KGX_MAX_KEYS) keys K (n_keys x 8 limbs, keyToSearch = key - start*G, the point at infinity as (0, 0)) and a
  *     range start below n: key_out[i] = kgi_resolve_multi's key index for collision i, or 0xFFFFFFFF when it gives none (same
- *     herd included), priv_out (n x 4 limbs) = its private key (0 with no key). --- */
+ *     herd included), priv_out (n x 4 limbs) = its private key (0 with no key).  A resolver created, run once and destroyed
+ *     (the arrays are in host memory here). --- */
 typedef struct {
   uint32_t n_keys, solved_in_inputs, solved_by_merge, left;
   uint64_t same_herd, no_key, already_solved, solving;   /* collisions by outcome; they sum to info->collisions */

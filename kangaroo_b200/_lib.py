@@ -100,6 +100,13 @@ _SIGS = {
                                             ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32]),
     "kgx_work_resolve": (ctypes.c_int, [ctypes.c_int, _u64p, _u64p, ctypes.c_uint64, _u64p, ctypes.c_uint32, _u64p,
                                         ctypes.POINTER(ctypes.c_uint32), _u64p]),
+    "kgx_resolver_create": (ctypes.c_void_p, [ctypes.c_int, _u64p, ctypes.c_uint32, _u64p]),
+    "kgx_resolver_destroy": (None, [ctypes.c_void_p]),
+    "kgx_resolver_last_error": (ctypes.c_char_p, [ctypes.c_void_p]),
+    "kgx_resolver_run": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "kgx_dptable_add_resolve": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint32), ctypes.c_uint32,
+                                               ctypes.c_uint64, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32,
+                                               ctypes.POINTER(ctypes.c_uint32), ctypes.c_void_p]),
     "kgx_batch_block_bytes": (ctypes.c_uint64, [ctypes.c_uint32, ctypes.c_uint64]),
     "kgx_batch_block": (ctypes.c_int, [_u64p, ctypes.POINTER(ctypes.c_uint8), _u64p, ctypes.c_uint32, _u16p, ctypes.c_uint64, ctypes.c_uint64,
                                        ctypes.c_void_p]),

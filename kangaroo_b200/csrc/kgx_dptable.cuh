@@ -23,6 +23,8 @@
 //      the (h, x) index in place of its binary search.  Buckets never share an entry, so threads of different buckets only
 //      meet in the index, where an insert claims an empty slot with a CAS after its entry is written.
 //   4. the events, written at their arrival index, are compacted in arrival order; the first `cap` go back to the host.
+//      kgx_dptable_add_resolve runs a resolver (kgx_resolver.cuh) over those `cap` on the same stream first, so that each
+//      collision goes back with its key and private key in the same copy.
 #include <cub/cub.cuh>
 #include "kgx_workfile.h"
 #include "kgx_bucketsort.cuh"
@@ -177,6 +179,7 @@ struct kgx_dptable {
   uint32_t scratchN = 0, evCap = 0;
   uint32_t *keyIn = nullptr, *keyOut = nullptr, *valIn = nullptr, *valOut = nullptr, *sel = nullptr;
   kgx_dp_event *evArr = nullptr, *evOut = nullptr;
+  kgx_dp_event_key* evKey = nullptr;                       // kgx_dptable_add_resolve's events, evCap of them
   uint8_t* evFlag = nullptr;
   void* cubTmp = nullptr;
   size_t cubTmpBytes = 0;
@@ -281,7 +284,7 @@ void kgx_dptable_destroy(kgx_dptable* t) {
   cudaDeviceSynchronize();
   cudaFree(t->ent); cudaFree(t->ent_h); cudaFree(t->slots); cudaFree(t->nb); cudaFree(t->mx); cudaFree(t->res);
   dpt_free_scratch(t);
-  cudaFree(t->evOut);
+  cudaFree(t->evOut); cudaFree(t->evKey);
   cudaFree(t->sIdxA); cudaFree(t->sIdxB); cudaFree(t->sCursor); cudaFree(t->sKeyA); cudaFree(t->sKeyB); cudaFree(t->sOut); cudaFree(t->sTmp);
   if (t->resHost) cudaFreeHost(t->resHost);
   if (t->hostEnt) cudaFreeHost(t->hostEnt);
@@ -346,13 +349,18 @@ kgx_dptable* kgx_dptable_create(int dev, uint64_t capacity) {
 
 uint64_t kgx_dptable_count(kgx_dptable* t) { return t->count; }
 uint64_t kgx_dptable_capacity(kgx_dptable* t) { return t->capacity; }
-uint64_t kgx_dptable_memory_bytes(kgx_dptable* t) { return t->bytes + (t->evOut ? sizeof(kgx_dp_event) * (uint64_t)t->evCap : 0); }
+uint64_t kgx_dptable_memory_bytes(kgx_dptable* t) {
+  return t->bytes + (t->evOut ? (sizeof(kgx_dp_event) + sizeof(kgx_dp_event_key)) * (uint64_t)t->evCap : 0);
+}
 
+// the first `cap` events of an add on the device, plain and with their keys (grow-only; every add ends with a
+// synchronisation of its stream, so no earlier call still writes the buffers freed here)
 static int dpt_events(kgx_dptable* t, uint32_t cap) {
   if (cap <= t->evCap) return 0;
-  cudaFree(t->evOut);
-  t->evOut = nullptr; t->evCap = 0;
+  cudaFree(t->evOut); cudaFree(t->evKey);
+  t->evOut = nullptr; t->evKey = nullptr; t->evCap = 0;
   DPT_CK(t, cudaMalloc((void**)&t->evOut, sizeof(kgx_dp_event) * (size_t)cap));
+  DPT_CK(t, cudaMalloc((void**)&t->evKey, sizeof(kgx_dp_event_key) * (size_t)cap));
   t->evCap = cap;
   return 0;
 }
@@ -367,10 +375,15 @@ int kgx_dptable_reserve(kgx_dptable* t, uint32_t n_records, uint32_t cap) {
   return dpt_events(t, cap);
 }
 
-int kgx_dptable_add(kgx_dptable* t, const void* recs, const uint32_t* counts, uint32_t n_ranks, uint64_t stride, kgx_dp_event* ev,
-                    uint32_t cap, uint32_t* n_ev, void* stream) {
+// kgx_dptable_add (r null: ev holds kgx_dp_event) and kgx_dptable_add_resolve (ev holds kgx_dp_event_key)
+static int dpt_add(kgx_dptable* t, const void* recs, const uint32_t* counts, uint32_t n_ranks, uint64_t stride, const kgx_resolver* r,
+                   void* ev, uint32_t cap, uint32_t* n_ev, void* stream) {
   using namespace kgx_dpt;
   *n_ev = 0;
+  if (r && r->dev != t->dev) {
+    snprintf(t->err, sizeof t->err, "kgx_dptable_add_resolve: the resolver is on device %d, the table on device %d", r->dev, t->dev);
+    return -3;
+  }
   if (n_ranks == 0 || n_ranks > KGX_DPT_MAX_RANKS) {
     snprintf(t->err, sizeof t->err, "kgx_dptable_add: %u ranks (1 .. %d)", n_ranks, KGX_DPT_MAX_RANKS);
     return -3;
@@ -418,6 +431,7 @@ int kgx_dptable_add(kgx_dptable* t, const void* recs, const uint32_t* counts, ui
   if (nout) {
     k_events_out<<<(nout + B - 1) / B, B, 0, st>>>(t->evArr, t->sel, t->res, cap, t->evOut);
     DPT_CK(t, cudaGetLastError());
+    if (r) DPT_CK(t, kgx_wt::resolve_events(r, t->evOut, &t->res->nsel, nout, t->evKey, st));
   }
   DPT_CK(t, cudaMemcpyAsync(t->resHost, t->res, sizeof(Res), cudaMemcpyDeviceToHost, st));
   DPT_CK(t, cudaStreamSynchronize(st));
@@ -425,10 +439,25 @@ int kgx_dptable_add(kgx_dptable* t, const void* recs, const uint32_t* counts, ui
   *n_ev = t->resHost->nsel;
   const uint32_t ncopy = *n_ev < cap ? *n_ev : cap;
   if (ncopy) {
-    DPT_CK(t, cudaMemcpyAsync(ev, t->evOut, sizeof(kgx_dp_event) * (size_t)ncopy, cudaMemcpyDeviceToHost, st));
+    if (r) DPT_CK(t, cudaMemcpyAsync(ev, t->evKey, sizeof(kgx_dp_event_key) * (size_t)ncopy, cudaMemcpyDeviceToHost, st));
+    else DPT_CK(t, cudaMemcpyAsync(ev, t->evOut, sizeof(kgx_dp_event) * (size_t)ncopy, cudaMemcpyDeviceToHost, st));
     DPT_CK(t, cudaStreamSynchronize(st));
   }
   return t->resHost->bad ? -1 : 0;
+}
+
+int kgx_dptable_add(kgx_dptable* t, const void* recs, const uint32_t* counts, uint32_t n_ranks, uint64_t stride, kgx_dp_event* ev,
+                    uint32_t cap, uint32_t* n_ev, void* stream) {
+  return dpt_add(t, recs, counts, n_ranks, stride, nullptr, ev, cap, n_ev, stream);
+}
+
+int kgx_dptable_add_resolve(kgx_dptable* t, const void* recs, const uint32_t* counts, uint32_t n_ranks, uint64_t stride, kgx_resolver* r,
+                            kgx_dp_event_key* ev, uint32_t cap, uint32_t* n_ev, void* stream) {
+  if (!r) {
+    snprintf(t->err, sizeof t->err, "kgx_dptable_add_resolve: no resolver");
+    return -3;
+  }
+  return dpt_add(t, recs, counts, n_ranks, stride, r, ev, cap, n_ev, stream);
 }
 
 // The buckets [b0, b1) of the table, each nbItem, maxItem and its entries (HashTable::SaveTable, HashTable.cpp:375-396), to f

@@ -16,7 +16,8 @@
 // pairwise merges do -- and classifies each later one against it: equal tagged d = a duplicate ("Dead kangaroo"), else a
 // collision returned to the host.  The kept entries are compacted, counted per bucket and written with maxItem = nbItem
 // rounded up to a multiple of 4 (HashTable.cpp:204-209).  Batch work files merge through the same blocks, each block's
-// collisions resolved against every key on the device (wt_resolve_kernel).  The file format is kgx_workfile.h's, the block sort
+// collisions resolved against every key on the device (wt_resolve_kernel, around wt_resolve_pair, which the persistent
+// resolver of kgx_resolver.cuh shares).  The file format is kgx_workfile.h's, the block sort
 // kgx_bucketsort.cuh's (shared with the device table's save) and the group law kgx_curve.cuh's (shared with herd creation).
 #include <vector>
 #include <algorithm>
@@ -367,26 +368,18 @@ __device__ uint32_t wt_find_key(const u32* kx, const uint32_t* ki, const u32* K,
   return NO_KEY;
 }
 
-// One collision per thread.  out_key / out_priv (optional): every collision's key (NO_KEY: none, same-herd included) and
-// private key.  solved (optional): the merge's classification, cnt = {same herd, no key, key already solved, hit} and every
-// hit on an unsolved key appended to hits.  The two points share one inverse.
-__global__ void __launch_bounds__(CHECK_THREADS) wt_resolve_kernel(const u32* __restrict__ comb, const Coll* __restrict__ coll, uint32_t n,
-                                                                  const u32* __restrict__ kx, const uint32_t* __restrict__ ki,
-                                                                  const u32* __restrict__ K, uint32_t n_keys, Start start,
-                                                                  uint32_t* out_key, u64* out_priv, const uint8_t* solved, ull* cnt,
-                                                                  Hit* hits) {
+// One collision (two tagged distances, in either order) -> the key it hits (NO_KEY: none, same-herd included) and, with a key,
+// its private key in priv (else 0).  sc: the comb in shared memory.  The two points share one inverse.
+__device__ uint32_t wt_resolve_pair(const u32* sc, const u64* d_first, const u64* d_other, const u32* __restrict__ kx,
+                                    const uint32_t* __restrict__ ki, const u32* __restrict__ K, uint32_t n_keys, const Start& start,
+                                    u64* priv) {
   using namespace kgx;
-  __shared__ u32 sc[COMB_WORDS];
-  wt_load_comb(sc, comb);
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const Coll c = coll[i];
   const u64 M = 0x3FFFFFFFFFFFFFFFull;
-  const bool cross = ((c.d_first[1] ^ c.d_other[1]) >> 62) & 1;
+  const bool cross = ((d_first[1] ^ d_other[1]) >> 62) & 1;
   uint32_t key = NO_KEY;
-  u64 priv[4] = {0, 0, 0, 0};
+  for (int w = 0; w < 4; w++) priv[w] = 0;
   if (cross) {                                         // a tame/wild pair
-    const u64 a[2] = {c.d_first[0], c.d_first[1] & M}, b[2] = {c.d_other[0], c.d_other[1] & M};
+    const u64 a[2] = {d_first[0], d_first[1] & M}, b[2] = {d_other[0], d_other[1] & M};
     u64 m[2][2];
     m[0][0] = a[0] + b[0];
     m[0][1] = a[1] + b[1] + (m[0][0] < a[0]);
@@ -433,11 +426,23 @@ __global__ void __launch_bounds__(CHECK_THREADS) wt_resolve_kernel(const u32* __
       if (cy || ge_order(priv)) { const u64 nn[4] = {kOrder[0], kOrder[1], kOrder[2], kOrder[3]}; sub256(priv, priv, nn); }
     }
   }
-  if (out_key) {
-    out_key[i] = key;
-    for (int w = 0; w < 4; w++) out_priv[4ull * i + w] = priv[w];
-  }
-  if (!solved) return;
+  return key;
+}
+
+// The batch merge: one collision per thread, classified as cnt = {same herd, no key, key already solved, hit}; every hit on a
+// key not in solved is appended to hits.
+__global__ void __launch_bounds__(CHECK_THREADS) wt_resolve_kernel(const u32* __restrict__ comb, const Coll* __restrict__ coll, uint32_t n,
+                                                                  const u32* __restrict__ kx, const uint32_t* __restrict__ ki,
+                                                                  const u32* __restrict__ K, uint32_t n_keys, Start start,
+                                                                  const uint8_t* solved, ull* cnt, Hit* hits) {
+  __shared__ u32 sc[COMB_WORDS];
+  wt_load_comb(sc, comb);
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const Coll c = coll[i];
+  const bool cross = ((c.d_first[1] ^ c.d_other[1]) >> 62) & 1;
+  u64 priv[4];
+  const uint32_t key = wt_resolve_pair(sc, c.d_first, c.d_other, kx, ki, K, n_keys, start, priv);
   if (!cross) atomicAdd(&cnt[0], 1ull);
   else if (key == NO_KEY) atomicAdd(&cnt[1], 1ull);
   else if (solved[key]) atomicAdd(&cnt[2], 1ull);
@@ -1084,37 +1089,6 @@ int kgx_batch_read(const char* path, uint32_t* n_keys, uint64_t* nb_walk, uint64
   return rc;
 }
 
-int kgx_work_resolve(int dev, const uint64_t* d_first, const uint64_t* d_other, uint64_t n, const uint64_t* keys, uint32_t n_keys,
-                     const uint64_t range_start[4], uint32_t* key_out, uint64_t* priv_out) {
-  using namespace kgx_wt;
-  if (n_keys == 0 || n_keys > kgx_wf::BATCH_MAX_KEYS) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_work_resolve: n_keys must be in [1, %u]", kgx_wf::BATCH_MAX_KEYS); return -1; }
-  if (n >= 0x80000000ull) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_work_resolve: %llu collisions (at most 2^31-1)", (unsigned long long)n); return -1; }
-  if (kgx::ge256(range_start, kgx::kOrderHost)) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_work_resolve: the range start is not below n"); return -1; }
-  if (set_device(dev)) return -3;
-  DevBufs B;
-  u32 *comb, *kx, *K;
-  uint32_t *ki, *dKey;
-  std::vector<uint32_t> order, hk(16ull * n_keys);
-  memcpy(hk.data(), keys, 64ull * n_keys);
-  if (build_comb(B, &comb, 0) || key_index(B, hk, n_keys, &kx, &ki, order) || B.dev(&K, 64ull * n_keys)) return -3;
-  WT_CK(cudaMemcpy(K, keys, 64ull * n_keys, cudaMemcpyHostToDevice));
-  if (n == 0) return 0;
-  Coll* dColl;
-  u64* dPriv;
-  if (B.dev(&dColl, sizeof(Coll) * n) || B.dev(&dKey, 4 * n) || B.dev(&dPriv, 32 * n)) return -3;
-  std::vector<Coll> hc(n);
-  for (uint64_t i = 0; i < n; i++) hc[i] = Coll{0, (uint32_t)i, {d_first[2 * i], d_first[2 * i + 1]}, {d_other[2 * i], d_other[2 * i + 1]}};
-  WT_CK(cudaMemcpy(dColl, hc.data(), sizeof(Coll) * n, cudaMemcpyHostToDevice));
-  Start st;
-  memcpy(st.v, range_start, 32);
-  wt_resolve_kernel<<<(unsigned)((n + CHECK_THREADS - 1) / CHECK_THREADS), CHECK_THREADS>>>(comb, dColl, (uint32_t)n, kx, ki, K, n_keys, st, dKey,
-                                                                                           dPriv, nullptr, nullptr, nullptr);
-  WT_CK(cudaGetLastError());
-  WT_CK(cudaMemcpy(key_out, dKey, 4 * n, cudaMemcpyDeviceToHost));
-  WT_CK(cudaMemcpy(priv_out, dPriv, 32 * n, cudaMemcpyDeviceToHost));
-  return 0;
-}
-
 int kgx_work_merge_batch(int dev, const char* const* paths, uint32_t n_paths, const char* tmp_path, uint64_t block_entries,
                          kgx_work_merge_info* info, kgx_batch_merge_info* binfo, kgx_batch_key_result* keys_out, uint32_t cap_keys) {
   using namespace kgx_wt;
@@ -1208,8 +1182,8 @@ int kgx_work_merge_batch(int dev, const char* const* paths, uint32_t n_paths, co
   std::vector<Hit> hits;
   auto on_coll = [&](uint32_t nc, const Coll* dColl) -> int {
     WT_CK(cudaMemset(dCnt, 0, 32));
-    wt_resolve_kernel<<<(nc + CHECK_THREADS - 1) / CHECK_THREADS, CHECK_THREADS>>>(comb, dColl, nc, kx, kidx, K, n, st, nullptr, nullptr,
-                                                                                   dSolved, dCnt, dHits);
+    wt_resolve_kernel<<<(nc + CHECK_THREADS - 1) / CHECK_THREADS, CHECK_THREADS>>>(comb, dColl, nc, kx, kidx, K, n, st, dSolved, dCnt,
+                                                                                   dHits);
     WT_CK(cudaGetLastError());
     ull cnt[4];
     WT_CK(cudaMemcpy(cnt, dCnt, 32, cudaMemcpyDeviceToHost));

@@ -3,7 +3,11 @@
 The table is the reference's own `class HashTable` (HashTable.{h,cpp}, compiled unmodified from the reference sources by
 kangaroo_b200/csrc/build_ingest.sh); the library adds the batched, bucket-sharded multi-threaded insert that replaces the
 single-mutex loop of Kangaroo::SolveKeyGPU (Kangaroo.cpp:594-612) when the DP records of all GPUs arrive on rank 0.
-No Python-side fallback: without the library DPTable() raises."""
+No Python-side fallback: without the library DPTable() raises.  KGX_INGEST_LIB in the environment names another copy of the
+library (or a path that does not exist, to run as a checkout built without the reference sources).
+
+DeviceDPTable and DeviceResolver are libkgx.so's: the device table and the collision resolver on the GPU, which need no
+reference sources; nothing here loads libkgx_ingest.so for them."""
 import collections
 import ctypes
 import os
@@ -12,7 +16,8 @@ import struct
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(HERE, "..", "build", "libkgx_ingest.so")
+LIB_PATH = os.environ.get("KGX_INGEST_LIB") or os.path.join(HERE, "..", "build", "libkgx_ingest.so")
+NO_KEY = 0xFFFFFFFF
 
 EV_RESET, EV_COLLISION = 1, 2
 DP40_BYTES, ITEM_BYTES = 40, 56
@@ -23,6 +28,11 @@ class Event(ctypes.Structure):
     """kgi_event"""
     _fields_ = [("kind", ctypes.c_uint32), ("rank", ctypes.c_uint32), ("kidx", ctypes.c_uint32), ("h", ctypes.c_uint32),
                 ("d_old", ctypes.c_uint64 * 2), ("d_new", ctypes.c_uint64 * 2)]
+
+
+class EventKey(ctypes.Structure):
+    """kgx_dp_event_key: an event of kgx_dptable_add_resolve, with its collision's key index (NO_KEY: none) and private key"""
+    _fields_ = [("ev", Event), ("key", ctypes.c_uint32), ("reserved", ctypes.c_uint32), ("priv", ctypes.c_uint64 * 4)]
 
 
 _u64p = ctypes.POINTER(ctypes.c_uint64)
@@ -58,9 +68,16 @@ def load_library():
     if _lib is not None:
         return _lib
     path = os.path.abspath(LIB_PATH)
-    if not os.path.exists(path):
-        raise RuntimeError("kangaroo_b200: %s is missing (kangaroo_b200/csrc/build_ingest.sh builds it against the reference sources)" % path)
-    lib = ctypes.CDLL(path)
+    why = "is missing" if not os.path.exists(path) else None
+    if why is None:
+        try:
+            lib = ctypes.CDLL(path)
+        except OSError as e:
+            why = "cannot be loaded (%s)" % e
+    if why is not None:
+        raise RuntimeError("kangaroo_b200: %s %s: the host DP table (--dp-table host) is the reference's HashTable, which "
+                           "kangaroo_b200/csrc/build_ingest.sh builds against the reference sources; --dp-table device and "
+                           "--dp-table sharded keep the table and resolve collisions on the GPU without it" % (path, why))
     for name, (res, args) in _SIGS.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = res, args
@@ -203,11 +220,71 @@ class TableFull(RuntimeError):
     """An add that would take a DeviceDPTable past its capacity: nothing of it was inserted."""
 
 
+def _limbs_u64(vals, k):
+    """ints -> (n, k) uint64 little-endian limbs"""
+    return np.array([[(int(v) >> (64 * w)) & _M64 for w in range(k)] for v in vals], dtype=np.uint64).reshape(-1, k)
+
+
+class DeviceResolver:
+    """kgx_resolver_*: tame/wild collisions resolved on one GPU against a key table -- kgi_resolve_multi's result (the first
+    key in input order that +-Td +-Wd * G hits, and its private key) without the host.  keys: K = key - start*G per key, as
+    DPTable.key_table gives them (or a list of points, None for the point at infinity); range_start below n.  The comb and
+    the key index are built once here; run_raw is one stream-ordered kernel, and DeviceDPTable.add(resolver=) runs it inside
+    the table's add."""
+
+    def __init__(self, keys, range_start, device=0):
+        from ._lib import load_library as load_engine
+        self._lib = load_engine()
+        kt = keys if isinstance(keys, np.ndarray) else DPTable.key_table(keys)
+        kt = np.ascontiguousarray(kt, dtype=np.uint64)
+        self.device, self.n_keys = int(device), int(kt.shape[0])
+        self._h = ctypes.c_void_p(self._lib.kgx_resolver_create(self.device, kt.ctypes.data_as(_u64p), self.n_keys, _limbs4(range_start)))
+        if not self._h:
+            raise RuntimeError(self._lib.kgx_resolver_last_error(None).decode())
+
+    def close(self):
+        if self._h:
+            self._lib.kgx_resolver_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def run_raw(self, pairs, n, key_out, priv_out, stream=0):
+        """n collisions at device address pairs (n x 4 limbs {d_first, d_other}) -> key_out (n uint32) and priv_out (n x 4 limbs),
+        device addresses, queued on `stream`"""
+        rc = self._lib.kgx_resolver_run(self._h, ctypes.c_void_p(int(pairs)), int(n), ctypes.c_void_p(int(key_out)),
+                                        ctypes.c_void_p(int(priv_out)), ctypes.c_void_p(int(stream)))
+        if rc != 0:
+            raise RuntimeError(self._lib.kgx_resolver_last_error(self._h).decode())
+
+    def resolve(self, d_first, d_other, stream=None):
+        """two lists of tagged distances (ints) -> [(key index, private key) or None]; on `stream` (a torch stream) or torch's
+        current one, waited for"""
+        import torch
+        n = len(d_first)
+        if n == 0:
+            return []
+        dev = torch.device("cuda", self.device)
+        pairs = torch.from_numpy(np.ascontiguousarray(np.hstack([_limbs_u64(d_first, 2), _limbs_u64(d_other, 2)])).view(np.int64))
+        st = stream or torch.cuda.current_stream(dev)
+        with torch.cuda.stream(st):
+            p = pairs.to(dev, non_blocking=False)
+            key = torch.empty(n, dtype=torch.int32, device=dev)
+            priv = torch.empty((n, 4), dtype=torch.int64, device=dev)
+            self.run_raw(p.data_ptr(), n, key.data_ptr(), priv.data_ptr(), st.cuda_stream)
+            key_h, priv_h = key.cpu().numpy().view(np.uint32), priv.cpu().numpy().view(np.uint64)
+        return [None if k == NO_KEY else (int(k), sum(int(v) << (64 * w) for w, v in enumerate(pv))) for k, pv in zip(key_h.tolist(), priv_h)]
+
+
 class DeviceDPTable:
     """The rank-0 DP table in the memory of one GPU (libkgx.so, kgx_dptable_*): DPTable's add / __len__ / save_work /
     load_work_ex with exactly its results for the same records in the same order, inserted by CUDA kernels straight from device
     memory.  Its capacity (entries) is fixed at creation; an add that could pass it raises TableFull and changes nothing.
-    resolve / resolve_multi are the host table's (kgi_resolve: the reference's CheckKey), on a DPTable that holds no entry.
+    add(resolver=) resolves the collisions of the add on the device (kgx_dptable_add_resolve).
     buckets=(lo, hi): a shard of the sharded table, holding the buckets [lo, hi) only (kgx_dptable_create_range)."""
 
     def __init__(self, capacity, device=None, max_events=4096, buckets=None):
@@ -223,9 +300,9 @@ class DeviceDPTable:
         self.buckets = (0, 1 << 18) if buckets is None else (int(buckets[0]), int(buckets[1]))
         self.capacity = int(capacity)
         self._ev = (Event * max_events)()
+        self._evk = None                     # EventKey * max_events, made by the first add with a resolver
         self._cap = max_events
         self.threads = 0                     # no host workers
-        self._resolver = None
 
     @staticmethod
     def bytes_for(capacity):
@@ -236,9 +313,6 @@ class DeviceDPTable:
         if self._h:
             self._lib.kgx_dptable_destroy(self._h)
             self._h = None
-        if self._resolver is not None:
-            self._resolver.close()
-            self._resolver = None
 
     def __del__(self):
         try:
@@ -260,27 +334,46 @@ class DeviceDPTable:
         if self._lib.kgx_dptable_reserve(self._h, int(n_records), self._cap) != 0:
             raise RuntimeError("kgx_dptable_reserve: " + self._err())
 
-    def add_raw(self, ptr, counts, stride, stream=0):
+    def add_raw(self, ptr, counts, stride, stream=0, resolver=None):
         """counts[r] records of rank r at device address ptr + r*stride*40 -> (return code, total events, Event array of the
-        first min(total, max_events)).  Raises TableFull (-2) and RuntimeError on a CUDA error (-3); -1 = malformed records
-        skipped."""
+        first min(total, max_events); with a resolver, EventKey records).  Raises TableFull (-2) and RuntimeError on a CUDA error
+        (-3); -1 = malformed records skipped."""
         counts = [int(c) for c in counts]
         cnt = (ctypes.c_uint32 * len(counts))(*counts)
         ne = ctypes.c_uint32(0)
-        rc = self._lib.kgx_dptable_add(self._h, ctypes.c_void_p(int(ptr)), cnt, len(counts), int(stride),
-                                       ctypes.cast(self._ev, ctypes.c_void_p), self._cap, ctypes.byref(ne), ctypes.c_void_p(int(stream)))
+        args = (self._h, ctypes.c_void_p(int(ptr)), cnt, len(counts), int(stride))
+        if resolver is None:
+            out = self._ev
+            rc = self._lib.kgx_dptable_add(*args, ctypes.cast(out, ctypes.c_void_p), self._cap, ctypes.byref(ne),
+                                           ctypes.c_void_p(int(stream)))
+        else:
+            if self._evk is None:
+                self._evk = (EventKey * self._cap)()
+            out = self._evk
+            rc = self._lib.kgx_dptable_add_resolve(*args, resolver._h, ctypes.cast(out, ctypes.c_void_p), self._cap, ctypes.byref(ne),
+                                                   ctypes.c_void_p(int(stream)))
         if rc == -2:
             raise TableFull(self._err())
         if rc < -1:
             raise RuntimeError("kgx_dptable_add: " + self._err())
-        return rc, ne.value, self._ev
+        return rc, ne.value, out
 
-    def add(self, ptr, counts, stride, stream=0):
-        """every rank's records of one step (device memory) -> list of (kind, rank, kidx, d_old, d_new) events"""
-        rc, n, _ = self.add_raw(ptr, counts, stride, stream)
+    def add(self, ptr, counts, stride, stream=0, resolver=None):
+        """every rank's records of one step (device memory) -> list of (kind, rank, kidx, d_old, d_new) events; with a
+        resolver (DeviceResolver on this table's GPU) (kind, rank, kidx, d_old, d_new, hit), hit = (key index, private key) of a
+        collision event, or None: no key, or another kind of event"""
+        rc, n, out = self.add_raw(ptr, counts, stride, stream, resolver)
         if rc != 0:
             raise RuntimeError("kgx_dptable_add: malformed DP record (h >= 2^18)")
-        return DPTable._events(self, n)
+        if resolver is None:
+            return DPTable._events(self, n)
+        evs = []
+        for i in range(min(n, self._cap)):
+            k = out[i]
+            e = k.ev
+            hit = None if k.key == NO_KEY else (int(k.key), sum(int(k.priv[w]) << (64 * w) for w in range(4)))
+            evs.append((int(e.kind), int(e.rank), int(e.kidx), (int(e.d_old[0]), int(e.d_old[1])), (int(e.d_new[0]), int(e.d_new[1])), hit))
+        return evs
 
     def add_dp40(self, buf, rank=0, stream=0):
         """DPTable.add_dp40 for records in device memory: buf = a CUDA uint8 tensor of n x 40 bytes"""
@@ -324,17 +417,6 @@ class DeviceDPTable:
         if rc != 0:
             raise RuntimeError("kgx_dptable_load_range: %s" % self._err())
         return info
-
-    def _host(self):
-        if self._resolver is None:
-            self._resolver = DPTable(threads=1)
-        return self._resolver
-
-    def resolve(self, d_old, d_new, key, range_start):
-        return self._host().resolve(d_old, d_new, key, range_start)
-
-    def resolve_multi(self, d_old, d_new, keys, range_start):
-        return self._host().resolve_multi(d_old, d_new, keys, range_start)
 
 
 class WorkHeader(collections.namedtuple("WorkHeader", "dp_bits range_start range_end key total_count total_time")):

@@ -18,6 +18,9 @@ Per step (= one GPUEngine::Launch on every rank) nothing on the data path is Pyt
 With --dp-table device, rank 0's table is ingest.DeviceDPTable in its GPU's memory (same events and work files): the step's
 records are copied device to device into a staging buffer and inserted from there by the ingest thread on its own stream, no
 host copy of them.  Its capacity is fixed; a full table stops the run (with --save-work, after writing the table it holds).
+The insert resolves its tame/wild collisions on the same stream (ingest.DeviceResolver, kgi_resolve_multi's result against the
+run's keys), so each collision event comes back with its key and private key; only --dp-table host loads
+build/libkgx_ingest.so, the reference's HashTable and CheckKey.
 
 With --dp-table sharded, every rank holds the device table of the buckets it owns and inserts them on an ingest thread of its
 own: the records go to their owners (dist.DPExchange) in place of the gather, and a per-step block from every rank brings rank
@@ -58,7 +61,7 @@ import numpy as np
 from . import ecmath as ec
 from .engine import GPUEngine, NB_JUMP, NB_RUN, WILD, random_herd_arrays
 from .dist import DPExchange, DPGather, HerdGather, SlabView, DP40_BYTES, WALK_BYTES, owner_ranges
-from .ingest import DPTable, DeviceDPTable, TableFull, EV_RESET, EV_COLLISION
+from .ingest import DPTable, DeviceDPTable, DeviceResolver, TableFull, EV_RESET, EV_COLLISION
 
 ORDER = ec.N
 MAX_RESETS = 255          # per step, carried in the control broadcast
@@ -243,17 +246,23 @@ class HostTable:
     def insert(self, segments):
         return [ev for r, buf in segments if buf.size != 0 for ev in self.dps.add_dp40(buf, r)]
 
+    def close(self):
+        self.dps.close()
+
 
 class DeviceTable:
     """ingest.DeviceDPTable in rank 0's GPU memory, fed from device staging buffers on a stream of the ingest thread's own.
     The two staging buffers and a third one, which takes parked records back to the GPU, are all the GPU memory the records
-    take; the table's per-add scratch is reserved up front, so the table needs no allocation while it runs."""
+    take; the table's per-add scratch is reserved up front, so the table needs no allocation while it runs.  Every insert
+    resolves its collisions against the run's keys on the same stream (ingest.DeviceResolver): its events carry their hits."""
     label = "device table"
 
-    def __init__(self, torch, n_records, device, capacity, wait_copy, buckets=None):
+    def __init__(self, torch, n_records, device, capacity, wait_copy, keys, start, buckets=None):
         """wait_copy: the records' source is rewritten unordered with torch's stream (the engine's own buffer, on one GPU).
+        keys: the key table the collisions are resolved against (DPTable.key_table: K = key - start*G per key).
         buckets: (lo, hi) of a shard (ShardedTable)"""
         self.torch, self._wait_copy = torch, wait_copy
+        self.resolver = DeviceResolver(keys, start, device=device)
         self._bufs = [torch.empty(n_records * DP40_BYTES, dtype=torch.uint8, device=torch.device("cuda", device)) for _ in range(3)]
         self._back = self._bufs.pop()
         if not capacity:
@@ -289,7 +298,11 @@ class DeviceTable:
             buf = self._back
         else:
             self._stream.wait_event(ev)                     # the records' copy into the staging buffer
-        return self.dps.add(buf.data_ptr(), counts, stride, self._stream.cuda_stream)
+        return self.dps.add(buf.data_ptr(), counts, stride, self._stream.cuda_stream, self.resolver)
+
+    def close(self):
+        self.dps.close()
+        self.resolver.close()
 
 
 class ShardedTable(DeviceTable):
@@ -297,8 +310,8 @@ class ShardedTable(DeviceTable):
     Its capacity is the shard's; save_piece writes its piece of a work file at an offset."""
     label = "sharded table"
 
-    def __init__(self, torch, n_records, device, capacity, buckets):
-        super().__init__(torch, n_records, device, capacity, False, buckets)
+    def __init__(self, torch, n_records, device, capacity, keys, start, buckets):
+        super().__init__(torch, n_records, device, capacity, False, keys, start, buckets)
         self.save_piece = functools.partial(self.dps.save_piece, stream=self._stream.cuda_stream)
 
 
@@ -366,6 +379,7 @@ class Solver:
         self.wdiv2 = width >> 1
         # Kangaroo::InitSearchKey (:892-909): keyToSearch = P - start*G
         self.key = ec.add(pub, ec.neg(ec.mul(start))) if start else pub
+        self.key_table = self._key_table()
         gx, gy = grid or GPUEngine.GetGridSize(self.local, 0, 0)
         self.eng = GPUEngine(gx, gy, self.local, max_found)
         self.table = create_jump_table(self.range_power)
@@ -391,8 +405,8 @@ class Solver:
         if self.sharded:
             self._init_shard(max_found, dp_table_capacity)
         elif self.rank == 0:
-            self.dpt = (DeviceTable(torch, self.world * max_found, self.local, dp_table_capacity, self.gather is None)
-                        if dp_table == "device" else HostTable(torch, self.world * max_found, ingest_threads))
+            self.dpt = (DeviceTable(torch, self.world * max_found, self.local, dp_table_capacity, self.gather is None, self.key_table,
+                                    self.start) if dp_table == "device" else HostTable(torch, self.world * max_found, ingest_threads))
             self.dps = self.dpt.dps
         self._work = queue.Queue()
         self._done = queue.Queue()
@@ -435,6 +449,18 @@ class Solver:
     def _create_herd(self, sc, d128):
         self.eng.CreateHerdRaw(sc, d128, self.key)
 
+    def _key_table(self):
+        """the keys a collision is resolved against: the one key of the run"""
+        return DPTable.key_table([self.key])
+
+    def _hit(self, ev):
+        """a collision event -> (key index, private key) or None.  The device tables resolved it with the insert; the host table
+        runs the reference's CheckKey (Kangaroo.cpp:255-302) on the key."""
+        if len(ev) > 5:
+            return ev[5]
+        priv = self.dps.resolve(ev[3], ev[4], self.key, self.start)
+        return None if priv is None else (0, priv)
+
     # -- --dp-table sharded ---------------------------------------------------------------------------------------------
     # Every rank holds the shard of the buckets it owns (dist.owner_ranges) and runs an ingest thread of its own, one step
     # behind like rank 0's.  Per step: DPExchange brings each rank the records of its buckets; each rank's main thread then
@@ -450,7 +476,7 @@ class Solver:
             raise ValueError(err)
         self.buckets = owner_ranges(self.world)[self.rank]
         self.headroom = shard_headroom(self.world, max_found)
-        self.dpt = ShardedTable(torch, self.world * max_found, self.local, capacity, self.buckets)
+        self.dpt = ShardedTable(torch, self.world * max_found, self.local, capacity, self.key_table, self.start, self.buckets)
         self.dps = self.dpt.dps
         if self.dps.capacity <= self.headroom:
             raise RuntimeError(sharded_capacity_error(self.dps.capacity, self.world, max_found))
@@ -804,13 +830,14 @@ class Solver:
         """rank 0, ingest thread: one step's events -> (hits [(key index, private key, rank, kIdx)], resets).  Resolving stops
         at the first key found."""
         hits, resets = [], []
-        for kind, rk, kidx, d_old, d_new in events:
+        for ev in events:
+            kind, rk, kidx = ev[:3]
             if kind == EV_COLLISION and not hits:
-                priv = self.dps.resolve(d_old, d_new, self.key, self.start)      # Kangaroo.cpp:255-302
-                if priv is None:
+                m = self._hit(ev)
+                if m is None:
                     resets.append((rk, kidx))                                    # "unexpected wrong collision, reset kangaroo"
                 else:
-                    hits.append((0, priv, rk, kidx))
+                    hits.append(m + (rk, kidx))
             elif kind == EV_RESET:
                 resets.append((rk, kidx))
         return hits, resets
@@ -1036,8 +1063,8 @@ class Solver:
             self._thread.join(timeout=10)
             self._thread = None
         self.eng.close()
-        if self.dps is not None:
-            self.dps.close()
+        if self.dpt is not None:
+            self.dpt.close()
 
 
 # -- --batch-keys: every key of the input in one run, one tame herd shared by all of them -------------------------------------
@@ -1132,7 +1159,6 @@ class BatchSolver(Solver):
         super().__init__(start, end, self.pubs[0], dp_bits, grid, max_found, seed, ingest_threads, dp_table=dp_table,
                          dp_table_capacity=dp_table_capacity, save_work=save_work, save_interval=save_interval,
                          save_kangaroos=bool(save_work), resume=resume)
-        self.key_table = DPTable.key_table(self.keys)
 
     def _resume(self, path):
         """Solver._resume with the targets: rank 0 loads the table and sends every rank its records and their targets; each
@@ -1223,12 +1249,19 @@ class BatchSolver(Solver):
     def _wild_key(self, kidx):
         return self.keys[int(self.targets[kidx])]
 
+    def _key_table(self):
+        return DPTable.key_table(self.keys)
+
+    def _hit(self, ev):
+        return ev[5] if len(ev) > 5 else self.dps.resolve_multi(ev[3], ev[4], self.key_table, self.start)
+
     def _ingest(self, events):
         """rank 0, ingest thread -> (hits [(key index, private key, rank, kIdx)], resets): every collision is resolved"""
         hits, resets = [], []
-        for kind, rk, kidx, d_old, d_new in events:
+        for ev in events:
+            kind, rk, kidx = ev[:3]
             if kind == EV_COLLISION:
-                m = self.dps.resolve_multi(d_old, d_new, self.key_table, self.start)
+                m = self._hit(ev)
                 if m is None:
                     resets.append((rk, kidx))                    # matches no key: "unexpected wrong collision, reset kangaroo"
                 else:
@@ -1409,7 +1442,9 @@ def config_difference(start, end, pubs, f_start, f_end, f_pubs):
     return None
 
 
-def main(argv=None):
+def parse_args(argv=None):
+    """the command line -> (arguments, range start, range end, public keys, dp bits, grid, batch block or None); argparse
+    exits on a usage error.  Loads build/libkgx_ingest.so only for --dp-table host, to refuse the run when it is missing."""
     ap = argparse.ArgumentParser()
     ap.add_argument("config", nargs="?", help="range start, end and public keys (optional with --resume)")
     ap.add_argument("--dp", type=int, default=None, help="distinguished-point bits (default 12, or the file's with --resume)")
@@ -1425,7 +1460,7 @@ def main(argv=None):
                     help="continue from a work file (-i): range, key and dp come from the file unless given")
     ap.add_argument("--dp-table", choices=("host", "device", "sharded"), default="host",
                     help="where the DP table is kept: host = the reference's HashTable in rank 0's host RAM, inserted by "
-                         "--ingest-threads workers; device = a hash table with the same results in rank 0's GPU memory, inserted "
+                         "--ingest-threads workers (build/libkgx_ingest.so, built only with the reference sources); device = a hash table with the same results in rank 0's GPU memory, inserted "
                          "by CUDA kernels straight from the gathered records (fixed capacity: a full table stops the run); "
                          "sharded = the device table split by bucket over every rank's GPU, each rank inserting the records of its "
                          "buckets (a full shard stops the run with the normal end-of-run work file; every rank writes its piece of "
@@ -1490,7 +1525,18 @@ def main(argv=None):
         ap.error("--batch-keys needs a config with at least one public key")
     if a.batch_keys and len(pubs) > MAX_KEYS:
         ap.error("--batch-keys takes at most %d keys, the config has %d" % (MAX_KEYS, len(pubs)))
+    if a.dp_table == "host":
+        from . import ingest
+        try:
+            ingest.load_library()
+        except RuntimeError as e:
+            ap.error(str(e))
     grid = tuple(int(v) for v in a.grid.split(",")) if a.grid else None
+    return a, start, end, pubs, dp, grid, block
+
+
+def main(argv=None):
+    a, start, end, pubs, dp, grid, block = parse_args(argv)
     rc = _run_batch(start, end, pubs, dp, grid, a, block) if a.batch_keys else 0
     for i, pub in enumerate([] if a.batch_keys else pubs):
         s = Solver(start, end, pub, dp, grid, seed=a.seed, ingest_threads=a.ingest_threads, save_work=a.save_work,

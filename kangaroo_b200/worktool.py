@@ -7,8 +7,8 @@
 `check` recomputes every stored DP (d*G, or key - start*G + d*G for a wild one) and every kangaroo on the GPU
 (libkgx.so, kgx_work_check) and exits 1 when anything is wrong.  It also takes the solver's batch work files (--batch-keys
 --batch-save): every kangaroo is checked against its own target key, every wild DP against all keys of the file.  `merge` combines files of the same key and range in the order
-given (the entry of the earlier file wins at equal x) with kgx_work_merge, resolves every tame/wild collision with the
-solver's resolver (the reference's CheckKey, build/libkgx_ingest.so), and either prints the key and writes nothing, or writes
+given (the entry of the earlier file wins at equal x) with kgx_work_merge, resolves every tame/wild collision on the device
+with the solver's resolver (kgx_work_resolve: the reference's CheckKey result), and either prints the key and writes nothing, or writes
 DEST through DEST.tmp, fsync and rename.  The merged file ends with a kangaroo count of 0, so the solver's --resume and the
 reference's -i take it; they start fresh herds.  Batch work files (the same keys in the same order and the same range) are
 merged with kgx_work_merge_batch, which resolves every tame/wild collision against all keys on the device; DEST is always
@@ -375,17 +375,10 @@ def merge(paths, dest, device=0, block_entries=0, out=print):
     unresolved, priv = 0, None
     cross = [c for c in res.collision_list if (c[1][1] ^ c[2][1]) & (TYPE_BIT >> 64)]
     same_herd = len(res.collision_list) - len(cross)
-    if cross:
-        from .ingest import DPTable
-        t = DPTable(threads=1)
-        try:
-            for h, d1, d2 in cross:
-                priv = t.resolve(d1, d2, key, start)
-                if priv is not None:
-                    break
-                unresolved += 1
-        finally:
-            t.close()
+    if cross:                                                             # Merge.cpp's CheckKey on each, in order, on the device
+        found = resolve([_val(d1) for _, d1, _ in cross], [_val(d2) for _, _, d2 in cross], [key], start, device=device)
+        first = next((i for i, m in enumerate(found) if m is not None), len(found))
+        unresolved, priv = first, (found[first][1] if first < len(found) else None)
     if res.n_listed < res.collisions:
         out("Warning: %d collisions, only the first %d examined" % (res.collisions, res.n_listed))
     if priv is not None and ec.mul(priv) == pub:
