@@ -202,13 +202,25 @@ typedef struct {                     /* = kgi_event (include/kgx_ingest.h) */
  *     key or its negative), KGX_NO_KEY when none does or both distances are of one herd; priv_out (device, n x 4 limbs) = its
  *     private key, (+-m + start) mod n, 0 with no key.  Stream-ordered on `stream` (NULL = the legacy default stream), no
  *     allocation, no synchronisation.  -1: too many collisions; -3: a CUDA error, text in kgx_resolver_last_error(r).
- * _destroy frees the resolver after the runs queued on it. --- */
+ * _destroy frees the resolver after the runs queued on it.
+ * _verify: a resolver of exactly one key (else -1) checks n received 40-byte DP records {u32 kIdx; u32 h; u128 x; u128 tagged d}
+ *     (device memory, 8-byte aligned) by the rule of kgx_work_check: S = +-|d|*G (sign bit 127, |d| the low 126 bits), + K when
+ *     the type bit 126 is set; a record is good iff h < 2^18, S is not the point at infinity, S.x.bits64[2] & 0x3FFFF == h and
+ *     the low 128 bits of S.x equal x.  good (device, n x 40 bytes, 8-byte aligned) gets the good records in input order (a
+ *     stable compaction), counts (device, 2 entries) = {good, bad}, bad_idx (device, cap entries) the indices of the first
+ *     `cap` bad records in input order.  scratch: device memory of at least kgx_resolver_verify_scratch_bytes(n) bytes,
+ *     256-byte aligned (as cudaMalloc returns it; the flags, their prefix sums and cub's scan storage live there).
+ *     Stream-ordered on `stream`, no allocation, no synchronisation.  -1: bad arguments; -3: a CUDA error, text in
+ *     kgx_resolver_last_error(r). --- */
 typedef struct kgx_resolver kgx_resolver;
 #define KGX_NO_KEY 0xFFFFFFFFu
 kgx_resolver* kgx_resolver_create(int dev, const uint64_t* keys, uint32_t n_keys, const uint64_t range_start[4]);
 void          kgx_resolver_destroy(kgx_resolver* r);
 const char*   kgx_resolver_last_error(kgx_resolver* r);
 int           kgx_resolver_run(kgx_resolver* r, const void* pairs, uint32_t n, uint32_t* key_out, uint64_t* priv_out, void* stream);
+uint64_t      kgx_resolver_verify_scratch_bytes(uint32_t n);
+int           kgx_resolver_verify(kgx_resolver* r, const void* recs, uint32_t n, void* good, uint32_t* counts, uint32_t* bad_idx,
+                                  uint32_t cap, void* scratch, uint64_t scratch_bytes, void* stream);
 /* An event of kgx_dptable_add_resolve: the event of kgx_dptable_add, then for a collision event the resolver's key index and
  * private key, KGX_NO_KEY and 0 for any other event. */
 typedef struct {

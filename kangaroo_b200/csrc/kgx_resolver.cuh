@@ -6,10 +6,17 @@
 // private key.  Runs are stream-ordered on the caller's stream and allocate nothing, so the solver resolves every step's
 // collisions on the device table's stream (kgx_dptable_add_resolve, kgx_dptable.cuh) and the host does no per-collision work.
 // kgx_work_resolve is a resolver of one call.
+//
+// A resolver of one key also checks received DP records (kgx_resolver_verify, the server's check of what clients send): the
+// stored-entry check of kgx_worktool.cuh (wt_check_entries_kernel, on Dp40Check records) flags each record, an exclusive scan
+// of the flags gives each good record its slot, and one pass writes the good records in input order and the indices of the
+// first `cap` bad ones.
+#include <cub/cub.cuh>
 
 struct kgx_resolver {
   int dev = 0;
   uint32_t n_keys = 0;
+  int kinf = 0;                                         // key 0's K is the point at infinity (the check needs it)
   kgx_wt::Start start;
   kgx_wt::u32 *comb = nullptr, *kx = nullptr, *K = nullptr;
   uint32_t* ki = nullptr;
@@ -68,6 +75,33 @@ static cudaError_t resolve_events(const kgx_resolver* r, const kgx_dp_event* ev,
   return cudaGetLastError();
 }
 
+// kgx_resolver_verify's last pass: flags / pos = each record's verdict and its exclusive prefix sum.  Good record i goes to
+// good[pos[i]], bad record i is bad record number i - pos[i]; the last thread writes both counts.
+__global__ void wt_verify_compact_kernel(const u64* __restrict__ rec, uint32_t n, const uint32_t* __restrict__ flags,
+                                         const uint32_t* __restrict__ pos, u64* good, uint32_t* counts, uint32_t* bad_idx, uint32_t cap) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t p = pos[i];
+  if (flags[i]) {
+#pragma unroll
+    for (int k = 0; k < 5; k++) good[5ull * p + k] = rec[5ull * i + k];
+  } else if (i - p < cap) {
+    bad_idx[i - p] = i;
+  }
+  if (i == n - 1) {
+    counts[0] = p + flags[i];
+    counts[1] = n - (p + flags[i]);
+  }
+}
+
+inline uint64_t align256(uint64_t v) { return (v + 255) & ~255ull; }
+
+inline uint64_t verify_scan_bytes(uint32_t n) {
+  size_t b = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, b, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)(n ? n : 1));
+  return b;
+}
+
 // the checks kgx_resolver_create and kgx_work_resolve share: -1 with the reason in g_wt_err, or 0
 static int resolver_args(const char* fn, uint32_t n_keys, const uint64_t range_start[4]) {
   if (n_keys == 0 || n_keys > kgx_wf::BATCH_MAX_KEYS) { snprintf(g_wt_err, sizeof g_wt_err, "%s: n_keys must be in [1, %u]", fn, kgx_wf::BATCH_MAX_KEYS); return -1; }
@@ -98,6 +132,7 @@ kgx_resolver* kgx_resolver_create(int dev, const uint64_t* keys, uint32_t n_keys
   kgx_resolver* r = new kgx_resolver();
   r->dev = dev;
   r->n_keys = n_keys;
+  r->kinf = !(keys[0] | keys[1] | keys[2] | keys[3] | keys[4] | keys[5] | keys[6] | keys[7]);
   memcpy(r->start.v, range_start, 32);
   r->comb = comb; r->kx = kx; r->K = K; r->ki = ki;
   r->mem.swap(B.d);                                     // the resolver keeps them
@@ -125,6 +160,50 @@ int kgx_resolver_run(kgx_resolver* r, const void* pairs, uint32_t n, uint32_t* k
   }
   if (s != cudaSuccess) {
     snprintf(r->err, sizeof r->err, "kgx_resolver_run: %s", cudaGetErrorString(s));
+    return -3;
+  }
+  return 0;
+}
+
+uint64_t kgx_resolver_verify_scratch_bytes(uint32_t n) {
+  using namespace kgx_wt;
+  if (n >= 0x80000000u) return 0;
+  return 2 * align256(4ull * n) + align256(verify_scan_bytes(n));
+}
+
+int kgx_resolver_verify(kgx_resolver* r, const void* recs, uint32_t n, void* good, uint32_t* counts, uint32_t* bad_idx, uint32_t cap,
+                        void* scratch, uint64_t scratch_bytes, void* stream) {
+  using namespace kgx_wt;
+  const char* why = nullptr;
+  if (r->n_keys != 1) why = "the resolver must hold exactly one key";
+  else if (n >= 0x80000000u) why = "at most 2^31-1 records";
+  else if (((uintptr_t)recs | (uintptr_t)good) & 7) why = "recs and good must be 8-byte aligned";
+  else if ((uintptr_t)scratch & 255) why = "scratch must be 256-byte aligned";
+  else if (scratch_bytes < kgx_resolver_verify_scratch_bytes(n)) why = "scratch smaller than kgx_resolver_verify_scratch_bytes(n)";
+  if (why) {
+    snprintf(r->err, sizeof r->err, "kgx_resolver_verify: %s", why);
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t s = cudaSetDevice(r->dev);
+  if (s == cudaSuccess && n == 0) s = cudaMemsetAsync(counts, 0, 8, st);
+  if (s == cudaSuccess && n > 0) {
+    uint8_t* sb = static_cast<uint8_t*>(scratch);
+    uint32_t* flags = reinterpret_cast<uint32_t*>(sb);
+    uint32_t* pos = reinterpret_cast<uint32_t*>(sb + align256(4ull * n));
+    size_t tb = scratch_bytes - 2 * align256(4ull * n);
+    const u64* rec = static_cast<const u64*>(recs);
+    wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS, 0, st>>>(r->comb, Dp40Check{rec, flags}, n, r->K, r->kinf);
+    s = cudaGetLastError();
+    if (s == cudaSuccess) s = cub::DeviceScan::ExclusiveSum(sb + 2 * align256(4ull * n), tb, flags, pos, (int)n, st);
+    if (s == cudaSuccess) {
+      wt_verify_compact_kernel<<<(n + 255) / 256, 256, 0, st>>>(rec, n, flags, pos, static_cast<u64*>(good), counts, bad_idx, cap);
+      s = cudaGetLastError();
+    }
+  }
+  if (s != cudaSuccess) {
+    snprintf(r->err, sizeof r->err, "kgx_resolver_verify: %s", cudaGetErrorString(s));
+    cudaGetLastError();
     return -3;
   }
   return 0;

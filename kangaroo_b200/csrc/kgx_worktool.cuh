@@ -79,12 +79,45 @@ __device__ __forceinline__ void wt_load_comb(u32* sc, const u32* comb) {
   __syncthreads();
 }
 
-// Table entries: bad[i] = 1 when entry i (bucket hs[i]) is wrong.  K: 16 words (x, y), kinf = K is the point at infinity.
-// Block b checks entries [b * 128 * GROUP, (b + 1) * 128 * GROUP); thread t those at t + g * 128, g < GROUP, with one
-// inverse for its group (entries at infinity, past n or wrong, are left out of the product).
-__global__ void __launch_bounds__(CHECK_THREADS) wt_check_entries_kernel(const u32* __restrict__ comb, const Entry* __restrict__ ent,
-                                                                        const uint32_t* __restrict__ hs, uint64_t n,
-                                                                        const u32* __restrict__ K, int kinf, uint8_t* bad, ull* nbad) {
+// How wt_check_entries_kernel reads record i and reports it: d() gives its tagged distance (d1: bit 63 the sign, bit 62 the
+// type, the rest |d| with d0), same() whether x (S.x, 8 words, canonical) is its (bucket, x lo 128), done() the verdict.
+// Work-file entries: Entry + hs[i]; bad[i] = 1 when wrong, *nbad counts them.
+struct EntryCheck {
+  const Entry* ent;
+  const uint32_t* hs;
+  uint8_t* bad;
+  ull* nbad;
+  __device__ __forceinline__ void d(uint64_t i, u64& d0, u64& d1) const { d0 = ent[i].d0; d1 = ent[i].d1; }
+  __device__ __forceinline__ bool same(uint64_t i, const u32* x) const {
+    const Entry e = ent[i];
+    return (x[4] & 0x3FFFFu) == hs[i] && (((u64)x[1] << 32) | x[0]) == e.x0 && (((u64)x[3] << 32) | x[2]) == e.x1;
+  }
+  __device__ __forceinline__ void done(uint64_t i, bool wrong) const {
+    bad[i] = wrong;
+    if (wrong) atomicAdd(nbad, 1ull);
+  }
+};
+
+// 40-byte DP records {u32 kIdx; u32 h; u128 x; u128 tagged d} (Kangaroo.h:94-101), 8-byte aligned, as 5 words each:
+// good[i] = 1 when record i is right.  h >= 2^18 never equals the 18 bits of S.x, so a malformed record is wrong.
+struct Dp40Check {
+  const u64* rec;
+  uint32_t* good;
+  __device__ __forceinline__ void d(uint64_t i, u64& d0, u64& d1) const { d0 = rec[5 * i + 3]; d1 = rec[5 * i + 4]; }
+  __device__ __forceinline__ bool same(uint64_t i, const u32* x) const {
+    return (x[4] & 0x3FFFFu) == (uint32_t)(rec[5 * i] >> 32) && (((u64)x[1] << 32) | x[0]) == rec[5 * i + 1] &&
+           (((u64)x[3] << 32) | x[2]) == rec[5 * i + 2];
+  }
+  __device__ __forceinline__ void done(uint64_t i, bool wrong) const { good[i] = !wrong; }
+};
+
+// Records of a table (Src: EntryCheck, Dp40Check): record i is wrong unless S = +-|d|*G (+ K when wild) is not the point at
+// infinity and src.same(i, S.x).  K: 16 words (x, y), kinf = K is the point at infinity.  Block b checks records
+// [b * 128 * GROUP, (b + 1) * 128 * GROUP); thread t those at t + g * 128, g < GROUP, with one inverse for its group
+// (records at infinity, past n or wrong, are left out of the product).
+template <class Src>
+__global__ void __launch_bounds__(CHECK_THREADS) wt_check_entries_kernel(const u32* __restrict__ comb, const Src src, uint64_t n,
+                                                                        const u32* __restrict__ K, int kinf) {
   using namespace kgx;
   __shared__ u32 sc[COMB_WORDS];
   wt_load_comb(sc, comb);
@@ -98,9 +131,10 @@ __global__ void __launch_bounds__(CHECK_THREADS) wt_check_entries_kernel(const u
     const uint64_t i = base + (uint64_t)g * CHECK_THREADS;
     inf[g] = true;
     if (i < n) {
-      const Entry e = ent[i];
-      const bool wild = (e.d1 >> 62) & 1, neg = e.d1 >> 63;
-      const u32 m[4] = {(u32)e.d0, (u32)(e.d0 >> 32), (u32)e.d1, (u32)(e.d1 >> 32) & 0x3FFFFFFFu};
+      u64 d0, d1;
+      src.d(i, d0, d1);
+      const bool wild = (d1 >> 62) & 1, neg = d1 >> 63;
+      const u32 m[4] = {(u32)d0, (u32)(d0 >> 32), (u32)d1, (u32)(d1 >> 32) & 0x3FFFFFFFu};
       u32 Y[8];
       bool f;
       wt_comb_mul(sc, m, X[g], Y, Z[g], f);
@@ -125,11 +159,9 @@ __global__ void __launch_bounds__(CHECK_THREADS) wt_check_entries_kernel(const u
       fe_sqr(zi, zi);
       fe_mul(x, X[g], zi);
       fe_canon(x);
-      const Entry e = ent[i];
-      wrong = (x[4] & 0x3FFFFu) != hs[i] || (((u64)x[1] << 32) | x[0]) != e.x0 || (((u64)x[3] << 32) | x[2]) != e.x1;
+      wrong = !src.same(i, x);
     }
-    bad[i] = wrong;
-    if (wrong) atomicAdd(nbad, 1ull);
+    src.done(i, wrong);
   }
 }
 
@@ -826,7 +858,7 @@ int kgx_work_check_records(int dev, int walks, const void* recs, const uint32_t*
     uint32_t* dH;
     if (B.dev(&dH, 4 * n)) return -3;
     WT_CK(cudaMemcpy(dH, hs, 4 * n, cudaMemcpyHostToDevice));
-    wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS>>>(comb, (const Entry*)dRec, dH, n, K, kinf, dBad, cnt);
+    wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS>>>(comb, EntryCheck{(const Entry*)dRec, dH, dBad, cnt}, n, K, kinf);
   }
   WT_CK(cudaGetLastError());
   WT_CK(cudaMemcpy(out, walks ? dRes : dBad, n, cudaMemcpyDeviceToHost));
@@ -918,7 +950,7 @@ int kgx_work_check(int dev, const char* path, uint64_t chunk, kgx_work_check_inf
         wt_check_entries_multi_kernel<<<(unsigned)((n + CHECK_THREADS - 1) / CHECK_THREADS), CHECK_THREADS, 0, st>>>(
             comb, dEnt[b], dH[b], n, K, Kinfs, bi.n_keys, dBad[b], dCnt[b]);
       else
-        wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS, 0, st>>>(comb, dEnt[b], dH[b], n, K, kinf, dBad[b], dCnt[b]);
+        wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS, 0, st>>>(comb, EntryCheck{dEnt[b], dH[b], dBad[b], dCnt[b]}, n, K, kinf);
     } else {
       WT_CK(cudaMemcpyAsync(dEnt[b], hEnt[b], 96 * n, cudaMemcpyHostToDevice, st));
       if (batch) WT_CK(cudaMemcpyAsync(dTg[b], btg.data() + first, 2 * n, cudaMemcpyHostToDevice, st));

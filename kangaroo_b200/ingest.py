@@ -230,7 +230,7 @@ class DeviceResolver:
     key in input order that +-Td +-Wd * G hits, and its private key) without the host.  keys: K = key - start*G per key, as
     DPTable.key_table gives them (or a list of points, None for the point at infinity); range_start below n.  The comb and
     the key index are built once here; run_raw is one stream-ordered kernel, and DeviceDPTable.add(resolver=) runs it inside
-    the table's add."""
+    the table's add.  A resolver of one key also checks received DP records (verify / verify_raw, kgx_resolver_verify)."""
 
     def __init__(self, keys, range_start, device=0):
         from ._lib import load_library as load_engine
@@ -260,6 +260,41 @@ class DeviceResolver:
                                         ctypes.c_void_p(int(priv_out)), ctypes.c_void_p(int(stream)))
         if rc != 0:
             raise RuntimeError(self._lib.kgx_resolver_last_error(self._h).decode())
+
+    def verify_scratch_bytes(self, n):
+        """device scratch bytes verify_raw needs for n records"""
+        return int(self._lib.kgx_resolver_verify_scratch_bytes(int(n)))
+
+    def verify_raw(self, recs, n, good, counts, bad_idx, cap, scratch, scratch_bytes, stream=0):
+        """kgx_resolver_verify: n 40-byte DP records at device address recs (8-byte aligned) checked against the one key ->
+        good (device, the good records in input order), counts (device, 2 uint32: good, bad), bad_idx (device, the indices of
+        the first cap bad records); queued on `stream`, not waited for"""
+        rc = self._lib.kgx_resolver_verify(self._h, ctypes.c_void_p(int(recs)), int(n), ctypes.c_void_p(int(good)),
+                                           ctypes.c_void_p(int(counts)), ctypes.c_void_p(int(bad_idx)), int(cap),
+                                           ctypes.c_void_p(int(scratch)), int(scratch_bytes), ctypes.c_void_p(int(stream)))
+        if rc != 0:
+            raise RuntimeError(self._lib.kgx_resolver_last_error(self._h).decode())
+
+    def verify(self, recs, cap=None, stream=None):
+        """recs: a CUDA uint8 tensor of n x 40-byte records -> (good records as a CUDA uint8 tensor, number of bad records, the
+        first cap (default: all) bad indices as a list); on `stream` or torch's current one, waited for"""
+        import torch
+        assert recs.is_cuda and recs.dtype == torch.uint8 and recs.numel() % DP40_BYTES == 0
+        n = recs.numel() // DP40_BYTES
+        cap = n if cap is None else int(cap)
+        dev = recs.device
+        st = stream or torch.cuda.current_stream(dev)
+        with torch.cuda.stream(st):
+            good = torch.empty(max(n, 1) * DP40_BYTES, dtype=torch.uint8, device=dev)
+            counts = torch.empty(2, dtype=torch.int32, device=dev)
+            bad = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
+            nb = self.verify_scratch_bytes(n)
+            scratch = torch.empty(max(nb, 1), dtype=torch.uint8, device=dev)
+            self.verify_raw(recs.data_ptr(), n, good.data_ptr(), counts.data_ptr(), bad.data_ptr(), cap, scratch.data_ptr(), nb,
+                            st.cuda_stream)
+            n_good, n_bad = (int(v) for v in counts.cpu().tolist())
+            idx = bad[:min(n_bad, cap)].cpu().tolist()
+        return good[:n_good * DP40_BYTES], n_bad, idx
 
     def resolve(self, d_first, d_other, stream=None):
         """two lists of tagged distances (ints) -> [(key index, private key) or None]; on `stream` (a torch stream) or torch's

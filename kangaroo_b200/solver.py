@@ -1,6 +1,7 @@
 """Stand-alone multi-GPU driver of the jump engine: the role Kangaroo::Run / SolveKeyGPU (Kangaroo.cpp:913-1083,
-510-644) plays in the reference, with the reference's TCP client/server (Network.cpp) replaced in-box by one process
-per GPU and an NCCL gather of the DP records to rank 0 (kangaroo_b200/dist.py).  Kept deliberately small: it exists to
+510-644) plays in the reference, on the GPUs of one job: one process per GPU and an NCCL gather of the DP records to rank 0
+(kangaroo_b200/dist.py).  Machines that join and leave use the reference's client/server mode instead, with
+kangaroo_b200/server.py as the server.  Kept deliberately small: it exists to
 exercise the engine end to end (BASELINE config 4) -- the full-featured caller remains the reference's own program
 linked against the engine (INTEGRATION.md).
 
