@@ -211,7 +211,15 @@ typedef struct {                     /* = kgi_event (include/kgx_ingest.h) */
  *     `cap` bad records in input order.  scratch: device memory of at least kgx_resolver_verify_scratch_bytes(n) bytes,
  *     256-byte aligned (as cudaMalloc returns it; the flags, their prefix sums and cub's scan storage live there).
  *     Stream-ordered on `stream`, no allocation, no synchronisation.  -1: bad arguments; -3: a CUDA error, text in
- *     kgx_resolver_last_error(r). --- */
+ *     kgx_resolver_last_error(r).
+ * _verify_partition: _verify and kgx_dp_partition in one call, for a DP table sharded over W tables (1 .. KGX_DPT_MAX_RANKS).
+ *     The same check, then the good records grouped by the shard that owns their bucket (shard r of W holds the buckets
+ *     [floor(r*2^18/W), floor((r+1)*2^18/W))), each group in input order, into out (device, 8-byte aligned): packed when
+ *     stride = 0, else group r at record r * stride (stride >= n).  counts (device, W + 1 entries): the good records of each
+ *     group, then the bad count; bad_idx (device, cap entries): the indices of the first `cap` bad records in input order.
+ *     The result is byte for byte that of _verify followed by kgx_dp_partition of its good records.  scratch: at least
+ *     kgx_resolver_verify_partition_scratch_bytes(n, W) bytes (0: bad arguments), 256-byte aligned.  Stream-ordered on
+ *     `stream`, no allocation, no synchronisation.  -1: bad arguments; -3: a CUDA error, text in kgx_resolver_last_error(r). --- */
 typedef struct kgx_resolver kgx_resolver;
 #define KGX_NO_KEY 0xFFFFFFFFu
 kgx_resolver* kgx_resolver_create(int dev, const uint64_t* keys, uint32_t n_keys, const uint64_t range_start[4]);
@@ -221,6 +229,10 @@ int           kgx_resolver_run(kgx_resolver* r, const void* pairs, uint32_t n, u
 uint64_t      kgx_resolver_verify_scratch_bytes(uint32_t n);
 int           kgx_resolver_verify(kgx_resolver* r, const void* recs, uint32_t n, void* good, uint32_t* counts, uint32_t* bad_idx,
                                   uint32_t cap, void* scratch, uint64_t scratch_bytes, void* stream);
+uint64_t      kgx_resolver_verify_partition_scratch_bytes(uint32_t n, uint32_t world);
+int           kgx_resolver_verify_partition(kgx_resolver* r, const void* recs, uint32_t n, uint32_t world, uint64_t stride, void* out,
+                                            uint32_t* counts, uint32_t* bad_idx, uint32_t cap, void* scratch, uint64_t scratch_bytes,
+                                            void* stream);
 /* An event of kgx_dptable_add_resolve: the event of kgx_dptable_add, then for a collision event the resolver's key index and
  * private key, KGX_NO_KEY and 0 for any other event. */
 typedef struct {

@@ -107,6 +107,10 @@ _SIGS = {
     "kgx_resolver_verify_scratch_bytes": (ctypes.c_uint64, [ctypes.c_uint32]),
     "kgx_resolver_verify": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                            ctypes.c_uint32, ctypes.c_void_p, ctypes.c_uint64, ctypes.c_void_p]),
+    "kgx_resolver_verify_partition_scratch_bytes": (ctypes.c_uint64, [ctypes.c_uint32, ctypes.c_uint32]),
+    "kgx_resolver_verify_partition": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint64,
+                                                     ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32, ctypes.c_void_p,
+                                                     ctypes.c_uint64, ctypes.c_void_p]),
     "kgx_dptable_add_resolve": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint32), ctypes.c_uint32,
                                                ctypes.c_uint64, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32,
                                                ctypes.POINTER(ctypes.c_uint32), ctypes.c_void_p]),

@@ -852,6 +852,6 @@ int kgx_bench_raw(int dev, int kind, int iters, float* ms, double* ops) {
 
 #include "kgx_bucketsort.cuh"  // work-file order for a block of buckets (the table's save and the merge)
 #include "kgx_worktool.cuh"  // work-file check and merge (kgx_work_*)
+#include "kgx_partition.cuh" // a rank's DP records grouped by the shard that owns them (kgx_dp_partition)
 #include "kgx_resolver.cuh"  // the persistent collision resolver (kgx_resolver_*), which the table's resolving add runs
 #include "kgx_dptable.cuh"   // the device-resident DP table (kgx_dptable_*)
-#include "kgx_partition.cuh" // a rank's DP records grouped by the shard that owns them (kgx_dp_partition)

@@ -23,32 +23,47 @@ __device__ __forceinline__ uint32_t dest_of(const uint8_t* recs, uint32_t i, uin
   return h < kgx_wf::NBUCKET ? owner_of(h, world) : world;
 }
 
-__global__ void k_hist(const uint8_t* recs, uint32_t n, uint32_t world, uint32_t ntiles, uint32_t* hist) {
+// Where record i goes: its owner, or `world` for a record left out (the malformed ones here; the wrong ones of
+// kgx_resolver_verify_partition, whose Dest reads the check's flags)
+struct ByBucket {
+  const uint8_t* recs;
+  __device__ __forceinline__ uint32_t operator()(uint32_t i, uint32_t world) const { return dest_of(recs, i, world); }
+};
+
+template <class Dest>
+__global__ void k_hist(Dest dest, uint32_t n, uint32_t world, uint32_t ntiles, uint32_t* hist) {
   __shared__ uint32_t cnt[KGX_DPT_MAX_RANKS + 1];
   for (uint32_t d = threadIdx.x; d <= world; d += blockDim.x) cnt[d] = 0;
   __syncthreads();
   const uint32_t i = blockIdx.x * TILE + threadIdx.x;
-  if (i < n) atomicAdd(&cnt[dest_of(recs, i, world)], 1u);
+  if (i < n) atomicAdd(&cnt[dest(i, world)], 1u);
   __syncthreads();
   for (uint32_t d = threadIdx.x; d <= world; d += blockDim.x) hist[(uint64_t)d * ntiles + blockIdx.x] = cnt[d];
 }
 
-// stride 0: the groups packed one after another; else group d starts at record d * stride
-__global__ void k_scatter(const uint8_t* recs, uint32_t n, uint32_t world, uint32_t ntiles, const uint32_t* pos, uint64_t stride,
-                          uint8_t* out) {
+// stride 0: the groups packed one after another; else group d starts at record d * stride.  left: null, or the indices of the
+// first `cap` records left out, in input order
+template <class Dest>
+__global__ void k_scatter(const uint8_t* recs, Dest dest, uint32_t n, uint32_t world, uint32_t ntiles, const uint32_t* pos, uint64_t stride,
+                          uint8_t* out, uint32_t* left, uint32_t cap) {
   __shared__ uint32_t wcnt[WARPS][KGX_DPT_MAX_RANKS + 1];
   const uint32_t lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   for (uint32_t k = threadIdx.x; k < WARPS * (world + 1); k += blockDim.x) wcnt[k / (world + 1)][k % (world + 1)] = 0;
   __syncthreads();
   const uint32_t i = blockIdx.x * TILE + threadIdx.x;
-  const uint32_t d = i < n ? dest_of(recs, i, world) : 0xFFFFFFFFu;
+  const uint32_t d = i < n ? dest(i, world) : 0xFFFFFFFFu;
   const uint32_t peers = __match_any_sync(0xFFFFFFFFu, d);
   if (i < n && lane == __ffs(peers) - 1) wcnt[w][d] = __popc(peers);
   __syncthreads();
-  if (i >= n || d == world) return;
+  if (i >= n || (d == world && !left)) return;
   uint32_t r = __popc(peers & ((1u << lane) - 1));
   for (uint32_t v = 0; v < w; v++) r += wcnt[v][d];
   const uint64_t p = pos[(uint64_t)d * ntiles + blockIdx.x];
+  if (d == world) {                                       // the record's number among those left out
+    const uint64_t b = p - pos[(uint64_t)world * ntiles] + r;
+    if (b < cap) left[b] = i;
+    return;
+  }
   const uint64_t slot = stride ? d * stride + (p - pos[(uint64_t)d * ntiles]) + r : p + r;
   // 32-bit words: kgx_convert_dps's records follow its u32 count, so they are 4-byte aligned only
   const uint32_t* s4 = reinterpret_cast<const uint32_t*>(recs + 40ull * i);
@@ -75,6 +90,25 @@ inline size_t scan_bytes(uint32_t n, uint32_t world) {
 
 inline uint64_t align256(uint64_t v) { return (v + 255) & ~255ull; }
 
+// the three passes and the counts on st, scratch as kgx_dp_partition_scratch_bytes(n, world) lays it out -> 0 or -3
+template <class Dest>
+int run(const uint8_t* recs, Dest dest, uint32_t n, uint32_t world, uint64_t stride, void* out, uint32_t* counts, uint32_t* left,
+        uint32_t cap, void* scratch, uint64_t scratch_bytes, cudaStream_t st) {
+  const uint32_t nt = tiles_for(n);
+  const uint64_t cells = (uint64_t)(world + 1) * nt;
+  uint8_t* s = static_cast<uint8_t*>(scratch);
+  uint32_t* hist = reinterpret_cast<uint32_t*>(s);
+  uint32_t* pos = reinterpret_cast<uint32_t*>(s + align256(4 * cells));
+  void* tmp = s + 2 * align256(4 * cells);
+  size_t tb = scratch_bytes - 2 * align256(4 * cells);
+  k_hist<<<nt, TILE, 0, st>>>(dest, n, world, nt, hist);
+  if (cudaGetLastError() != cudaSuccess) return -3;
+  if (cub::DeviceScan::ExclusiveSum(tmp, tb, hist, pos, (int)cells, st) != cudaSuccess) return -3;
+  if (n) k_scatter<<<nt, TILE, 0, st>>>(recs, dest, n, world, nt, pos, stride, static_cast<uint8_t*>(out), left, cap);
+  k_counts<<<(world + 1 + 255) / 256, 256, 0, st>>>(hist, pos, world, nt, counts);
+  return cudaGetLastError() == cudaSuccess ? 0 : -3;
+}
+
 }  // namespace kgx_part
 
 extern "C" {
@@ -92,21 +126,8 @@ int kgx_dp_partition(const void* recs, uint32_t n, uint32_t world, uint64_t stri
   if (world == 0 || world > KGX_DPT_MAX_RANKS || n >= 0x80000000u || (stride != 0 && stride < n) ||
       scratch_bytes < kgx_dp_partition_scratch_bytes(n, world))
     return -1;
-  cudaStream_t st = (cudaStream_t)stream;
-  const uint32_t nt = tiles_for(n);
-  const uint64_t cells = (uint64_t)(world + 1) * nt;
-  uint8_t* s = static_cast<uint8_t*>(scratch);
-  uint32_t* hist = reinterpret_cast<uint32_t*>(s);
-  uint32_t* pos = reinterpret_cast<uint32_t*>(s + align256(4 * cells));
-  void* tmp = s + 2 * align256(4 * cells);
-  size_t tb = scratch_bytes - 2 * align256(4 * cells);
   const uint8_t* in = static_cast<const uint8_t*>(recs);
-  k_hist<<<nt, TILE, 0, st>>>(in, n, world, nt, hist);
-  if (cudaGetLastError() != cudaSuccess) return -3;
-  if (cub::DeviceScan::ExclusiveSum(tmp, tb, hist, pos, (int)cells, st) != cudaSuccess) return -3;
-  if (n) k_scatter<<<nt, TILE, 0, st>>>(in, n, world, nt, pos, stride, static_cast<uint8_t*>(out));
-  k_counts<<<(world + 1 + 255) / 256, 256, 0, st>>>(hist, pos, world, nt, counts);
-  return cudaGetLastError() == cudaSuccess ? 0 : -3;
+  return run(in, ByBucket{in}, n, world, stride, out, counts, nullptr, 0, scratch, scratch_bytes, (cudaStream_t)stream);
 }
 
 }  // extern "C"

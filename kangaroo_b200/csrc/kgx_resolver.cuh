@@ -10,7 +10,9 @@
 // A resolver of one key also checks received DP records (kgx_resolver_verify, the server's check of what clients send): the
 // stored-entry check of kgx_worktool.cuh (wt_check_entries_kernel, on Dp40Check records) flags each record, an exclusive scan
 // of the flags gives each good record its slot, and one pass writes the good records in input order and the indices of the
-// first `cap` bad ones.
+// first `cap` bad ones.  kgx_resolver_verify_partition runs the same check, then kgx_dp_partition's passes (kgx_partition.cuh)
+// with the wrong records as the group left out: the good records grouped by the shard that owns their bucket, and the bad
+// indices, from one scan of (owner, tile) counts.
 #include <cub/cub.cuh>
 
 struct kgx_resolver {
@@ -95,6 +97,16 @@ __global__ void wt_verify_compact_kernel(const u64* __restrict__ rec, uint32_t n
 }
 
 inline uint64_t align256(uint64_t v) { return (v + 255) & ~255ull; }
+
+// kgx_resolver_verify_partition's destination of record i: the owner of its bucket when the check found it good (then
+// h < 2^18, since h equals 18 bits of S.x), else the group left out
+struct Verified {
+  const uint8_t* recs;
+  const uint32_t* good;
+  __device__ __forceinline__ uint32_t operator()(uint32_t i, uint32_t world) const {
+    return good[i] ? kgx_part::owner_of(reinterpret_cast<const uint32_t*>(recs + 40ull * i)[1], world) : world;
+  }
+};
 
 inline uint64_t verify_scan_bytes(uint32_t n) {
   size_t b = 0;
@@ -203,6 +215,50 @@ int kgx_resolver_verify(kgx_resolver* r, const void* recs, uint32_t n, void* goo
   }
   if (s != cudaSuccess) {
     snprintf(r->err, sizeof r->err, "kgx_resolver_verify: %s", cudaGetErrorString(s));
+    cudaGetLastError();
+    return -3;
+  }
+  return 0;
+}
+
+uint64_t kgx_resolver_verify_partition_scratch_bytes(uint32_t n, uint32_t world) {
+  using namespace kgx_wt;
+  const uint64_t part = kgx_dp_partition_scratch_bytes(n, world);
+  return n >= 0x80000000u || part == 0 ? 0 : align256(4ull * n) + part;
+}
+
+int kgx_resolver_verify_partition(kgx_resolver* r, const void* recs, uint32_t n, uint32_t world, uint64_t stride, void* out,
+                                  uint32_t* counts, uint32_t* bad_idx, uint32_t cap, void* scratch, uint64_t scratch_bytes, void* stream) {
+  using namespace kgx_wt;
+  const char* why = nullptr;
+  if (r->n_keys != 1) why = "the resolver must hold exactly one key";
+  else if (n >= 0x80000000u) why = "at most 2^31-1 records";
+  else if (world == 0 || world > KGX_DPT_MAX_RANKS) why = "world must be 1 .. KGX_DPT_MAX_RANKS";
+  else if (stride != 0 && stride < n) why = "stride must be 0 or at least n";
+  else if (((uintptr_t)recs | (uintptr_t)out) & 7) why = "recs and out must be 8-byte aligned";
+  else if ((uintptr_t)scratch & 255) why = "scratch must be 256-byte aligned";
+  else if (scratch_bytes < kgx_resolver_verify_partition_scratch_bytes(n, world))
+    why = "scratch smaller than kgx_resolver_verify_partition_scratch_bytes(n, world)";
+  if (why) {
+    snprintf(r->err, sizeof r->err, "kgx_resolver_verify_partition: %s", why);
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t s = cudaSetDevice(r->dev);
+  uint8_t* sb = static_cast<uint8_t*>(scratch);
+  uint32_t* flags = reinterpret_cast<uint32_t*>(sb);
+  const uint8_t* in = static_cast<const uint8_t*>(recs);
+  if (s == cudaSuccess && n > 0) {
+    wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS, 0, st>>>(r->comb, Dp40Check{static_cast<const u64*>(recs), flags}, n, r->K,
+                                                                      r->kinf);
+    s = cudaGetLastError();
+  }
+  const int rc = s == cudaSuccess ? kgx_part::run(in, Verified{in, flags}, n, world, stride, out, counts, bad_idx, cap,
+                                                  sb + align256(4ull * n), scratch_bytes - align256(4ull * n), st)
+                                   : 0;
+  if (s != cudaSuccess || rc) {
+    snprintf(r->err, sizeof r->err, "kgx_resolver_verify_partition: %s",
+             s != cudaSuccess ? cudaGetErrorString(s) : "a launch of the partition passes failed");
     cudaGetLastError();
     return -3;
   }

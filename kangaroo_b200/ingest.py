@@ -230,7 +230,9 @@ class DeviceResolver:
     key in input order that +-Td +-Wd * G hits, and its private key) without the host.  keys: K = key - start*G per key, as
     DPTable.key_table gives them (or a list of points, None for the point at infinity); range_start below n.  The comb and
     the key index are built once here; run_raw is one stream-ordered kernel, and DeviceDPTable.add(resolver=) runs it inside
-    the table's add.  A resolver of one key also checks received DP records (verify / verify_raw, kgx_resolver_verify)."""
+    the table's add.  A resolver of one key also checks received DP records (verify / verify_raw, kgx_resolver_verify), and
+    groups the good ones by the shard of a sharded table that owns them in the same call (verify_partition /
+    verify_partition_raw, kgx_resolver_verify_partition)."""
 
     def __init__(self, keys, range_start, device=0):
         from ._lib import load_library as load_engine
@@ -295,6 +297,44 @@ class DeviceResolver:
             n_good, n_bad = (int(v) for v in counts.cpu().tolist())
             idx = bad[:min(n_bad, cap)].cpu().tolist()
         return good[:n_good * DP40_BYTES], n_bad, idx
+
+    def verify_partition_scratch_bytes(self, n, world):
+        """device scratch bytes verify_partition_raw needs for n records and `world` shards"""
+        return int(self._lib.kgx_resolver_verify_partition_scratch_bytes(int(n), int(world)))
+
+    def verify_partition_raw(self, recs, n, world, stride, out, counts, bad_idx, cap, scratch, scratch_bytes, stream=0):
+        """kgx_resolver_verify_partition: verify_raw's check, then the good records grouped by the shard of `world` that owns
+        their bucket, each group in input order, at out + shard * stride records (packed when stride = 0) -> counts (device,
+        world + 1 uint32: each group's records, then the bad count) and bad_idx (device, the first cap bad indices); queued on
+        `stream`, not waited for"""
+        rc = self._lib.kgx_resolver_verify_partition(self._h, ctypes.c_void_p(int(recs)), int(n), int(world), int(stride),
+                                                     ctypes.c_void_p(int(out)), ctypes.c_void_p(int(counts)),
+                                                     ctypes.c_void_p(int(bad_idx)), int(cap), ctypes.c_void_p(int(scratch)),
+                                                     int(scratch_bytes), ctypes.c_void_p(int(stream)))
+        if rc != 0:
+            raise RuntimeError(self._lib.kgx_resolver_last_error(self._h).decode())
+
+    def verify_partition(self, recs, world, stride=0, cap=None, stream=None):
+        """recs: a CUDA uint8 tensor of n x 40-byte records -> (out as a CUDA uint8 tensor of max(n, 1) records, or world x stride
+        records with a stride, the good records per shard as a list, the number of bad records, the first cap (default: all)
+        bad indices as a list); on `stream` or torch's current one, waited for"""
+        import torch
+        assert recs.is_cuda and recs.dtype == torch.uint8 and recs.numel() % DP40_BYTES == 0
+        n = recs.numel() // DP40_BYTES
+        cap = n if cap is None else int(cap)
+        dev = recs.device
+        st = stream or torch.cuda.current_stream(dev)
+        with torch.cuda.stream(st):
+            out = torch.empty((world * stride if stride else max(n, 1)) * DP40_BYTES, dtype=torch.uint8, device=dev)
+            counts = torch.empty(world + 1, dtype=torch.int32, device=dev)
+            bad = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
+            nb = self.verify_partition_scratch_bytes(n, world)
+            scratch = torch.empty(max(nb, 1), dtype=torch.uint8, device=dev)
+            self.verify_partition_raw(recs.data_ptr(), n, world, stride, out.data_ptr(), counts.data_ptr(), bad.data_ptr(), cap,
+                                      scratch.data_ptr(), nb, st.cuda_stream)
+            c = [int(v) for v in counts.cpu().tolist()]
+            idx = bad[:min(c[world], cap)].cpu().tolist()
+        return out, c[:world], c[world], idx
 
     def resolve(self, d_first, d_other, stream=None):
         """two lists of tagged distances (ints) -> [(key index, private key) or None]; on `stream` (a torch stream) or torch's

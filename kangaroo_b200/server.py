@@ -16,6 +16,11 @@ Threads:
                queued like records, so a work file holds the table after every record queued before it.
   main         the status line, periodic saves, signals and the end of the run.
 
+With --devices D0,D1,... (two or more entries) the table is split into one shard per entry (ShardedSink), in the buckets
+the solver's --dp-table sharded gives its ranks; the ingest thread then verifies each batch and groups its good records by
+shard in one kernel (kgx_resolver_verify_partition), and adds every group to its shard.  Its work files are byte for byte
+those of the one table.
+
 The protocol layer (Server) talks to its sink through three calls -- put(message, chunks), status(), reset_dead() -- so that
 a test can run it with a fake sink in place of the GPU path.
 """
@@ -49,6 +54,7 @@ END_GRACE = 10.0                # seconds the server waits for clients to leave 
 STATUS_PERIOD = 5.0             # seconds between status lines
 DP40 = 40
 EVENT_BYTES = 136               # device scratch per event slot of an add (kgx_dptable_reserve)
+MAX_SHARDS = 256                # KGX_DPT_MAX_RANKS: the shards of one table
 
 
 class ClientGone(Exception):
@@ -483,8 +489,7 @@ class GpuSink:
     def _save(self):
         from .solver import WorkFile
         wf = WorkFile(self.save_path, time.perf_counter())
-        wf.begin(lambda p: self.table.save_work(p, self.dp, self.start, self.end, self.pub, 0, self.elapsed(), 0,
-                                                stream=self.stream.cuda_stream))
+        wf.begin(self._write_table)
         path, mb, secs, err = wf.finish()
         self.last_save = (path, err)
         if err is None:
@@ -493,15 +498,35 @@ class GpuSink:
             self.out("Work file %s NOT written: %s (the previous file is kept)" % (path, err))
         self.saving -= 1
 
-    def _ingest(self, batch):
-        torch = self.torch
+    def _write_table(self, path):
+        self.table.save_work(path, self.dp, self.start, self.end, self.pub, 0, self.elapsed(), 0, stream=self.stream.cuda_stream)
+
+    def _stage(self, batch):
+        """the batch's records into the pinned host buffer -> (bytes, records, end of each chunk in records)"""
         sizes = [buf.nbytes for _, buf, _ in batch]
         ends = np.cumsum(sizes) // DP40
-        n = int(ends[-1])
         off = 0
         for (_, buf, _), sz in zip(batch, sizes):
             self._host_np[off:off + sz] = buf
             off += sz
+        return off, int(ends[-1]), ends
+
+    def _charge(self, batch, ends, n_bad, bad):
+        """n_bad wrong records, the device tensor bad holding their indices, charged to their messages and clients"""
+        if n_bad:
+            bad = bad[:n_bad].cpu().numpy()
+            per_chunk = np.bincount(np.searchsorted(ends, bad, side="right"), minlength=len(batch))
+            for (msg, _, _), k in zip(batch, per_chunk.tolist()):
+                msg.bad += k
+                msg.client.wrong += k
+            self.wrong += n_bad
+        for msg, _, last in batch:
+            if last and msg.bad:
+                self.out(msg.wrong_line())
+
+    def _ingest(self, batch):
+        torch = self.torch
+        off, n, ends = self._stage(batch)
         st = self.stream
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
         with torch.cuda.stream(st):
@@ -517,17 +542,8 @@ class GpuSink:
         self.t_verify += ev[1].elapsed_time(ev[2]) / 1e3
         n_good, n_bad = (int(v) for v in self._counts_h.tolist())
         self.received += n
-        if n_bad:
-            with torch.cuda.stream(st):
-                bad = self._bad[:n_bad].cpu().numpy()
-            per_chunk = np.bincount(np.searchsorted(ends, bad, side="right"), minlength=len(batch))
-            for (msg, _, _), k in zip(batch, per_chunk.tolist()):
-                msg.bad += k
-                msg.client.wrong += k
-            self.wrong += n_bad
-        for msg, _, last in batch:
-            if last and msg.bad:
-                self.out(msg.wrong_line())
+        with torch.cuda.stream(st):
+            self._charge(batch, ends, n_bad, self._bad)
         if n_good:
             t0 = time.perf_counter()
             try:
@@ -557,6 +573,181 @@ class GpuSink:
                              (e[2], e[3][1], e[3][0], e[4][1], e[4][0]))
 
 
+def shard_plan(devices):
+    """--devices -> [(device, lo, hi)] per shard: shard s of W holds the buckets [floor(s*2^18/W), floor((s+1)*2^18/W)), the
+    range rank s of the solver's --dp-table sharded holds, so the pieces of a work file sit where the solver puts them"""
+    from .dist import owner_ranges
+    return [(d, lo, hi) for d, (lo, hi) in zip(devices, owner_ranges(len(devices)))]
+
+
+class ShardTables:
+    """the shards of a ShardedSink as one table for the status line and the messages: entries, capacity and memory summed"""
+
+    def __init__(self, tables):
+        self.shards = tables
+        self.capacity = sum(t.capacity for t in tables)
+
+    def __len__(self):
+        return sum(len(t) for t in self.shards)
+
+    def memory_bytes(self):
+        return sum(t.memory_bytes() for t in self.shards)
+
+    def fullest(self):
+        """-> (shard, entries, capacity) of the shard with the largest fill"""
+        s = max(range(len(self.shards)), key=lambda i: len(self.shards[i]) / self.shards[i].capacity)
+        return s, len(self.shards[s]), self.shards[s].capacity
+
+
+class ShardedSink(GpuSink):
+    """--devices with two or more entries: the table split into one shard per entry (shard_plan), a DeviceDPTable of its
+    buckets on that entry's GPU; a GPU listed k times holds k shards.  Each distinct GPU has one resolver, shared by its shards,
+    and one set of batch buffers; each shard has its own stream and, when there are several GPUs, a staging buffer on its GPU.
+    Everything is allocated here.  capacity is per shard; by default each GPU's free memory, less its buffers, is split
+    evenly among its shards.
+
+    The ingest thread, per batch: one copy to the next GPU in turn (spreading the verify), kgx_resolver_verify_partition there
+    (the check, the good records grouped by shard in input order, the per-shard and bad counts), the counts back; then, unless
+    some shard would overflow (nothing of the batch is added then), each shard's group -- read in place on the batch's GPU, or
+    copied to the shard's staging buffer on another one -- added with its GPU's resolver on the shard's stream.  Each add
+    waits for its own work, and a batch is done before the next starts, so every bucket sees its records in queue order, as
+    the one table does.  A save writes the header, then each shard's piece at its offset: the one table's file, byte for byte."""
+
+    def __init__(self, start, end, pub, dp, devices, capacity=None, resume=None, save_path="", out=print):
+        import torch
+        from .ingest import DeviceDPTable, DeviceResolver, DPTable, TableFull
+        from .solver import DP_TABLE_MARGIN, default_table_capacity, scratch_bytes
+        self.torch, self.TableFull = torch, TableFull
+        self.start, self.end, self.pub, self.dp = start, end, pub, dp
+        self.save_path, self.out = save_path, out
+        self.plan = shard_plan(devices)
+        W = len(self.plan)
+        gpus = sorted(set(devices))
+        K = ec.add(pub, ec.neg(ec.mul(start))) if start else pub
+        self.gpus = {}                                        # device -> its resolver, batch buffers and stream
+        for d in gpus:
+            dev = torch.device("cuda", d)
+            r = DeviceResolver(DPTable.key_table([K]), start, device=d)
+            nb = r.verify_partition_scratch_bytes(CHUNK_RECORDS, W)
+            self.gpus[d] = dict(resolver=r, nb=nb, stream=torch.cuda.Stream(device=dev),
+                                recs=torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8, device=dev),
+                                out=torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8, device=dev),
+                                bad=torch.empty(CHUNK_RECORDS, dtype=torch.int32, device=dev),
+                                counts=torch.empty(W + 1, dtype=torch.int32, device=dev),
+                                scratch=torch.empty(nb, dtype=torch.uint8, device=dev))
+        self._host = torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8).pin_memory()
+        self._host_np = self._host.numpy()
+        self._counts_h = torch.empty(W + 1, dtype=torch.int32).pin_memory()
+        staged = len(gpus) > 1
+        per_shard = scratch_bytes(CHUNK_RECORDS) + EVENT_BYTES * CHUNK_RECORDS + (CHUNK_RECORDS * DP40 if staged else 0)
+        caps = {}
+        for d in gpus:                                        # before any table takes memory
+            k = devices.count(d)
+            caps[d] = capacity or default_table_capacity((torch.cuda.mem_get_info(d)[0] - DP_TABLE_MARGIN) // k - per_shard,
+                                                         margin=0)
+        self.shards = []
+        for s, (d, lo, hi) in enumerate(self.plan):
+            dev = torch.device("cuda", d)
+            t = DeviceDPTable(caps[d], device=d, max_events=CHUNK_RECORDS, buckets=(lo, hi))
+            t.reserve(CHUNK_RECORDS)
+            self.shards.append(dict(table=t, device=d, lo=lo, hi=hi, stream=torch.cuda.Stream(device=dev),
+                                    staging=torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8, device=dev) if staged else None))
+        self.table = ShardTables([sh["table"] for sh in self.shards])
+        self.shard_capacity = max(caps.values())
+        self.time0 = 0.0
+        if resume:
+            info = None
+            for s, sh in enumerate(self.shards):
+                try:
+                    info = sh["table"].load_piece(resume, sh["table"].capacity, stream=sh["stream"].cuda_stream)
+                except TableFull as e:
+                    raise TableFull("%s (shard %d of %d, buckets [%d, %d) on cuda:%d)" % (e, s, W, sh["lo"], sh["hi"], sh["device"]))
+            self.time0 = info.total_time
+            self.resumed = (len(self.table), info.nb_walk)
+        self.t_start = time.perf_counter()
+        self.queue = RecordQueue()
+        self.dead = self.wrong = self.wrong_collisions = self.received = 0
+        self.saving = 0
+        self.solved = None
+        self.full = None
+        self.failed = None
+        self.last_save = None
+        self.batches, self.t_copy, self.t_verify, self.t_add, self.t_peer = 0, 0.0, 0.0, 0.0, 0.0
+        self._turn = 0                                        # batches taken: the next one goes to gpus[_turn % len(gpus)]
+        self._thread = threading.Thread(target=self._loop, name="ingest", daemon=True)
+        self._thread.start()
+
+    def describe(self):
+        return "%d shards on cuda:%s, capacity %d entries each (%.2f GB in all)" % (
+            len(self.shards), ",".join(str(d) for d, _, _ in self.plan), self.shard_capacity, self.table.memory_bytes() / 1e9)
+
+    def close(self):
+        for sh in self.shards:
+            sh["table"].close()
+        for g in self.gpus.values():
+            g["resolver"].close()
+
+    def _write_table(self, path):
+        from .solver import piece_offsets, work_header
+        with open(path, "wb") as f:
+            f.write(work_header(self.dp, self.start, self.end, self.pub, 0, self.elapsed()))
+        offsets = piece_offsets([sh["table"].piece_bytes() for sh in self.shards])
+        for sh, o in zip(self.shards, offsets):
+            sh["table"].save_piece(path, o, stream=sh["stream"].cuda_stream)
+        with open(path, "r+b") as f:
+            f.seek(offsets[-1])
+            f.write(struct.pack("<Q", 0))                    # no kangaroos
+
+    def _ingest(self, batch):
+        torch = self.torch
+        W = len(self.shards)
+        off, n, ends = self._stage(batch)
+        d = sorted(self.gpus)[self._turn % len(self.gpus)]
+        self._turn += 1
+        g = self.gpus[d]
+        st = g["stream"]
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+        with torch.cuda.stream(st):
+            ev[0].record(st)
+            g["recs"][:off].copy_(self._host[:off], non_blocking=True)
+            ev[1].record(st)
+            g["resolver"].verify_partition_raw(g["recs"].data_ptr(), n, W, 0, g["out"].data_ptr(), g["counts"].data_ptr(),
+                                               g["bad"].data_ptr(), CHUNK_RECORDS, g["scratch"].data_ptr(), g["nb"], st.cuda_stream)
+            ev[2].record(st)
+            self._counts_h.copy_(g["counts"], non_blocking=True)
+        st.synchronize()
+        self.t_copy += ev[0].elapsed_time(ev[1]) / 1e3
+        self.t_verify += ev[1].elapsed_time(ev[2]) / 1e3
+        c = [int(v) for v in self._counts_h.tolist()]
+        self.received += n
+        with torch.cuda.stream(st):
+            self._charge(batch, ends, c[W], g["bad"])
+        for s, sh in enumerate(self.shards):                 # a saved file is always a cut between whole batches
+            t = sh["table"]
+            if len(t) + c[s] > t.capacity:
+                self.full = ("shard %d of %d (buckets [%d, %d) on cuda:%d) holds %d entries, capacity %d; this batch brought it %d "
+                             "more" % (s, W, sh["lo"], sh["hi"], sh["device"], len(t), t.capacity, c[s]))
+                return
+        t0 = time.perf_counter()
+        first = 0
+        for s, sh in enumerate(self.shards):
+            k, src = c[s], g["out"][first * DP40:(first + c[s]) * DP40]
+            first += k
+            if not k:
+                continue
+            if sh["device"] != d:                           # another GPU: into the shard's staging buffer, on its stream
+                p0 = time.perf_counter()
+                with torch.cuda.stream(sh["stream"]):
+                    sh["staging"][:k * DP40].copy_(src, non_blocking=True)
+                sh["stream"].synchronize()
+                self.t_peer += time.perf_counter() - p0
+                src = sh["staging"]
+            evs = sh["table"].add(src.data_ptr(), [k], k, sh["stream"].cuda_stream, self.gpus[sh["device"]]["resolver"])
+            self._events(evs)
+        self.t_add += time.perf_counter() - t0
+        self.batches += 1
+
+
 def expected_dps(start, end, kangaroos, dp):
     """log2 of the DPs the reference expects a search to need (Kangaroo::ComputeExpected, no symmetry)"""
     n = 2.0 ** max((end - start).bit_length(), 1)
@@ -575,10 +766,14 @@ def time_str(t):
 
 def status_line(server, sink):
     k = server.kangaroos()
-    return ("[Client %d][Kang 2^%.2f][DP Count 2^%.2f/2^%.2f][Dead %d][Wrong %d][%s][%d / %d entries]" %
+    line = ("[Client %d][Kang 2^%.2f][DP Count 2^%.2f/2^%.2f][Dead %d][Wrong %d][%s][%d / %d entries]" %
             (server.n_clients(), np.log2(max(k, 1)), np.log2(max(len(sink.table), 1)),
              expected_dps(sink.start, sink.end, k, sink.dp), sink.dead, sink.wrong, time_str(sink.elapsed()), len(sink.table),
              sink.table.capacity))
+    if isinstance(sink.table, ShardTables):
+        s, n, cap = sink.table.fullest()
+        line += "[fullest shard %d: %d / %d, %.1f%%]" % (s, n, cap, 100.0 * n / cap)
+    return line
 
 
 def parse_args(argv=None):
@@ -590,9 +785,13 @@ def parse_args(argv=None):
     ap.add_argument("--dp", type=int, default=None, help="distinguished-point bits the clients use (required without --resume)")
     ap.add_argument("--bind", default="0.0.0.0", help="address to listen on (default 0.0.0.0)")
     ap.add_argument("--port", type=int, default=DEFAULT_PORT, help="TCP port (default %d; 0 = an ephemeral port)" % DEFAULT_PORT)
-    ap.add_argument("--device", type=int, default=0, help="the GPU that holds the table")
+    ap.add_argument("--device", type=int, default=None, help="the GPU that holds the table (default 0)")
+    ap.add_argument("--devices", default=None, metavar="D0,D1,...",
+                    help="split the table into one shard per entry, on that GPU (a GPU may be listed more than once), in the "
+                         "solver's --dp-table sharded bucket ranges; two or more entries (at most %d)" % MAX_SHARDS)
     ap.add_argument("--dp-table-capacity", type=int, default=None, metavar="E",
-                    help="entries the table holds, 48 bytes of GPU memory each (default: what fits in the free GPU memory)")
+                    help="entries the table holds, 48 bytes of GPU memory each (default: what fits in the free GPU memory); "
+                         "with --devices, the entries of each shard (default: each GPU's free memory split among its shards)")
     ap.add_argument("--save-work", default="", metavar="FILE", help="write the table as a HEADW work file at exit")
     ap.add_argument("--save-interval", type=float, default=0.0, metavar="SECS", help="also save every SECS seconds")
     ap.add_argument("--resume", default="", metavar="FILE", help="start from a work file: range, key and dp come from it")
@@ -603,6 +802,22 @@ def parse_args(argv=None):
         ap.error("--save-interval needs --save-work FILE")
     if a.dp is not None and not 0 <= a.dp <= 64:
         ap.error("--dp must be 0 .. 64")
+    if a.devices is not None:
+        if a.device is not None:
+            ap.error("give --device or --devices, not both")
+        try:
+            a.devices = [int(v) for v in a.devices.split(",")] if a.devices.strip() else []
+        except ValueError:
+            ap.error("--devices must be GPU indices separated by commas, not %r" % a.devices)
+        if not a.devices:
+            ap.error("--devices: the list is empty")
+        if len(a.devices) > MAX_SHARDS:
+            ap.error("--devices: %d entries, at most %d shards" % (len(a.devices), MAX_SHARDS))
+        if min(a.devices) < 0:
+            ap.error("--devices: GPU indices are not negative")
+        a.device = a.devices[0]
+    elif a.device is None:
+        a.device = 0
     pubs = None
     if a.config:
         start, end, pubs = ec.parse_config(a.config)
@@ -632,9 +847,14 @@ def main(argv=None):
     a, start, end, pub, dp = parse_args(argv)
     out = lambda s: print(s, flush=True)
     from .ingest import TableFull
+    sharded = a.devices is not None and len(a.devices) >= 2
     try:
-        sink = GpuSink(start, end, pub, dp, device=a.device, capacity=a.dp_table_capacity, resume=a.resume or None,
-                       save_path=a.save_work, out=out)
+        if sharded:
+            sink = ShardedSink(start, end, pub, dp, a.devices, capacity=a.dp_table_capacity, resume=a.resume or None,
+                               save_path=a.save_work, out=out)
+        else:
+            sink = GpuSink(start, end, pub, dp, device=a.device, capacity=a.dp_table_capacity, resume=a.resume or None,
+                           save_path=a.save_work, out=out)
     except TableFull as e:
         out("--resume %s refused: %s; give a larger --dp-table-capacity" % (a.resume, e))
         return 1
@@ -642,8 +862,11 @@ def main(argv=None):
         out("Resume %s: %d DPs" % (a.resume, sink.resumed[0]))
         if sink.resumed[1]:
             out("%d kangaroos in %s skipped: the server keeps no herd" % (sink.resumed[1], a.resume))
-    out("Range 0x%X .. 0x%X  dp %d  key 04%064X%064X  table capacity %d entries (%.2f GB) on cuda:%d" %
-        (start, end, dp, pub[0], pub[1], sink.table.capacity, sink.table.memory_bytes() / 1e9, a.device))
+    if sharded:
+        out("Range 0x%X .. 0x%X  dp %d  key 04%064X%064X  table in %s" % (start, end, dp, pub[0], pub[1], sink.describe()))
+    else:
+        out("Range 0x%X .. 0x%X  dp %d  key 04%064X%064X  table capacity %d entries (%.2f GB) on cuda:%d" %
+            (start, end, dp, pub[0], pub[1], sink.table.capacity, sink.table.memory_bytes() / 1e9, a.device))
     stop = threading.Event()
     signals = []
 
@@ -692,7 +915,7 @@ def main(argv=None):
     if sink.full is not None:
         out("DP table full, server stopped: %s.  Resume with --resume %s --dp-table-capacity %d or more; the clients reconnect "
             "and resend the DPs they hold." % (sink.full, a.save_work or "FILE (give --save-work to write one)",
-                                               2 * sink.table.capacity))
+                                               2 * (sink.shard_capacity if sharded else sink.table.capacity)))
         rc = 1
     if sink.failed is not None:
         out("Ingest failed, server stopped: %s" % sink.failed)
@@ -703,6 +926,9 @@ def main(argv=None):
         "per batch; handlers blocked %.2f s on a full queue" %
         (sink.received, sink.wrong, sink.dead, sink.wrong_collisions, sink.batches, 1e3 * sink.t_copy / max(sink.batches, 1),
          1e3 * sink.t_verify / max(sink.batches, 1), 1e3 * sink.t_add / max(sink.batches, 1), sink.queue.blocked_s))
+    if sharded:
+        out("Shards: verify is verify+partition; add includes %.3f ms per batch of copies to other GPUs" %
+            (1e3 * sink.t_peer / max(sink.batches, 1)))
     sink.close()
     return rc
 
