@@ -173,7 +173,8 @@ uint64_t kgx_kernel_launches(kgx_engine* e);
  *     adds gives exactly the events, count, per-bucket nbItem / maxItem and work files of the host table of
  *     include/kgx_ingest.h (kgi_add / kgi_save_work_ex / kgi_load_work_ex) fed the same records in the same order.
  * _create: a table of `capacity` entries (fixed; 1 .. 2^32-2) on device dev; NULL without a device or memory, reason in
- *     kgx_dptable_last_error(NULL).  _bytes_for: device bytes a table of that capacity takes (48 per entry + fixed scratch).
+ *     kgx_dptable_last_error(NULL).  _bytes_for: device bytes a table of that capacity takes (48 per entry + fixed scratch:
+ *     a save chunk of 2^21 entries at 56 bytes each, the save's selection of min(capacity, 2^23) entries at 4 bytes each).
  * _add: records of n_ranks rank segments (1 .. KGX_DPT_MAX_RANKS), segment r = counts[r] records at recs + r*stride*40
  *     (device memory; counts on the host), inserted in segment order then record order, stream-ordered on `stream`
  *     (a cudaStream_t; NULL = the legacy default stream); the call waits for its own work only.  Events in arrival order:
@@ -193,6 +194,7 @@ typedef struct {                     /* = kgi_event (include/kgx_ingest.h) */
 #define KGX_DPT_EV_RESET     1
 #define KGX_DPT_EV_COLLISION 2
 #define KGX_DPT_MAX_RANKS    256
+#define KGX_DPT_HOST_ENTRIES 1   /* kgx_dptable_create_ex: the 32-byte entries in mapped, pinned host memory */
 /* --- the collision resolver on one GPU (kgx_resolver.cuh): kgi_resolve_multi's result without the host.
  * _create: keys K = key - start*G (n_keys x 8 limbs, x then y; the point at infinity as (0, 0); 1 <= n_keys <= KGX_MAX_KEYS)
  *     and a range start below the group order n.  Builds the fixed-base comb and the keys' index by x once, on device dev,
@@ -276,6 +278,20 @@ int kgx_dptable_save_range(kgx_dptable* t, const char* path, uint64_t offset, vo
 int kgx_dptable_load_range(kgx_dptable* t, const char* path, uint32_t* dp_bits, uint64_t range_start[4], uint64_t range_end[4],
                            uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time, uint64_t* nb_walk,
                            uint64_t* walk_offset, uint64_t max_entries, void* stream);
+/* --- the table's layout.
+ * _create_ex: kgx_dptable_create_range with flags: 0 (= _create_range: everything on the device) or KGX_DPT_HOST_ENTRIES,
+ *     which keeps the 32-byte entries in pinned host memory mapped into the device (cudaHostAllocMapped) and the index
+ *     (24 bytes per 2/3 entry), the entries' buckets (4 bytes), the counters and all scratch on the device: 16 bytes of GPU
+ *     memory per entry instead of 48.  Every call above works on either layout with exactly the same events, counts, return
+ *     codes and file bytes; an add reads an entry from host memory only when a probe meets a slot of its tag, and a load
+ *     reads the file's entries straight into the pinned buffer.  Unknown flags: NULL.  The pinned entries are freed by _destroy.
+ * _bytes_for_ex: the device bytes of a table of that capacity and layout (_bytes_for(c) = _bytes_for_ex(c, 0, NULL)); the
+ *     pinned host bytes of its entries (32 per entry, 0 on the device layout) in *host_bytes when not NULL.
+ * _host_bytes: the pinned host bytes of the table's entries (0 on the device layout).  Saves and loads also pin 36 bytes per
+ *     entry of a save chunk (at most 2^21 entries) on either layout, allocated by the first of them. --- */
+kgx_dptable* kgx_dptable_create_ex(int dev, uint64_t capacity, uint32_t lo, uint32_t hi, int flags);
+uint64_t     kgx_dptable_bytes_for_ex(uint64_t capacity, int flags, uint64_t* host_bytes);
+uint64_t     kgx_dptable_host_bytes(kgx_dptable* t);
 /* --- kgx_dp_partition (kgx_partition.cuh): n 40-byte DP records of kgx_convert_dps (device memory) grouped by the rank of W
  *     (1 .. KGX_DPT_MAX_RANKS) that owns their bucket, each group in input order (a stable partition), into out: packed when
  *     stride = 0, else group r at record r * stride (stride >= n).  recs and out need 4-byte alignment only (kgx_convert_dps's

@@ -85,6 +85,9 @@ _SIGS = {
     "kgx_dptable_save_range": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_uint64, ctypes.c_void_p]),
     "kgx_dptable_load_range": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_uint32), _u64p, _u64p, _u64p, _u64p,
                                               _u64p, ctypes.POINTER(ctypes.c_double), _u64p, _u64p, ctypes.c_uint64, ctypes.c_void_p]),
+    "kgx_dptable_create_ex": (ctypes.c_void_p, [ctypes.c_int, ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_int]),
+    "kgx_dptable_bytes_for_ex": (ctypes.c_uint64, [ctypes.c_uint64, ctypes.c_int, _u64p]),
+    "kgx_dptable_host_bytes": (ctypes.c_uint64, [ctypes.c_void_p]),
     "kgx_dp_partition_scratch_bytes": (ctypes.c_uint64, [ctypes.c_uint32, ctypes.c_uint32]),
     "kgx_dp_partition": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint64, ctypes.c_void_p, ctypes.c_void_p,
                                         ctypes.c_void_p, ctypes.c_uint64, ctypes.c_void_p]),

@@ -11,10 +11,21 @@
 //
 // Layout (fixed capacity C entries, no growth):
 //   ent[C]      32-byte entries {x, d}, dense in insertion order; ent_h[C] their bucket
-//   slots[S]    open-addressing index over (h, x), S = C + C/2 (load <= 2/3), linear probing: 64-bit word
+//   slots[N]    open-addressing index over (h, x), N = C + C/2 (load <= 2/3), linear probing: 64-bit word
 //               (entry index << 32) | tag, tag = (h + 1) | 13 bits of x.hi << 19, 0 = empty
 //   nb/mx[2^18] the reference's nbItem / maxItem
-// 48 bytes per entry of capacity, plus 2 MB of bucket counters and the save scratch (SAVE_CHUNK entries, 56 bytes each).
+// 48 bytes per entry of capacity, plus 2 MB of bucket counters and the save scratch (SAVE_CHUNK entries, 56 bytes each,
+// and the save's selection of SAVE_SELECT entries, 4 bytes each, with its 2^18 bucket cursors).
+// With KGX_DPT_HOST_ENTRIES (kgx_dptable_create_ex), ent[C] is mapped, pinned host memory that the kernels reach through its
+// device pointer, and the GPU holds 16 bytes per entry.  An add touches an entry only to write a new one and to read one
+// back when a probe meets a slot of the same tag; probes, tags and counters stay on the device.
+//
+// A save goes through the table in passes.  Each pass takes whole save chunks of consecutive buckets, at most SAVE_SELECT
+// entries in all, and groups their entries by bucket in one scan of ent_h: the bucket counts are nbItem, their prefix sums
+// (on the host) start one cursor per bucket, and each entry of the pass's buckets takes the next place of its bucket.  Each
+// chunk's entries are then a contiguous run of the selection, sorted and gathered on their own (kgx_bucketsort.cuh).  Four
+// chunks always fit a pass and two neighbouring chunks hold more than SAVE_CHUNK entries, so a save reads ent_h at most
+// count / 2^22 + 1 times, about count / SAVE_SELECT when buckets are small against a chunk.
 //
 // One add call, stream-ordered on the caller's stream:
 //   1. key  = h of every record (2^18 for a malformed one), value = arrival index (rank segments in order, then records)
@@ -36,6 +47,7 @@ using kgx_wf::NBUCKET;
 typedef unsigned long long ull;
 constexpr uint64_t TYPE_BIT = 0x4000000000000000ull;    // b126 of the tagged distance: herd type (HashTable::CalcDistAndType)
 constexpr uint64_t SAVE_CHUNK = 1ull << 21;             // entries per device->host chunk of a save / host->device chunk of a load
+constexpr uint64_t SAVE_SELECT = 1ull << 23;            // entries one select pass of a save groups (32 MB of indices)
 
 struct Res { ull count; uint32_t nsel; uint32_t bad; };
 struct Ranks { uint32_t n; uint32_t pre[KGX_DPT_MAX_RANKS + 1]; };
@@ -150,16 +162,17 @@ __global__ void k_index_entries(const Entry* ent, const uint32_t* ent_h, uint64_
   index_insert(slots, nslots, slot_home(h, v.x0, v.x1, nslots), ((ull)e << 32) | slot_tag(h, v.x1));
 }
 
-// a save: the entries of buckets [b0, b1), in any order
-__global__ void k_save_select(const uint32_t* ent_h, uint64_t count, uint32_t b0, uint32_t b1, uint32_t* idx, uint32_t* cursor) {
+// a save's select pass: the entries of buckets [b0, b1) grouped by bucket, cursor[h] the next place of bucket h in sel
+__global__ void k_save_select(const uint32_t* ent_h, uint64_t count, uint32_t b0, uint32_t b1, uint32_t* cursor, uint32_t* sel) {
   const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= count) return;
   const uint32_t h = ent_h[e];
-  if (h >= b0 && h < b1) idx[atomicAdd(cursor, 1u)] = (uint32_t)e;
+  if (h >= b0 && h < b1) sel[atomicAdd(&cursor[h], 1u)] = (uint32_t)e;
 }
 
 inline uint64_t slots_for(uint64_t capacity) { return capacity + capacity / 2 + 64; }
 inline uint64_t save_chunk_for(uint64_t capacity) { return capacity < SAVE_CHUNK ? (capacity ? capacity : 1) : SAVE_CHUNK; }
+inline uint64_t save_select_for(uint64_t capacity) { return capacity < SAVE_SELECT ? (capacity ? capacity : 1) : SAVE_SELECT; }
 
 }  // namespace kgx_dpt
 
@@ -169,7 +182,10 @@ struct kgx_dptable {
   int dev = 0;
   uint32_t lo = 0, hi = kgx_dpt::NBUCKET;                 // the buckets the table holds (a shard of the sharded table: a range)
   uint64_t capacity = 0, nslots = 0, count = 0;           // count: host mirror of res->count after the last call
-  kgx_dpt::Entry* ent = nullptr;
+  int flags = 0;
+  kgx_dpt::Entry* ent = nullptr;                           // as the kernels reach it: device memory, or entHost mapped
+  kgx_dpt::Entry* entHost = nullptr;                       // KGX_DPT_HOST_ENTRIES: the pinned entries (else null)
+  uint64_t hostBytes = 0;
   uint32_t* ent_h = nullptr;
   kgx_dpt::ull* slots = nullptr;
   uint32_t *nb = nullptr, *mx = nullptr;
@@ -184,9 +200,9 @@ struct kgx_dptable {
   void* cubTmp = nullptr;
   size_t cubTmpBytes = 0;
   uint64_t scratchBytes = 0;
-  // save / load scratch: chunk entries on the device, pinned on the host
-  uint64_t chunk = 0;
-  uint32_t *sIdxA = nullptr, *sIdxB = nullptr, *sCursor = nullptr;
+  // save / load scratch: chunk entries on the device, pinned on the host; the select pass's selection and bucket cursors
+  uint64_t chunk = 0, select = 0;
+  uint32_t *sIdxA = nullptr, *sIdxB = nullptr, *sSel = nullptr, *sCursor = nullptr;
   uint64_t *sKeyA = nullptr, *sKeyB = nullptr;
   kgx_dpt::Entry* sOut = nullptr;
   void* sTmp = nullptr;
@@ -270,11 +286,16 @@ static int dpt_pinned(kgx_dptable* t) {
 
 extern "C" {
 
-uint64_t kgx_dptable_bytes_for(uint64_t capacity) {
-  const uint64_t c = kgx_dpt::save_chunk_for(capacity);
-  return capacity * (sizeof(kgx_dpt::Entry) + 4) + 8 * kgx_dpt::slots_for(capacity) + 8ull * kgx_dpt::NBUCKET +
+uint64_t kgx_dptable_bytes_for_ex(uint64_t capacity, int flags, uint64_t* host_bytes) {
+  const uint64_t c = kgx_dpt::save_chunk_for(capacity), ent = sizeof(kgx_dpt::Entry) * capacity;
+  const bool host = flags & KGX_DPT_HOST_ENTRIES;
+  if (host_bytes) *host_bytes = host ? ent : 0;
+  return (host ? 0 : ent) + 4 * capacity + 8 * kgx_dpt::slots_for(capacity) + 8ull * kgx_dpt::NBUCKET +
+         4 * kgx_dpt::save_select_for(capacity) + 4ull * kgx_dpt::NBUCKET +
          c * (4 + 4 + 8 + 8 + sizeof(kgx_dpt::Entry)) + 2 * 8 * c + (64ull << 20);   // the last two: radix-sort scratch, estimated
 }
+
+uint64_t kgx_dptable_bytes_for(uint64_t capacity) { return kgx_dptable_bytes_for_ex(capacity, 0, nullptr); }
 
 const char* kgx_dptable_last_error(kgx_dptable* t) { return t ? t->err : g_dpt_create_err; }
 
@@ -282,27 +303,41 @@ void kgx_dptable_destroy(kgx_dptable* t) {
   if (!t) return;
   cudaSetDevice(t->dev);
   cudaDeviceSynchronize();
-  cudaFree(t->ent); cudaFree(t->ent_h); cudaFree(t->slots); cudaFree(t->nb); cudaFree(t->mx); cudaFree(t->res);
+  if (t->entHost) cudaFreeHost(t->entHost);
+  else cudaFree(t->ent);
+  cudaFree(t->ent_h); cudaFree(t->slots); cudaFree(t->nb); cudaFree(t->mx); cudaFree(t->res);
   dpt_free_scratch(t);
   cudaFree(t->evOut); cudaFree(t->evKey);
-  cudaFree(t->sIdxA); cudaFree(t->sIdxB); cudaFree(t->sCursor); cudaFree(t->sKeyA); cudaFree(t->sKeyB); cudaFree(t->sOut); cudaFree(t->sTmp);
+  cudaFree(t->sIdxA); cudaFree(t->sIdxB); cudaFree(t->sSel); cudaFree(t->sCursor); cudaFree(t->sKeyA); cudaFree(t->sKeyB); cudaFree(t->sOut); cudaFree(t->sTmp);
   if (t->resHost) cudaFreeHost(t->resHost);
   if (t->hostEnt) cudaFreeHost(t->hostEnt);
   if (t->hostH) cudaFreeHost(t->hostH);
   delete t;
 }
 
-kgx_dptable* kgx_dptable_create_range(int dev, uint64_t capacity, uint32_t lo, uint32_t hi) {
+// the pinned entries of a KGX_DPT_HOST_ENTRIES table, mapped into the device's address space
+static int dpt_alloc_host_entries(kgx_dptable* t) {
+  const size_t n = sizeof(kgx_dpt::Entry) * t->capacity;
+  cudaError_t s = cudaHostAlloc((void**)&t->entHost, n, cudaHostAllocMapped);
+  if (s == cudaSuccess) s = cudaHostGetDevicePointer((void**)&t->ent, t->entHost, 0);
+  if (s != cudaSuccess) {
+    snprintf(t->err, sizeof t->err, "cudaHostAlloc(%zu bytes, mapped): %s", n, cudaGetErrorString(s));
+    cudaGetLastError();
+    return -3;
+  }
+  t->hostBytes = n;
+  return 0;
+}
+
+kgx_dptable* kgx_dptable_create_ex(int dev, uint64_t capacity, uint32_t lo, uint32_t hi, int flags) {
   if (lo >= hi || hi > kgx_dpt::NBUCKET) {
     snprintf(g_dpt_create_err, sizeof g_dpt_create_err, "kgx_dptable_create_range: buckets [%u, %u) are not a range of [0, 2^18)", lo, hi);
     return nullptr;
   }
-  kgx_dptable* t = kgx_dptable_create(dev, capacity);
-  if (t) { t->lo = lo; t->hi = hi; }
-  return t;
-}
-
-kgx_dptable* kgx_dptable_create(int dev, uint64_t capacity) {
+  if (flags & ~KGX_DPT_HOST_ENTRIES) {
+    snprintf(g_dpt_create_err, sizeof g_dpt_create_err, "kgx_dptable_create_ex: unknown flags 0x%x", flags);
+    return nullptr;
+  }
   int cnt = 0;
   cudaError_t s = cudaGetDeviceCount(&cnt);
   if (s != cudaSuccess || cnt == 0) {
@@ -321,25 +356,35 @@ kgx_dptable* kgx_dptable_create(int dev, uint64_t capacity) {
     return nullptr;
   }
   kgx_dptable* t = new kgx_dptable();
-  t->dev = dev; t->capacity = capacity; t->nslots = kgx_dpt::slots_for(capacity);
+  t->dev = dev; t->lo = lo; t->hi = hi; t->flags = flags;
+  t->capacity = capacity; t->nslots = kgx_dpt::slots_for(capacity);
   t->chunk = kgx_dpt::save_chunk_for(capacity);
+  t->select = kgx_dpt::save_select_for(capacity);
   const uint64_t c = t->chunk;
   t->sTmpBytes = kgx_wf::bucket_sort_scratch(c);
-  bool ok = !dpt_alloc(t, (void**)&t->ent, sizeof(kgx_dpt::Entry) * capacity) && !dpt_alloc(t, (void**)&t->ent_h, 4ull * capacity) &&
-            !dpt_alloc(t, (void**)&t->slots, 8ull * t->nslots) && !dpt_alloc(t, (void**)&t->nb, 4ull * kgx_dpt::NBUCKET) &&
-            !dpt_alloc(t, (void**)&t->mx, 4ull * kgx_dpt::NBUCKET) && !dpt_alloc(t, (void**)&t->res, sizeof(kgx_dpt::Res)) &&
-            !dpt_alloc(t, (void**)&t->sIdxA, 4ull * c) && !dpt_alloc(t, (void**)&t->sIdxB, 4ull * c) &&
-            !dpt_alloc(t, (void**)&t->sCursor, 4) && !dpt_alloc(t, (void**)&t->sKeyA, 8ull * c) &&
-            !dpt_alloc(t, (void**)&t->sKeyB, 8ull * c) && !dpt_alloc(t, (void**)&t->sOut, sizeof(kgx_dpt::Entry) * c) &&
-            !dpt_alloc(t, &t->sTmp, t->sTmpBytes);
+  bool ok = (flags & KGX_DPT_HOST_ENTRIES) ? !dpt_alloc_host_entries(t) : !dpt_alloc(t, (void**)&t->ent, sizeof(kgx_dpt::Entry) * capacity);
+  ok = ok && !dpt_alloc(t, (void**)&t->ent_h, 4ull * capacity) &&
+       !dpt_alloc(t, (void**)&t->slots, 8ull * t->nslots) && !dpt_alloc(t, (void**)&t->nb, 4ull * kgx_dpt::NBUCKET) &&
+       !dpt_alloc(t, (void**)&t->mx, 4ull * kgx_dpt::NBUCKET) && !dpt_alloc(t, (void**)&t->res, sizeof(kgx_dpt::Res)) &&
+       !dpt_alloc(t, (void**)&t->sIdxA, 4ull * c) && !dpt_alloc(t, (void**)&t->sIdxB, 4ull * c) &&
+       !dpt_alloc(t, (void**)&t->sSel, 4ull * t->select) && !dpt_alloc(t, (void**)&t->sCursor, 4ull * kgx_dpt::NBUCKET) &&
+       !dpt_alloc(t, (void**)&t->sKeyA, 8ull * c) &&
+       !dpt_alloc(t, (void**)&t->sKeyB, 8ull * c) && !dpt_alloc(t, (void**)&t->sOut, sizeof(kgx_dpt::Entry) * c) &&
+       !dpt_alloc(t, &t->sTmp, t->sTmpBytes);
   if (ok && cudaHostAlloc((void**)&t->resHost, sizeof(kgx_dpt::Res), cudaHostAllocDefault) != cudaSuccess) {
     snprintf(t->err, sizeof t->err, "cudaHostAlloc failed");
     ok = false;
   }
   if (ok) ok = dpt_reset(t, 0) == 0;
   if (!ok) {
-    snprintf(g_dpt_create_err, sizeof g_dpt_create_err, "kgx_dptable_create(%llu entries, %.2f GB): %.180s",
-             (unsigned long long)capacity, kgx_dptable_bytes_for(capacity) / 1e9, t->err);
+    uint64_t hb = 0;
+    const uint64_t db = kgx_dptable_bytes_for_ex(capacity, flags, &hb);
+    if (hb)
+      snprintf(g_dpt_create_err, sizeof g_dpt_create_err, "kgx_dptable_create(%llu entries, %.2f GB + %.2f GB pinned host): %.160s",
+               (unsigned long long)capacity, db / 1e9, hb / 1e9, t->err);
+    else
+      snprintf(g_dpt_create_err, sizeof g_dpt_create_err, "kgx_dptable_create(%llu entries, %.2f GB): %.180s",
+               (unsigned long long)capacity, db / 1e9, t->err);
     cudaGetLastError();
     kgx_dptable_destroy(t);
     return nullptr;
@@ -347,8 +392,15 @@ kgx_dptable* kgx_dptable_create(int dev, uint64_t capacity) {
   return t;
 }
 
+kgx_dptable* kgx_dptable_create_range(int dev, uint64_t capacity, uint32_t lo, uint32_t hi) {
+  return kgx_dptable_create_ex(dev, capacity, lo, hi, 0);
+}
+
+kgx_dptable* kgx_dptable_create(int dev, uint64_t capacity) { return kgx_dptable_create_ex(dev, capacity, 0, kgx_dpt::NBUCKET, 0); }
+
 uint64_t kgx_dptable_count(kgx_dptable* t) { return t->count; }
 uint64_t kgx_dptable_capacity(kgx_dptable* t) { return t->capacity; }
+uint64_t kgx_dptable_host_bytes(kgx_dptable* t) { return t->hostBytes; }
 uint64_t kgx_dptable_memory_bytes(kgx_dptable* t) {
   return t->bytes + (t->evOut ? (sizeof(kgx_dp_event) + sizeof(kgx_dp_event_key)) * (uint64_t)t->evCap : 0);
 }
@@ -461,15 +513,16 @@ int kgx_dptable_add_resolve(kgx_dptable* t, const void* recs, const uint32_t* co
 }
 
 // The buckets [b0, b1) of the table, each nbItem, maxItem and its entries (HashTable::SaveTable, HashTable.cpp:375-396), to f
-// in chunks of whole buckets: select, sort by (h, x.hi, x.lo), copy out.  -> 0, -3 on a CUDA error (text in t->err), or 1
-// when a write failed (errno tells).
+// in chunks of whole buckets: a select pass groups the entries of several chunks by bucket, then each chunk is sorted by
+// (h, x.hi, x.lo) and copied out.  -> 0, -3 on a CUDA error (text in t->err), or 1 when a write failed (errno tells).
 static int dpt_write_buckets(kgx_dptable* t, FILE* f, uint32_t b0, uint32_t b1, cudaStream_t st) {
   using namespace kgx_dpt;
   using namespace kgx_wf;
   if (dpt_pinned(t)) return -3;
-  uint32_t* nbH = (uint32_t*)malloc(8ull * NBUCKET);
+  uint32_t* nbH = (uint32_t*)malloc(12ull * NBUCKET);
   if (!nbH) { snprintf(t->err, sizeof t->err, "out of host memory"); return -3; }
   uint32_t* mxH = nbH + NBUCKET;
+  uint32_t* curH = mxH + NBUCKET;                         // a pass's bucket cursors: where each bucket starts in the selection
   if (cudaMemcpy(nbH, t->nb, 4ull * NBUCKET, cudaMemcpyDeviceToHost) != cudaSuccess ||
       cudaMemcpy(mxH, t->mx, 4ull * NBUCKET, cudaMemcpyDeviceToHost) != cudaSuccess) {
     free(nbH);
@@ -479,6 +532,7 @@ static int dpt_write_buckets(kgx_dptable* t, FILE* f, uint32_t b0, uint32_t b1, 
   bool ok = true;
   int rc = 0;
   const uint32_t end = b1;
+  uint32_t p0 = b0, p1 = b0;                              // the buckets of the current select pass
   while (ok && rc == 0 && b0 < end) {
     uint64_t m = 0;
     b1 = b0;
@@ -489,13 +543,33 @@ static int dpt_write_buckets(kgx_dptable* t, FILE* f, uint32_t b0, uint32_t b1, 
       rc = -3;
       break;
     }
+    if (m && b0 >= p1) {                                  // a new select pass: whole chunks from b0, at most t->select entries
+      uint64_t sel = 0;
+      p0 = p1 = b0;
+      for (uint32_t c1 = b0; c1 < end && sel < t->select;) {
+        uint64_t cm = 0;
+        uint32_t c2 = c1;
+        while (c2 < end && (cm + nbH[c2] <= t->chunk || c2 == c1)) cm += nbH[c2++];
+        if (cm > t->chunk || sel + cm > t->select) break;
+        sel += cm;
+        c1 = p1 = c2;
+      }
+      uint32_t run = 0;
+      for (uint32_t h = p0; h < p1; h++) { curH[h] = run; run += nbH[h]; }
+      const uint32_t B = 256;
+      bool good = cudaMemcpyAsync(t->sCursor + p0, curH + p0, 4ull * (p1 - p0), cudaMemcpyHostToDevice, st) == cudaSuccess;
+      if (good) k_save_select<<<(unsigned)((t->count + B - 1) / B), B, 0, st>>>(t->ent_h, t->count, p0, p1, t->sCursor, t->sSel);
+      if (!good || cudaGetLastError() != cudaSuccess) {
+        snprintf(t->err, sizeof t->err, "kgx_dptable_save_work: %s", cudaGetErrorString(cudaGetLastError()));
+        rc = -3;
+        break;
+      }
+    }
     if (m) {
       const uint32_t n = (uint32_t)m, B = 256, G = (n + B - 1) / B;
       uint32_t* order = nullptr;
-      bool good = cudaMemsetAsync(t->sCursor, 0, 4, st) == cudaSuccess;
-      k_save_select<<<(unsigned)((t->count + B - 1) / B), B, 0, st>>>(t->ent_h, t->count, b0, b1, t->sIdxA, t->sCursor);
-      good = good && bucket_sort(t->ent, t->ent_h, t->sIdxA, n, b0, b1, t->sIdxA, t->sIdxB, t->sKeyA, t->sKeyB, t->sTmp, t->sTmpBytes, st,
-                                 &order) == cudaSuccess;
+      bool good = bucket_sort(t->ent, t->ent_h, t->sSel + curH[b0], n, b0, b1, t->sIdxA, t->sIdxB, t->sKeyA, t->sKeyB, t->sTmp,
+                              t->sTmpBytes, st, &order) == cudaSuccess;
       if (good) bucket_gather<<<G, B, 0, st>>>(t->ent, order, n, t->sOut);
       good = good && cudaMemcpyAsync(t->hostEnt, t->sOut, sizeof(Entry) * m, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
              cudaStreamSynchronize(st) == cudaSuccess;
@@ -562,7 +636,9 @@ int kgx_dptable_save_range(kgx_dptable* t, const char* path, uint64_t offset, vo
 }
 
 // HashTable::LoadTable (HashTable.cpp:439-459) of the table's buckets [lo, hi): the others are walked past.  More than
-// max_entries entries in the range: -ENOSPC and an empty table, like any failed load.
+// max_entries entries in the range: -ENOSPC and an empty table, like any failed load.  The entries are read into the pinned
+// chunk buffer and copied to the device, or with host entries read straight into their place in ent; either way the index
+// is rebuilt on the device.
 static int dpt_load(kgx_dptable* t, const char* path, uint64_t max_entries, uint32_t* dp_bits, uint64_t range_start[4],
                     uint64_t range_end[4], uint64_t keyx[4], uint64_t keyy[4], uint64_t* total_count, double* total_time,
                     uint64_t* nb_walk, uint64_t* walk_offset, cudaStream_t st) {
@@ -592,7 +668,8 @@ static int dpt_load(kgx_dptable* t, const char* path, uint64_t max_entries, uint
       return false;
     }
     const uint64_t B = 256;
-    bool good = cudaMemcpyAsync(t->ent + t->count, t->hostEnt, sizeof(Entry) * staged, cudaMemcpyHostToDevice, st) == cudaSuccess &&
+    bool good = (t->entHost || cudaMemcpyAsync(t->ent + t->count, t->hostEnt, sizeof(Entry) * staged, cudaMemcpyHostToDevice, st) ==
+                                   cudaSuccess) &&
                 cudaMemcpyAsync(t->ent_h + t->count, t->hostH, 4 * staged, cudaMemcpyHostToDevice, st) == cudaSuccess;
     if (good) k_index_entries<<<(unsigned)((staged + B - 1) / B), (unsigned)B, 0, st>>>(t->ent, t->ent_h, t->count, staged, t->slots, t->nslots);
     good = good && cudaStreamSynchronize(st) == cudaSuccess;    // the pinned buffers are refilled next
@@ -614,7 +691,8 @@ static int dpt_load(kgx_dptable* t, const char* path, uint64_t max_entries, uint
     while (ok && left) {
       if (staged == t->chunk && !flush()) { ok = false; break; }
       const uint32_t k = (uint32_t)std::min<uint64_t>(left, t->chunk - staged);
-      ok = fread(t->hostEnt + staged, sizeof(Entry), k, f) == k;
+      // total <= max_entries <= capacity: the entries read fit, host ones straight in ent
+      ok = fread((t->entHost ? t->entHost + t->count : t->hostEnt) + staged, sizeof(Entry), k, f) == k;
       for (uint32_t q = 0; q < k; q++) t->hostH[staged + q] = h;
       staged += k;
       left -= k;

@@ -394,10 +394,10 @@ class GpuSink:
     """The ingest thread and what it owns: the device table, the resolver of the one key, the staging buffers on `device`.
     put / status / reset_dead are the Server's sink calls."""
 
-    def __init__(self, start, end, pub, dp, device=0, capacity=None, resume=None, save_path="", out=print):
+    def __init__(self, start, end, pub, dp, device=0, capacity=None, resume=None, save_path="", out=print, entries="device"):
         import torch
         from .ingest import DeviceDPTable, DeviceResolver, DPTable, TableFull
-        from .solver import default_table_capacity, scratch_bytes
+        from .solver import default_table_capacity, host_entries_limit, mem_available, scratch_bytes
         self.torch, self.TableFull = torch, TableFull
         self.start, self.end, self.pub, self.dp = start, end, pub, dp
         self.save_path, self.out = save_path, out
@@ -415,12 +415,14 @@ class GpuSink:
         self._host = torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8).pin_memory()
         self._host_np = self._host.numpy()
         self._counts_h = torch.empty(2, dtype=torch.int32).pin_memory()
+        self.entries = entries
         if not capacity:
             capacity = default_table_capacity(torch.cuda.mem_get_info(self.dev)[0] - scratch_bytes(CHUNK_RECORDS) -
-                                              EVENT_BYTES * CHUNK_RECORDS)
+                                              EVENT_BYTES * CHUNK_RECORDS, entries=entries,
+                                              host_limit=host_entries_limit(mem_available(), 1) if entries == "host" else None)
         # a record makes at most one event, so room for a whole batch's events means no event of an add is ever cut off: a
         # hit cannot be pushed out by the RESETs of clients that keep resending, and the dead count is exact
-        self.table = DeviceDPTable(capacity, device=device, max_events=CHUNK_RECORDS)
+        self.table = DeviceDPTable(capacity, device=device, max_events=CHUNK_RECORDS, entries=entries)
         self.table.reserve(CHUNK_RECORDS)
         self.stream = torch.cuda.Stream(device=self.dev)
         self.time0 = 0.0
@@ -580,6 +582,12 @@ def shard_plan(devices):
     return [(d, lo, hi) for d, (lo, hi) in zip(devices, owner_ranges(len(devices)))]
 
 
+def host_note(table):
+    """the words the start line adds for a table (or ShardTables) with its entries in pinned host memory"""
+    hb = table.host_bytes()
+    return ", entries in pinned host memory (%.2f GB)" % (hb / 1e9) if hb else ""
+
+
 class ShardTables:
     """the shards of a ShardedSink as one table for the status line and the messages: entries, capacity and memory summed"""
 
@@ -592,6 +600,9 @@ class ShardTables:
 
     def memory_bytes(self):
         return sum(t.memory_bytes() for t in self.shards)
+
+    def host_bytes(self):
+        return sum(t.host_bytes() for t in self.shards)
 
     def fullest(self):
         """-> (shard, entries, capacity) of the shard with the largest fill"""
@@ -613,10 +624,10 @@ class ShardedSink(GpuSink):
     waits for its own work, and a batch is done before the next starts, so every bucket sees its records in queue order, as
     the one table does.  A save writes the header, then each shard's piece at its offset: the one table's file, byte for byte."""
 
-    def __init__(self, start, end, pub, dp, devices, capacity=None, resume=None, save_path="", out=print):
+    def __init__(self, start, end, pub, dp, devices, capacity=None, resume=None, save_path="", out=print, entries="device"):
         import torch
         from .ingest import DeviceDPTable, DeviceResolver, DPTable, TableFull
-        from .solver import DP_TABLE_MARGIN, default_table_capacity, scratch_bytes
+        from .solver import DP_TABLE_MARGIN, default_table_capacity, host_entries_limit, mem_available, scratch_bytes
         self.torch, self.TableFull = torch, TableFull
         self.start, self.end, self.pub, self.dp = start, end, pub, dp
         self.save_path, self.out = save_path, out
@@ -640,15 +651,17 @@ class ShardedSink(GpuSink):
         self._counts_h = torch.empty(W + 1, dtype=torch.int32).pin_memory()
         staged = len(gpus) > 1
         per_shard = scratch_bytes(CHUNK_RECORDS) + EVENT_BYTES * CHUNK_RECORDS + (CHUNK_RECORDS * DP40 if staged else 0)
+        self.entries = entries
+        host_limit = host_entries_limit(mem_available(), W) if entries == "host" else None   # the host's RAM shared by all shards
         caps = {}
         for d in gpus:                                        # before any table takes memory
             k = devices.count(d)
             caps[d] = capacity or default_table_capacity((torch.cuda.mem_get_info(d)[0] - DP_TABLE_MARGIN) // k - per_shard,
-                                                         margin=0)
+                                                         margin=0, entries=entries, host_limit=host_limit)
         self.shards = []
         for s, (d, lo, hi) in enumerate(self.plan):
             dev = torch.device("cuda", d)
-            t = DeviceDPTable(caps[d], device=d, max_events=CHUNK_RECORDS, buckets=(lo, hi))
+            t = DeviceDPTable(caps[d], device=d, max_events=CHUNK_RECORDS, buckets=(lo, hi), entries=entries)
             t.reserve(CHUNK_RECORDS)
             self.shards.append(dict(table=t, device=d, lo=lo, hi=hi, stream=torch.cuda.Stream(device=dev),
                                     staging=torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8, device=dev) if staged else None))
@@ -678,8 +691,9 @@ class ShardedSink(GpuSink):
         self._thread.start()
 
     def describe(self):
-        return "%d shards on cuda:%s, capacity %d entries each (%.2f GB in all)" % (
-            len(self.shards), ",".join(str(d) for d, _, _ in self.plan), self.shard_capacity, self.table.memory_bytes() / 1e9)
+        return "%d shards on cuda:%s, capacity %d entries each (%.2f GB in all)%s" % (
+            len(self.shards), ",".join(str(d) for d, _, _ in self.plan), self.shard_capacity, self.table.memory_bytes() / 1e9,
+            host_note(self.table))
 
     def close(self):
         for sh in self.shards:
@@ -792,6 +806,11 @@ def parse_args(argv=None):
     ap.add_argument("--dp-table-capacity", type=int, default=None, metavar="E",
                     help="entries the table holds, 48 bytes of GPU memory each (default: what fits in the free GPU memory); "
                          "with --devices, the entries of each shard (default: each GPU's free memory split among its shards)")
+    ap.add_argument("--dp-table-entries", choices=("device", "host"), default="device",
+                    help="where the table's 32-byte entries live: device (default) = GPU memory, 48 bytes per entry in all; "
+                         "host = pinned host RAM mapped into the GPU, which then holds 16 bytes per entry, for about 2.6x the "
+                         "entries per GPU.  The default capacity with host is also at most the host RAM available (MemAvailable) "
+                         "less a margin, at 32 bytes per entry, shared by all shards; a larger --dp-table-capacity is refused")
     ap.add_argument("--save-work", default="", metavar="FILE", help="write the table as a HEADW work file at exit")
     ap.add_argument("--save-interval", type=float, default=0.0, metavar="SECS", help="also save every SECS seconds")
     ap.add_argument("--resume", default="", metavar="FILE", help="start from a work file: range, key and dp come from it")
@@ -818,6 +837,12 @@ def parse_args(argv=None):
         a.device = a.devices[0]
     elif a.device is None:
         a.device = 0
+    if a.dp_table_entries == "host":
+        from .solver import host_capacity_error, mem_available
+        shards = len(a.devices) if a.devices is not None and len(a.devices) >= 2 else 1
+        err = host_capacity_error(a.dp_table_capacity, mem_available(), shards)
+        if err:
+            ap.error(err.replace("table(s)", "shard(s)"))
     pubs = None
     if a.config:
         start, end, pubs = ec.parse_config(a.config)
@@ -851,10 +876,10 @@ def main(argv=None):
     try:
         if sharded:
             sink = ShardedSink(start, end, pub, dp, a.devices, capacity=a.dp_table_capacity, resume=a.resume or None,
-                               save_path=a.save_work, out=out)
+                               save_path=a.save_work, out=out, entries=a.dp_table_entries)
         else:
             sink = GpuSink(start, end, pub, dp, device=a.device, capacity=a.dp_table_capacity, resume=a.resume or None,
-                           save_path=a.save_work, out=out)
+                           save_path=a.save_work, out=out, entries=a.dp_table_entries)
     except TableFull as e:
         out("--resume %s refused: %s; give a larger --dp-table-capacity" % (a.resume, e))
         return 1
@@ -865,8 +890,8 @@ def main(argv=None):
     if sharded:
         out("Range 0x%X .. 0x%X  dp %d  key 04%064X%064X  table in %s" % (start, end, dp, pub[0], pub[1], sink.describe()))
     else:
-        out("Range 0x%X .. 0x%X  dp %d  key 04%064X%064X  table capacity %d entries (%.2f GB) on cuda:%d" %
-            (start, end, dp, pub[0], pub[1], sink.table.capacity, sink.table.memory_bytes() / 1e9, a.device))
+        out("Range 0x%X .. 0x%X  dp %d  key 04%064X%064X  table capacity %d entries (%.2f GB) on cuda:%d%s" %
+            (start, end, dp, pub[0], pub[1], sink.table.capacity, sink.table.memory_bytes() / 1e9, a.device, host_note(sink.table)))
     stop = threading.Event()
     signals = []
 
@@ -913,8 +938,8 @@ def main(argv=None):
         out("Stopped by signal %d" % signals[0])
         rc = 1
     if sink.full is not None:
-        out("DP table full, server stopped: %s.  Resume with --resume %s --dp-table-capacity %d or more; the clients reconnect "
-            "and resend the DPs they hold." % (sink.full, a.save_work or "FILE (give --save-work to write one)",
+        out("DP table full%s, server stopped: %s.  Resume with --resume %s --dp-table-capacity %d or more; the clients reconnect "
+            "and resend the DPs they hold." % (" (host entries)" if a.dp_table_entries == "host" else "", sink.full, a.save_work or "FILE (give --save-work to write one)",
                                                2 * (sink.shard_capacity if sharded else sink.table.capacity)))
         rc = 1
     if sink.failed is not None:

@@ -74,6 +74,8 @@ SAVE_BUFFERS = 4          # rank 0's pinned chunk buffers queued to the writer
 DP_TABLE_MARGIN = 4 << 30 # --dp-table device without a capacity: rank 0's free GPU memory after the engine, its staging
                           # buffers and the table's reserved per-add scratch, less this margin for NCCL, the gather buffer
                           # and torch's allocator.  Nothing else grows on the GPU: steps queued behind a save wait in host RAM
+HOST_ENTRIES_MARGIN = 8 << 30   # --dp-table-entries host: host RAM (MemAvailable) left to the OS, torch, the pinned staging
+                                # and save buffers and parked steps; the rest may hold pinned table entries
 
 
 def init_dist():
@@ -102,13 +104,52 @@ def scratch_bytes(n_records):
     return m * 80 + (16 << 20)
 
 
-def default_table_capacity(free_bytes, margin=DP_TABLE_MARGIN):
-    """the largest capacity whose device table fits in free_bytes - margin"""
+def default_table_capacity(free_bytes, margin=DP_TABLE_MARGIN, entries="device", host_limit=None):
+    """the largest capacity whose device table of that layout (ingest.TABLE_ENTRIES) fits in free_bytes - margin, at most
+    2^32-2 entries and, with entries="host", at most host_limit (host_entries_limit)"""
     room = free_bytes - margin
-    cap = max(room // 48, 0)
-    while cap > 0 and DeviceDPTable.bytes_for(cap) > room:
+    cap = max(room // (16 if entries == "host" else 48), 0)
+    while cap > 0 and DeviceDPTable.bytes_for(cap, entries) > room:
         cap = cap * 63 // 64
-    return int(min(cap, (1 << 32) - 2))
+    cap = min(cap, (1 << 32) - 2)
+    if entries == "host" and host_limit is not None:
+        cap = min(cap, host_limit)
+    return int(cap)
+
+
+def mem_available():
+    """the kernel's estimate of the host RAM available without swapping (/proc/meminfo MemAvailable), in bytes"""
+    with open("/proc/meminfo") as f:
+        for line in f:
+            if line.startswith("MemAvailable:"):
+                return int(line.split()[1]) * 1024
+    raise RuntimeError("/proc/meminfo has no MemAvailable")
+
+
+def host_entries_limit(available, tables, margin=HOST_ENTRIES_MARGIN):
+    """--dp-table-entries host: the entries each of `tables` tables on this host may pin, at 32 bytes each, out of `available`
+    bytes of host RAM less the margin"""
+    return int(max(available - margin, 0) // max(int(tables), 1) // 32)
+
+
+def tables_on_node(dp_table):
+    """the device tables this host holds: one (rank 0's) for --dp-table device, one per local rank for sharded"""
+    return int(os.environ.get("LOCAL_WORLD_SIZE", "1")) if dp_table == "sharded" else 1
+
+
+def host_capacity_error(capacity, available, tables):
+    """why an explicit --dp-table-capacity cannot hold host entries here, or None"""
+    limit = host_entries_limit(available, tables)
+    if capacity is not None and capacity > limit:
+        return ("--dp-table-entries host: --dp-table-capacity %d entries would pin %.1f GB of host RAM, more than the host limit "
+                "of %d entries (MemAvailable %.1f GB less %d GiB, shared by %d table(s) on this host, 32 bytes per entry)" %
+                (capacity, 32 * capacity / 1e9, limit, available / 1e9, HOST_ENTRIES_MARGIN >> 30, tables))
+    return None
+
+
+def layout_note(entries):
+    """the words the report lines add for a table's layout"""
+    return " (host entries)" if entries == "host" else ""
 
 
 def shard_headroom(world, max_found):
@@ -258,22 +299,26 @@ class DeviceTable:
     resolves its collisions against the run's keys on the same stream (ingest.DeviceResolver): its events carry their hits."""
     label = "device table"
 
-    def __init__(self, torch, n_records, device, capacity, wait_copy, keys, start, buckets=None):
+    def __init__(self, torch, n_records, device, capacity, wait_copy, keys, start, buckets=None, entries="device", tables=1):
         """wait_copy: the records' source is rewritten unordered with torch's stream (the engine's own buffer, on one GPU).
         keys: the key table the collisions are resolved against (DPTable.key_table: K = key - start*G per key).
-        buckets: (lo, hi) of a shard (ShardedTable)"""
+        buckets: (lo, hi) of a shard (ShardedTable).  entries: the table's layout (ingest.TABLE_ENTRIES); with "host" the
+        default capacity also keeps to this host's share of its RAM among `tables` tables (host_entries_limit)"""
         self.torch, self._wait_copy = torch, wait_copy
         self.resolver = DeviceResolver(keys, start, device=device)
         self._bufs = [torch.empty(n_records * DP40_BYTES, dtype=torch.uint8, device=torch.device("cuda", device)) for _ in range(3)]
         self._back = self._bufs.pop()
         if not capacity:
-            capacity = default_table_capacity(torch.cuda.mem_get_info(device)[0] - scratch_bytes(n_records))
-        self.dps = DeviceDPTable(capacity, device=device, buckets=buckets)
+            capacity = default_table_capacity(torch.cuda.mem_get_info(device)[0] - scratch_bytes(n_records), entries=entries,
+                                              host_limit=host_entries_limit(mem_available(), tables) if entries == "host" else None)
+        self.dps = DeviceDPTable(capacity, device=device, buckets=buckets, entries=entries)
         self.dps.reserve(n_records)
         self._stream = torch.cuda.Stream(device=device)
         self._i = 0
         self.save = functools.partial(self.dps.save_work, stream=self._stream.cuda_stream)
         self.info = "dp table: device, capacity %d entries (%.2f GB)" % (self.dps.capacity, self.dps.memory_bytes() / 1e9)
+        if entries == "host":
+            self.info += ", entries in pinned host memory (%.2f GB)" % (self.dps.host_bytes() / 1e9)
 
     def stage(self, counts, stride, src, park):
         """the records are copied device to device (torch's stream), since the gather buffer and the engine's record buffer
@@ -311,8 +356,8 @@ class ShardedTable(DeviceTable):
     Its capacity is the shard's; save_piece writes its piece of a work file at an offset."""
     label = "sharded table"
 
-    def __init__(self, torch, n_records, device, capacity, keys, start, buckets):
-        super().__init__(torch, n_records, device, capacity, False, keys, start, buckets)
+    def __init__(self, torch, n_records, device, capacity, keys, start, buckets, entries="device"):
+        super().__init__(torch, n_records, device, capacity, False, keys, start, buckets, entries, tables_on_node("sharded"))
         self.save_piece = functools.partial(self.dps.save_piece, stream=self._stream.cuda_stream)
 
 
@@ -366,7 +411,8 @@ class WorkFile:
 
 class Solver:
     def __init__(self, start, end, pub, dp_bits, grid=None, max_found=1 << 17, seed=None, ingest_threads=0,
-                 save_work="", save_interval=0.0, save_kangaroos=False, resume=None, dp_table="host", dp_table_capacity=None):
+                 save_work="", save_interval=0.0, save_kangaroos=False, resume=None, dp_table="host", dp_table_capacity=None,
+                 dp_table_entries="device"):
         import torch
         self.torch = torch
         self.rank = int(os.environ.get("RANK", "0"))
@@ -403,11 +449,13 @@ class Solver:
         self.found = None                   # rank 0: the private key, once found
         self._announce = []                 # rank 0: keys solved, not yet in a control broadcast
         self.dpt = self.dps = None          # rank 0: HostTable / DeviceTable, and the table it holds
+        self.entries = dp_table_entries     # the device table's layout: "device" or "host" (its entries in pinned host RAM)
         if self.sharded:
             self._init_shard(max_found, dp_table_capacity)
         elif self.rank == 0:
             self.dpt = (DeviceTable(torch, self.world * max_found, self.local, dp_table_capacity, self.gather is None, self.key_table,
-                                    self.start) if dp_table == "device" else HostTable(torch, self.world * max_found, ingest_threads))
+                                    self.start, entries=dp_table_entries) if dp_table == "device"
+                        else HostTable(torch, self.world * max_found, ingest_threads))
             self.dps = self.dpt.dps
         self._work = queue.Queue()
         self._done = queue.Queue()
@@ -477,7 +525,8 @@ class Solver:
             raise ValueError(err)
         self.buckets = owner_ranges(self.world)[self.rank]
         self.headroom = shard_headroom(self.world, max_found)
-        self.dpt = ShardedTable(torch, self.world * max_found, self.local, capacity, self.key_table, self.start, self.buckets)
+        self.dpt = ShardedTable(torch, self.world * max_found, self.local, capacity, self.key_table, self.start, self.buckets,
+                                self.entries)
         self.dps = self.dpt.dps
         if self.dps.capacity <= self.headroom:
             raise RuntimeError(sharded_capacity_error(self.dps.capacity, self.world, max_found))
@@ -491,6 +540,8 @@ class Solver:
         self.shard_caps = caps
         self.dpt.info = ("dp table: sharded over %d GPUs, %d entries in all (rank 0: buckets [%d, %d), %d entries, %.2f GB)" %
                          (self.world, sum(caps), self.buckets[0], self.buckets[1], caps[0], self.dps.memory_bytes() / 1e9))
+        if self.entries == "host":
+            self.dpt.info += ", entries in pinned host memory (rank 0: %.2f GB)" % (self.dps.host_bytes() / 1e9)
         self.shard_total = 0                # entries of all shards, as the last blocks reported them
         self.shard_hits = [0] * self.world  # rank 0: collisions resolved to a key on each shard
         self.shard_msg = None               # rank 0: why a full shard stopped the run
@@ -1138,7 +1189,7 @@ class BatchSolver(Solver):
     block (worktool.BatchBlock, from batch_resume_file: the targets on rank 0 only)."""
 
     def __init__(self, start, end, pubs, dp_bits, grid=None, max_found=1 << 17, seed=None, ingest_threads=0, dp_table="host",
-                 dp_table_capacity=None, save_work="", save_interval=0.0, resume=None, resume_block=None):
+                 dp_table_capacity=None, save_work="", save_interval=0.0, resume=None, resume_block=None, dp_table_entries="device"):
         self.pubs = list(pubs)
         if not 1 <= len(self.pubs) <= MAX_KEYS:
             raise ValueError("--batch-keys takes 1 to %d keys, not %d" % (MAX_KEYS, len(self.pubs)))
@@ -1158,8 +1209,8 @@ class BatchSolver(Solver):
                     self.announced.add(self.rep[i])
         self.live = [i for i, k in enumerate(self.keys) if k is not None and self.rep[i] == i and i not in self.announced]
         super().__init__(start, end, self.pubs[0], dp_bits, grid, max_found, seed, ingest_threads, dp_table=dp_table,
-                         dp_table_capacity=dp_table_capacity, save_work=save_work, save_interval=save_interval,
-                         save_kangaroos=bool(save_work), resume=resume)
+                         dp_table_capacity=dp_table_capacity, dp_table_entries=dp_table_entries, save_work=save_work,
+                         save_interval=save_interval, save_kangaroos=bool(save_work), resume=resume)
 
     def _resume(self, path):
         """Solver._resume with the targets: rank 0 loads the table and sends every rank its records and their targets; each
@@ -1305,7 +1356,7 @@ def _run_batch(start, end, pubs, dp, grid, a, block=None):
     t0 = time.perf_counter()
     s = BatchSolver(start, end, pubs, dp, grid, seed=a.seed, ingest_threads=a.ingest_threads, dp_table=a.dp_table,
                     dp_table_capacity=a.dp_table_capacity, save_work=a.batch_save, save_interval=a.batch_save_interval,
-                    resume=a.batch_resume or None, resume_block=block)
+                    resume=a.batch_resume or None, resume_block=block, dp_table_entries=a.dp_table_entries)
     t_setup = time.perf_counter() - t0
     if s.rank == 0:
         print("Range width: 2^%d  kangaroos/GPU: %d  GPUs: %d  dp: %d  %s  keys: %d in one run" %
@@ -1344,8 +1395,8 @@ def report(s, a):
     if s.sharded:
         print("Hits resolved per shard: %s" % " ".join(str(v) for v in s.shard_hits))
     if s.shard_stop and not s.table_stopped:
-        print("DP table shard full, run stopped: %s.  Resume the work file with a larger --dp-table-capacity, on more GPUs or with "
-              "--dp-table host" % s.shard_msg)
+        print("DP table shard full%s, run stopped: %s.  Resume the work file with a larger --dp-table-capacity, on more GPUs or "
+              "with --dp-table host" % (layout_note(s.entries), s.shard_msg))
     if s.table_stopped:
         print(table_message(s, a))
         return 1
@@ -1370,7 +1421,7 @@ def print_key(i, pub, priv):
 def table_message(s, a):
     """rank 0, after the run: why the table stopped it, and which work file, if any, to resume"""
     what = "full" if s.table_kind == "full" else "failed"
-    msg = "DP table %s, run stopped: %s." % (what, s.table_msg)
+    msg = "DP table %s%s, run stopped: %s." % (what, layout_note(s.entries), s.table_msg)
     saved = s.full_saved
     if saved and saved[2] is None:
         msg += (" %s holds the table as it was before this step's launch (count 2^%.2f, no kangaroos); resume it with "
@@ -1470,6 +1521,12 @@ def parse_args(argv=None):
                     help="--dp-table device: entries the table holds, 48 bytes of GPU memory each (default: what fits in rank "
                          "0's free GPU memory after the engine, less %d GiB); --dp-table sharded: entries of each GPU's shard "
                          "(default: the same rule on each GPU)" % (DP_TABLE_MARGIN >> 30))
+    ap.add_argument("--dp-table-entries", choices=("device", "host"), default=None,
+                    help="--dp-table device or sharded: where the table's 32-byte entries live.  device (default) = GPU "
+                         "memory, 48 bytes per entry in all; host = pinned host RAM mapped into the GPU, which then holds 16 bytes "
+                         "per entry (the index), for about 2.6x the entries per GPU.  The default capacity with host is also at "
+                         "most 2^32-2 and the host RAM available (MemAvailable) less %d GiB, at 32 bytes per entry, shared by "
+                         "the tables of this host; a larger --dp-table-capacity is refused" % (HOST_ENTRIES_MARGIN >> 30))
     ap.add_argument("--batch-keys", action="store_true",
                     help="solve every key of the config in one run: one tame herd and one DP table shared by all keys, the "
                          "wild kangaroos spread over the unsolved ones")
@@ -1497,6 +1554,11 @@ def parse_args(argv=None):
         ap.error("--dp-table-capacity must be 1 .. 2^32-2 entries, not %d" % a.dp_table_capacity)
     if a.dp_table == "sharded" and sharded_capacity_error(a.dp_table_capacity, int(os.environ.get("WORLD_SIZE", "1"))):
         ap.error(sharded_capacity_error(a.dp_table_capacity, int(os.environ.get("WORLD_SIZE", "1"))))
+    if a.dp_table_entries is not None and a.dp_table not in ("device", "sharded"):
+        ap.error("--dp-table-entries needs --dp-table device or sharded (--dp-table host keeps the reference's table in host RAM)")
+    a.dp_table_entries = a.dp_table_entries or "device"
+    if a.dp_table_entries == "host" and host_capacity_error(a.dp_table_capacity, mem_available(), tables_on_node(a.dp_table)):
+        ap.error(host_capacity_error(a.dp_table_capacity, mem_available(), tables_on_node(a.dp_table)))
     block = None
     if a.batch_resume:
         res = batch_resume_file(a.batch_resume)
@@ -1542,7 +1604,7 @@ def main(argv=None):
     for i, pub in enumerate([] if a.batch_keys else pubs):
         s = Solver(start, end, pub, dp, grid, seed=a.seed, ingest_threads=a.ingest_threads, save_work=a.save_work,
                    save_interval=a.save_interval, save_kangaroos=a.save_kangaroos, resume=a.resume or None, dp_table=a.dp_table,
-                   dp_table_capacity=a.dp_table_capacity)
+                   dp_table_capacity=a.dp_table_capacity, dp_table_entries=a.dp_table_entries)
         if s.rank == 0:
             print("Range width: 2^%d  kangaroos/GPU: %d  GPUs: %d  dp: %d  %s" %
                   (s.range_power, s.eng.nbKangaroo, s.world, dp, s.dpt.info), flush=True)
