@@ -210,10 +210,11 @@ typedef struct {                     /* = kgi_event (include/kgx_ingest.h) */
  *     the type bit 126 is set; a record is good iff h < 2^18, S is not the point at infinity, S.x.bits64[2] & 0x3FFFF == h and
  *     the low 128 bits of S.x equal x.  good (device, n x 40 bytes, 8-byte aligned) gets the good records in input order (a
  *     stable compaction), counts (device, 2 entries) = {good, bad}, bad_idx (device, cap entries) the indices of the first
- *     `cap` bad records in input order.  scratch: device memory of at least kgx_resolver_verify_scratch_bytes(n) bytes,
- *     256-byte aligned (as cudaMalloc returns it; the flags, their prefix sums and cub's scan storage live there).
- *     Stream-ordered on `stream`, no allocation, no synchronisation.  -1: bad arguments; -3: a CUDA error, text in
- *     kgx_resolver_last_error(r).
+ *     `cap` bad records in input order.  It is _verify_partition with W = 1 and stride 0.  scratch: device memory of at
+ *     least kgx_resolver_verify_scratch_bytes(n) bytes (0: bad arguments), which is
+ *     kgx_resolver_verify_partition_scratch_bytes(n, 1), 256-byte aligned (as cudaMalloc returns it; the flags, the
+ *     partition's (owner, tile) counts and cub's scan storage of them live there).  Stream-ordered on `stream`, no
+ *     allocation, no synchronisation.  -1: bad arguments; -3: a CUDA error, text in kgx_resolver_last_error(r).
  * _verify_partition: _verify and kgx_dp_partition in one call, for a DP table sharded over W tables (1 .. KGX_DPT_MAX_RANKS).
  *     The same check, then the good records grouped by the shard that owns their bucket (shard r of W holds the buckets
  *     [floor(r*2^18/W), floor((r+1)*2^18/W))), each group in input order, into out (device, 8-byte aligned): packed when

@@ -8,12 +8,10 @@
 // kgx_work_resolve is a resolver of one call.
 //
 // A resolver of one key also checks received DP records (kgx_resolver_verify, the server's check of what clients send): the
-// stored-entry check of kgx_worktool.cuh (wt_check_entries_kernel, on Dp40Check records) flags each record, an exclusive scan
-// of the flags gives each good record its slot, and one pass writes the good records in input order and the indices of the
-// first `cap` bad ones.  kgx_resolver_verify_partition runs the same check, then kgx_dp_partition's passes (kgx_partition.cuh)
-// with the wrong records as the group left out: the good records grouped by the shard that owns their bucket, and the bad
-// indices, from one scan of (owner, tile) counts.
-#include <cub/cub.cuh>
+// stored-entry check of kgx_worktool.cuh (wt_check_entries_kernel, on Dp40Check records) flags each record, then
+// kgx_dp_partition's passes (kgx_partition.cuh) run with the wrong records as the group left out: the good records grouped by
+// the shard that owns their bucket (kgx_resolver_verify_partition; one group, in input order, for kgx_resolver_verify) and
+// the bad indices, from one scan of (owner, tile) counts.
 
 struct kgx_resolver {
   int dev = 0;
@@ -77,27 +75,6 @@ static cudaError_t resolve_events(const kgx_resolver* r, const kgx_dp_event* ev,
   return cudaGetLastError();
 }
 
-// kgx_resolver_verify's last pass: flags / pos = each record's verdict and its exclusive prefix sum.  Good record i goes to
-// good[pos[i]], bad record i is bad record number i - pos[i]; the last thread writes both counts.
-__global__ void wt_verify_compact_kernel(const u64* __restrict__ rec, uint32_t n, const uint32_t* __restrict__ flags,
-                                         const uint32_t* __restrict__ pos, u64* good, uint32_t* counts, uint32_t* bad_idx, uint32_t cap) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint32_t p = pos[i];
-  if (flags[i]) {
-#pragma unroll
-    for (int k = 0; k < 5; k++) good[5ull * p + k] = rec[5ull * i + k];
-  } else if (i - p < cap) {
-    bad_idx[i - p] = i;
-  }
-  if (i == n - 1) {
-    counts[0] = p + flags[i];
-    counts[1] = n - (p + flags[i]);
-  }
-}
-
-inline uint64_t align256(uint64_t v) { return (v + 255) & ~255ull; }
-
 // kgx_resolver_verify_partition's destination of record i: the owner of its bucket when the check found it good (then
 // h < 2^18, since h equals 18 bits of S.x), else the group left out
 struct Verified {
@@ -108,10 +85,42 @@ struct Verified {
   }
 };
 
-inline uint64_t verify_scan_bytes(uint32_t n) {
-  size_t b = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, b, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)(n ? n : 1));
-  return b;
+// kgx_resolver_verify_partition, and kgx_resolver_verify as its world 1, stride 0; fn names the call in its error messages.
+// scratch: the check's flags, then kgx_dp_partition_scratch_bytes(n, world) for the partition's passes.
+static int verify_partition(const char* fn, kgx_resolver* r, const void* recs, uint32_t n, uint32_t world, uint64_t stride, void* out,
+                            uint32_t* counts, uint32_t* bad_idx, uint32_t cap, void* scratch, uint64_t scratch_bytes, void* stream) {
+  const char* why = nullptr;
+  if (r->n_keys != 1) why = "the resolver must hold exactly one key";
+  else if (n >= 0x80000000u) why = "at most 2^31-1 records";
+  else if (world == 0 || world > KGX_DPT_MAX_RANKS) why = "world must be 1 .. KGX_DPT_MAX_RANKS";
+  else if (stride != 0 && stride < n) why = "stride must be 0 or at least n";
+  else if (((uintptr_t)recs | (uintptr_t)out) & 7) why = "the records and the output must be 8-byte aligned";
+  else if ((uintptr_t)scratch & 255) why = "scratch must be 256-byte aligned";
+  else if (scratch_bytes < kgx_resolver_verify_partition_scratch_bytes(n, world)) why = "scratch smaller than the call's _scratch_bytes";
+  if (why) {
+    snprintf(r->err, sizeof r->err, "%s: %s", fn, why);
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t s = cudaSetDevice(r->dev);
+  uint8_t* sb = static_cast<uint8_t*>(scratch);
+  uint32_t* flags = reinterpret_cast<uint32_t*>(sb);
+  const uint8_t* in = static_cast<const uint8_t*>(recs);
+  const uint64_t fb = kgx_part::align256(4ull * n);
+  if (s == cudaSuccess && n > 0) {
+    wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS, 0, st>>>(r->comb, Dp40Check{static_cast<const u64*>(recs), flags}, n, r->K,
+                                                                      r->kinf);
+    s = cudaGetLastError();
+  }
+  const int rc = s == cudaSuccess ? kgx_part::run(in, Verified{in, flags}, n, world, stride, out, counts, bad_idx, cap, sb + fb,
+                                                  scratch_bytes - fb, st)
+                                   : 0;
+  if (s != cudaSuccess || rc) {
+    snprintf(r->err, sizeof r->err, "%s: %s", fn, s != cudaSuccess ? cudaGetErrorString(s) : "a launch of the partition passes failed");
+    cudaGetLastError();
+    return -3;
+  }
+  return 0;
 }
 
 // the checks kgx_resolver_create and kgx_work_resolve share: -1 with the reason in g_wt_err, or 0
@@ -177,92 +186,22 @@ int kgx_resolver_run(kgx_resolver* r, const void* pairs, uint32_t n, uint32_t* k
   return 0;
 }
 
-uint64_t kgx_resolver_verify_scratch_bytes(uint32_t n) {
-  using namespace kgx_wt;
-  if (n >= 0x80000000u) return 0;
-  return 2 * align256(4ull * n) + align256(verify_scan_bytes(n));
-}
+uint64_t kgx_resolver_verify_scratch_bytes(uint32_t n) { return kgx_resolver_verify_partition_scratch_bytes(n, 1); }
 
 int kgx_resolver_verify(kgx_resolver* r, const void* recs, uint32_t n, void* good, uint32_t* counts, uint32_t* bad_idx, uint32_t cap,
                         void* scratch, uint64_t scratch_bytes, void* stream) {
-  using namespace kgx_wt;
-  const char* why = nullptr;
-  if (r->n_keys != 1) why = "the resolver must hold exactly one key";
-  else if (n >= 0x80000000u) why = "at most 2^31-1 records";
-  else if (((uintptr_t)recs | (uintptr_t)good) & 7) why = "recs and good must be 8-byte aligned";
-  else if ((uintptr_t)scratch & 255) why = "scratch must be 256-byte aligned";
-  else if (scratch_bytes < kgx_resolver_verify_scratch_bytes(n)) why = "scratch smaller than kgx_resolver_verify_scratch_bytes(n)";
-  if (why) {
-    snprintf(r->err, sizeof r->err, "kgx_resolver_verify: %s", why);
-    return -1;
-  }
-  cudaStream_t st = (cudaStream_t)stream;
-  cudaError_t s = cudaSetDevice(r->dev);
-  if (s == cudaSuccess && n == 0) s = cudaMemsetAsync(counts, 0, 8, st);
-  if (s == cudaSuccess && n > 0) {
-    uint8_t* sb = static_cast<uint8_t*>(scratch);
-    uint32_t* flags = reinterpret_cast<uint32_t*>(sb);
-    uint32_t* pos = reinterpret_cast<uint32_t*>(sb + align256(4ull * n));
-    size_t tb = scratch_bytes - 2 * align256(4ull * n);
-    const u64* rec = static_cast<const u64*>(recs);
-    wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS, 0, st>>>(r->comb, Dp40Check{rec, flags}, n, r->K, r->kinf);
-    s = cudaGetLastError();
-    if (s == cudaSuccess) s = cub::DeviceScan::ExclusiveSum(sb + 2 * align256(4ull * n), tb, flags, pos, (int)n, st);
-    if (s == cudaSuccess) {
-      wt_verify_compact_kernel<<<(n + 255) / 256, 256, 0, st>>>(rec, n, flags, pos, static_cast<u64*>(good), counts, bad_idx, cap);
-      s = cudaGetLastError();
-    }
-  }
-  if (s != cudaSuccess) {
-    snprintf(r->err, sizeof r->err, "kgx_resolver_verify: %s", cudaGetErrorString(s));
-    cudaGetLastError();
-    return -3;
-  }
-  return 0;
+  return kgx_wt::verify_partition("kgx_resolver_verify", r, recs, n, 1, 0, good, counts, bad_idx, cap, scratch, scratch_bytes, stream);
 }
 
 uint64_t kgx_resolver_verify_partition_scratch_bytes(uint32_t n, uint32_t world) {
-  using namespace kgx_wt;
   const uint64_t part = kgx_dp_partition_scratch_bytes(n, world);
-  return n >= 0x80000000u || part == 0 ? 0 : align256(4ull * n) + part;
+  return n >= 0x80000000u || part == 0 ? 0 : kgx_part::align256(4ull * n) + part;
 }
 
 int kgx_resolver_verify_partition(kgx_resolver* r, const void* recs, uint32_t n, uint32_t world, uint64_t stride, void* out,
                                   uint32_t* counts, uint32_t* bad_idx, uint32_t cap, void* scratch, uint64_t scratch_bytes, void* stream) {
-  using namespace kgx_wt;
-  const char* why = nullptr;
-  if (r->n_keys != 1) why = "the resolver must hold exactly one key";
-  else if (n >= 0x80000000u) why = "at most 2^31-1 records";
-  else if (world == 0 || world > KGX_DPT_MAX_RANKS) why = "world must be 1 .. KGX_DPT_MAX_RANKS";
-  else if (stride != 0 && stride < n) why = "stride must be 0 or at least n";
-  else if (((uintptr_t)recs | (uintptr_t)out) & 7) why = "recs and out must be 8-byte aligned";
-  else if ((uintptr_t)scratch & 255) why = "scratch must be 256-byte aligned";
-  else if (scratch_bytes < kgx_resolver_verify_partition_scratch_bytes(n, world))
-    why = "scratch smaller than kgx_resolver_verify_partition_scratch_bytes(n, world)";
-  if (why) {
-    snprintf(r->err, sizeof r->err, "kgx_resolver_verify_partition: %s", why);
-    return -1;
-  }
-  cudaStream_t st = (cudaStream_t)stream;
-  cudaError_t s = cudaSetDevice(r->dev);
-  uint8_t* sb = static_cast<uint8_t*>(scratch);
-  uint32_t* flags = reinterpret_cast<uint32_t*>(sb);
-  const uint8_t* in = static_cast<const uint8_t*>(recs);
-  if (s == cudaSuccess && n > 0) {
-    wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS, 0, st>>>(r->comb, Dp40Check{static_cast<const u64*>(recs), flags}, n, r->K,
-                                                                      r->kinf);
-    s = cudaGetLastError();
-  }
-  const int rc = s == cudaSuccess ? kgx_part::run(in, Verified{in, flags}, n, world, stride, out, counts, bad_idx, cap,
-                                                  sb + align256(4ull * n), scratch_bytes - align256(4ull * n), st)
-                                   : 0;
-  if (s != cudaSuccess || rc) {
-    snprintf(r->err, sizeof r->err, "kgx_resolver_verify_partition: %s",
-             s != cudaSuccess ? cudaGetErrorString(s) : "a launch of the partition passes failed");
-    cudaGetLastError();
-    return -3;
-  }
-  return 0;
+  return kgx_wt::verify_partition("kgx_resolver_verify_partition", r, recs, n, world, stride, out, counts, bad_idx, cap, scratch,
+                                  scratch_bytes, stream);
 }
 
 int kgx_work_resolve(int dev, const uint64_t* d_first, const uint64_t* d_other, uint64_t n, const uint64_t* keys, uint32_t n_keys,

@@ -2,7 +2,7 @@
 every received DP checked on the GPU before it is kept.
 
 Unmodified reference clients (`kangaroo -c SERVER`) and the drop-in build/kangaroo_b200 connect to it as to `kangaroo -s`.
-The server holds the one DP table of the search in the memory of one GPU (ingest.DeviceDPTable), resolves its collisions there
+The server holds the one DP table of the search in GPU memory (ingest.DeviceDPTable), resolves its collisions there
 (ingest.DeviceResolver) and writes the work files the solver, worktool and the reference read.
 
 Threads:
@@ -10,16 +10,16 @@ Threads:
   handlers     one per connection: the protocol.  A SENDDP message is read whole, in host chunks of at most 2^20 records,
                answered with the status, then queued with its connection; the queue has a byte budget and a handler blocks
                while it is full.  Records are never touched one by one in Python.
-  ingest       owns the GPU (GpuSink): per batch of up to 2^20 queued records, one copy to the device, kgx_resolver_verify
-               (the check of every record against the key, and a stable compaction of the good ones), the two counts back,
-               then DeviceDPTable.add of the good records with the resolver, on the ingest thread's own stream.  Saves are
-               queued like records, so a work file holds the table after every record queued before it.
+  ingest       owns the GPUs (GpuSink): per batch of up to 2^20 queued records, one copy to a GPU,
+               kgx_resolver_verify_partition (the check of every record against the key, and the good ones grouped by the
+               shard that owns their bucket, in input order), the counts back, then DeviceDPTable.add of each group with the
+               resolver, on the shard's stream.  Saves are queued like records, so a work file holds the table after every
+               record queued before it.
   main         the status line, periodic saves, signals and the end of the run.
 
-With --devices D0,D1,... (two or more entries) the table is split into one shard per entry (ShardedSink), in the buckets
-the solver's --dp-table sharded gives its ranks; the ingest thread then verifies each batch and groups its good records by
-shard in one kernel (kgx_resolver_verify_partition), and adds every group to its shard.  Its work files are byte for byte
-those of the one table.
+The table is one shard per --devices entry (--device D, the default, is the one entry D), in the buckets the solver's
+--dp-table sharded gives its ranks; one shard holds every bucket.  The work files are byte for byte those of one table
+whatever the shards.
 
 The protocol layer (Server) talks to its sink through three calls -- put(message, chunks), status(), reset_dead() -- so that
 a test can run it with a fake sink in place of the GPU path.
@@ -391,43 +391,79 @@ class RecordQueue:
 
 
 class GpuSink:
-    """The ingest thread and what it owns: the device table, the resolver of the one key, the staging buffers on `device`.
-    put / status / reset_dead are the Server's sink calls."""
+    """The ingest thread and what it owns.  The table is split into one shard per `devices` entry (shard_plan), a DeviceDPTable
+    of its buckets on that entry's GPU: one entry is the one table over every bucket, and a GPU listed k times holds k shards.
+    Each distinct GPU has one resolver of the one key, shared by its shards, and one set of batch buffers; each shard has its
+    own stream and, when there are several GPUs, a staging buffer on its GPU.  Everything is allocated here.  capacity is per
+    shard; by default each GPU's free memory, less its buffers, is split evenly among its shards.  put / status / reset_dead
+    are the Server's sink calls.
 
-    def __init__(self, start, end, pub, dp, device=0, capacity=None, resume=None, save_path="", out=print, entries="device"):
+    The ingest thread, per batch: one copy to the next GPU in turn (spreading the verify), kgx_resolver_verify_partition there
+    (the check, the good records grouped by shard in input order, the per-shard and bad counts), the counts back; then, unless
+    some shard would overflow (nothing of the batch is added then), each shard's group -- read in place on the batch's GPU, or
+    copied to the shard's staging buffer on another one -- added with its GPU's resolver on the shard's stream.  Each add
+    waits for its own work, and a batch is done before the next starts, so every bucket sees its records in queue order, as
+    the one table does.  A save writes the header, then each shard's piece at its offset: the one table's file, byte for byte."""
+
+    def __init__(self, start, end, pub, dp, devices=(0,), capacity=None, resume=None, save_path="", out=print, entries="device"):
         import torch
         from .ingest import DeviceDPTable, DeviceResolver, DPTable, TableFull
-        from .solver import default_table_capacity, host_entries_limit, mem_available, scratch_bytes
-        self.torch, self.TableFull = torch, TableFull
+        from .solver import DP_TABLE_MARGIN, default_table_capacity, host_entries_limit, mem_available, scratch_bytes
+        self.torch = torch
         self.start, self.end, self.pub, self.dp = start, end, pub, dp
         self.save_path, self.out = save_path, out
-        self.dev = torch.device("cuda", device)
-        torch.cuda.set_device(self.dev)
+        devices = list(devices)
+        torch.cuda.set_device(devices[0])
+        self.plan = shard_plan(devices)
+        W = len(self.plan)
+        gpus = sorted(set(devices))
         K = ec.add(pub, ec.neg(ec.mul(start))) if start else pub
-        self.resolver = DeviceResolver(DPTable.key_table([K]), start, device=device)
-        nb = self.resolver.verify_scratch_bytes(CHUNK_RECORDS)
-        self._recs = torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8, device=self.dev)
-        self._good = torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8, device=self.dev)
-        self._bad = torch.empty(CHUNK_RECORDS, dtype=torch.int32, device=self.dev)
-        self._counts = torch.empty(2, dtype=torch.int32, device=self.dev)
-        self._scratch = torch.empty(nb, dtype=torch.uint8, device=self.dev)
-        self._scratch_bytes = nb
+        self.gpus = {}                                        # device -> its resolver, batch buffers and stream
+        for d in gpus:
+            dev = torch.device("cuda", d)
+            r = DeviceResolver(DPTable.key_table([K]), start, device=d)
+            nb = r.verify_partition_scratch_bytes(CHUNK_RECORDS, W)
+            self.gpus[d] = dict(resolver=r, nb=nb,
+                                recs=torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8, device=dev),
+                                out=torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8, device=dev),
+                                bad=torch.empty(CHUNK_RECORDS, dtype=torch.int32, device=dev),
+                                counts=torch.empty(W + 1, dtype=torch.int32, device=dev),
+                                scratch=torch.empty(nb, dtype=torch.uint8, device=dev))
         self._host = torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8).pin_memory()
         self._host_np = self._host.numpy()
-        self._counts_h = torch.empty(2, dtype=torch.int32).pin_memory()
+        self._counts_h = torch.empty(W + 1, dtype=torch.int32).pin_memory()
+        staged = len(gpus) > 1
+        per_shard = scratch_bytes(CHUNK_RECORDS) + EVENT_BYTES * CHUNK_RECORDS + (CHUNK_RECORDS * DP40 if staged else 0)
         self.entries = entries
-        if not capacity:
-            capacity = default_table_capacity(torch.cuda.mem_get_info(self.dev)[0] - scratch_bytes(CHUNK_RECORDS) -
-                                              EVENT_BYTES * CHUNK_RECORDS, entries=entries,
-                                              host_limit=host_entries_limit(mem_available(), 1) if entries == "host" else None)
+        host_limit = host_entries_limit(mem_available(), W) if entries == "host" else None   # the host's RAM shared by all shards
+        caps = {}
+        for d in gpus:                                        # before any table takes memory
+            k = devices.count(d)
+            caps[d] = capacity or default_table_capacity((torch.cuda.mem_get_info(d)[0] - DP_TABLE_MARGIN) // k - per_shard,
+                                                         margin=0, entries=entries, host_limit=host_limit)
         # a record makes at most one event, so room for a whole batch's events means no event of an add is ever cut off: a
         # hit cannot be pushed out by the RESETs of clients that keep resending, and the dead count is exact
-        self.table = DeviceDPTable(capacity, device=device, max_events=CHUNK_RECORDS, entries=entries)
-        self.table.reserve(CHUNK_RECORDS)
-        self.stream = torch.cuda.Stream(device=self.dev)
+        self.shards = []
+        for s, (d, lo, hi) in enumerate(self.plan):
+            dev = torch.device("cuda", d)
+            t = DeviceDPTable(caps[d], device=d, max_events=CHUNK_RECORDS, buckets=(lo, hi), entries=entries)
+            t.reserve(CHUNK_RECORDS)
+            self.shards.append(dict(table=t, device=d, lo=lo, hi=hi, stream=torch.cuda.Stream(device=dev),
+                                    staging=torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8, device=dev) if staged else None))
+            # a GPU checks its batches on its first shard's stream; torch makes its pool of streams at the first one, so
+            # no stream is made before the capacity is read from the free memory
+            self.gpus[d].setdefault("stream", self.shards[-1]["stream"])
+        self.table = ShardTables([sh["table"] for sh in self.shards])
+        self.shard_capacity = max(caps.values())
         self.time0 = 0.0
         if resume:
-            info = self.table.load_work_ex(resume, stream=self.stream.cuda_stream)   # TableFull: refused before listening
+            info = None
+            for s, sh in enumerate(self.shards):
+                try:
+                    info = sh["table"].load_piece(resume, sh["table"].capacity, stream=sh["stream"].cuda_stream)
+                except TableFull as e:                       # refused before listening
+                    where = " (shard %d of %d, buckets [%d, %d) on cuda:%d)" % (s, W, sh["lo"], sh["hi"], sh["device"]) if W > 1 else ""
+                    raise TableFull("%s%s" % (e, where))
             self.time0 = info.total_time
             self.resumed = (len(self.table), info.nb_walk)
         self.t_start = time.perf_counter()
@@ -438,9 +474,19 @@ class GpuSink:
         self.full = None                                     # why the table stopped the run
         self.failed = None                                   # an ingest error
         self.last_save = None                                # (path, error or None)
-        self.batches, self.t_copy, self.t_verify, self.t_add = 0, 0.0, 0.0, 0.0
+        self.batches, self.t_copy, self.t_verify, self.t_add, self.t_peer = 0, 0.0, 0.0, 0.0, 0.0
+        self._turn = 0                                        # batches taken: the next one goes to gpus[_turn % len(gpus)]
         self._thread = threading.Thread(target=self._loop, name="ingest", daemon=True)
         self._thread.start()
+
+    def describe(self):
+        """the start line's words for the table"""
+        if len(self.shards) == 1:
+            return "capacity %d entries (%.2f GB) on cuda:%d%s" % (self.table.capacity, self.table.memory_bytes() / 1e9, self.plan[0][0],
+                                                                  host_note(self.table))
+        return "in %d shards on cuda:%s, capacity %d entries each (%.2f GB in all)%s" % (
+            len(self.shards), ",".join(str(d) for d, _, _ in self.plan), self.shard_capacity, self.table.memory_bytes() / 1e9,
+            host_note(self.table))
 
     # -- the Server's sink -----------------------------------------------------------------------------------------------
     def put(self, msg, chunks):
@@ -471,8 +517,10 @@ class GpuSink:
         self._thread.join()
 
     def close(self):
-        self.table.close()
-        self.resolver.close()
+        for sh in self.shards:
+            sh["table"].close()
+        for g in self.gpus.values():
+            g["resolver"].close()
 
     # -- the ingest thread -------------------------------------------------------------------------------------------------
     def _loop(self):
@@ -501,7 +549,15 @@ class GpuSink:
         self.saving -= 1
 
     def _write_table(self, path):
-        self.table.save_work(path, self.dp, self.start, self.end, self.pub, 0, self.elapsed(), 0, stream=self.stream.cuda_stream)
+        from .solver import piece_offsets, work_header
+        with open(path, "wb") as f:
+            f.write(work_header(self.dp, self.start, self.end, self.pub, 0, self.elapsed()))
+        offsets = piece_offsets([sh["table"].piece_bytes() for sh in self.shards])
+        for sh, o in zip(self.shards, offsets):
+            sh["table"].save_piece(path, o, stream=sh["stream"].cuda_stream)
+        with open(path, "r+b") as f:
+            f.seek(offsets[-1])
+            f.write(struct.pack("<Q", 0))                    # no kangaroos
 
     def _stage(self, batch):
         """the batch's records into the pinned host buffer -> (bytes, records, end of each chunk in records)"""
@@ -525,192 +581,6 @@ class GpuSink:
         for msg, _, last in batch:
             if last and msg.bad:
                 self.out(msg.wrong_line())
-
-    def _ingest(self, batch):
-        torch = self.torch
-        off, n, ends = self._stage(batch)
-        st = self.stream
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
-        with torch.cuda.stream(st):
-            ev[0].record(st)
-            self._recs[:off].copy_(self._host[:off], non_blocking=True)
-            ev[1].record(st)
-            self.resolver.verify_raw(self._recs.data_ptr(), n, self._good.data_ptr(), self._counts.data_ptr(), self._bad.data_ptr(),
-                                     CHUNK_RECORDS, self._scratch.data_ptr(), self._scratch_bytes, st.cuda_stream)
-            ev[2].record(st)
-            self._counts_h.copy_(self._counts, non_blocking=True)
-        st.synchronize()
-        self.t_copy += ev[0].elapsed_time(ev[1]) / 1e3
-        self.t_verify += ev[1].elapsed_time(ev[2]) / 1e3
-        n_good, n_bad = (int(v) for v in self._counts_h.tolist())
-        self.received += n
-        with torch.cuda.stream(st):
-            self._charge(batch, ends, n_bad, self._bad)
-        if n_good:
-            t0 = time.perf_counter()
-            try:
-                evs = self.table.add(self._good.data_ptr(), [n_good], n_good, st.cuda_stream, self.resolver)
-            except self.TableFull as e:
-                self.full = "%s (%d entries, capacity %d; this batch brought %d more)" % (e, len(self.table), self.table.capacity, n_good)
-                return
-            self.t_add += time.perf_counter() - t0
-            self._events(evs)
-        self.batches += 1
-
-    def _events(self, evs):
-        from .ingest import EV_RESET, EV_COLLISION
-        from .solver import print_key
-        for e in evs:
-            if e[0] == EV_RESET:
-                self.dead += 1                               # the reference's collisionInSameHerd
-            elif e[0] == EV_COLLISION:
-                if e[5] is not None:
-                    if self.solved is None and ec.mul(e[5][1]) == self.pub:
-                        self.solved = e[5][1]
-                        print_key(0, self.pub, self.solved)
-                        sys.stdout.flush()
-                else:
-                    self.wrong_collisions += 1
-                    self.out("Unexpected wrong collision (kIdx %d, bucket h of d %016X%016X / %016X%016X)" %
-                             (e[2], e[3][1], e[3][0], e[4][1], e[4][0]))
-
-
-def shard_plan(devices):
-    """--devices -> [(device, lo, hi)] per shard: shard s of W holds the buckets [floor(s*2^18/W), floor((s+1)*2^18/W)), the
-    range rank s of the solver's --dp-table sharded holds, so the pieces of a work file sit where the solver puts them"""
-    from .dist import owner_ranges
-    return [(d, lo, hi) for d, (lo, hi) in zip(devices, owner_ranges(len(devices)))]
-
-
-def host_note(table):
-    """the words the start line adds for a table (or ShardTables) with its entries in pinned host memory"""
-    hb = table.host_bytes()
-    return ", entries in pinned host memory (%.2f GB)" % (hb / 1e9) if hb else ""
-
-
-class ShardTables:
-    """the shards of a ShardedSink as one table for the status line and the messages: entries, capacity and memory summed"""
-
-    def __init__(self, tables):
-        self.shards = tables
-        self.capacity = sum(t.capacity for t in tables)
-
-    def __len__(self):
-        return sum(len(t) for t in self.shards)
-
-    def memory_bytes(self):
-        return sum(t.memory_bytes() for t in self.shards)
-
-    def host_bytes(self):
-        return sum(t.host_bytes() for t in self.shards)
-
-    def fullest(self):
-        """-> (shard, entries, capacity) of the shard with the largest fill"""
-        s = max(range(len(self.shards)), key=lambda i: len(self.shards[i]) / self.shards[i].capacity)
-        return s, len(self.shards[s]), self.shards[s].capacity
-
-
-class ShardedSink(GpuSink):
-    """--devices with two or more entries: the table split into one shard per entry (shard_plan), a DeviceDPTable of its
-    buckets on that entry's GPU; a GPU listed k times holds k shards.  Each distinct GPU has one resolver, shared by its shards,
-    and one set of batch buffers; each shard has its own stream and, when there are several GPUs, a staging buffer on its GPU.
-    Everything is allocated here.  capacity is per shard; by default each GPU's free memory, less its buffers, is split
-    evenly among its shards.
-
-    The ingest thread, per batch: one copy to the next GPU in turn (spreading the verify), kgx_resolver_verify_partition there
-    (the check, the good records grouped by shard in input order, the per-shard and bad counts), the counts back; then, unless
-    some shard would overflow (nothing of the batch is added then), each shard's group -- read in place on the batch's GPU, or
-    copied to the shard's staging buffer on another one -- added with its GPU's resolver on the shard's stream.  Each add
-    waits for its own work, and a batch is done before the next starts, so every bucket sees its records in queue order, as
-    the one table does.  A save writes the header, then each shard's piece at its offset: the one table's file, byte for byte."""
-
-    def __init__(self, start, end, pub, dp, devices, capacity=None, resume=None, save_path="", out=print, entries="device"):
-        import torch
-        from .ingest import DeviceDPTable, DeviceResolver, DPTable, TableFull
-        from .solver import DP_TABLE_MARGIN, default_table_capacity, host_entries_limit, mem_available, scratch_bytes
-        self.torch, self.TableFull = torch, TableFull
-        self.start, self.end, self.pub, self.dp = start, end, pub, dp
-        self.save_path, self.out = save_path, out
-        self.plan = shard_plan(devices)
-        W = len(self.plan)
-        gpus = sorted(set(devices))
-        K = ec.add(pub, ec.neg(ec.mul(start))) if start else pub
-        self.gpus = {}                                        # device -> its resolver, batch buffers and stream
-        for d in gpus:
-            dev = torch.device("cuda", d)
-            r = DeviceResolver(DPTable.key_table([K]), start, device=d)
-            nb = r.verify_partition_scratch_bytes(CHUNK_RECORDS, W)
-            self.gpus[d] = dict(resolver=r, nb=nb, stream=torch.cuda.Stream(device=dev),
-                                recs=torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8, device=dev),
-                                out=torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8, device=dev),
-                                bad=torch.empty(CHUNK_RECORDS, dtype=torch.int32, device=dev),
-                                counts=torch.empty(W + 1, dtype=torch.int32, device=dev),
-                                scratch=torch.empty(nb, dtype=torch.uint8, device=dev))
-        self._host = torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8).pin_memory()
-        self._host_np = self._host.numpy()
-        self._counts_h = torch.empty(W + 1, dtype=torch.int32).pin_memory()
-        staged = len(gpus) > 1
-        per_shard = scratch_bytes(CHUNK_RECORDS) + EVENT_BYTES * CHUNK_RECORDS + (CHUNK_RECORDS * DP40 if staged else 0)
-        self.entries = entries
-        host_limit = host_entries_limit(mem_available(), W) if entries == "host" else None   # the host's RAM shared by all shards
-        caps = {}
-        for d in gpus:                                        # before any table takes memory
-            k = devices.count(d)
-            caps[d] = capacity or default_table_capacity((torch.cuda.mem_get_info(d)[0] - DP_TABLE_MARGIN) // k - per_shard,
-                                                         margin=0, entries=entries, host_limit=host_limit)
-        self.shards = []
-        for s, (d, lo, hi) in enumerate(self.plan):
-            dev = torch.device("cuda", d)
-            t = DeviceDPTable(caps[d], device=d, max_events=CHUNK_RECORDS, buckets=(lo, hi), entries=entries)
-            t.reserve(CHUNK_RECORDS)
-            self.shards.append(dict(table=t, device=d, lo=lo, hi=hi, stream=torch.cuda.Stream(device=dev),
-                                    staging=torch.empty(CHUNK_RECORDS * DP40, dtype=torch.uint8, device=dev) if staged else None))
-        self.table = ShardTables([sh["table"] for sh in self.shards])
-        self.shard_capacity = max(caps.values())
-        self.time0 = 0.0
-        if resume:
-            info = None
-            for s, sh in enumerate(self.shards):
-                try:
-                    info = sh["table"].load_piece(resume, sh["table"].capacity, stream=sh["stream"].cuda_stream)
-                except TableFull as e:
-                    raise TableFull("%s (shard %d of %d, buckets [%d, %d) on cuda:%d)" % (e, s, W, sh["lo"], sh["hi"], sh["device"]))
-            self.time0 = info.total_time
-            self.resumed = (len(self.table), info.nb_walk)
-        self.t_start = time.perf_counter()
-        self.queue = RecordQueue()
-        self.dead = self.wrong = self.wrong_collisions = self.received = 0
-        self.saving = 0
-        self.solved = None
-        self.full = None
-        self.failed = None
-        self.last_save = None
-        self.batches, self.t_copy, self.t_verify, self.t_add, self.t_peer = 0, 0.0, 0.0, 0.0, 0.0
-        self._turn = 0                                        # batches taken: the next one goes to gpus[_turn % len(gpus)]
-        self._thread = threading.Thread(target=self._loop, name="ingest", daemon=True)
-        self._thread.start()
-
-    def describe(self):
-        return "%d shards on cuda:%s, capacity %d entries each (%.2f GB in all)%s" % (
-            len(self.shards), ",".join(str(d) for d, _, _ in self.plan), self.shard_capacity, self.table.memory_bytes() / 1e9,
-            host_note(self.table))
-
-    def close(self):
-        for sh in self.shards:
-            sh["table"].close()
-        for g in self.gpus.values():
-            g["resolver"].close()
-
-    def _write_table(self, path):
-        from .solver import piece_offsets, work_header
-        with open(path, "wb") as f:
-            f.write(work_header(self.dp, self.start, self.end, self.pub, 0, self.elapsed()))
-        offsets = piece_offsets([sh["table"].piece_bytes() for sh in self.shards])
-        for sh, o in zip(self.shards, offsets):
-            sh["table"].save_piece(path, o, stream=sh["stream"].cuda_stream)
-        with open(path, "r+b") as f:
-            f.seek(offsets[-1])
-            f.write(struct.pack("<Q", 0))                    # no kangaroos
 
     def _ingest(self, batch):
         torch = self.torch
@@ -739,8 +609,12 @@ class ShardedSink(GpuSink):
         for s, sh in enumerate(self.shards):                 # a saved file is always a cut between whole batches
             t = sh["table"]
             if len(t) + c[s] > t.capacity:
-                self.full = ("shard %d of %d (buckets [%d, %d) on cuda:%d) holds %d entries, capacity %d; this batch brought it %d "
-                             "more" % (s, W, sh["lo"], sh["hi"], sh["device"], len(t), t.capacity, c[s]))
+                if W > 1:
+                    self.full = ("shard %d of %d (buckets [%d, %d) on cuda:%d) holds %d entries, capacity %d; this batch brought it "
+                                 "%d more" % (s, W, sh["lo"], sh["hi"], sh["device"], len(t), t.capacity, c[s]))
+                else:                                        # the words of the add's refusal (TableFull), then the table's state
+                    self.full = ("DP table full: %d entries + %d records of this call > capacity %d (%d entries, capacity %d; this batch "
+                                 "brought %d more)" % (len(t), c[s], t.capacity, len(t), t.capacity, c[s]))
                 return
         t0 = time.perf_counter()
         first = 0
@@ -760,6 +634,58 @@ class ShardedSink(GpuSink):
             self._events(evs)
         self.t_add += time.perf_counter() - t0
         self.batches += 1
+
+    def _events(self, evs):
+        from .ingest import EV_RESET, EV_COLLISION
+        from .solver import print_key
+        for e in evs:
+            if e[0] == EV_RESET:
+                self.dead += 1                               # the reference's collisionInSameHerd
+            elif e[0] == EV_COLLISION:
+                if e[5] is not None:
+                    if self.solved is None and ec.mul(e[5][1]) == self.pub:
+                        self.solved = e[5][1]
+                        print_key(0, self.pub, self.solved)
+                        sys.stdout.flush()
+                else:
+                    self.wrong_collisions += 1
+                    self.out("Unexpected wrong collision (kIdx %d, bucket h of d %016X%016X / %016X%016X)" %
+                             (e[2], e[3][1], e[3][0], e[4][1], e[4][0]))
+
+
+def shard_plan(devices):
+    """--devices -> [(device, lo, hi)] per shard: shard s of W holds the buckets [floor(s*2^18/W), floor((s+1)*2^18/W)), the
+    range rank s of the solver's --dp-table sharded holds, so the pieces of a work file sit where the solver puts them"""
+    from .dist import owner_ranges
+    return [(d, lo, hi) for d, (lo, hi) in zip(devices, owner_ranges(len(devices)))]
+
+
+def host_note(table):
+    """the words the start line adds for a table with its entries in pinned host memory"""
+    hb = table.host_bytes()
+    return ", entries in pinned host memory (%.2f GB)" % (hb / 1e9) if hb else ""
+
+
+class ShardTables:
+    """the shards of a GpuSink as one table for the status line and the messages: entries, capacity and memory summed"""
+
+    def __init__(self, tables):
+        self.shards = tables
+        self.capacity = sum(t.capacity for t in tables)
+
+    def __len__(self):
+        return sum(len(t) for t in self.shards)
+
+    def memory_bytes(self):
+        return sum(t.memory_bytes() for t in self.shards)
+
+    def host_bytes(self):
+        return sum(t.host_bytes() for t in self.shards)
+
+    def fullest(self):
+        """-> (shard, entries, capacity) of the shard with the largest fill"""
+        s = max(range(len(self.shards)), key=lambda i: len(self.shards[i]) / self.shards[i].capacity)
+        return s, len(self.shards[s]), self.shards[s].capacity
 
 
 def expected_dps(start, end, kangaroos, dp):
@@ -784,7 +710,7 @@ def status_line(server, sink):
             (server.n_clients(), np.log2(max(k, 1)), np.log2(max(len(sink.table), 1)),
              expected_dps(sink.start, sink.end, k, sink.dp), sink.dead, sink.wrong, time_str(sink.elapsed()), len(sink.table),
              sink.table.capacity))
-    if isinstance(sink.table, ShardTables):
+    if len(sink.table.shards) > 1:
         s, n, cap = sink.table.fullest()
         line += "[fullest shard %d: %d / %d, %.1f%%]" % (s, n, cap, 100.0 * n / cap)
     return line
@@ -839,8 +765,7 @@ def parse_args(argv=None):
         a.device = 0
     if a.dp_table_entries == "host":
         from .solver import host_capacity_error, mem_available
-        shards = len(a.devices) if a.devices is not None and len(a.devices) >= 2 else 1
-        err = host_capacity_error(a.dp_table_capacity, mem_available(), shards)
+        err = host_capacity_error(a.dp_table_capacity, mem_available(), len(a.devices or [a.device]))
         if err:
             ap.error(err.replace("table(s)", "shard(s)"))
     pubs = None
@@ -872,14 +797,9 @@ def main(argv=None):
     a, start, end, pub, dp = parse_args(argv)
     out = lambda s: print(s, flush=True)
     from .ingest import TableFull
-    sharded = a.devices is not None and len(a.devices) >= 2
     try:
-        if sharded:
-            sink = ShardedSink(start, end, pub, dp, a.devices, capacity=a.dp_table_capacity, resume=a.resume or None,
-                               save_path=a.save_work, out=out, entries=a.dp_table_entries)
-        else:
-            sink = GpuSink(start, end, pub, dp, device=a.device, capacity=a.dp_table_capacity, resume=a.resume or None,
-                           save_path=a.save_work, out=out, entries=a.dp_table_entries)
+        sink = GpuSink(start, end, pub, dp, a.devices or [a.device], capacity=a.dp_table_capacity, resume=a.resume or None,
+                       save_path=a.save_work, out=out, entries=a.dp_table_entries)
     except TableFull as e:
         out("--resume %s refused: %s; give a larger --dp-table-capacity" % (a.resume, e))
         return 1
@@ -887,11 +807,7 @@ def main(argv=None):
         out("Resume %s: %d DPs" % (a.resume, sink.resumed[0]))
         if sink.resumed[1]:
             out("%d kangaroos in %s skipped: the server keeps no herd" % (sink.resumed[1], a.resume))
-    if sharded:
-        out("Range 0x%X .. 0x%X  dp %d  key 04%064X%064X  table in %s" % (start, end, dp, pub[0], pub[1], sink.describe()))
-    else:
-        out("Range 0x%X .. 0x%X  dp %d  key 04%064X%064X  table capacity %d entries (%.2f GB) on cuda:%d%s" %
-            (start, end, dp, pub[0], pub[1], sink.table.capacity, sink.table.memory_bytes() / 1e9, a.device, host_note(sink.table)))
+    out("Range 0x%X .. 0x%X  dp %d  key 04%064X%064X  table %s" % (start, end, dp, pub[0], pub[1], sink.describe()))
     stop = threading.Event()
     signals = []
 
@@ -940,7 +856,7 @@ def main(argv=None):
     if sink.full is not None:
         out("DP table full%s, server stopped: %s.  Resume with --resume %s --dp-table-capacity %d or more; the clients reconnect "
             "and resend the DPs they hold." % (" (host entries)" if a.dp_table_entries == "host" else "", sink.full, a.save_work or "FILE (give --save-work to write one)",
-                                               2 * (sink.shard_capacity if sharded else sink.table.capacity)))
+                                               2 * sink.shard_capacity))
         rc = 1
     if sink.failed is not None:
         out("Ingest failed, server stopped: %s" % sink.failed)
@@ -951,7 +867,7 @@ def main(argv=None):
         "per batch; handlers blocked %.2f s on a full queue" %
         (sink.received, sink.wrong, sink.dead, sink.wrong_collisions, sink.batches, 1e3 * sink.t_copy / max(sink.batches, 1),
          1e3 * sink.t_verify / max(sink.batches, 1), 1e3 * sink.t_add / max(sink.batches, 1), sink.queue.blocked_s))
-    if sharded:
+    if len(sink.shards) > 1:
         out("Shards: verify is verify+partition; add includes %.3f ms per batch of copies to other GPUs" %
             (1e3 * sink.t_peer / max(sink.batches, 1)))
     sink.close()

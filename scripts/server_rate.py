@@ -6,9 +6,9 @@ processes, each sending its share in SENDDP messages of --msg records over 127.0
 (Server + GpuSink, the code `python -m kangaroo_b200.server` runs), so the script reads when the last record is inserted.
 Per sender count it prints records/s inserted end to end (from the first message the server has read to the last record
 inserted; the senders' start-up is left out), the ingest thread's time
-per batch (host-to-device copy and kgx_resolver_verify from CUDA events, the add from the host clock) and how long the
-handlers blocked on a full queue.  A second pass with 8 senders runs under torch.profiler and gives the verify kernels' own
-time per batch.  The control: the same senders against oracle/_ref/kangaroo_ref_cpu -s (where it was built), its rate read
+per batch (host-to-device copy and kgx_resolver_verify_partition at one shard from CUDA events, the add from the host
+clock) and how long the handlers blocked on a full queue.  A second pass with 8 senders runs under torch.profiler and gives
+the verify kernels' own time per batch: the check, the scans and the partition passes.  The control: the same senders against oracle/_ref/kangaroo_ref_cpu -s (where it was built), its rate read
 from its DP Count line, timed from the senders' start (their start-up, about half a second, is inside its window); that server listens on all interfaces while it runs (it has no bind option).  Writes
 results/server_rate.json.
 
@@ -106,20 +106,20 @@ def run_ours(n_send, path, total, n_wrong, msg):
 
 
 def profiled_verify(path, total, n_wrong, msg, outdir):
-    """8 senders under torch.profiler -> the verify kernels' device time per batch (check, scan, compaction)"""
+    """8 senders under torch.profiler -> the verify kernels' device time per batch (check, scan, partition)"""
     import torch
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
         r = run_ours(8, path, total, n_wrong, msg)
     prof.export_chrome_trace(os.path.join(outdir, "server_rate.pt.trace.json"))
-    us = {"check": 0.0, "scan": 0.0, "compact": 0.0}
+    us = {"check": 0.0, "scan": 0.0, "partition": 0.0}
     for e in prof.key_averages():
         name = e.key
         t = getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0.0)
         if "wt_check_entries_kernel" in name and "Dp40Check" in name:
             us["check"] += t
-        elif "wt_verify_compact_kernel" in name:
-            us["compact"] += t
+        elif "k_counts" in name or (("k_hist" in name or "k_scatter" in name) and "Verified" in name):
+            us["partition"] += t
         elif "DeviceScan" in name or "ScanKernel" in name or "DeviceScanInitKernel" in name:
             us["scan"] += t                                    # cub's scan (the device table's own scans count here too)
     return {k: v / 1e3 / max(r["batches"], 1) for k, v in us.items()}, r
@@ -196,8 +196,8 @@ def main():
                                       r["blocked_s"]), flush=True)
         kern, r = profiled_verify(path, a.records, len(wrong), a.msg, os.path.dirname(a.out))
         out["verify_kernels_ms_per_batch"] = kern
-        print("profiled (8 senders, %d batches): check %.3f ms, scan %.3f ms, compaction %.3f ms per batch" %
-              (r["batches"], kern["check"], kern["scan"], kern["compact"]), flush=True)
+        print("profiled (8 senders, %d batches): check %.3f ms, scan %.3f ms, partition %.3f ms per batch" %
+              (r["batches"], kern["check"], kern["scan"], kern["partition"]), flush=True)
         if not a.no_ref:
             for n in [int(v) for v in a.senders.split(",")]:
                 r = run_ref(n, path, a.records, a.msg, tmp)

@@ -1,14 +1,13 @@
 """End-to-end rate of the DP server with its table in shards (--devices), the counterpart of scripts/server_rate.py, whose
 records, senders and clock it uses: 2^23 engine-made records (dp 8, 2^100 range), 5 % of them wrong, sent over 127.0.0.1 by 1,
-4 and 8 sender processes in SENDDP messages of 2^14 records, to a server in this process (Server + GpuSink or ShardedSink, the
-code `python -m kangaroo_b200.server` runs).
+4 and 8 sender processes in SENDDP messages of 2^14 records, to a server in this process (Server + GpuSink, the code
+`python -m kangaroo_b200.server` runs).
 
 Layouts: W = 1 (the one-GPU server) and W = 2, 4 and 8 GPUs, each where that many are visible (--devices 0,1,...), then W
 shards on GPU 0 alone (--devices 0,0,...; --one-gpu, default 2 and 4), which measures the sharded path's own cost where
 one GPU is all there is.  Per layout and sender count it prints records/s (from the first message read to the last record
-inserted), the ingest thread's time per batch: host-to-device copy and verify (kgx_resolver_verify, or
-kgx_resolver_verify_partition with shards) from CUDA events, the adds from the host clock, and inside them the copies of
-groups to other GPUs; and the default total capacity the layout would take (each GPU's free memory at start-up split among
+inserted), the ingest thread's time per batch: host-to-device copy and verify (kgx_resolver_verify_partition) from CUDA
+events, the adds from the host clock, and inside them the copies of groups to other GPUs; and the default total capacity the layout would take (each GPU's free memory at start-up split among
 its shards).  Writes results/server_shards_rate.json.
 
     python scripts/server_shards_rate.py [--records 8388608] [--msg 16384] [--senders 1,4,8] [--one-gpu 2,4]"""
@@ -38,20 +37,13 @@ def default_capacity(devices):
     for d in set(devices):
         k = devices.count(d)
         free = torch.cuda.mem_get_info(d)[0]
-        if k == 1 and len(devices) == 1:                                  # the one-GPU server's rule
-            total += default_table_capacity(free - scratch_bytes(CHUNK_RECORDS) - EVENT_BYTES * CHUNK_RECORDS)
-        else:
-            total += k * default_table_capacity((free - DP_TABLE_MARGIN) // k - per_shard, margin=0)
+        total += k * default_table_capacity((free - DP_TABLE_MARGIN) // k - per_shard, margin=0)
     return total
 
 
 def run(devices, n_send, path, total, n_wrong, msg):
-    from kangaroo_b200.server import GpuSink, Server, ShardedSink
-    cap = total + (1 << 20)
-    if len(devices) == 1:
-        sink = GpuSink(sr.START, sr.END, sr.KEY, sr.DP, device=devices[0], capacity=cap, out=lambda s: None)
-    else:
-        sink = ShardedSink(sr.START, sr.END, sr.KEY, sr.DP, devices, capacity=cap, out=lambda s: None)
+    from kangaroo_b200.server import GpuSink, Server
+    sink = GpuSink(sr.START, sr.END, sr.KEY, sr.DP, devices, capacity=total + (1 << 20), out=lambda s: None)
     srv = Server(sr.START, sr.END, sr.KEY, sr.DP, sink, bind="127.0.0.1", port=0, out=lambda s: None)
     srv.listen()
     first, put = [], sink.put
@@ -76,7 +68,7 @@ def run(devices, n_send, path, total, n_wrong, msg):
     b = max(sink.batches, 1)
     res = dict(devices=devices, senders=n_send, records=total, seconds=t1 - first[0], rate=total / (t1 - first[0]),
                batches=sink.batches, entries=len(sink.table), copy_ms=1e3 * sink.t_copy / b, verify_ms=1e3 * sink.t_verify / b,
-               add_ms=1e3 * sink.t_add / b, peer_ms=1e3 * getattr(sink, "t_peer", 0.0) / b, blocked_s=sink.queue.blocked_s)
+               add_ms=1e3 * sink.t_add / b, peer_ms=1e3 * sink.t_peer / b, blocked_s=sink.queue.blocked_s)
     sink.close()
     return res
 
@@ -111,10 +103,10 @@ def main():
             for n in [int(v) for v in a.senders.split(",")]:
                 r = run(devices, n, path, a.records, len(wrong), a.msg)
                 out["runs"].append(r)
-                print("  %d senders: %.2f M records/s (%.2f s); per batch (%d): copy %.3f ms, verify%s %.3f ms, add %.3f ms (copies "
-                      "to other GPUs %.3f ms); handlers blocked %.2f s" %
-                      (n, r["rate"] / 1e6, r["seconds"], r["batches"], r["copy_ms"], "+partition" if len(devices) > 1 else "",
-                       r["verify_ms"], r["add_ms"], r["peer_ms"], r["blocked_s"]), flush=True)
+                print("  %d senders: %.2f M records/s (%.2f s); per batch (%d): copy %.3f ms, verify+partition %.3f ms, add %.3f ms "
+                      "(copies to other GPUs %.3f ms); handlers blocked %.2f s" %
+                      (n, r["rate"] / 1e6, r["seconds"], r["batches"], r["copy_ms"], r["verify_ms"], r["add_ms"], r["peer_ms"],
+                       r["blocked_s"]), flush=True)
     with open(a.out, "w") as f:
         json.dump(out, f, indent=1)
 

@@ -178,6 +178,7 @@ def test_table_equals_in_process_table(tmp_path, engine_recs):
     finally:
         srv.close()
     text = srv.text()
+    assert re.search(r"  table capacity 1048576 entries \(\d+\.\d\d GB\) on cuda:0\n", text), text[:2000]
     assert "40 wrong DPs of 10040 from 127.0.0.1" in text and "processId 4242, threadId 1, gpuId 1" in text
     t = DeviceDPTable(1 << 20)
     try:
@@ -328,6 +329,7 @@ def test_full_table_saves_and_exits_1(tmp_path, engine_recs):
     text = srv.text()
     assert rc == 1
     assert "DP table full" in text and "--dp-table-capacity 2000" in text
+    assert "(600 entries, capacity 1000; this batch brought 1000 more)" in text
     from kangaroo_b200.ingest import read_work_header
     assert read_work_header(str(work)).key == KEY
     assert "Work file %s written: 600 DPs" % work in text
