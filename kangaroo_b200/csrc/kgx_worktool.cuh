@@ -538,61 +538,26 @@ static int set_device(int dev) {
   return 0;
 }
 
-// *ok = key on the curve; K (16 words on the device) = key - start*G, *kinf = K is the point at infinity
-static int key_setup(DevBufs& B, const uint64_t kx[4], const uint64_t ky[4], const uint64_t rs[4], cudaStream_t st, int* ok,
-                     u32** K, int* kinf) {
-  u32 *dKey, *tab = nullptr, *scal = nullptr, *ky_ = nullptr;
-  int* dOk;
-  if (B.dev(&dKey, 64) || B.dev(&dOk, 4)) return -3;
-  uint64_t key[8];
-  memcpy(key, kx, 32); memcpy(key + 4, ky, 32);
-  const int one = 1;
-  WT_CK(cudaMemcpyAsync(dKey, key, 64, cudaMemcpyHostToDevice, st));
-  WT_CK(cudaMemcpyAsync(dOk, &one, 4, cudaMemcpyHostToDevice, st));
-  wt_on_curve_kernel<<<1, 32, 0, st>>>(dKey, 1, dOk);
-  WT_CK(cudaGetLastError());
-  WT_CK(cudaMemcpyAsync(ok, dOk, 4, cudaMemcpyDeviceToHost, st));
-  WT_CK(cudaStreamSynchronize(st));
-  if (!K || !*ok) return 0;
-  // s = (n - start mod n) mod n
-  using kgx::kOrderHost;
-  u64 a[4], s[4] = {0, 0, 0, 0};
-  memcpy(a, rs, 32);
-  if (kgx::ge256(a, kOrderHost)) kgx::sub256(a, a, kOrderHost);
-  if (a[0] | a[1] | a[2] | a[3]) kgx::sub256(s, kOrderHost, a);
-  if (B.dev(&tab, 256 * 16 * 4) || B.dev(&scal, 32) || B.dev(K, 64) || B.dev(&ky_, 64)) return -3;
-  WT_CK(cudaMemcpyAsync(scal, s, 32, cudaMemcpyHostToDevice, st));
-  kgx::herd_table_kernel<<<1, 32, 0, st>>>(tab);
-  kgx::herd_kernel<<<1, 32, 0, st>>>(tab, scal, dKey, nullptr, 1, 1, *K, ky_, 0, nullptr);   // wild: key + s*G
-  WT_CK(cudaGetLastError());
-  WT_CK(cudaMemcpyAsync(*K + 8, ky_, 32, cudaMemcpyDeviceToDevice, st));
-  uint64_t kh[8];
-  WT_CK(cudaMemcpyAsync(kh, *K, 64, cudaMemcpyDeviceToHost, st));
-  WT_CK(cudaStreamSynchronize(st));
-  bool z = true;
-  for (int k = 0; k < 8; k++) z = z && kh[k] == 0;
-  *kinf = z;                                            // herd_kernel stores the point at infinity as (0, 0)
-  return 0;
-}
-
-// A batch file's keys (n x 8 limbs, public x, y) -> *ok = all on the curve; K (n x 16 words on the device) = key - start*G,
-// kinfs[k] = K is the point at infinity.  herd_kernel makes odd slots wild, so key k is computed in slot 2k + 1.
-static int keys_setup(DevBufs& B, const std::vector<uint64_t>& keys, uint32_t n, const uint64_t rs[4], cudaStream_t st, int* ok,
-                      u32** K, int** kinfs) {
+// n public keys (8 limbs each: x, y) -> *ok = all on the curve.  With K: K (n x 16 words on the device) = key - start*G, and
+// kinfs (device) and hinf (host, when given) = K is the point at infinity.  herd_kernel makes odd slots wild, so key k is
+// computed in slot 2k + 1.
+static int keys_setup(DevBufs& B, const uint64_t* keys, uint32_t n, const uint64_t rs[4], cudaStream_t st, int* ok, u32** K = nullptr,
+                      int** kinfs = nullptr, std::vector<int>* hinf = nullptr) {
   u32 *dKeys, *tab, *scal, *px, *py;
   uint16_t* tg;
   int* dOk;
-  if (B.dev(&dKeys, 64ull * n) || B.dev(&dOk, 4) || B.dev(&tab, 256 * 16 * 4) || B.dev(&scal, 64ull * n) || B.dev(&px, 64ull * n) ||
-      B.dev(&py, 64ull * n) || B.dev(&tg, 4ull * n) || B.dev(K, 64ull * n) || B.dev(kinfs, 4ull * n))
-    return -3;
+  if (B.dev(&dKeys, 64ull * n) || B.dev(&dOk, 4)) return -3;
   const int one = 1;
-  WT_CK(cudaMemcpyAsync(dKeys, keys.data(), 64ull * n, cudaMemcpyHostToDevice, st));
+  WT_CK(cudaMemcpyAsync(dKeys, keys, 64ull * n, cudaMemcpyHostToDevice, st));
   WT_CK(cudaMemcpyAsync(dOk, &one, 4, cudaMemcpyHostToDevice, st));
   wt_on_curve_kernel<<<(n + 127) / 128, 128, 0, st>>>(dKeys, n, dOk);
   WT_CK(cudaGetLastError());
   WT_CK(cudaMemcpyAsync(ok, dOk, 4, cudaMemcpyDeviceToHost, st));
   WT_CK(cudaStreamSynchronize(st));
-  if (!*ok) return 0;
+  if (!K || !*ok) return 0;
+  if (B.dev(&tab, 256 * 16 * 4) || B.dev(&scal, 64ull * n) || B.dev(&px, 64ull * n) || B.dev(&py, 64ull * n) || B.dev(&tg, 4ull * n) ||
+      B.dev(K, 64ull * n) || B.dev(kinfs, 4ull * n))
+    return -3;
   using kgx::kOrderHost;
   u64 a[4], s[4] = {0, 0, 0, 0};
   memcpy(a, rs, 32);
@@ -610,7 +575,9 @@ static int keys_setup(DevBufs& B, const std::vector<uint64_t>& keys, uint32_t n,
   kgx::herd_kernel<<<(2 * n + 127) / 128, 128, 0, st>>>(tab, scal, dKeys, tg, 0, 2ull * n, px, py, 0, nullptr);
   WT_CK(cudaGetLastError());
   std::vector<uint32_t> hx(16ull * n), hy(16ull * n), hk(16ull * n);
-  std::vector<int> hinf(n);
+  std::vector<int> own;
+  std::vector<int>& inf = hinf ? *hinf : own;
+  inf.assign(n, 0);
   WT_CK(cudaMemcpyAsync(hx.data(), px, 64ull * n, cudaMemcpyDeviceToHost, st));
   WT_CK(cudaMemcpyAsync(hy.data(), py, 64ull * n, cudaMemcpyDeviceToHost, st));
   WT_CK(cudaStreamSynchronize(st));
@@ -621,10 +588,10 @@ static int keys_setup(DevBufs& B, const std::vector<uint64_t>& keys, uint32_t n,
       hk[16ull * k + 8 + w] = hy[16ull * k + 8 + w];
       z = z && hk[16ull * k + w] == 0 && hk[16ull * k + 8 + w] == 0;
     }
-    hinf[k] = z;                                        // herd_kernel stores the point at infinity as (0, 0)
+    inf[k] = z;                                         // herd_kernel stores the point at infinity as (0, 0)
   }
   WT_CK(cudaMemcpyAsync(*K, hk.data(), 64ull * n, cudaMemcpyHostToDevice, st));
-  WT_CK(cudaMemcpyAsync(*kinfs, hinf.data(), 4ull * n, cudaMemcpyHostToDevice, st));
+  WT_CK(cudaMemcpyAsync(*kinfs, inf.data(), 4ull * n, cudaMemcpyHostToDevice, st));
   WT_CK(cudaStreamSynchronize(st));
   return 0;
 }
@@ -688,6 +655,43 @@ static int privs_check(DevBufs& B, const std::vector<uint64_t>& keys, const std:
   WT_CK(cudaMemcpy(hy.data(), py, 64 * m, cudaMemcpyDeviceToHost));
   for (uint64_t j = 0; j < m && *bad < 0; j++)
     if (memcmp(&hx[8 * j], &keys[8ull * sel[j]], 32) || memcmp(&hy[8 * j], &keys[8ull * sel[j] + 4], 32)) *bad = sel[j];
+  return 0;
+}
+
+// Input i of a merge, checked before anything is written (Merge.cpp:56-143): opened into fs[i], positioned after its header
+// hd[i], and refused when it is of the other kind (a batch work file in a plain merge, a plain one in a batch merge), of
+// another version than the first input, with its key off the curve (a plain merge; a batch merge checks its block's keys) or
+// of another range.  *nk: its key count (a batch merge).
+static int merge_input(DevBufs& B, const char* const* paths, uint32_t i, bool batch, std::vector<FILE*>& fs,
+                       std::vector<kgx_wf::WorkHeader>& hd, uint32_t* nk) {
+  errno = 0;
+  fs[i] = fopen(paths[i], "rb");
+  if (!fs[i]) { const int e = kgx_wf::io_error(); snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", paths[i], strerror(-e)); return e; }
+  setvbuf(fs[i], nullptr, _IOFBF, 1 << 22);
+  if (!kgx_wf::read_header(fs[i], hd[i])) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s is not a HEADW work file", paths[i]); return -1; }
+  *nk = 0;
+  const int bf = kgx_batch_read(paths[i], nk, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+  if (batch && bf < 0) return bf;
+  if (batch && bf == 0) {
+    snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s is a plain HEADW work file: batch work files merge only with batch work files", paths[i]);
+    return -1;
+  }
+  if (!batch && bf == 1) {
+    snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s is a batch work file (%u keys): merging batch files is not supported", paths[i], *nk);
+    return -1;
+  }
+  if (hd[i].version != hd[0].version) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: cannot merge workfile of different version (%s)", paths[i]); return -1; }
+  if (!batch) {
+    uint64_t key[8];
+    memcpy(key, hd[i].kx, 32); memcpy(key + 4, hd[i].ky, 32);
+    int ok = 0;
+    if (keys_setup(B, key, 1, hd[i].rs, 0, &ok)) return -3;
+    if (!ok) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: key of %s does not lie on elliptic curve", paths[i]); return -1; }
+  }
+  if (memcmp(hd[i].rs, hd[0].rs, 32) || memcmp(hd[i].re, hd[0].re, 32)) {
+    snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: File range differs (%s, %s)", paths[0], paths[i]);
+    return -1;
+  }
   return 0;
 }
 
@@ -836,9 +840,12 @@ int kgx_work_check_records(int dev, int walks, const void* recs, const uint32_t*
   using namespace kgx_wt;
   if (set_device(dev)) return -3;
   DevBufs B;
-  int ok = 0, kinf = 0;
-  u32 *K = nullptr, *comb;
-  if (key_setup(B, keyx, keyy, range_start, 0, &ok, &K, &kinf)) return -3;
+  uint64_t key[8];
+  memcpy(key, keyx, 32); memcpy(key + 4, keyy, 32);
+  int ok = 0, *Kinfs;
+  u32 *K, *comb;
+  std::vector<int> kinf;
+  if (keys_setup(B, key, 1, range_start, 0, &ok, &K, &Kinfs, &kinf)) return -3;
   if (!ok) { snprintf(g_wt_err, sizeof g_wt_err, "kgx_work_check_records: the key does not lie on the curve"); return -1; }
   if (build_comb(B, &comb, 0)) return -3;
   if (n == 0) return 0;
@@ -849,16 +856,13 @@ int kgx_work_check_records(int dev, int walks, const void* recs, const uint32_t*
   WT_CK(cudaMemcpy(dRec, recs, n * (walks ? 96 : 32), cudaMemcpyHostToDevice));
   WT_CK(cudaMemset(cnt, 0, 24));
   if (walks) {
-    int* dKinf;
-    if (B.dev(&dKinf, 4)) return -3;
-    WT_CK(cudaMemcpy(dKinf, &kinf, 4, cudaMemcpyHostToDevice));
-    wt_check_walks_kernel<<<(unsigned)std::min<uint64_t>((n + 127) / 128, 4096), 128>>>(comb, (const u32*)dRec, n, K, dKinf, nullptr, dRes,
+    wt_check_walks_kernel<<<(unsigned)std::min<uint64_t>((n + 127) / 128, 4096), 128>>>(comb, (const u32*)dRec, n, K, Kinfs, nullptr, dRes,
                                                                                          dBad, cnt);
   } else {
     uint32_t* dH;
     if (B.dev(&dH, 4 * n)) return -3;
     WT_CK(cudaMemcpy(dH, hs, 4 * n, cudaMemcpyHostToDevice));
-    wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS>>>(comb, EntryCheck{(const Entry*)dRec, dH, dBad, cnt}, n, K, kinf);
+    wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS>>>(comb, EntryCheck{(const Entry*)dRec, dH, dBad, cnt}, n, K, kinf[0]);
   }
   WT_CK(cudaGetLastError());
   WT_CK(cudaMemcpy(out, walks ? dRes : dBad, n, cudaMemcpyDeviceToHost));
@@ -884,37 +888,36 @@ int kgx_work_check(int dev, const char* path, uint64_t chunk, kgx_work_check_inf
   cudaStream_t st;
   WT_CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   struct StreamGuard { cudaStream_t s; ~StreamGuard() { cudaStreamSynchronize(s); cudaStreamDestroy(s); } } sg{st};
-  int ok = 0, kinf = 0;
-  u32 *K = nullptr, *comb;
-  if (key_setup(B, hd.kx, hd.ky, hd.rs, st, &ok, &K, &kinf)) return -3;
-  if (!ok) { snprintf(g_wt_err, sizeof g_wt_err, "CheckWorkFile: key1 does not lie on elliptic curve"); return -1; }
-  if (build_comb(B, &comb, st)) return -3;
-  int* Kinfs;                                           // per key of K: the point at infinity
-  if (B.dev(&Kinfs, 4)) return -3;
-  WT_CK(cudaMemcpyAsync(Kinfs, &kinf, 4, cudaMemcpyHostToDevice, st));
-  // a batch file: every key of its block, and every kangaroo's target
+  // the file's keys: the header key, or every key of a batch file's block, with every kangaroo's target
+  uint64_t hkey[8];
+  memcpy(hkey, hd.kx, 32); memcpy(hkey + 4, hd.ky, 32);
   kgx_wf::BatchInfo bi;
   std::vector<uint64_t> bkeys;
   std::vector<uint16_t> btg;
-  {
-    FILE* g = fopen(path, "rb");
-    if (!g) { const int e = kgx_wf::io_error(); snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", path, strerror(-e)); return e; }
-    char berr[256] = "";
-    int bf = kgx_wf::batch_find(g, bi, berr, sizeof berr);
-    if (bf == 1) {
-      bkeys.resize(8ull * bi.n_keys);
-      btg.resize(bi.nb_walk);
-      if (kgx_wf::batch_read(g, bi, bkeys.data(), nullptr, nullptr, btg.data(), berr, sizeof berr)) bf = -1;
-    }
-    fclose(g);
-    if (bf < 0) { snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", path, berr); return -1; }
-    if (bf == 1) {
-      if (keys_setup(B, bkeys, bi.n_keys, hd.rs, st, &ok, &K, &Kinfs)) return -3;
-      if (!ok) { snprintf(g_wt_err, sizeof g_wt_err, "CheckWorkFile: a key of the batch block does not lie on elliptic curve"); return -1; }
-      info->n_keys = bi.n_keys;
-    }
+  char berr[256] = "";
+  FILE* g = fopen(path, "rb");
+  if (!g) { const int e = kgx_wf::io_error(); snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", path, strerror(-e)); return e; }
+  int bf = kgx_wf::batch_find(g, bi, berr, sizeof berr);
+  if (bf == 1) {
+    bkeys.resize(8ull * bi.n_keys);
+    btg.resize(bi.nb_walk);
+    if (kgx_wf::batch_read(g, bi, bkeys.data(), nullptr, nullptr, btg.data(), berr, sizeof berr)) bf = -1;
   }
-  const bool batch = info->n_keys != 0;
+  fclose(g);
+  const bool batch = bf == 1;
+  // the header key is checked first, a batch file's too; a damaged batch block is reported after it
+  int ok = 0, *Kinfs;
+  u32 *K, *comb;
+  std::vector<int> kinf;
+  if (keys_setup(B, hkey, 1, hd.rs, st, &ok, batch ? nullptr : &K, &Kinfs, &kinf)) return -3;
+  if (!ok) { snprintf(g_wt_err, sizeof g_wt_err, "CheckWorkFile: key1 does not lie on elliptic curve"); return -1; }
+  if (bf < 0) { snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", path, berr); return -1; }
+  if (batch) {
+    if (keys_setup(B, bkeys.data(), bi.n_keys, hd.rs, st, &ok, &K, &Kinfs, &kinf)) return -3;
+    if (!ok) { snprintf(g_wt_err, sizeof g_wt_err, "CheckWorkFile: a key of the batch block does not lie on elliptic curve"); return -1; }
+    info->n_keys = bi.n_keys;
+  }
+  if (build_comb(B, &comb, st)) return -3;
   // two buffers: the host fills one from disk while the device checks the other
   const uint64_t wchunk = chunk / 3 ? chunk / 3 : 1;    // walks per chunk: 96-byte records in the 32-byte entries' room
   Entry *hEnt[2], *dEnt[2];
@@ -950,7 +953,7 @@ int kgx_work_check(int dev, const char* path, uint64_t chunk, kgx_work_check_inf
         wt_check_entries_multi_kernel<<<(unsigned)((n + CHECK_THREADS - 1) / CHECK_THREADS), CHECK_THREADS, 0, st>>>(
             comb, dEnt[b], dH[b], n, K, Kinfs, bi.n_keys, dBad[b], dCnt[b]);
       else
-        wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS, 0, st>>>(comb, EntryCheck{dEnt[b], dH[b], dBad[b], dCnt[b]}, n, K, kinf);
+        wt_check_entries_kernel<<<check_blocks(n), CHECK_THREADS, 0, st>>>(comb, EntryCheck{dEnt[b], dH[b], dBad[b], dCnt[b]}, n, K, kinf[0]);
     } else {
       WT_CK(cudaMemcpyAsync(dEnt[b], hEnt[b], 96 * n, cudaMemcpyHostToDevice, st));
       if (batch) WT_CK(cudaMemcpyAsync(dTg[b], btg.data() + first, 2 * n, cudaMemcpyHostToDevice, st));
@@ -1045,26 +1048,9 @@ int kgx_work_merge(int dev, const char* const* paths, uint32_t n_paths, const ch
   struct Closer { std::vector<FILE*>& v; ~Closer() { for (FILE* f : v) if (f) fclose(f); } } closer{fs};
   std::vector<kgx_wf::WorkHeader> hd(n_paths);
   DevBufs B;
-  // Merge.cpp:56-143: every input is checked before anything is written
   for (uint32_t i = 0; i < n_paths; i++) {
-    errno = 0;
-    fs[i] = fopen(paths[i], "rb");
-    if (!fs[i]) { const int e = kgx_wf::io_error(); snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", paths[i], strerror(-e)); return e; }
-    setvbuf(fs[i], nullptr, _IOFBF, 1 << 22);
-    if (!kgx_wf::read_header(fs[i], hd[i])) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s is not a HEADW work file", paths[i]); return -1; }
-    uint32_t nk = 0;                                    // batch work files (--batch-keys) are not merged
-    if (kgx_batch_read(paths[i], &nk, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr) == 1) {
-      snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s is a batch work file (%u keys): merging batch files is not supported", paths[i], nk);
-      return -1;
-    }
-    if (hd[i].version != hd[0].version) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: cannot merge workfile of different version (%s)", paths[i]); return -1; }
-    int ok = 0;
-    if (key_setup(B, hd[i].kx, hd[i].ky, hd[i].rs, 0, &ok, nullptr, nullptr)) return -3;
-    if (!ok) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: key of %s does not lie on elliptic curve", paths[i]); return -1; }
-    if (memcmp(hd[i].rs, hd[0].rs, 32) || memcmp(hd[i].re, hd[0].re, 32)) {
-      snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: File range differs (%s, %s)", paths[0], paths[i]);
-      return -1;
-    }
+    uint32_t nk;
+    if (const int e = merge_input(B, paths, i, false, fs, hd, &nk)) return e;
     if (memcmp(hd[i].kx, hd[0].kx, 32) || memcmp(hd[i].ky, hd[0].ky, 32)) {
       snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: key differs, multiple keys not yet supported (%s, %s)", paths[0], paths[i]);
       return -1;
@@ -1134,28 +1120,13 @@ int kgx_work_merge_batch(int dev, const char* const* paths, uint32_t n_paths, co
   struct Closer { std::vector<FILE*>& v; ~Closer() { for (FILE* f : v) if (f) fclose(f); } } closer{fs};
   std::vector<kgx_wf::WorkHeader> hd(n_paths);
   DevBufs B;
-  // every input is checked before anything is written: the HEADW part as kgx_work_merge checks it, then the batch blocks
+  // every input is checked before anything is written: its HEADW part, then its batch block
   uint32_t n = 0;
   std::vector<uint64_t> keys, ki, privs, pi;             // the first input's keys; privs: the union of the recorded ones
   std::vector<uint8_t> solved, si;
   for (uint32_t i = 0; i < n_paths; i++) {
-    errno = 0;
-    fs[i] = fopen(paths[i], "rb");
-    if (!fs[i]) { const int e = kgx_wf::io_error(); snprintf(g_wt_err, sizeof g_wt_err, "%s: %s", paths[i], strerror(-e)); return e; }
-    setvbuf(fs[i], nullptr, _IOFBF, 1 << 22);
-    if (!kgx_wf::read_header(fs[i], hd[i])) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s is not a HEADW work file", paths[i]); return -1; }
-    uint32_t nk = 0;
-    const int bf = kgx_batch_read(paths[i], &nk, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
-    if (bf < 0) return bf;
-    if (bf == 0) {
-      snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s is a plain HEADW work file: batch work files merge only with batch work files", paths[i]);
-      return -1;
-    }
-    if (hd[i].version != hd[0].version) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: cannot merge workfile of different version (%s)", paths[i]); return -1; }
-    if (memcmp(hd[i].rs, hd[0].rs, 32) || memcmp(hd[i].re, hd[0].re, 32)) {
-      snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: File range differs (%s, %s)", paths[0], paths[i]);
-      return -1;
-    }
+    uint32_t nk;
+    if (const int e = merge_input(B, paths, i, true, fs, hd, &nk)) return e;
     if (i == 0) n = nk;
     if (nk != n) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: %s holds %u keys, %s %u: the key lists differ", paths[i], nk, paths[0], n); return -1; }
     ki.assign(8ull * n, 0); pi.assign(4ull * n, 0); si.assign(n, 0);
@@ -1186,7 +1157,7 @@ int kgx_work_merge_batch(int dev, const char* const* paths, uint32_t n_paths, co
   int ok = 0;
   u32* K;
   int* kinfs;
-  if (keys_setup(B, keys, n, hd[0].rs, 0, &ok, &K, &kinfs)) return -3;
+  if (keys_setup(B, keys.data(), n, hd[0].rs, 0, &ok, &K, &kinfs)) return -3;
   if (!ok) { snprintf(g_wt_err, sizeof g_wt_err, "MergeWork: a key of %s does not lie on elliptic curve", paths[0]); return -1; }
   int64_t bad = -1;
   if (privs_check(B, keys, solved, privs, n, &bad)) return -3;

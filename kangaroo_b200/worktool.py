@@ -279,6 +279,14 @@ def dir_inputs(dirname):
     return sorted(files, key=lambda f: (-os.path.getsize(f), os.path.basename(f)))
 
 
+def _same_version_and_range(paths, p, h, first):
+    """MergeWork's refusals of input p (header h) against paths[0] (header first): another version or range -> ValueError"""
+    if h.version != first.version:
+        raise ValueError("MergeWork: cannot merge workfile of different version (%s)" % p)
+    if (h.range_start, h.range_end) != (first.range_start, first.range_end):
+        raise ValueError("MergeWork: File range differs (%s, %s)" % (paths[0], p))
+
+
 def validate(paths):
     """MergeWork's refusals (Merge.cpp:56-143), before the device is touched: fewer than two inputs, a directory, a file that
     is not HEADW, another version, a key off the curve, another range or another key -> ValueError"""
@@ -294,13 +302,8 @@ def validate(paths):
         x, y = h.key
         if not (x < ec.P and y < ec.P and (y * y - x * x * x - 7) % ec.P == 0):
             raise ValueError("MergeWork: key of %s does not lie on elliptic curve" % p)
-        if first is None:
-            first = h
-            continue
-        if h.version != first.version:
-            raise ValueError("MergeWork: cannot merge workfile of different version (%s)" % p)
-        if (h.range_start, h.range_end) != (first.range_start, first.range_end):
-            raise ValueError("MergeWork: File range differs (%s, %s)" % (paths[0], p))
+        first = first or h
+        _same_version_and_range(paths, p, h, first)
         if h.key != first.key:
             raise ValueError("MergeWork: key differs, multiple keys not yet supported (%s, %s)" % (paths[0], p))
 
@@ -314,11 +317,7 @@ def validate_batch(paths, blocks):
             raise ValueError("MergeWork: %s is a plain HEADW work file: batch work files merge only with batch work files" % p)
     h0, b0 = read_work_header(paths[0]), blocks[0]
     for p, b in zip(paths[1:], blocks[1:]):
-        h = read_work_header(p)
-        if h.version != h0.version:
-            raise ValueError("MergeWork: cannot merge workfile of different version (%s)" % p)
-        if (h.range_start, h.range_end) != (h0.range_start, h0.range_end):
-            raise ValueError("MergeWork: File range differs (%s, %s)" % (paths[0], p))
+        _same_version_and_range(paths, p, read_work_header(p), h0)
         if b.n_keys != b0.n_keys:
             raise ValueError("MergeWork: %s holds %d keys, %s %d: the key lists differ" % (p, b.n_keys, paths[0], b0.n_keys))
         for k, (q, q0) in enumerate(zip(b.pubs, b0.pubs)):

@@ -57,6 +57,8 @@ def refusal_inputs(tmp_path, what):
         return [a, work(tame=(33,)).write(str(tmp_path / "b.work"))], "plain HEADW"
     if what == "range":
         return [a, write_batch(tmp_path / "b.work", work(end=END + 1, tame=(33,)))], "range differs"
+    if what == "range+fewer":                             # two faults in one input: the range is refused first
+        return [a, write_batch(tmp_path / "b.work", work(end=END + 1, tame=(33,)), pubs=PUBS[:63])], "range differs"
     if what == "conflict":
         privs = list(ANSWERS)
         privs[1] = (2 * START - ANSWERS[1]) % ec.N
@@ -68,4 +70,4 @@ def refusal_inputs(tmp_path, what):
     raise ValueError(what)
 
 
-CPU_REFUSALS = ["order", "fewer", "plain", "range", "conflict"]
+CPU_REFUSALS = ["order", "fewer", "plain", "range", "range+fewer", "conflict"]

@@ -213,7 +213,7 @@ def test_the_merge_finds_a_key_and_leaves_solved_ones_alone(tmp_path):
     assert wt.check(dest).ok
 
 
-@pytest.mark.parametrize("what", ["order", "fewer", "plain", "range", "conflict", "tampered"])
+@pytest.mark.parametrize("what", ["order", "fewer", "plain", "range", "range+fewer", "conflict", "tampered"])
 def test_refusals_on_the_device_write_nothing(tmp_path, what):
     inputs, match = refusal_inputs(tmp_path, what)
     tmp = str(tmp_path / "m.work.tmp")

@@ -155,6 +155,26 @@ def test_check_corrupted_fixture_gives_the_reference_count(tmp_path):
         assert "DP Wrong: %d" % want in ref
 
 
+def test_check_refuses_keys_off_the_curve(tmp_path):
+    """kgx_work_check's key refusals in their order: the header key first, in a plain or a batch file, and before a damaged
+    batch block is reported; then the keys of the batch block"""
+    from tests.batch_merge_util import PUBS, work, write_batch
+    off = (PUBS[0][0], PUBS[0][1] ^ 2)
+    head_off = write_batch(tmp_path / "h.work", work(pub0=off))
+    good = write_batch(tmp_path / "g.work", work())
+    for name, src in (("hd.work", head_off), ("gd.work", good)):                   # the batch block's footer cut short
+        (tmp_path / name).write_bytes(open(src, "rb").read()[:-1])
+    cases = [(work(pub0=off).write(str(tmp_path / "p.work")), "key1 does not lie on elliptic curve"),
+             (head_off, "key1 does not lie on elliptic curve"),
+             (str(tmp_path / "hd.work"), "key1 does not lie on elliptic curve"),
+             (str(tmp_path / "gd.work"), "no batch block footer"),
+             (write_batch(tmp_path / "b.work", work(), pubs=[PUBS[0], off]), "a key of the batch block does not lie on elliptic curve")]
+    for path, match in cases:
+        with pytest.raises(ValueError, match=match):
+            wt.check(path)
+    assert wt.check(good).ok
+
+
 def solver(args, timeout=900):
     p = subprocess.run([sys.executable, "-m", "kangaroo_b200.solver"] + args, capture_output=True, text=True, timeout=timeout, cwd=ROOT)
     out = p.stdout + p.stderr
@@ -248,6 +268,9 @@ def test_merge_refuses_bad_inputs_on_the_device(tmp_path):
     w = Work.read(pb); w.end += 1
     with pytest.raises(ValueError, match="range differs"):
         wt.merge_files([pa, w.write(str(tmp_path / "r.work"))], str(tmp_path / "o.work"))
+    w.key = (w.key[0], w.key[1] ^ 2)                                                # off the curve and another range: the curve first
+    with pytest.raises(ValueError, match="does not lie on elliptic curve"):
+        wt.merge_files([pa, w.write(str(tmp_path / "cr.work"))], str(tmp_path / "o.work"))
     assert not os.path.exists(str(tmp_path / "o.work"))
 
 

@@ -25,7 +25,8 @@ def small(tmp_path, name, **kw):
 
 @pytest.mark.parametrize("what,match", [
     ("one", "at least two"), ("range", "range differs"), ("key", "key differs"), ("version", "different version"),
-    ("curve", "does not lie on elliptic curve"), ("nothw", "not a HEADW"), ("dir", "directory")])
+    ("curve", "does not lie on elliptic curve"), ("curve+range", "does not lie on elliptic curve"), ("nothw", "not a HEADW"),
+    ("dir", "directory")])
 def test_merge_refusals_write_nothing(tmp_path, what, match):
     from tests.golden import make_work_golden as g
     a = small(tmp_path, "a.work")
@@ -40,6 +41,9 @@ def test_merge_refusals_write_nothing(tmp_path, what, match):
     elif what == "curve":
         x, y = ec.mul(g.PRIV)
         inputs = [a, small(tmp_path, "b.work", key=(x, y + 1))]
+    elif what == "curve+range":                             # two faults in one input: the curve is refused first
+        x, y = ec.mul(g.PRIV)
+        inputs = [a, small(tmp_path, "b.work", key=(x, y + 1), end=g.START + (1 << 40))]
     elif what == "nothw":
         (tmp_path / "b.work").write_bytes(b"\x00" * 400)
         inputs = [a, str(tmp_path / "b.work")]
